@@ -123,6 +123,23 @@ int tds_b200_step_jacobian_device(tds_b200_sim* sim, int mode, int use_pd, const
 int tds_b200_step_jacobian_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd,
                                 const double* tau_or_action, double* jac);
 
+/* Vector-Jacobian product of one step per environment, g_in = g_out^T J with J, rows and columns as above, by reverse mode:
+ * the step kernel on a taping fp64 scalar, one lane per environment, then a reverse sweep in the same lane (DESIGN.md 7.8).
+ * The gradient is that of the fp64 world-frame step at the fp32-rounded inputs, of the branch taken.  Argument checks as for
+ * the Jacobian: mode WORLD -> -2, use_pd without tds_b200_set_env -> -3, a NULL required pointer -> -1.
+ *   device: q, qd, tau_or_action as in tds_b200_step_device; g_out [rows][n_stride], g_in [cols][n_stride] fp64.  Environments
+ *           run in chunks of at most 2 GB of tape; the call synchronises its stream after every chunk (it reads the tape's
+ *           overflow flag, and reruns a chunk with twice the capacity when it is set; the capacity stays grown).
+ *   host:   q [n][n_q], qd [n][n_qd], tau_or_action [n][n_tau | n_act] fp64 (rounded to fp32 before the step),
+ *           g_out [n][rows], g_in [n][cols] fp64.  Synchronous.
+ * tds_b200_vjp_tape_info: info[0] = tape capacity in use (nodes per lane), info[1] = environments per chunk at that capacity
+ * (a batch of more environments runs in several chunks). */
+int tds_b200_step_vjp_device(tds_b200_sim* sim, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                             const double* g_out, double* g_in, void* stream);
+int tds_b200_step_vjp_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd,
+                           const double* tau_or_action, const double* g_out, double* g_in);
+int tds_b200_vjp_tape_info(const tds_b200_sim* sim, int info[2]);
+
 /* Stand-alone integration stages of the fine-grained surface (device SoA arrays as above):
  * integrate_euler (src/dynamics/integrator.hpp:10-133): qd += qdd dt (qdd may be NULL = zero), q += qd dt, floating base
  * quaternion increment + normalisation; integrate_euler_qdd (:141-195): qd += qdd dt only. */
@@ -292,6 +309,16 @@ int tds_b200_rigid_set_params(tds_b200_rigid* h, double dt, const double* gravit
 int tds_b200_rigid_step_device(tds_b200_rigid* h, const double* state_in, double* state_out, const double* force, int steps, void* stream);
 int tds_b200_rigid_step_host(tds_b200_rigid* h, const double* state, const double* force, int steps, double* state_out);
 int tds_b200_rigid_jacobian_host(tds_b200_rigid* h, const double* state, const double* force, int steps, double* state_out, double* jac);
+/* Vector-Jacobian product of `steps` World::step calls: (g_state, g_force) = g_state_out^T d state_out / d (state, force), by the
+ * taping instance of the rigid-body kernel one step at a time: the forward keeps the steps + 1 states on the device, then steps
+ * single-step reverse sweeps run backwards, chaining the state cotangent (the tape never holds more than one step).  The force
+ * acts in the first step only.  force may be NULL (zero force); g_force may be NULL.
+ *   device: state / g_state_out / g_state [13 n_bodies][n_stride], force / g_force [3 n_bodies][n_stride] fp64
+ *   host:   state, g_state_out, g_state [n_worlds][n_bodies][13], force, g_force [n_worlds][n_bodies][3] fp64.  Synchronous. */
+int tds_b200_rigid_vjp_device(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
+                              double* g_state, double* g_force, void* stream);
+int tds_b200_rigid_vjp_host(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
+                            double* g_state, double* g_force);
 
 #ifdef __cplusplus
 }

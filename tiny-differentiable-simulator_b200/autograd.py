@@ -1,0 +1,124 @@
+"""torch.autograd bindings of the batched step (reverse mode, DESIGN.md section 7.8).
+
+    q1, qd1 = tds_b200.autograd.step(sim, q, qd, tau)          # [n_envs, dim] float32 CUDA tensors
+    loss = ((q1 - target) ** 2).sum(); loss.backward()           # q.grad, qd.grad, tau.grad
+
+The forward is the simulator's own step (BatchSim.step_device at its precision: Laikago keeps its fast mixed kernel).  The
+backward is the vector-Jacobian product of the step at the saved inputs (BatchSim.step_vjp_device): the gradient of the fp64
+world-frame step at the fp32-rounded inputs, and the gradient of the branch taken (contact set, clamps of the PD controller and
+of the Gauss-Seidel sweep), as with any operator-overloading AD.  Gradients come back as float32.  The PD gains are simulator
+settings, not autograd inputs; their cotangents are available from step_vjp_host / step_vjp_device.
+
+rigid_step does the same for a batch of rigid-body worlds (RigidWorld) on float64 [n_worlds, n_bodies, 13] / [..., 3] tensors:
+the reverse pass checkpoints the states of the rollout on the device and sweeps one step at a time.
+"""
+import torch
+
+from .sim import MODE_FD, MODE_FULL
+
+
+def _soa(x, n_stride, dtype):
+    """[n, dim] -> [max(dim, 1), n_stride] contiguous, padding environments zero."""
+    n, dim = x.shape
+    out = torch.zeros((max(dim, 1), n_stride), dtype=dtype, device=x.device)
+    if dim:
+        out[:dim, :n] = x.detach().to(dtype).t()
+    return out
+
+
+class _Step(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, sim, mode, use_pd, q, qd, tau):
+        n, ns = sim.n_envs, sim.n_stride
+        qs, qds = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32)
+        ts = None if tau is None else _soa(tau, ns, torch.float32)
+        q_out, qd_out = torch.empty_like(qs), torch.empty_like(qds)
+        qdd_out = torch.empty_like(qds) if mode == MODE_FD else None
+        sim.step_device(mode, qs, qds, ts, q_out=q_out, qd_out=qd_out, qdd_out=qdd_out, use_pd=use_pd)
+        ctx.sim, ctx.mode, ctx.use_pd, ctx.has_tau = sim, mode, use_pd, tau is not None
+        ctx.save_for_backward(qs, qds, ts if ts is not None else qs)
+        if mode == MODE_FD:
+            return qdd_out[:sim.n_qd, :n].t().contiguous()
+        return q_out[:sim.n_q, :n].t().contiguous(), qd_out[:sim.n_qd, :n].t().contiguous()
+
+    @staticmethod
+    def backward(ctx, *grads):
+        sim, mode = ctx.sim, ctx.mode
+        qs, qds, ts = ctx.saved_tensors
+        n, ns = sim.n_envs, sim.n_stride
+        rows, cols = sim.jacobian_dims(mode, ctx.use_pd)
+        dims = [sim.n_qd] if mode == MODE_FD else [sim.n_q, sim.n_qd]
+        g_out = torch.zeros((rows, ns), dtype=torch.float64, device=qs.device)
+        r = 0
+        for g, d in zip(grads, dims):
+            if g is not None:
+                g_out[r:r + d, :n] = g.to(torch.float64).t()
+            r += d
+        g_in = torch.zeros((cols, ns), dtype=torch.float64, device=qs.device)
+        sim.step_vjp_device(mode, qs, qds, ts if ctx.has_tau else None, g_out, g_in, use_pd=ctx.use_pd)
+        gq = g_in[:sim.n_q, :n].t().to(torch.float32)
+        gqd = g_in[sim.n_q:sim.n_q + sim.n_qd, :n].t().to(torch.float32)
+        gt = None
+        if ctx.has_tau:
+            k0 = sim.n_q + sim.n_qd
+            gt = g_in[k0:k0 + (sim.n_act if ctx.use_pd else sim.n_tau), :n].t().to(torch.float32)
+        return None, None, None, gq, gqd, gt
+
+
+def step(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False):
+    """One differentiable step of every environment of `sim` (a BatchSim).  q [n_envs, n_q], qd [n_envs, n_qd], tau_or_action
+    [n_envs, n_tau] (or [n_envs, n_act] with use_pd) float32 CUDA tensors.  Returns (q', qd'), or qdd in MODE_FD.  The gradient
+    is that of the fp64 world-frame step at the fp32-rounded inputs, of the branch taken; see the module docstring."""
+    for name, t in (("q", q), ("qd", qd), ("tau_or_action", tau_or_action)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or t.shape[0] != sim.n_envs):
+            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, dim] is expected")
+    return _Step.apply(sim, int(mode), bool(use_pd), q, qd, tau_or_action)
+
+
+def _on_side_stream(dev, fn, tensors):
+    """The rigid-world C-ABI reads a NULL stream as the world's own stream, and torch's default stream has the handle NULL: run
+    fn(stream) on a side stream ordered after and before torch's current stream instead."""
+    cur = torch.cuda.current_stream(dev)
+    side = torch.cuda.Stream(dev)
+    side.wait_stream(cur)
+    fn(side)
+    cur.wait_stream(side)
+    for t in tensors:
+        if t is not None:
+            t.record_stream(side)
+
+
+class _RigidStep(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, world, steps, state, force):
+        n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
+        s = _soa(state.reshape(n, 13 * nb), ns, torch.float64)
+        f = None if force is None else _soa(force.reshape(n, 3 * nb), ns, torch.float64)
+        out = torch.empty_like(s)
+        _on_side_stream(state.device, lambda st: world.step_device(s, out, f, steps, stream=st), (s, out, f))
+        ctx.world, ctx.steps, ctx.has_force = world, steps, force is not None
+        ctx.save_for_backward(s, f if f is not None else s)
+        return out[:, :n].t().reshape(n, nb, 13).contiguous()
+
+    @staticmethod
+    def backward(ctx, g):
+        world = ctx.world
+        s, f = ctx.saved_tensors
+        n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
+        g_out = _soa(g.reshape(n, 13 * nb), ns, torch.float64)
+        g_state = torch.zeros_like(g_out)
+        g_force = torch.zeros((3 * nb, ns), dtype=torch.float64, device=g.device) if ctx.has_force else None
+        _on_side_stream(g.device, lambda st: world.step_vjp_device(s, f if ctx.has_force else None, g_out, g_state, g_force,
+                                                                   ctx.steps, stream=st), (s, f, g_out, g_state, g_force))
+        gs = g_state[:, :n].t().reshape(n, nb, 13)
+        gf = g_force[:, :n].t().reshape(n, nb, 3) if ctx.has_force else None
+        return None, None, gs, gf
+
+
+def rigid_step(world, state, force=None, steps=1):
+    """`steps` differentiable World::step calls of every world of `world` (a RigidWorld).  state [n_worlds, n_bodies, 13], force
+    [n_worlds, n_bodies, 3] (applied before the first step) float64 CUDA tensors.  Returns the new state."""
+    for name, t in (("state", state), ("force", force)):
+        if t is not None and (t.dtype != torch.float64 or not t.is_cuda or t.shape[:2] != (world.n_worlds, world.n_bodies)):
+            raise ValueError(f"{name}: a float64 CUDA tensor [n_worlds, n_bodies, dim] is expected")
+    return _RigidStep.apply(world, int(steps), state, force)

@@ -14,6 +14,7 @@
 #include "tds_model.h"
 #include "tds_types.h"
 #include "tds_team.h"
+#include "tds_tape.cuh"
 
 extern "C" int tds_launch_stept(const TeamModel* TM, const TeamLink* tl_dev, const DevModel* M, const SimParams* P,
                                 const EnvParams* E, const StepIO* io, int mode, int use_pd, int precision,
@@ -30,6 +31,8 @@ extern "C" int tds_launch_step_spec(int spec, const SimParams* P, const EnvParam
                                     int precision, cudaStream_t stream);
 extern "C" int tds_launch_stepw_jacobian(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, int mode,
                                          int use_pd, int n_dirs, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_stepw_vjp(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, int mode,
+                                    int use_pd, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_stepw(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io,
                                 int mode, int use_pd, int precision, char* gscratch, int use_smem,
                                 int warps_per_block, cudaStream_t stream);
@@ -374,6 +377,12 @@ struct tds_b200_sim {
   DevModel dm_ad;         // layout of the differentiable instance (dual numbers, 16-byte scalars)
   char* jac_scratch = nullptr; size_t jac_scratch_bytes = 0;
   double* jac_dev = nullptr; size_t jac_dev_bytes = 0;
+  // vector-Jacobian product: tape capacity in nodes per lane (grows by doubling when a run overflows, and stays grown),
+  // its node / adjoint / arena buffers, the overflow flag, device staging of the host path
+  int tape_cap = 4096;
+  char* vjp_buf = nullptr; size_t vjp_buf_bytes = 0;
+  int* vjp_flag = nullptr;
+  double* vjp_g = nullptr; size_t vjp_g_bytes = 0;
   bool smem_ok[3] = {false, false, false};
   bool smem_ok_w[3] = {false, false, false};
   // 3: role-warp kernel (tds_stepr.cu), 2: lane-team kernel (tds_stept.cu), 1: one-lane world-frame kernel
@@ -613,6 +622,7 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->rq); cudaFree(s->rqd); cudaFree(s->zero_act); cudaFree(s->pol_act); cudaFree(s->sticky); cudaFree(s->r_total);
   cudaFree(s->pol_params); cudaFree(s->act_qidx); cudaFree(s->r_steps);
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
+  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
   if (s->stage_host) cudaFreeHost(s->stage_host);
   if (s->stream) cudaStreamDestroy(s->stream);
@@ -838,6 +848,124 @@ int tds_b200_step_jacobian_host(tds_b200_sim* s, int mode, int use_pd, const dou
   const size_t rc_n = (size_t)dims[0] * dims[1];
   for (int e = 0; e < n; ++e)
     for (size_t k = 0; k < rc_n; ++k) jac[(size_t)e * rc_n + k] = tmp[k * ns + e];
+  return 0;
+}
+
+// ---- vector-Jacobian product: g_in = g_out^T d(q', qd' | qdd) / d(q | qd | tau or action (| kp, kd, max_force)) by the taping
+// instance of the world-frame kernel (tds_tape.cuh), one lane per environment.  Environments run in chunks that keep arena +
+// tape + adjoints inside 2 GB; a chunk whose tape overflowed is rerun with twice the capacity (the flag is read after every
+// chunk, so the call synchronises its stream once per chunk).
+int tds_b200_step_vjp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                             const double* g_out, double* g_in, void* stream) {
+  if (!s || !q || !qd || !g_out || !g_in) return -1;
+  if (mode == 3) { set_err("vjp: modes FD, NOCONTACT, FULL"); return -2; }
+  if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+  cudaStream_t sm = (cudaStream_t)stream;
+  const size_t arena_warp = (size_t)s->dm_ad.x_total * 32 * 4;
+  const size_t cap_bytes = (size_t)2 << 30;
+  if (!s->vjp_flag) CUDA_TRY(cudaMalloc((void**)&s->vjp_flag, sizeof(int)));
+  const int n = s->n, ns = s->ns;
+  for (int e0 = 0; e0 < n;) {
+    const size_t lane_bytes = (size_t)s->tape_cap * (sizeof(tds::TapeNode) + sizeof(double));
+    size_t warps = cap_bytes / (arena_warp + 32 * lane_bytes);
+    if (warps < 1) warps = 1;
+    const size_t left = (size_t)(n - e0 + 31) / 32;
+    if (warps > left) warps = left;
+    const int chunk = (int)(warps * 32 < (size_t)(n - e0) ? warps * 32 : (size_t)(n - e0));
+    const size_t tape_b = warps * 32 * s->tape_cap * sizeof(tds::TapeNode), adj_b = warps * 32 * s->tape_cap * sizeof(double);
+    const size_t need = warps * arena_warp + tape_b + adj_b;
+    if (need > s->vjp_buf_bytes) {
+      CUDA_TRY(cudaStreamSynchronize(sm));
+      if (s->vjp_buf) cudaFree(s->vjp_buf);
+      s->vjp_buf = nullptr; s->vjp_buf_bytes = 0;
+      CUDA_TRY(cudaMalloc((void**)&s->vjp_buf, need));
+      s->vjp_buf_bytes = need;
+    }
+    StepIO io;
+    memset(&io, 0, sizeof(io));
+    io.q_in = q + e0; io.qd_in = qd + e0; io.tau_in = tau_or_action ? tau_or_action + e0 : nullptr;   // [dim][ns]: column offset
+    io.n = chunk; io.n_stride = ns;
+    io.g_out = g_out + e0; io.g_in = g_in + e0;
+    io.tape = s->vjp_buf + warps * arena_warp;
+    io.tape_adj = (double*)(s->vjp_buf + warps * arena_warp + tape_b);
+    io.tape_cap = s->tape_cap; io.tape_overflow = s->vjp_flag;
+    CUDA_TRY(cudaMemsetAsync(s->vjp_flag, 0, sizeof(int), sm));
+    int rc = tds_launch_stepw_vjp(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, s->vjp_buf, sm);
+    if (rc) { set_err(std::string("vjp launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
+    int overflow = 0;
+    CUDA_TRY(cudaMemcpyAsync(&overflow, s->vjp_flag, sizeof(int), cudaMemcpyDeviceToHost, sm));
+    CUDA_TRY(cudaStreamSynchronize(sm));
+    if (overflow) {
+      if (s->tape_cap > (1 << 28)) { set_err("vjp: tape capacity exhausted"); return -4; }
+      s->tape_cap *= 2;
+      continue;
+    }
+    e0 += chunk;
+  }
+  return 0;
+}
+
+int tds_b200_step_vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
+                           const double* tau_or_action, const double* g_out, double* g_in) {
+  if (!s || !q || !qd || !g_out || !g_in) return -1;
+  if (mode == 3) { set_err("vjp: modes FD, NOCONTACT, FULL"); return -2; }
+  if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+  CUDA_TRY(cudaSetDevice(s->device));
+  const DevModel& M = s->dm[0];
+  const int n = s->n, ns = s->ns;
+  int dims[2];
+  tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  const int n_in = use_pd ? s->E.n_act : s->n_tau;
+  const size_t maxdim = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + 1;
+  int rc = ensure_stage(s, sizeof(double) * n * maxdim, 0);
+  if (rc) return rc;
+  const size_t gb = sizeof(double) * (size_t)(dims[0] + dims[1]) * ns;
+  if (gb > s->vjp_g_bytes) {
+    if (s->vjp_g) cudaFree(s->vjp_g);
+    s->vjp_g = nullptr; s->vjp_g_bytes = 0;
+    CUDA_TRY(cudaMalloc((void**)&s->vjp_g, gb));
+    s->vjp_g_bytes = gb;
+  }
+  double* st = (double*)s->stage_dev;
+  const int T = 128, B = (n + T - 1) / T;
+  cudaStream_t sm = s->stream;
+  auto up = [&](const double* src, int dim, float* dst) -> int {
+    if (dim == 0) return 0;
+    CUDA_TRY(cudaMemcpyAsync(st, src, sizeof(double) * n * dim, cudaMemcpyHostToDevice, sm));
+    aos_to_soa_kernel<double><<<B, T, 0, sm>>>(st, dim, 0, dst, dim, n, ns);
+    return 0;
+  };
+  if ((rc = up(q, M.n_q, s->q))) return rc;
+  if ((rc = up(qd, M.n_qd, s->qd))) return rc;
+  if (tau_or_action) { if ((rc = up(tau_or_action, n_in, s->act))) return rc; }
+  else CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * ns * (n_in > 0 ? n_in : 1), sm));
+  std::vector<double> tmp((size_t)(dims[0] > dims[1] ? dims[0] : dims[1]) * ns, 0.0);
+  for (int e = 0; e < n; ++e)
+    for (int k = 0; k < dims[0]; ++k) tmp[(size_t)k * ns + e] = g_out[(size_t)e * dims[0] + k];
+  double* gout_d = s->vjp_g;
+  double* gin_d = s->vjp_g + (size_t)dims[0] * ns;
+  CUDA_TRY(cudaMemcpyAsync(gout_d, tmp.data(), sizeof(double) * dims[0] * ns, cudaMemcpyHostToDevice, sm));
+  CUDA_TRY(cudaMemsetAsync(gin_d, 0, sizeof(double) * dims[1] * ns, sm));
+  rc = tds_b200_step_vjp_device(s, mode, use_pd, s->q, s->qd, s->act, gout_d, gin_d, sm);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(tmp.data(), gin_d, sizeof(double) * dims[1] * ns, cudaMemcpyDeviceToHost, sm));
+  CUDA_TRY(cudaStreamSynchronize(sm));
+  CUDA_TRY(cudaGetLastError());
+  for (int e = 0; e < n; ++e)
+    for (int k = 0; k < dims[1]; ++k) g_in[(size_t)e * dims[1] + k] = tmp[(size_t)k * ns + e];
+  return 0;
+}
+
+// diagnostics of the VJP path: the tape capacity now in use (nodes per lane) and the environments per chunk it implies
+// (a batch larger than that runs in several chunks)
+int tds_b200_vjp_tape_info(const tds_b200_sim* s, int info[2]) {
+  if (!s || !info) return -1;
+  const size_t arena_warp = (size_t)s->dm_ad.x_total * 32 * 4;
+  const size_t lane_bytes = (size_t)s->tape_cap * (sizeof(tds::TapeNode) + sizeof(double));
+  size_t warps = ((size_t)2 << 30) / (arena_warp + 32 * lane_bytes);
+  if (warps < 1) warps = 1;
+  info[0] = s->tape_cap;
+  info[1] = (int)(warps * 32 < (size_t)1 << 30 ? warps * 32 : (size_t)1 << 30);
   return 0;
 }
 

@@ -36,6 +36,11 @@ template <typename T> struct Dual {
 template <typename T> struct is_dual { static constexpr bool value = false; };
 template <typename T> struct is_dual<Dual<T>> { static constexpr bool value = true; };
 
+// input idx of a lane whose input direction is dir: the dual instance seeds .d, the plain instances do nothing, the taping
+// instance (tds_tape.cuh) makes it leaf idx
+template <typename T> TDS_D T ad_seed(T x, int, int) { return x; }
+template <typename T> TDS_D Dual<T> ad_seed(Dual<T> x, int idx, int dir) { if (idx == dir) x.d = T(1); return x; }
+
 template <typename T> TDS_D double val_of(Dual<T> a) { return (double)a.v; }
 template <typename T> TDS_D Dual<T> min_t(Dual<T> a, Dual<T> b) { return a.v < b.v ? a : b; }
 template <typename T> TDS_D Dual<T> max_t(Dual<T> a, Dual<T> b) { return a.v > b.v ? a : b; }

@@ -15,6 +15,7 @@
 
 #include "tds_math.cuh"
 #include "tds_dual.cuh"
+#include "tds_tape.cuh"
 #include "tds_b200_model.h"
 
 #define TDS_RIGID_MAX_BODIES 16
@@ -63,6 +64,14 @@ static inline int tds_rigid_world_from_desc(const double* desc, int n_bodies, Ri
 namespace tdsrb {
 using namespace tds;
 
+// buffers of the taping instance (vector-Jacobian product of ONE step): cotangent g_out [13 nb][ns] -> g_state [13 nb][ns] and
+// g_force [3 nb][ns] (may be null; g_state must not alias g_out: a chunk that overflowed is rerun from the same g_out).  tape / adj: cap nodes /
+// adjoints per lane, interleaved by lane within a warp.  cap 0 or g_out null: values only (s_out), nothing recorded.
+struct RigidVjpIO {
+  const double* g_out; double* g_state; double* g_force;
+  TapeNode* tape; double* adj; int cap; int* overflow;
+};
+
 template <typename T> struct Contact { V3<T> n, ra, rb; T dist; int a, b; };   // normal on b, point - position of a / b
 
 // contact_sphere_sphere (contact_point.hpp:44-94) between two spheres given by centre and radius; pa / pb: the bodies' positions
@@ -100,13 +109,16 @@ TDS_D void plane_sphere(const V3<T>& pn, T pc, const V3<T>& c, T r, Contact<T>* 
 template <typename T, typename TS>
 __global__ void __launch_bounds__(128) tds_rigid_step_kernel(const __grid_constant__ RigidWorld W, const TS* s_in,
                                                              TS* s_out, const TS* __restrict__ force, int steps,
-                                                             int n, int ns, double* __restrict__ jac, int jac_dir0) {
+                                                             int n, int ns, double* __restrict__ jac, int jac_dir0,
+                                                             const RigidVjpIO vio = RigidVjpIO{}) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n) return;
   constexpr bool AD = is_dual<T>::value;
+  constexpr bool TP = is_tape<T>::value;                     // taping instance: one lane per world, one step
   const int dir = AD ? (int)blockIdx.y + jac_dir0 : -1;      // differentiable instance: input direction of this lane
   const int nb = W.n_bodies;
-  auto seed = [&](T x, int idx) -> T { if constexpr (AD) { if (idx == dir) x.d = 1.0; } return x; };
+  auto seed = [&](T x, int idx) -> T { return ad_seed(x, idx, dir); };   // d input_idx / d direction, or leaf idx of the tape
+  if constexpr (TP) tape_begin(vio.tape + ((size_t)(e >> 5) * vio.cap * 32 + (e & 31)), vio.g_out ? vio.cap : 0, vio.overflow, 16 * nb);
   V3<T> pos[TDS_RIGID_MAX_BODIES], lin[TDS_RIGID_MAX_BODIES], ang[TDS_RIGID_MAX_BODIES];
   T qx[TDS_RIGID_MAX_BODIES], qy[TDS_RIGID_MAX_BODIES], qz[TDS_RIGID_MAX_BODIES], qw[TDS_RIGID_MAX_BODIES];
   // input directions: the 13 * n_bodies state entries, then the 3 * n_bodies force entries
@@ -218,13 +230,33 @@ __global__ void __launch_bounds__(128) tds_rigid_step_kernel(const __grid_consta
       qx[b] = x * inv; qy[b] = y * inv; qz[b] = z * inv; qw[b] = ww * inv;
     }
   }
+  if constexpr (TP) {
+    auto entry = [&](int r) -> T {   // state row r = 13 b + k
+      const int b = r / 13, k = r % 13;
+      switch (k) {
+        case 0: return pos[b].x; case 1: return pos[b].y; case 2: return pos[b].z;
+        case 3: return qx[b]; case 4: return qy[b]; case 5: return qz[b]; case 6: return qw[b];
+        case 7: return lin[b].x; case 8: return lin[b].y; case 9: return lin[b].z;
+        case 10: return ang[b].x; case 11: return ang[b].y; default: return ang[b].z;
+      }
+    };
+    if (vio.g_out) {
+      double* adj = vio.adj + ((size_t)(e >> 5) * vio.cap * 32 + (e & 31));
+      if (tape_reverse(adj, 13 * nb, [&](int r) { return entry(r).id; }, [&](int r) { return vio.g_out[(size_t)r * ns + e]; }, 16 * nb)) {
+        for (int r = 0; r < 13 * nb; ++r) vio.g_state[(size_t)r * ns + e] = adj[(size_t)r * 32];
+        if (vio.g_force) for (int r = 0; r < 3 * nb; ++r) vio.g_force[(size_t)r * ns + e] = adj[(size_t)(13 * nb + r) * 32];
+      }
+    }
+    if (s_out) for (int r = 0; r < 13 * nb; ++r) s_out[(size_t)r * ns + e] = (TS)val_of(entry(r));
+    return;
+  }
   for (int b = 0; b < nb; ++b) {
     const T out[13] = {pos[b].x, pos[b].y, pos[b].z, qx[b], qy[b], qz[b], qw[b], lin[b].x, lin[b].y, lin[b].z, ang[b].x, ang[b].y, ang[b].z};
     for (int k = 0; k < 13; ++k) {
       if constexpr (AD) {
         if (jac) jac[((size_t)(b * 13 + k) * (16 * nb) + dir) * ns + e] = out[k].d;     // [row][column][world]
         if (blockIdx.y == 0 && s_out) s_out[(size_t)(b * 13 + k) * ns + e] = (TS)val_of(out[k]);
-      } else {
+      } else if constexpr (!TP) {
         s_out[(size_t)(b * 13 + k) * ns + e] = (TS)out[k];
       }
     }
@@ -242,6 +274,13 @@ struct tds_b200_rigid {
   RigidWorld W;
   int n = 0, ns = 0, device = 0;
   double *state = nullptr, *state2 = nullptr, *force = nullptr, *jac = nullptr;   // state2: output of the differentiable instance
+  // vector-Jacobian product: checkpointed states, tape capacity (nodes per lane; doubles on overflow and stays grown), tape +
+  // adjoint buffer, overflow flag, device staging of the host path
+  double* ckpt = nullptr; size_t ckpt_bytes = 0;
+  int tape_cap = 4096;
+  char* vjp_buf = nullptr; size_t vjp_buf_bytes = 0;
+  int* vjp_flag = nullptr;
+  double* vjp_g = nullptr;     // [2 * 13 n_bodies + 3 n_bodies][ns]: g_state | next state cotangent | g_force of the host path
   cudaStream_t stream = nullptr;
 };
 
@@ -275,6 +314,7 @@ void tds_b200_rigid_destroy(tds_b200_rigid* h) {
   if (!h) return;
   cudaSetDevice(h->device);
   cudaFree(h->state); cudaFree(h->state2); cudaFree(h->force); cudaFree(h->jac);
+  cudaFree(h->ckpt); cudaFree(h->vjp_buf); cudaFree(h->vjp_flag); cudaFree(h->vjp_g);
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
@@ -352,6 +392,117 @@ int tds_b200_rigid_jacobian_host(tds_b200_rigid* h, const double* state, const d
   for (int e = 0; e < n; ++e) {
     for (int k = 0; k < rows * cols; ++k) jac[(size_t)e * rows * cols + k] = t[(size_t)k * ns + e];
     if (state_out) for (int k = 0; k < rows; ++k) state_out[(size_t)e * rows + k] = so[(size_t)k * ns + e];
+  }
+  return 0;
+}
+
+using tdsrb::RigidVjpIO;
+using tds::Tape;
+using tds::TapeNode;
+
+// One launch of the taping instance over every world, in chunks of worlds whose tape + adjoints stay inside 2 GB; a chunk whose
+// tape overflowed is rerun with twice the capacity.  vio: g_out / g_state / g_force for all worlds (offset per chunk here).
+static int rigid_tape_pass(tds_b200_rigid* h, const double* s_in, double* s_out, const double* force, RigidVjpIO vio, cudaStream_t sm) {
+  const int n = h->n, ns = h->ns;
+  if (!h->vjp_flag) RB_TRY(cudaMalloc((void**)&h->vjp_flag, sizeof(int)));
+  const bool record = vio.g_out != nullptr;
+  for (int e0 = 0; e0 < n;) {
+    const size_t lane_bytes = record ? (size_t)h->tape_cap * (sizeof(TapeNode) + sizeof(double)) : 0;
+    size_t warps = record ? (((size_t)2 << 30) / (32 * lane_bytes)) : (size_t)(n + 31) / 32;
+    if (warps < 1) warps = 1;
+    const size_t left = (size_t)(n - e0 + 31) / 32;
+    if (warps > left) warps = left;
+    const int chunk = (int)(warps * 32 < (size_t)(n - e0) ? warps * 32 : (size_t)(n - e0));
+    const size_t tape_b = warps * 32 * h->tape_cap * sizeof(TapeNode), need = record ? warps * 32 * lane_bytes : 0;
+    if (need > h->vjp_buf_bytes) {
+      RB_TRY(cudaStreamSynchronize(sm));
+      cudaFree(h->vjp_buf);
+      h->vjp_buf = nullptr; h->vjp_buf_bytes = 0;
+      RB_TRY(cudaMalloc((void**)&h->vjp_buf, need));
+      h->vjp_buf_bytes = need;
+    }
+    RigidVjpIO v = vio;
+    if (record) {
+      v.g_out += e0; v.g_state += e0; if (v.g_force) v.g_force += e0;
+      v.tape = (TapeNode*)h->vjp_buf; v.adj = (double*)(h->vjp_buf + tape_b); v.cap = h->tape_cap; v.overflow = h->vjp_flag;
+      RB_TRY(cudaMemsetAsync(h->vjp_flag, 0, sizeof(int), sm));
+    }
+    const int T = 128, B = (chunk + T - 1) / T;
+    tdsrb::tds_rigid_step_kernel<Tape<double>, double><<<B, T, 0, sm>>>(h->W, s_in + e0, s_out ? s_out + e0 : nullptr,
+                                                                        force ? force + e0 : nullptr, 1, chunk, ns, nullptr, 0, v);
+    RB_TRY(cudaGetLastError());
+    if (record) {
+      int overflow = 0;
+      RB_TRY(cudaMemcpyAsync(&overflow, h->vjp_flag, sizeof(int), cudaMemcpyDeviceToHost, sm));
+      RB_TRY(cudaStreamSynchronize(sm));
+      if (overflow) {
+        if (h->tape_cap > (1 << 28)) return rigid_fail("rigid_vjp: tape capacity exhausted", -4);
+        h->tape_cap *= 2;
+        continue;
+      }
+    }
+    e0 += chunk;
+  }
+  return 0;
+}
+
+int tds_b200_rigid_vjp_device(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
+                              double* g_state, double* g_force, void* stream) {
+  if (!h || !state || !g_state_out || !g_state || steps < 0) return rigid_fail("rigid_vjp_device: bad argument", -1);
+  cudaStream_t sm = stream ? (cudaStream_t)stream : h->stream;
+  const int nb = h->W.n_bodies, ns = h->ns, rows = 13 * nb;
+  const size_t sb = sizeof(double) * (size_t)rows * ns;
+  if (g_state != g_state_out) RB_TRY(cudaMemcpyAsync(g_state, g_state_out, sb, cudaMemcpyDeviceToDevice, sm));
+  if (g_force) RB_TRY(cudaMemsetAsync(g_force, 0, sizeof(double) * 3 * nb * ns, sm));
+  if (steps == 0) return 0;
+  // forward, one step at a time, by the same instance without recording: states 0 .. steps - 1 are kept
+  if (sb * steps > h->ckpt_bytes) {
+    RB_TRY(cudaStreamSynchronize(sm));
+    cudaFree(h->ckpt);
+    h->ckpt = nullptr; h->ckpt_bytes = 0;
+    RB_TRY(cudaMalloc((void**)&h->ckpt, sb * steps));
+    h->ckpt_bytes = sb * steps;
+  }
+  RB_TRY(cudaMemcpyAsync(h->ckpt, state, sb, cudaMemcpyDeviceToDevice, sm));
+  if (!h->vjp_g) RB_TRY(cudaMalloc((void**)&h->vjp_g, sizeof(double) * (size_t)(2 * rows + 3 * nb) * ns));
+  const size_t st = (size_t)rows * ns;
+  for (int k = 0; k + 1 < steps; ++k) {
+    int rc = rigid_tape_pass(h, h->ckpt + k * st, h->ckpt + (k + 1) * st, k == 0 ? force : nullptr, RigidVjpIO{}, sm);
+    if (rc) return rc;
+  }
+  // reverse: one recorded step per launch, the state cotangent chained through g_state
+  double* gnext = h->vjp_g == g_state ? h->vjp_g + st : h->vjp_g;   // (the host path passes its own staging as g_state)
+  for (int k = steps - 1; k >= 0; --k) {
+    RigidVjpIO v{};
+    v.g_out = g_state; v.g_state = gnext; v.g_force = k == 0 ? g_force : nullptr;
+    int rc = rigid_tape_pass(h, h->ckpt + k * st, nullptr, k == 0 ? force : nullptr, v, sm);
+    if (rc) return rc;
+    RB_TRY(cudaMemcpyAsync(g_state, gnext, sb, cudaMemcpyDeviceToDevice, sm));
+  }
+  return 0;
+}
+
+int tds_b200_rigid_vjp_host(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
+                            double* g_state, double* g_force) {
+  if (!h || !state || !g_state_out || !g_state || steps < 0) return rigid_fail("rigid_vjp_host: bad argument", -1);
+  RB_TRY(cudaSetDevice(h->device));
+  int rc = rigid_upload(h, state, force);
+  if (rc) return rc;
+  const int nb = h->W.n_bodies, n = h->n, ns = h->ns, rows = 13 * nb;
+  if (!h->vjp_g) RB_TRY(cudaMalloc((void**)&h->vjp_g, sizeof(double) * (size_t)(2 * rows + 3 * nb) * ns));
+  std::vector<double> t((size_t)rows * ns, 0.0), f((size_t)3 * nb * ns, 0.0);
+  for (int e = 0; e < n; ++e) for (int k = 0; k < rows; ++k) t[(size_t)k * ns + e] = g_state_out[(size_t)e * rows + k];
+  double* gs = h->vjp_g;
+  double* gf = h->vjp_g + (size_t)2 * rows * ns;
+  RB_TRY(cudaMemcpyAsync(gs, t.data(), sizeof(double) * t.size(), cudaMemcpyHostToDevice, h->stream));
+  rc = tds_b200_rigid_vjp_device(h, h->state, force ? h->force : nullptr, steps, gs, gs, gf, h->stream);
+  if (rc) return rc;
+  RB_TRY(cudaMemcpyAsync(t.data(), gs, sizeof(double) * t.size(), cudaMemcpyDeviceToHost, h->stream));
+  RB_TRY(cudaMemcpyAsync(f.data(), gf, sizeof(double) * f.size(), cudaMemcpyDeviceToHost, h->stream));
+  RB_TRY(cudaStreamSynchronize(h->stream));
+  for (int e = 0; e < n; ++e) {
+    for (int k = 0; k < rows; ++k) g_state[(size_t)e * rows + k] = t[(size_t)k * ns + e];
+    if (g_force) for (int k = 0; k < 3 * nb; ++k) g_force[(size_t)e * 3 * nb + k] = f[(size_t)k * ns + e];
   }
   return 0;
 }

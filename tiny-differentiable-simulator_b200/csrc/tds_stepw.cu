@@ -34,7 +34,9 @@ namespace tdsw {
 // per-link region, element offsets: [rigid inertia (10 RC) | later U (6 RA), invD, u] then v / c / a (6 RA)
 
 // RQ: scalar of the state vectors (q, qd, tau): float, or the dual number type in the differentiable instance
-// (RA = RC = RS = RQ = Dual<double>: blockIdx.y + io.jac_dir0 is the input direction of the lane, see tds_dual.cuh).
+// (RA = RC = RS = RQ = Dual<double>: blockIdx.y + io.jac_dir0 is the input direction of the lane, see tds_dual.cuh),
+// or the taping scalar of the vector-Jacobian product (RA = RC = RS = RQ = Tape<double>, one lane per environment: the
+// lane records its step and sweeps it backwards from io.g_out at the end, see tds_tape.cuh).
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
@@ -47,17 +49,28 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   const bool live = env < io.n;
   const int e = live ? env : io.n - 1;
   constexpr bool AD = is_dual<RQ>::value;
+  constexpr bool TP = is_tape<RQ>::value;
   const int dir = AD ? (int)blockIdx.y + io.jac_dir0 : -1;     // differentiable instance: this lane's input direction
   Arena A;
   if (SMEM) { A.blk = smem_raw + (size_t)warp_in_blk * M.x_total * 32 * 4; A.stride = 32; A.col = lane; }
   else { A.blk = gscratch + ((size_t)blockIdx.y * ((size_t)gridDim.x * (blockDim.x >> 5)) + (size_t)(env >> 5)) * M.x_total * 32 * 4; A.stride = 32; A.col = lane; }  // per-warp block, same addressing as shared memory
-  auto seed = [&](RQ x, int idx) -> RQ { if constexpr (AD) { if (idx == dir) x.d = 1.0; } return x; };   // d input_idx / d direction
+  auto seed = [&](RQ x, int idx) -> RQ { return ad_seed(x, idx, dir); };   // d input_idx / d direction, or leaf idx of the tape
   const int ST = A.stride;
   const int ns = io.n_stride;
   const int n_links = M.n_links;
   const int n = M.n_qd;
   const int nb = M.nb;
   const int n3 = 3 * nb;
+  // VJP instance: input columns q | qd | tau or action (| kp, kd, max_force) are the first nodes of the lane's tape
+  const int n_in_ad = M.n_q + n + (use_pd ? E.n_act + 3 : n - (M.floating ? 6 : 0));
+  if constexpr (TP) tape_begin((TapeNode*)io.tape + ((size_t)(env >> 5) * io.tape_cap * 32 + lane), io.tape_cap, io.tape_overflow, n_in_ad);
+  // reverse sweep from the cotangent of the outputs out_id(r), r < n_rows; the input adjoints are this lane's g_in column
+  auto vjp_write = [&](int n_rows, auto out_id) {
+    double* adj = io.tape_adj + ((size_t)(env >> 5) * io.tape_cap * 32 + lane);
+    const bool ok = tape_reverse(adj, n_rows, out_id, [&](int r) { return io.g_out[(size_t)r * ns + e]; }, n_in_ad);
+    if (ok && live)
+      for (int k = 0; k < n_in_ad; ++k) io.g_in[(size_t)k * ns + e] = adj[(size_t)k * 32];
+  };
   int phase_id = 0;
 #define TDSW_PHASE() do { if (io.phase_clk && lane == 0) io.phase_clk[(size_t)(env >> 5) * 16 + (phase_id++)] = clock64(); } while (0)
   TDSW_PHASE();
@@ -663,6 +676,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
         a.bot = axpy(S.bot, qdd, a.bot);
         if (mode == MODE_FD) {
           if constexpr (AD) { if (live && io.jac) io.jac[((size_t)(d0 + j) * io.jac_n_in + dir) * ns + e] = qdd.d; }
+          else if constexpr (TP) qdv[(d0 + j) * ST] = qdd;   // the VJP's output rows (qd is not read again in this mode)
           else if (live && io.qdd_out) io.qdd_out[(size_t)(d0 + j) * ns + e] = (float)val_of(qdd);
         } else if (!world_step) qdv[(d0 + j) * ST] = RQ(RA(qdv[(d0 + j) * ST]) + qdd * dtA);
       }
@@ -678,6 +692,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       const int qdi = M.qd_idx[i];
       if (mode == MODE_FD) {
         if constexpr (AD) { if (live && io.jac) io.jac[((size_t)qdi * io.jac_n_in + dir) * ns + e] = qdd.d; }
+        else if constexpr (TP) qdv[qdi * ST] = qdd;
         else if (live && io.qdd_out) io.qdd_out[(size_t)qdi * ns + e] = (float)val_of(qdd);
       } else if (!world_step) qdv[qdi * ST] = RQ(RA(qdv[qdi * ST]) + qdd * dtA);
     }
@@ -691,11 +706,13 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     for (int k = 0; k < 6; ++k) {
       if (mode == MODE_FD) {
         if constexpr (AD) { if (live && io.jac) io.jac[((size_t)k * io.jac_n_in + dir) * ns + e] = qb[k].d; }
+        else if constexpr (TP) qdv[k * ST] = qb[k];
         else if (live && io.qdd_out) io.qdd_out[(size_t)k * ns + e] = (float)val_of(qb[k]);
       } else if (!world_step) qdv[k * ST] = RQ(RC(qdv[k * ST]) + qb[k] * RC(P.dt));
     }
   }
   TDSW_PHASE();  // 4
+  if constexpr (TP) { if (mode == MODE_FD) { vjp_write(n, [&](int r) { return qdv[r * ST].id; }); return; } }
   if (mode == MODE_FD) return;
 
   // ---- contact solve -------------------------------------------------------------------------------------------
@@ -951,6 +968,10 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     }
     return;
   }
+  if constexpr (TP) {   // rows q' | qd'
+    vjp_write(M.n_q + n, [&](int r) { return r < M.n_q ? qv[r * ST].id : qdv[(r - M.n_q) * ST].id; });
+    return;
+  }
   if (live) {
     bool done = false;
     if (E.reward_kind == 1) {   // laikago_environment2.h:130-171 (fixed-base emulation)
@@ -1018,6 +1039,18 @@ extern "C" int tds_launch_stepw_jacobian(const DevModel* M, const SimParams* P, 
   typedef tds::Dual<double> D;
   const dim3 grid((io->n + 31) / 32, n_dirs);
   tds_stepw_kernel<D, D, D, D, false><<<grid, 32, 0, stream>>>(*M, *P, *E, *io, mode, use_pd, gscratch);
+  return (int)cudaGetLastError();
+}
+
+// Vector-Jacobian product: the same kernel on the taping scalar (fp64), one lane per environment, 32 lanes per block.  M must
+// carry the 16-byte layout; gscratch: ceil(n / 32) blocks of x_total * 128 bytes; io->tape / io->tape_adj: ceil(n / 32) * 32
+// lanes of io->tape_cap nodes / adjoints; io->g_out -> io->g_in.  *io->tape_overflow is set when a lane's tape was too short
+// (its g_in column is then not written).
+extern "C" int tds_launch_stepw_vjp(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, int mode,
+                                    int use_pd, char* gscratch, cudaStream_t stream) {
+  using namespace tdsw;
+  typedef tds::Tape<double> T;
+  tds_stepw_kernel<T, T, T, T, false><<<(io->n + 31) / 32, 32, 0, stream>>>(*M, *P, *E, *io, mode, use_pd, gscratch);
   return (int)cudaGetLastError();
 }
 #endif  // TDS_STEPW_KERNEL_ONLY

@@ -139,4 +139,9 @@ struct StepIO {
   // rows = q' | qd' (or qdd in forward-dynamics mode), columns = q | qd | tau or action (| kp, kd, max_force with PD)
   double* jac; int jac_n_in; int jac_dir0;
   int n; int n_stride;
+  // vector-Jacobian product (tds_stepw.cu instantiated on Tape<double>, tds_tape.cuh): cotangent g_out [rows][n_stride] ->
+  // g_in [cols][n_stride], fp64, rows / columns as for jac.  tape: nodes (tds::TapeNode), tape_adj: fp64 adjoints, both
+  // tape_cap entries per lane and interleaved by lane within a warp; tape_overflow: set when a lane ran out of capacity
+  const double* g_out; double* g_in;
+  void* tape; double* tape_adj; int tape_cap; int* tape_overflow;
 };

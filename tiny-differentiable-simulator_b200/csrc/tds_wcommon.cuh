@@ -6,6 +6,7 @@
 
 #include "tds_math.cuh"
 #include "tds_dual.cuh"
+#include "tds_tape.cuh"
 #include "tds_types.h"
 #include "tds_b200_model.h"
 

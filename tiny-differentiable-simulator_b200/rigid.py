@@ -92,6 +92,25 @@ class RigidWorld:
                                                          int(steps), ctypes.c_void_p(out.ctypes.data), ctypes.c_void_p(jac.ctypes.data)), "rigid_jacobian_host")
         return out, jac
 
+    def step_vjp(self, state, force, g_state_out, steps=1):
+        """(g_state, g_force) = g_state_out^T d state_out / d (state, force) of `steps` World::step calls, by reverse mode on the
+        GPU (one recorded step at a time, the states checkpointed on the device).  Host arrays [n_worlds][n_bodies][13 | 3]."""
+        s, f = self._args(state, force)
+        g = np.ascontiguousarray(g_state_out, dtype=np.float64)
+        assert g.shape == s.shape, g.shape
+        gs, gf = np.zeros_like(s), np.zeros((self.n_worlds, self.n_bodies, 3))
+        v = lambda a: ctypes.c_void_p(a.ctypes.data) if a is not None else None
+        self._check(self._L.tds_b200_rigid_vjp_host(self._h, v(s), v(f), int(steps), v(g), v(gs), v(gf)), "rigid_vjp_host")
+        return gs, gf
+
+    def step_vjp_device(self, state, force, g_state_out, g_state, g_force=None, steps=1, stream=None):
+        """Device version of step_vjp: float64 CUDA tensors state / g_state_out / g_state [13 * n_bodies][n_stride], force / g_force
+        [3 * n_bodies][n_stride] (force None: zero force; g_force None: not computed).  stream None = the world's own stream.
+        Synchronous."""
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+        self._check(self._L.tds_b200_rigid_vjp_device(self._h, p(state), p(force), int(steps), p(g_state_out), p(g_state), p(g_force),
+                                                      ctypes.c_void_p(stream.cuda_stream) if stream is not None else None), "rigid_vjp_device")
+
     def step_device(self, state_in, state_out, force=None, steps=1, stream=None):
         """CUDA tensors, fp64: state [13 * n_bodies][n_stride], force [3 * n_bodies][n_stride] or None; in place allowed."""
         p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None

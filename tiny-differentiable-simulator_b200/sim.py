@@ -158,6 +158,41 @@ class BatchSim:
         self._check(self._L.tds_b200_step_jacobian_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), _dp(jac)), "step_jacobian_host")
         return jac
 
+    def jacobian_dims(self, mode, use_pd=False):
+        """(rows, cols) of the step's Jacobian and of its vector-Jacobian product."""
+        dims = (ctypes.c_int * 2)()
+        self._check(self._L.tds_b200_jacobian_dims(self._h, mode, int(use_pd), dims), "jacobian_dims")
+        return dims[0], dims[1]
+
+    def step_vjp_host(self, mode, q, qd, tau_or_action, g_out, use_pd=False):
+        """Vector-Jacobian product of one step per environment by reverse mode on the GPU: g_in [n, cols] = g_out [n, rows]^T J,
+        rows / cols as in step_jacobian_host.  The gradient is that of the fp64 world-frame step at the fp32-rounded inputs, of the
+        branch taken (contact set, clamps)."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        qd = np.ascontiguousarray(qd, dtype=np.float64)
+        t = None if tau_or_action is None else np.ascontiguousarray(tau_or_action, dtype=np.float64)
+        rows, cols = self.jacobian_dims(mode, use_pd)
+        g = np.ascontiguousarray(g_out, dtype=np.float64)
+        assert g.shape == (self.n_envs, rows), (g.shape, rows)
+        g_in = np.zeros((self.n_envs, cols))
+        self._check(self._L.tds_b200_step_vjp_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), _dp(g), _dp(g_in)), "step_vjp_host")
+        return g_in
+
+    def step_vjp_device(self, mode, q, qd, tau_or_action, g_out, g_in, use_pd=False, stream=None):
+        """Device version of step_vjp_host on the SoA layout: q, qd, tau_or_action float32 CUDA tensors [dim, n_stride] as for
+        step_device, g_out [rows, n_stride] and g_in [cols, n_stride] float64 CUDA tensors.  Synchronises the stream once per chunk
+        of environments (see include/tds_b200.h)."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_step_vjp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), _ptr(g_out),
+                                                     _ptr(g_in), st), "step_vjp_device")
+
+    def vjp_tape_info(self):
+        """(tape capacity in nodes per lane, environments per chunk) of the reverse-mode path as it stands."""
+        info = (ctypes.c_int * 2)()
+        self._check(self._L.tds_b200_vjp_tape_info(self._h, info), "vjp_tape_info")
+        return info[0], info[1]
+
     def integrate_host(self, q, qd, qdd, update_q=True):
         """integrate_euler (update_q) / integrate_euler_qdd of one state vector per environment, on the device
         (tds_b200_integrate_euler{,_qdd}_device); host arrays [n_q], [n_qd] for a one-environment simulator or [n, dim]."""
