@@ -140,6 +140,40 @@ int tds_b200_step_vjp_host(tds_b200_sim* sim, int mode, int use_pd, const double
                            const double* tau_or_action, const double* g_out, double* g_in);
 int tds_b200_vjp_tape_info(const tds_b200_sim* sim, int info[2]);
 
+/* ---- per-environment physical parameters (DESIGN.md 7.9): system identification and domain randomisation ----------------------
+ * Parameter ids over the flat model (for a world of several multibodies: the links of the merged model):
+ *   0                              friction (World::default_friction; SimParams friction)
+ *   1                              restitution (World::default_restitution)
+ *   2 + 10 b + c                   body b: b = 0 the floating base (floating models only), b = i + 1 link i;
+ *                                  c = mass, com x, com y, com z, inertia about the com xx, xy, xz, yy, yz, zz (off-diagonal ids are
+ *                                  the symmetric component: the value stands for both entries)
+ *   2 + 10 (n_links + 1) + 2 i + c link i: c = 0 joint stiffness, c = 1 joint damping (used at fp32, as the model stores them)
+ * tds_b200_param_count: the number of ids, 2 + 10 (n_links + 1) + 2 n_links.
+ *
+ * tds_b200_set_physical_params_*: install k parameters; the simulator copies the values into a buffer it owns.  device: values
+ * [k][n_stride] fp64 device pointer, copied on `stream`; host: values [n][k] fp64, synchronous.  k = 0 clears the set.  Refused (-2,
+ * reason in tds_b200_last_error): an id out of range, an id given twice, a base id on a fixed-base model.  While a set is installed
+ * every stepping entry point (step, Jacobian, VJP, env_step_*, env_reset settle steps, rollouts, ars_train_step, the visual stream)
+ * uses each environment's values for those ids and the model's values for the rest, on the generic world-frame kernel.  Installing
+ * another set of ids, clearing it or growing its buffer drops the captured graphs of tds_b200_env_step_host; new values for the
+ * same ids keep the buffer, so a captured graph sees them.
+ *
+ * tds_b200_step_param_jacobian_*: d(outputs) / d(installed parameters) by dual numbers, rows as tds_b200_step_jacobian_*, k columns
+ * (k directions per environment).  device: jac [rows * k][n_stride]; host: jac [n][rows][k].  -4 when no set is installed.
+ * tds_b200_step_vjp_params_*: the reverse sweep of tds_b200_step_vjp_*, which also writes g_par = g_out^T d(outputs) / d(parameters):
+ * device [k][n_stride], host [n][k].  g_in may be NULL.  Argument checks as for the VJP; -4 when no set is installed. */
+int tds_b200_param_count(const tds_b200_sim* sim);
+int tds_b200_set_physical_params_device(tds_b200_sim* sim, int k, const int* ids, const double* values, void* stream);
+int tds_b200_set_physical_params_host(tds_b200_sim* sim, int k, const int* ids, const double* values);
+int tds_b200_step_param_jacobian_device(tds_b200_sim* sim, int mode, int use_pd, const float* q, const float* qd,
+                                        const float* tau_or_action, double* jac, void* stream);
+int tds_b200_step_param_jacobian_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd,
+                                      const double* tau_or_action, double* jac);
+int tds_b200_step_vjp_params_device(tds_b200_sim* sim, int mode, int use_pd, const float* q, const float* qd,
+                                    const float* tau_or_action, const double* g_out, double* g_in, double* g_par, void* stream);
+int tds_b200_step_vjp_params_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd,
+                                  const double* tau_or_action, const double* g_out, double* g_in, double* g_par);
+
 /* Stand-alone integration stages of the fine-grained surface (device SoA arrays as above):
  * integrate_euler (src/dynamics/integrator.hpp:10-133): qd += qdd dt (qdd may be NULL = zero), q += qd dt, floating base
  * quaternion increment + normalisation; integrate_euler_qdd (:141-195): qd += qdd dt only. */

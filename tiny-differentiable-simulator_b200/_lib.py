@@ -89,6 +89,20 @@ def lib():
     L.tds_b200_step_vjp_host.restype = ci
     L.tds_b200_step_vjp_host.argtypes = [vp, ci, ci, dp, dp, dp, dp, dp]
     L.tds_b200_vjp_tape_info.restype = ci
+    L.tds_b200_param_count.restype = ci
+    L.tds_b200_param_count.argtypes = [vp]
+    L.tds_b200_set_physical_params_device.restype = ci
+    L.tds_b200_set_physical_params_device.argtypes = [vp, ci, vp, vp, vp]
+    L.tds_b200_set_physical_params_host.restype = ci
+    L.tds_b200_set_physical_params_host.argtypes = [vp, ci, vp, dp]
+    L.tds_b200_step_param_jacobian_device.restype = ci
+    L.tds_b200_step_param_jacobian_device.argtypes = [vp, ci, ci, fp, fp, fp, vp, vp]
+    L.tds_b200_step_param_jacobian_host.restype = ci
+    L.tds_b200_step_param_jacobian_host.argtypes = [vp, ci, ci, dp, dp, dp, dp]
+    L.tds_b200_step_vjp_params_device.restype = ci
+    L.tds_b200_step_vjp_params_device.argtypes = [vp, ci, ci, fp, fp, fp, vp, vp, vp, vp]
+    L.tds_b200_step_vjp_params_host.restype = ci
+    L.tds_b200_step_vjp_params_host.argtypes = [vp, ci, ci, dp, dp, dp, dp, dp, dp]
     L.tds_b200_vjp_tape_info.argtypes = [vp, ctypes.POINTER(ci)]
     L.tds_b200_integrate_euler_device.restype = ci
     L.tds_b200_integrate_euler_device.argtypes = [vp, fp, fp, fp, vp]
@@ -162,7 +176,10 @@ DECLARED_SYMBOLS = [
     "b200_laikago_jacobian", "b200_laikago_jacobian_meta", "b200_laikago_jacobian_allocate", "b200_laikago_jacobian_deallocate",
     "b200_laikago_jacobian_send_local", "b200_laikago_jacobian_send_global",
     "tds_b200_jacobian_dims", "tds_b200_step_jacobian_device", "tds_b200_step_jacobian_host",
-    "tds_b200_step_vjp_device", "tds_b200_step_vjp_host", "tds_b200_vjp_tape_info", "tds_b200_integrate_euler_device", "tds_b200_integrate_euler_qdd_device", "tds_b200_contact_pairs", "tds_b200_model_contact_pairs", "tds_b200_contact_tuples", "tds_b200_model_contact_tuples", "tds_b200_contact_list_device", "tds_b200_contact_list_host", "tds_b200_contact_list_candidates_host",
+    "tds_b200_step_vjp_device", "tds_b200_step_vjp_host", "tds_b200_vjp_tape_info",
+    "tds_b200_param_count", "tds_b200_set_physical_params_device", "tds_b200_set_physical_params_host",
+    "tds_b200_step_param_jacobian_device", "tds_b200_step_param_jacobian_host", "tds_b200_step_vjp_params_device",
+    "tds_b200_step_vjp_params_host", "tds_b200_integrate_euler_device", "tds_b200_integrate_euler_qdd_device", "tds_b200_contact_pairs", "tds_b200_model_contact_pairs", "tds_b200_contact_tuples", "tds_b200_model_contact_tuples", "tds_b200_contact_list_device", "tds_b200_contact_list_host", "tds_b200_contact_list_candidates_host",
     "tds_b200_rigid_create", "tds_b200_rigid_destroy", "tds_b200_rigid_set_params", "tds_b200_rigid_step_device", "tds_b200_rigid_step_host", "tds_b200_rigid_jacobian_host",
     "tds_b200_rigid_vjp_device", "tds_b200_rigid_vjp_host",
     "tds_b200_step_device", "tds_b200_step_host", "tds_b200_env_set_state_host",

@@ -9,6 +9,10 @@ world-frame step at the fp32-rounded inputs, and the gradient of the branch take
 of the Gauss-Seidel sweep), as with any operator-overloading AD.  Gradients come back as float32.  The PD gains are simulator
 settings, not autograd inputs; their cotangents are available from step_vjp_host / step_vjp_device.
 
+With params (a float64 CUDA tensor [n_envs, k] of values for the physical parameters installed by BatchSim.set_physical_params,
+DESIGN.md section 7.9) the forward installs those values and steps, and the backward also returns params.grad (float64): system
+identification by gradient descent through rollouts.
+
 rigid_step does the same for a batch of rigid-body worlds (RigidWorld) on float64 [n_worlds, n_bodies, 13] / [..., 3] tensors:
 the reverse pass checkpoints the states of the rollout on the device and sweeps one step at a time.
 """
@@ -28,15 +32,17 @@ def _soa(x, n_stride, dtype):
 
 class _Step(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, sim, mode, use_pd, q, qd, tau):
+    def forward(ctx, sim, mode, use_pd, q, qd, tau, params):
         n, ns = sim.n_envs, sim.n_stride
+        if params is not None:
+            sim.set_physical_params(sim.param_ids, params.detach())
         qs, qds = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32)
         ts = None if tau is None else _soa(tau, ns, torch.float32)
         q_out, qd_out = torch.empty_like(qs), torch.empty_like(qds)
         qdd_out = torch.empty_like(qds) if mode == MODE_FD else None
         sim.step_device(mode, qs, qds, ts, q_out=q_out, qd_out=qd_out, qdd_out=qdd_out, use_pd=use_pd)
-        ctx.sim, ctx.mode, ctx.use_pd, ctx.has_tau = sim, mode, use_pd, tau is not None
-        ctx.save_for_backward(qs, qds, ts if ts is not None else qs)
+        ctx.sim, ctx.mode, ctx.use_pd, ctx.has_tau, ctx.has_params = sim, mode, use_pd, tau is not None, params is not None
+        ctx.save_for_backward(qs, qds, ts if ts is not None else qs, params.detach() if params is not None else qs)
         if mode == MODE_FD:
             return qdd_out[:sim.n_qd, :n].t().contiguous()
         return q_out[:sim.n_q, :n].t().contiguous(), qd_out[:sim.n_qd, :n].t().contiguous()
@@ -44,7 +50,7 @@ class _Step(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *grads):
         sim, mode = ctx.sim, ctx.mode
-        qs, qds, ts = ctx.saved_tensors
+        qs, qds, ts, par = ctx.saved_tensors
         n, ns = sim.n_envs, sim.n_stride
         rows, cols = sim.jacobian_dims(mode, ctx.use_pd)
         dims = [sim.n_qd] if mode == MODE_FD else [sim.n_q, sim.n_qd]
@@ -55,24 +61,37 @@ class _Step(torch.autograd.Function):
                 g_out[r:r + d, :n] = g.to(torch.float64).t()
             r += d
         g_in = torch.zeros((cols, ns), dtype=torch.float64, device=qs.device)
-        sim.step_vjp_device(mode, qs, qds, ts if ctx.has_tau else None, g_out, g_in, use_pd=ctx.use_pd)
+        gp = None
+        if ctx.has_params:
+            # the values of this step (a later step of the graph may have installed others)
+            sim.set_physical_params(sim.param_ids, par)
+            g_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=qs.device)
+            sim.step_vjp_params_device(mode, qs, qds, ts if ctx.has_tau else None, g_out, g_in, g_par, use_pd=ctx.use_pd)
+            gp = g_par[:, :n].t().contiguous()
+        else:
+            sim.step_vjp_device(mode, qs, qds, ts if ctx.has_tau else None, g_out, g_in, use_pd=ctx.use_pd)
         gq = g_in[:sim.n_q, :n].t().to(torch.float32)
         gqd = g_in[sim.n_q:sim.n_q + sim.n_qd, :n].t().to(torch.float32)
         gt = None
         if ctx.has_tau:
             k0 = sim.n_q + sim.n_qd
             gt = g_in[k0:k0 + (sim.n_act if ctx.use_pd else sim.n_tau), :n].t().to(torch.float32)
-        return None, None, None, gq, gqd, gt
+        return None, None, None, gq, gqd, gt, gp
 
 
-def step(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False):
+def step(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False, params=None):
     """One differentiable step of every environment of `sim` (a BatchSim).  q [n_envs, n_q], qd [n_envs, n_qd], tau_or_action
     [n_envs, n_tau] (or [n_envs, n_act] with use_pd) float32 CUDA tensors.  Returns (q', qd'), or qdd in MODE_FD.  The gradient
-    is that of the fp64 world-frame step at the fp32-rounded inputs, of the branch taken; see the module docstring."""
+    is that of the fp64 world-frame step at the fp32-rounded inputs, of the branch taken; see the module docstring.  params: None,
+    or a float64 CUDA tensor [n_envs, k] of values for the parameters installed by sim.set_physical_params (then also
+    differentiated)."""
     for name, t in (("q", q), ("qd", qd), ("tau_or_action", tau_or_action)):
         if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or t.shape[0] != sim.n_envs):
             raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, dim] is expected")
-    return _Step.apply(sim, int(mode), bool(use_pd), q, qd, tau_or_action)
+    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
+                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
+        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    return _Step.apply(sim, int(mode), bool(use_pd), q, qd, tau_or_action, params)
 
 
 def _on_side_stream(dev, fn, tensors):

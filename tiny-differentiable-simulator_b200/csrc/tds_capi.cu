@@ -5,6 +5,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -36,6 +37,14 @@ extern "C" int tds_launch_stepw_vjp(const DevModel* M, const SimParams* P, const
 extern "C" int tds_launch_stepw(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io,
                                 int mode, int use_pd, int precision, char* gscratch, int use_smem,
                                 int warps_per_block, cudaStream_t stream);
+// the same with installed physical parameters (tds_stepw_par.cu)
+extern "C" int tds_launch_stepw_par(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
+                                    int mode, int use_pd, int precision, char* gscratch, int use_smem, int warps_per_block,
+                                    cudaStream_t stream);
+extern "C" int tds_launch_stepw_jacobian_par(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
+                                             int mode, int use_pd, int n_dirs, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_stepw_vjp_par(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
+                                        int mode, int use_pd, char* gscratch, cudaStream_t stream);
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
 // (plane candidates first, then - worlds of several multibodies - the candidates between multibodies, list after list)
@@ -383,6 +392,9 @@ struct tds_b200_sim {
   char* vjp_buf = nullptr; size_t vjp_buf_bytes = 0;
   int* vjp_flag = nullptr;
   double* vjp_g = nullptr; size_t vjp_g_bytes = 0;
+  // installed physical parameters (tds_b200_set_physical_params_*): slot map (par.n == 0: none) and values [k][ns] fp64
+  ParMap par;
+  double* par_dev = nullptr; size_t par_dev_bytes = 0;
   bool smem_ok[3] = {false, false, false};
   bool smem_ok_w[3] = {false, false, false};
   // 3: role-warp kernel (tds_stepr.cu), 2: lane-team kernel (tds_stept.cu), 1: one-lane world-frame kernel
@@ -573,6 +585,7 @@ tds_b200_sim* tds_b200_create(const double* model, int n_model, int n_envs, int 
   s->dm_ad = base;
   tds_build_layout_w(&s->dm_ad, 16, 16, 16, -1, 16);
   s->model.assign(model, model + n_model);
+  { const char* e = nullptr; tds_build_par_map(&base, 0, nullptr, &s->par, &e); }
   if (const char* kv = getenv("TDS_B200_KERNEL"))
     s->kernel_req = strcmp(kv, "world") == 0 ? 1 : (strcmp(kv, "team") == 0 ? 2 : (strcmp(kv, "role") == 0 ? 3 : 4));
   s->kernel = s->kernel_req;
@@ -622,7 +635,7 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->rq); cudaFree(s->rqd); cudaFree(s->zero_act); cudaFree(s->pol_act); cudaFree(s->sticky); cudaFree(s->r_total);
   cudaFree(s->pol_params); cudaFree(s->act_qidx); cudaFree(s->r_steps);
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
-  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g);
+  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
   if (s->stage_host) cudaFreeHost(s->stage_host);
   if (s->stream) cudaStreamDestroy(s->stream);
@@ -697,6 +710,54 @@ int tds_b200_set_precision(tds_b200_sim* s, int precision) {
   return 0;
 }
 
+int tds_b200_param_count(const tds_b200_sim* s) { return s ? tds_param_count(&s->dm[0]) : -1; }
+
+// values: device [k][ns] (copied on `stream`) or host [n][k] (synchronous), fp64
+static int set_physical_params(tds_b200_sim* s, int k, const int* ids, const double* values, bool device, void* stream) {
+  if (!s) return -1;
+  if (k > 0 && !values) { set_err("physical params: null values"); return -1; }
+  ParMap pm;
+  const char* err = nullptr;
+  if (tds_build_par_map(&s->dm[0], k, ids, &pm, &err)) { set_err(std::string("physical params: ") + err); return -2; }
+  CUDA_TRY(cudaSetDevice(s->device));
+  const bool same_ids = memcmp(&pm, &s->par, sizeof(pm)) == 0;   // (the map keeps no pointers: they are set per launch)
+  // a captured host graph holds the parameter buffer and the kernel instance: it stays valid only for new values of the same ids
+  if (!same_ids) drop_host_graph(s);
+  if (k == 0) {
+    s->par = pm;
+    return 0;
+  }
+  const size_t bytes = sizeof(double) * (size_t)k * s->ns;
+  if (bytes > s->par_dev_bytes) {
+    drop_host_graph(s);
+    cudaFree(s->par_dev);
+    s->par_dev = nullptr; s->par_dev_bytes = 0;
+    CUDA_TRY(cudaMalloc((void**)&s->par_dev, bytes));
+    CUDA_TRY(cudaMemset(s->par_dev, 0, bytes));
+    s->par_dev_bytes = bytes;
+  }
+  if (device) {
+    CUDA_TRY(cudaMemcpyAsync(s->par_dev, values, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  } else {
+    std::vector<double> tmp((size_t)k * s->ns, 0.0);
+    for (int e = 0; e < s->n; ++e)
+      for (int j = 0; j < k; ++j) tmp[(size_t)j * s->ns + e] = values[(size_t)e * k + j];
+    // steps run on non-blocking streams, which a plain cudaMemcpy does not wait for
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemcpy(s->par_dev, tmp.data(), bytes, cudaMemcpyHostToDevice));
+  }
+  s->par = pm;
+  return 0;
+}
+
+int tds_b200_set_physical_params_device(tds_b200_sim* s, int k, const int* ids, const double* values, void* stream) {
+  return set_physical_params(s, k, ids, values, true, stream);
+}
+
+int tds_b200_set_physical_params_host(tds_b200_sim* s, int k, const int* ids, const double* values) {
+  return set_physical_params(s, k, ids, values, false, nullptr);
+}
+
 int tds_b200_get_dims(const tds_b200_sim* s, int dims[8]) {
   if (!s) return -1;
   const DevModel& M = s->dm[0];
@@ -720,7 +781,7 @@ int tds_b200_step_device(tds_b200_sim* s, int mode, int use_pd, const float* q_i
   io.n = s->n; io.n_stride = s->ns;
   if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
   int kern = s->kernel_req;
-  if (s->dm[0].world_only || mode == 3 || s->P.contact_model != 0) kern = 1;   // (mode 3 = TDS_B200_MODE_WORLD)   // box shapes / spherical joints: served by the generic world-frame kernel only
+  if (s->dm[0].world_only || mode == 3 || s->P.contact_model != 0 || s->par.n > 0) kern = 1;   // (mode 3 = TDS_B200_MODE_WORLD)   // box shapes / spherical joints: served by the generic world-frame kernel only
   if (kern == 4 && !(s->spec_ok && tds_spec_smem_bytes(s->spec_idx, p) <= (size_t)s->max_smem_optin)) kern = 3;
   if (kern == 4) {
     s->kernel = kern;
@@ -757,8 +818,12 @@ int tds_b200_step_device(tds_b200_sim* s, int mode, int use_pd, const float* q_i
   }
   const int use_smem = s->smem_ok_w[p] ? 1 : 0;
   if (!use_smem) { int rc = ensure_scratch(s, p); if (rc) return rc; }
-  int rc = tds_launch_stepw(&s->dm[p], &s->P, &s->E, &io, mode, use_pd, p, s->scratch, use_smem,
-                            s->warps_per_block[p], (cudaStream_t)stream);
+  ParMap pm = s->par;
+  pm.values = s->par_dev; pm.grad = nullptr;
+  int rc = s->par.n > 0
+      ? tds_launch_stepw_par(&s->dm[p], &s->P, &s->E, &io, &pm, mode, use_pd, p, s->scratch, use_smem, s->warps_per_block[p],
+                             (cudaStream_t)stream)
+      : tds_launch_stepw(&s->dm[p], &s->P, &s->E, &io, mode, use_pd, p, s->scratch, use_smem, s->warps_per_block[p], (cudaStream_t)stream);
   if (rc) set_err(std::string("step launch: ") + cudaGetErrorString((cudaError_t)rc));
   return rc;
 }
@@ -773,47 +838,72 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
   return 0;
 }
 
-int tds_b200_step_jacobian_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
-                                  double* jac, void* stream) {
-  if (!s || !q || !qd || !jac) return -1;
-  if (mode == 3) { set_err("jacobian: modes FD, NOCONTACT, FULL"); return -2; }
-  if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+// Jacobian columns: the step's inputs (params == false) or the installed physical parameters, which are the dual instance's
+// directions dims[1] + s (params == true)
+static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                        double* jac, void* stream, bool params) {
   int dims[2];
   tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  const int n_dirs = params ? s->par.n : dims[1], dir_base = params ? dims[1] : 0;
   StepIO io;
   memset(&io, 0, sizeof(io));
   io.q_in = q; io.qd_in = qd; io.tau_in = tau_or_action;
-  io.jac = jac; io.jac_n_in = dims[1];
+  io.jac = jac; io.jac_n_in = n_dirs;
   io.n = s->n; io.n_stride = s->ns;
+  ParMap pmv = s->par;
+  pmv.values = s->par_dev; pmv.grad = nullptr;
+  const ParMap* pm = s->par.n > 0 ? &pmv : nullptr;
   const size_t warps = (size_t)(s->n + 31) / 32;
   const size_t per_dir = warps * (size_t)s->dm_ad.x_total * 32 * 4;
   const size_t cap = (size_t)2 << 30;                       // scratch bound: directions are processed in chunks
   int chunk = (int)(cap / per_dir);
   if (chunk < 1) chunk = 1;
-  if (chunk > dims[1]) chunk = dims[1];
+  if (chunk > n_dirs) chunk = n_dirs;
   if (per_dir * chunk > s->jac_scratch_bytes) {
     if (s->jac_scratch) cudaFree(s->jac_scratch);
     s->jac_scratch = nullptr; s->jac_scratch_bytes = 0;
     CUDA_TRY(cudaMalloc((void**)&s->jac_scratch, per_dir * chunk));
     s->jac_scratch_bytes = per_dir * chunk;
   }
-  for (int d0 = 0; d0 < dims[1]; d0 += chunk) {
-    io.jac_dir0 = d0;
-    const int nd = dims[1] - d0 < chunk ? dims[1] - d0 : chunk;
-    int rc = tds_launch_stepw_jacobian(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream);
+  for (int d0 = 0; d0 < n_dirs; d0 += chunk) {
+    io.jac_dir0 = dir_base + d0;
+    const int nd = n_dirs - d0 < chunk ? n_dirs - d0 : chunk;
+    int rc = pm ? tds_launch_stepw_jacobian_par(&s->dm_ad, &s->P, &s->E, &io, pm, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream)
+                : tds_launch_stepw_jacobian(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream);
     if (rc) { set_err(std::string("jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
   }
   return 0;
 }
 
-int tds_b200_step_jacobian_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
-                                const double* tau_or_action, double* jac) {
+static int jacobian_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* jac, bool params) {
   if (!s || !q || !qd || !jac) return -1;
+  if (mode == 3) { set_err("jacobian: modes FD, NOCONTACT, FULL"); return -2; }
+  if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+  if (params && s->par.n == 0) { set_err("parameter jacobian: no physical parameters installed"); return -4; }
+  return 0;
+}
+
+int tds_b200_step_jacobian_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                                  double* jac, void* stream) {
+  if (int rc = jacobian_check(s, mode, use_pd, q, qd, jac, false)) return rc;
+  return jacobian_run(s, mode, use_pd, q, qd, tau_or_action, jac, stream, false);
+}
+
+int tds_b200_step_param_jacobian_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd,
+                                        const float* tau_or_action, double* jac, void* stream) {
+  if (int rc = jacobian_check(s, mode, use_pd, q, qd, jac, true)) return rc;
+  return jacobian_run(s, mode, use_pd, q, qd, tau_or_action, jac, stream, true);
+}
+
+static int jacobian_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
+                         const double* tau_or_action, double* jac, bool params) {
+  if (int rc = jacobian_check(s, mode, use_pd, q, qd, jac, params)) return rc;
   CUDA_TRY(cudaSetDevice(s->device));
   const DevModel& M = s->dm[0];
   const int n = s->n, ns = s->ns;
   int dims[2];
   tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  if (params) dims[1] = s->par.n;
   const int n_in = use_pd ? s->E.n_act : s->n_tau;
   const size_t maxdim = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + 1;
   int rc = ensure_stage(s, sizeof(double) * n * maxdim, 0);
@@ -839,7 +929,7 @@ int tds_b200_step_jacobian_host(tds_b200_sim* s, int mode, int use_pd, const dou
   if (tau_or_action) { if ((rc = up(tau_or_action, n_in, s->act))) return rc; }
   else CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * ns * (n_in > 0 ? n_in : 1), sm));
   CUDA_TRY(cudaMemsetAsync(s->jac_dev, 0, jb, sm));
-  rc = tds_b200_step_jacobian_device(s, mode, use_pd, s->q, s->qd, s->act, s->jac_dev, sm);
+  rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, s->jac_dev, sm, params);
   if (rc) return rc;
   std::vector<double> tmp((size_t)dims[0] * dims[1] * ns);
   CUDA_TRY(cudaMemcpyAsync(tmp.data(), s->jac_dev, jb, cudaMemcpyDeviceToHost, sm));
@@ -851,15 +941,32 @@ int tds_b200_step_jacobian_host(tds_b200_sim* s, int mode, int use_pd, const dou
   return 0;
 }
 
+int tds_b200_step_jacobian_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
+                                const double* tau_or_action, double* jac) {
+  return jacobian_host(s, mode, use_pd, q, qd, tau_or_action, jac, false);
+}
+
+int tds_b200_step_param_jacobian_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
+                                      const double* tau_or_action, double* jac) {
+  return jacobian_host(s, mode, use_pd, q, qd, tau_or_action, jac, true);
+}
+
 // ---- vector-Jacobian product: g_in = g_out^T d(q', qd' | qdd) / d(q | qd | tau or action (| kp, kd, max_force)) by the taping
 // instance of the world-frame kernel (tds_tape.cuh), one lane per environment.  Environments run in chunks that keep arena +
 // tape + adjoints inside 2 GB; a chunk whose tape overflowed is rerun with twice the capacity (the flag is read after every
 // chunk, so the call synchronises its stream once per chunk).
-int tds_b200_step_vjp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
-                             const double* g_out, double* g_in, void* stream) {
-  if (!s || !q || !qd || !g_out || !g_in) return -1;
+static int vjp_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* g_out, const void* g_req) {
+  if (!s || !q || !qd || !g_out || !g_req) return -1;
   if (mode == 3) { set_err("vjp: modes FD, NOCONTACT, FULL"); return -2; }
   if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+  return 0;
+}
+
+// g_in (may be null while parameters are installed) and g_par [k][ns] (or null); every pointer is offset per chunk of environments
+static int vjp_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                   const double* g_out, double* g_in, double* g_par, void* stream) {
+  ParMap pmv = s->par;
+  const ParMap* pm = s->par.n > 0 ? &pmv : nullptr;
   cudaStream_t sm = (cudaStream_t)stream;
   const size_t arena_warp = (size_t)s->dm_ad.x_total * 32 * 4;
   const size_t cap_bytes = (size_t)2 << 30;
@@ -885,12 +992,14 @@ int tds_b200_step_vjp_device(tds_b200_sim* s, int mode, int use_pd, const float*
     memset(&io, 0, sizeof(io));
     io.q_in = q + e0; io.qd_in = qd + e0; io.tau_in = tau_or_action ? tau_or_action + e0 : nullptr;   // [dim][ns]: column offset
     io.n = chunk; io.n_stride = ns;
-    io.g_out = g_out + e0; io.g_in = g_in + e0;
+    io.g_out = g_out + e0; io.g_in = g_in ? g_in + e0 : nullptr;
+    pmv.values = s->par_dev ? s->par_dev + e0 : nullptr; pmv.grad = g_par ? g_par + e0 : nullptr;
     io.tape = s->vjp_buf + warps * arena_warp;
     io.tape_adj = (double*)(s->vjp_buf + warps * arena_warp + tape_b);
     io.tape_cap = s->tape_cap; io.tape_overflow = s->vjp_flag;
     CUDA_TRY(cudaMemsetAsync(s->vjp_flag, 0, sizeof(int), sm));
-    int rc = tds_launch_stepw_vjp(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, s->vjp_buf, sm);
+    int rc = pm ? tds_launch_stepw_vjp_par(&s->dm_ad, &s->P, &s->E, &io, pm, mode, use_pd, s->vjp_buf, sm)
+                : tds_launch_stepw_vjp(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, s->vjp_buf, sm);
     if (rc) { set_err(std::string("vjp launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
     int overflow = 0;
     CUDA_TRY(cudaMemcpyAsync(&overflow, s->vjp_flag, sizeof(int), cudaMemcpyDeviceToHost, sm));
@@ -905,11 +1014,21 @@ int tds_b200_step_vjp_device(tds_b200_sim* s, int mode, int use_pd, const float*
   return 0;
 }
 
-int tds_b200_step_vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
-                           const double* tau_or_action, const double* g_out, double* g_in) {
-  if (!s || !q || !qd || !g_out || !g_in) return -1;
-  if (mode == 3) { set_err("vjp: modes FD, NOCONTACT, FULL"); return -2; }
-  if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+int tds_b200_step_vjp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                             const double* g_out, double* g_in, void* stream) {
+  if (int rc = vjp_check(s, mode, use_pd, q, qd, g_out, g_in)) return rc;
+  return vjp_run(s, mode, use_pd, q, qd, tau_or_action, g_out, g_in, nullptr, stream);
+}
+
+int tds_b200_step_vjp_params_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd,
+                                    const float* tau_or_action, const double* g_out, double* g_in, double* g_par, void* stream) {
+  if (int rc = vjp_check(s, mode, use_pd, q, qd, g_out, g_par)) return rc;
+  if (s->par.n == 0) { set_err("parameter vjp: no physical parameters installed"); return -4; }
+  return vjp_run(s, mode, use_pd, q, qd, tau_or_action, g_out, g_in, g_par, stream);
+}
+
+static int vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
+                    const double* tau_or_action, const double* g_out, double* g_in, double* g_par) {
   CUDA_TRY(cudaSetDevice(s->device));
   const DevModel& M = s->dm[0];
   const int n = s->n, ns = s->ns;
@@ -919,7 +1038,8 @@ int tds_b200_step_vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* 
   const size_t maxdim = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + 1;
   int rc = ensure_stage(s, sizeof(double) * n * maxdim, 0);
   if (rc) return rc;
-  const size_t gb = sizeof(double) * (size_t)(dims[0] + dims[1]) * ns;
+  const int n_par = g_par ? s->par.n : 0;
+  const size_t gb = sizeof(double) * (size_t)(dims[0] + dims[1] + n_par) * ns;
   if (gb > s->vjp_g_bytes) {
     if (s->vjp_g) cudaFree(s->vjp_g);
     s->vjp_g = nullptr; s->vjp_g_bytes = 0;
@@ -939,21 +1059,41 @@ int tds_b200_step_vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* 
   if ((rc = up(qd, M.n_qd, s->qd))) return rc;
   if (tau_or_action) { if ((rc = up(tau_or_action, n_in, s->act))) return rc; }
   else CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * ns * (n_in > 0 ? n_in : 1), sm));
-  std::vector<double> tmp((size_t)(dims[0] > dims[1] ? dims[0] : dims[1]) * ns, 0.0);
+  std::vector<double> tmp((size_t)std::max(std::max(dims[0], dims[1]), n_par) * ns, 0.0);
   for (int e = 0; e < n; ++e)
     for (int k = 0; k < dims[0]; ++k) tmp[(size_t)k * ns + e] = g_out[(size_t)e * dims[0] + k];
   double* gout_d = s->vjp_g;
   double* gin_d = s->vjp_g + (size_t)dims[0] * ns;
+  double* gpar_d = g_par ? s->vjp_g + (size_t)(dims[0] + dims[1]) * ns : nullptr;
   CUDA_TRY(cudaMemcpyAsync(gout_d, tmp.data(), sizeof(double) * dims[0] * ns, cudaMemcpyHostToDevice, sm));
-  CUDA_TRY(cudaMemsetAsync(gin_d, 0, sizeof(double) * dims[1] * ns, sm));
-  rc = tds_b200_step_vjp_device(s, mode, use_pd, s->q, s->qd, s->act, gout_d, gin_d, sm);
+  CUDA_TRY(cudaMemsetAsync(gin_d, 0, sizeof(double) * (dims[1] + n_par) * ns, sm));
+  rc = vjp_run(s, mode, use_pd, s->q, s->qd, s->act, gout_d, g_in ? gin_d : nullptr, gpar_d, sm);
   if (rc) return rc;
-  CUDA_TRY(cudaMemcpyAsync(tmp.data(), gin_d, sizeof(double) * dims[1] * ns, cudaMemcpyDeviceToHost, sm));
-  CUDA_TRY(cudaStreamSynchronize(sm));
+  auto down = [&](const double* src, int dim, double* dst) -> int {
+    if (!dst) return 0;
+    CUDA_TRY(cudaMemcpyAsync(tmp.data(), src, sizeof(double) * dim * ns, cudaMemcpyDeviceToHost, sm));
+    CUDA_TRY(cudaStreamSynchronize(sm));
+    for (int e = 0; e < n; ++e)
+      for (int j = 0; j < dim; ++j) dst[(size_t)e * dim + j] = tmp[(size_t)j * ns + e];
+    return 0;
+  };
+  if ((rc = down(gin_d, dims[1], g_in))) return rc;
+  if ((rc = down(gpar_d, n_par, g_par))) return rc;
   CUDA_TRY(cudaGetLastError());
-  for (int e = 0; e < n; ++e)
-    for (int k = 0; k < dims[1]; ++k) g_in[(size_t)e * dims[1] + k] = tmp[(size_t)k * ns + e];
   return 0;
+}
+
+int tds_b200_step_vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
+                           const double* tau_or_action, const double* g_out, double* g_in) {
+  if (int rc = vjp_check(s, mode, use_pd, q, qd, g_out, g_in)) return rc;
+  return vjp_host(s, mode, use_pd, q, qd, tau_or_action, g_out, g_in, nullptr);
+}
+
+int tds_b200_step_vjp_params_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
+                                  const double* tau_or_action, const double* g_out, double* g_in, double* g_par) {
+  if (int rc = vjp_check(s, mode, use_pd, q, qd, g_out, g_par)) return rc;
+  if (s->par.n == 0) { set_err("parameter vjp: no physical parameters installed"); return -4; }
+  return vjp_host(s, mode, use_pd, q, qd, tau_or_action, g_out, g_in, g_par);
 }
 
 // diagnostics of the VJP path: the tape capacity now in use (nodes per lane) and the environments per chunk it implies
@@ -1382,7 +1522,7 @@ int tds_b200_env_step_host(tds_b200_sim* s, const float* actions, float* obs, fl
   cudaStream_t sm = s->stream;
   const int T = 128, B = (n + T - 1) / T;
   // the specialised kernel reads environment-major actions and writes the observation block itself
-  const bool direct = s->kernel_req == 4 && s->spec_ok && s->P.contact_model == 0 && tds_spec_smem_bytes(s->spec_idx, s->precision) <= (size_t)s->max_smem_optin;
+  const bool direct = s->kernel_req == 4 && s->spec_ok && s->P.contact_model == 0 && s->par.n == 0 && tds_spec_smem_bytes(s->spec_idx, s->precision) <= (size_t)s->max_smem_optin;
   auto enqueue = [&]() -> int {
     CUDA_TRY(cudaMemcpyAsync(d_in, actions, in_b, cudaMemcpyHostToDevice, sm));
     if (direct) {

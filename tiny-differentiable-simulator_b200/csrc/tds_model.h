@@ -333,3 +333,36 @@ TDS_HOST_INLINE void tds_build_layout_w(DevModel* D, int size_ra, int size_rc, i
   w = even(w);
   D->x_total = w;
 }
+
+// ---- physical parameter ids (include/tds_b200.h, tds_b200_set_physical_params_*) ----------------------------------------------------
+// 0 friction, 1 restitution, 2 + 10 b + c body b (0 = base, i + 1 = link i; c: mass, com x y z, I_com xx xy xz yy yz zz),
+// 2 + 10 (n_links + 1) + 2 i + c link i (c: joint stiffness, joint damping)
+TDS_HOST_INLINE int tds_param_count(const DevModel* D) { return 2 + 10 * (D->n_links + 1) + 2 * D->n_links; }
+
+// ids[0..k) -> slot map.  Returns 0, or -1 with *err set: an id out of range, an id given twice, a base id on a fixed-base model.
+TDS_HOST_INLINE int tds_build_par_map(const DevModel* D, int k, const int* ids, ParMap* pm, const char** err) {
+  memset(pm, 0, sizeof(*pm));
+  pm->friction = pm->restitution = -1;
+  for (int b = 0; b <= TDS_MAX_LINKS; ++b) for (int c = 0; c < 10; ++c) pm->body[b][c] = -1;
+  for (int i = 0; i < TDS_MAX_LINKS; ++i) pm->joint[i][0] = pm->joint[i][1] = -1;
+  const int n_ids = tds_param_count(D), j0 = 2 + 10 * (D->n_links + 1);
+  if (k < 0 || (k > 0 && !ids)) { *err = "bad parameter count"; return -1; }
+  pm->n = k;
+  for (int s = 0; s < k; ++s) {
+    const int id = ids[s];
+    if (id < 0 || id >= n_ids) { *err = "parameter id out of range"; return -1; }
+    short* slot = nullptr;
+    int* islot = nullptr;
+    if (id == 0) islot = &pm->friction;
+    else if (id == 1) islot = &pm->restitution;
+    else if (id < j0) {
+      const int b = (id - 2) / 10;
+      if (b == 0 && !D->floating) { *err = "base parameter on a fixed-base model (its base does not move)"; return -1; }
+      slot = &pm->body[b][(id - 2) % 10];
+      if (b == 0) pm->any_base = 1;
+    } else slot = &pm->joint[(id - j0) / 2][(id - j0) % 2];
+    if ((islot && *islot >= 0) || (slot && *slot >= 0)) { *err = "parameter id given twice"; return -1; }
+    if (islot) *islot = s; else *slot = (short)s;
+  }
+  return 0;
+}

@@ -33,15 +33,29 @@ namespace tdsw {
 
 // per-link region, element offsets: [rigid inertia (10 RC) | later U (6 RA), invD, u] then v / c / a (6 RA)
 
+// kernel argument of the instances without installed physical parameters: nothing
+struct NoPar {};
+template <bool PAR> struct ParArg { typedef NoPar type; };
+template <> struct ParArg<true> { typedef ParMap type; };
+
+// joint stiffness and damping enter the step at fp32, as DevModel stores them; the derivative is taken at the rounded value
+TDS_D double f32_round(double x) { return (double)(float)x; }
+template <typename T> TDS_D Dual<T> f32_round(Dual<T> x) { x.v = (T)(float)x.v; return x; }
+template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; return x; }
+
 // RQ: scalar of the state vectors (q, qd, tau): float, or the dual number type in the differentiable instance
 // (RA = RC = RS = RQ = Dual<double>: blockIdx.y + io.jac_dir0 is the input direction of the lane, see tds_dual.cuh),
 // or the taping scalar of the vector-Jacobian product (RA = RC = RS = RQ = Tape<double>, one lane per environment: the
 // lane records its step and sweeps it backwards from io.g_out at the end, see tds_tape.cuh).
-template <typename RA, typename RC, typename RS, typename RQ, bool SMEM>
+// PAR: per-environment physical parameters (DESIGN.md section 7.9).  Parameter slot s of the lane is pm.values[s * n_stride + e];
+// pm also says which model quantity each slot replaces.  In the dual instance slot s is input direction n_in_ad + s, in the taping
+// instance leaf n_in_ad + s (after the state / control inputs, so g_in keeps its layout).  The values are read where the model
+// values are read (once per step each; the reads of a warp are coalesced), so the arena layout does not change.
+template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
-                 char* __restrict__ gscratch) {
+                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR>::type pm = {}) {
   extern __shared__ __align__(16) char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp_in_blk = threadIdx.x >> 5;
@@ -63,13 +77,49 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   const int n3 = 3 * nb;
   // VJP instance: input columns q | qd | tau or action (| kp, kd, max_force) are the first nodes of the lane's tape
   const int n_in_ad = M.n_q + n + (use_pd ? E.n_act + 3 : n - (M.floating ? 6 : 0));
-  if constexpr (TP) tape_begin((TapeNode*)io.tape + ((size_t)(env >> 5) * io.tape_cap * 32 + lane), io.tape_cap, io.tape_overflow, n_in_ad);
+  // (the instances without parameters keep their original statements: their code must not change)
+  if constexpr (TP && PAR) tape_begin((TapeNode*)io.tape + ((size_t)(env >> 5) * io.tape_cap * 32 + lane), io.tape_cap, io.tape_overflow, n_in_ad + pm.n);
+  else if constexpr (TP) tape_begin((TapeNode*)io.tape + ((size_t)(env >> 5) * io.tape_cap * 32 + lane), io.tape_cap, io.tape_overflow, n_in_ad);
   // reverse sweep from the cotangent of the outputs out_id(r), r < n_rows; the input adjoints are this lane's g_in column
+  // (and its g_par column: the installed parameters are the leaves after the inputs)
   auto vjp_write = [&](int n_rows, auto out_id) {
     double* adj = io.tape_adj + ((size_t)(env >> 5) * io.tape_cap * 32 + lane);
-    const bool ok = tape_reverse(adj, n_rows, out_id, [&](int r) { return io.g_out[(size_t)r * ns + e]; }, n_in_ad);
-    if (ok && live)
-      for (int k = 0; k < n_in_ad; ++k) io.g_in[(size_t)k * ns + e] = adj[(size_t)k * 32];
+    if constexpr (PAR) {
+      const bool ok = tape_reverse(adj, n_rows, out_id, [&](int r) { return io.g_out[(size_t)r * ns + e]; }, n_in_ad + pm.n);
+      if (ok && live && io.g_in)
+        for (int k = 0; k < n_in_ad; ++k) io.g_in[(size_t)k * ns + e] = adj[(size_t)k * 32];
+      if (ok && live && pm.grad)
+        for (int k = 0; k < pm.n; ++k) pm.grad[(size_t)k * ns + e] = adj[(size_t)(n_in_ad + k) * 32];
+    } else {
+      const bool ok = tape_reverse(adj, n_rows, out_id, [&](int r) { return io.g_out[(size_t)r * ns + e]; }, n_in_ad);
+      if (ok && live)
+        for (int k = 0; k < n_in_ad; ++k) io.g_in[(size_t)k * ns + e] = adj[(size_t)k * 32];
+    }
+  };
+  // Jacobian column of this lane's direction: parameter directions n_in_ad + s are column s of the parameter Jacobian
+  const int jcol = (PAR && dir >= n_in_ad) ? dir - n_in_ad : dir;
+  // physical quantities: the lane's installed value (the dual / taping instances seed it) or the model's.  RP keeps fp64 in the
+  // plain instances, as the model stores these quantities.
+  typedef typename std::conditional<AD || TP, RQ, double>::type RP;
+  auto par_of = [&](int slot, double model_v) -> RP {
+    if constexpr (PAR) { if (slot >= 0) return ad_seed(RP(pm.values[(size_t)slot * ns + e]), n_in_ad + slot, dir); }
+    return RP(model_v);
+  };
+  auto body_slot = [&](int b, int c) -> int {
+    if constexpr (PAR) return pm.body[b][c];
+    else return -1;
+  };
+  auto joint_slot = [&](int i, int c) -> int {
+    if constexpr (PAR) return pm.joint[i][c];
+    else return -1;
+  };
+  int par_friction = -1, par_restitution = -1;
+  if constexpr (PAR) { par_friction = pm.friction; par_restitution = pm.restitution; }
+  // joint stiffness (c = 0) / damping (c = 1) of link i, at fp32
+  auto joint_par = [&](int i, int c, float model_v) -> RP {
+    const int s = joint_slot(i, c);
+    if (s >= 0) return f32_round(par_of(s, 0.0));
+    return RP(model_v);
   };
   int phase_id = 0;
 #define TDSW_PHASE() do { if (io.phase_clk && lane == 0) io.phase_clk[(size_t)(env >> 5) * 16 + (phase_id++)] = clock64(); } while (0)
@@ -276,13 +326,14 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     // rigid-body inertia about O in world axes: com c = p_i + R_i com_l, I = R Icom R^T + m (|c|^2 1 - c c^T)
     {
       const double* rb = M.rbic[i];
+      auto rbc = [&](int c) -> RP { return par_of(body_slot(i + 1, c), rb[c]); };
       Rbi<RC> r;
-      r.m = RC(rb[0]);
-      const V3<RC> c = pi + mul(Ri, v3<RC>(RC(rb[1]), RC(rb[2]), RC(rb[3])));
+      r.m = RC(rbc(0));
+      const V3<RC> c = pi + mul(Ri, v3<RC>(RC(rbc(1)), RC(rbc(2)), RC(rbc(3))));
       r.h = c * r.m;
       // R Icom R^T enters every product additively (no cancellation) -> RA precision is enough; the parallel-axis
       // terms m(|c|^2 1 - c c^T) and h = m c cancel against each other in M_ij and stay in RC.
-      S3<RA> Icf; Icf.xx = RA(rb[4]); Icf.xy = RA(rb[5]); Icf.xz = RA(rb[6]); Icf.yy = RA(rb[7]); Icf.yz = RA(rb[8]); Icf.zz = RA(rb[9]);
+      S3<RA> Icf; Icf.xx = RA(rbc(4)); Icf.xy = RA(rbc(5)); Icf.xz = RA(rbc(6)); Icf.yy = RA(rbc(7)); Icf.yz = RA(rbc(8)); Icf.zz = RA(rbc(9));
       const S3<RA> Irot = rot_sym(cvt<RA>(Ri), Icf);
       r.I.xx = RC(Irot.xx); r.I.xy = RC(Irot.xy); r.I.xz = RC(Irot.xz); r.I.yy = RC(Irot.yy); r.I.yz = RC(Irot.yz); r.I.zz = RC(Irot.zz);
       const RC cc = dot(c, c);
@@ -466,15 +517,16 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       for (int a = 0; a < 3; ++a) {
 #pragma unroll
         for (int b = 0; b < 3; ++b) Dm[a][b] = dot(S[a], U[b]);
-        u[a] = RA(tauv[(d0 + a) * ST]) - RA(M.damping[i]) * qdj[a] - dot(S[a], pA);
+        u[a] = RA(tauv[(d0 + a) * ST]) - RA(joint_par(i, 1, M.damping[i])) * qdj[a] - dot(S[a], pA);
       }
-      if (M.stiffness[i] != 0.f) {   // tau -= stiffness * quaternion_axis_angle(q), forward_dynamics.hpp:69-74, tiny_algebra.hpp:509-527
+      // (an installed stiffness always takes this path: its derivative at 0 is not lost)
+      if (M.stiffness[i] != 0.f || joint_slot(i, 0) >= 0) {   // tau -= stiffness * quaternion_axis_angle(q), forward_dynamics.hpp:69-74, tiny_algebra.hpp:509-527
         const int q0 = M.q_idx[i];
         const RC qx = RC(qv[q0 * ST]), qy = RC(qv[(q0 + 1) * ST]), qz = RC(qv[(q0 + 2) * ST]), qw = RC(qv[(q0 + 3) * ST]);
         const RC nrm = sqrt_t(qx * qx + qy * qy + qz * qz);
         const RC theta = RC(2) * atan2_t(nrm, qw);
         const RC scaling = nrm < RC(1.220703125e-4) ? RC(1) / (RC(0.5) + theta * theta * RC(1.0 / 48.0)) : theta / nrm;   // eps^(1/4)
-        const RA k = RA(M.stiffness[i]);
+        const RA k = RA(joint_par(i, 0, M.stiffness[i]));
         u[0] -= k * RA(scaling * qx); u[1] -= k * RA(scaling * qy); u[2] -= k * RA(scaling * qz);
       }
       RA Di[3][3];   // general 3 x 3 inverse (Matrix3::inverse)
@@ -523,8 +575,8 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       const RA D = dot(S, U);
       const RA invD = RA(1) / D;
       RA tau = RA(tauv[qdi * ST]);
-      tau -= RA(M.stiffness[i]) * RA(qv[M.q_idx[i] * ST]);
-      tau -= RA(M.damping[i]) * qdj;
+      tau -= RA(joint_par(i, 0, M.stiffness[i])) * RA(qv[M.q_idx[i] * ST]);
+      tau -= RA(joint_par(i, 1, M.damping[i])) * qdj;
       const RA u = tau - dot(S, pA);                         // :129
       st6<RA>(vrec, ST, c);
       st6<RA>(urec, ST, U);
@@ -577,10 +629,30 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       abi_add(Ach, sa); pch = pch + sp;
       rbi_add(Icch, ld_rbi<RC>(A.ptr<RC>(M.x_acc + M.base_acc * M.x_acc_words + M.x_acc_ic_word), ST));
     }
+    // installed base quantities: (m, h, I about the origin) packed per lane as tds_rbi_pack does on the host, and I_com of the
+    // gyroscopic term at fp32 as DevModel::base_inertia_com
+    bool base_par = false;
+    Rbi<RP> bp;
+    if constexpr (PAR) {
+      if (pm.any_base) {
+        base_par = true;
+        RP b[10];
+        for (int c = 0; c < 10; ++c) b[c] = par_of(body_slot(0, c), M.base_rbic[c]);
+        const RP cc = b[1] * b[1] + b[2] * b[2] + b[3] * b[3];
+        bp.m = b[0];
+        bp.h = v3<RP>(b[0] * b[1], b[0] * b[2], b[0] * b[3]);
+        bp.I.xx = b[4] + b[0] * (cc - b[1] * b[1]);
+        bp.I.xy = b[5] - b[0] * b[1] * b[2];
+        bp.I.xz = b[6] - b[0] * b[1] * b[3];
+        bp.I.yy = b[7] + b[0] * (cc - b[2] * b[2]);
+        bp.I.yz = b[8] - b[0] * b[2] * b[3];
+        bp.I.zz = b[9] + b[0] * (cc - b[3] * b[3]);
+      }
+    }
     const M3<RA> Rt = cvt<RA>(transpose(Rb));
     Abi<RA> Ab;
     {
-      Rbi<RA> rbb = model_rbi_of<RA>(M.base_rbi);
+      Rbi<RA> rbb = base_par ? cvt_rbi<RA>(bp) : model_rbi_of<RA>(M.base_rbi);
       Ab = abi_from_rbi(rbb);
       Abi<RA> Arot;
       Arot.I = rot_sym(Rt, Ach.I); Arot.M = rot_sym(Rt, Ach.M); Arot.H = rot_gen(Rt, Ach.H);
@@ -594,13 +666,19 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       Ic0.xx = RA(M.base_inertia_com[0]); Ic0.xy = RA(M.base_inertia_com[1]); Ic0.xz = RA(M.base_inertia_com[2]);
       Ic0.yx = RA(M.base_inertia_com[3]); Ic0.yy = RA(M.base_inertia_com[4]); Ic0.yz = RA(M.base_inertia_com[5]);
       Ic0.zx = RA(M.base_inertia_com[6]); Ic0.zy = RA(M.base_inertia_com[7]); Ic0.zz = RA(M.base_inertia_com[8]);
+      if constexpr (PAR) {
+        if (base_par) {
+          auto f = [&](int c) -> RA { return RA(f32_round(par_of(body_slot(0, c), M.base_rbic[c]))); };
+          Ic0.xx = f(4); Ic0.xy = Ic0.yx = f(5); Ic0.xz = Ic0.zx = f(6); Ic0.yy = f(7); Ic0.yz = Ic0.zy = f(8); Ic0.zz = f(9);
+        }
+      }
       const M3<RA> Iw = rot_gen(RbA, Ic0);
       const V3<RA> wb = v3<RA>(RA(qdv[0]), RA(qdv[ST]), RA(qdv[2 * ST]));
       pb.top = cross(wb, mul(Iw, wb)) + mul(Rt, pch.top);
       pb.bot = mul(Rt, pch.bot);
     }
     if (any_contact) {  // mass_matrix.hpp:114-120: base block = composite inertia in the base frame
-      Rbi<RC> Ib = model_rbi_of<RC>(M.base_rbi);
+      Rbi<RC> Ib = base_par ? cvt_rbi<RC>(bp) : model_rbi_of<RC>(M.base_rbi);
       const M3<RC> RtC = transpose(Rb);
       Rbi<RC> rot; rot.m = Icch.m; rot.h = mul(RtC, Icch.h); rot.I = rot_sym(RtC, Icch.I);
       rbi_add(Ib, rot);
@@ -675,7 +753,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
         a.top = axpy(S.top, qdd, a.top);
         a.bot = axpy(S.bot, qdd, a.bot);
         if (mode == MODE_FD) {
-          if constexpr (AD) { if (live && io.jac) io.jac[((size_t)(d0 + j) * io.jac_n_in + dir) * ns + e] = qdd.d; }
+          if constexpr (AD) { if (live && io.jac) io.jac[((size_t)(d0 + j) * io.jac_n_in + jcol) * ns + e] = qdd.d; }
           else if constexpr (TP) qdv[(d0 + j) * ST] = qdd;   // the VJP's output rows (qd is not read again in this mode)
           else if (live && io.qdd_out) io.qdd_out[(size_t)(d0 + j) * ns + e] = (float)val_of(qdd);
         } else if (!world_step) qdv[(d0 + j) * ST] = RQ(RA(qdv[(d0 + j) * ST]) + qdd * dtA);
@@ -691,7 +769,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       a.bot = axpy(S.bot, qdd, a.bot);
       const int qdi = M.qd_idx[i];
       if (mode == MODE_FD) {
-        if constexpr (AD) { if (live && io.jac) io.jac[((size_t)qdi * io.jac_n_in + dir) * ns + e] = qdd.d; }
+        if constexpr (AD) { if (live && io.jac) io.jac[((size_t)qdi * io.jac_n_in + jcol) * ns + e] = qdd.d; }
         else if constexpr (TP) qdv[qdi * ST] = qdd;
         else if (live && io.qdd_out) io.qdd_out[(size_t)qdi * ns + e] = (float)val_of(qdd);
       } else if (!world_step) qdv[qdi * ST] = RQ(RA(qdv[qdi * ST]) + qdd * dtA);
@@ -705,7 +783,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
 #pragma unroll
     for (int k = 0; k < 6; ++k) {
       if (mode == MODE_FD) {
-        if constexpr (AD) { if (live && io.jac) io.jac[((size_t)k * io.jac_n_in + dir) * ns + e] = qb[k].d; }
+        if constexpr (AD) { if (live && io.jac) io.jac[((size_t)k * io.jac_n_in + jcol) * ns + e] = qb[k].d; }
         else if constexpr (TP) qdv[k * ST] = qb[k];
         else if (live && io.qdd_out) io.qdd_out[(size_t)k * ns + e] = (float)val_of(qb[k]);
       } else if (!world_step) qdv[k * ST] = RQ(RC(qdv[k * ST]) + qb[k] * RC(P.dt));
@@ -779,7 +857,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
           // rel_vel = vel_a - vel_b = -vel ; mb_constraint_solver.hpp:299-345
           RS* const cs = A.ptr<RS>(M.x_conS) + c * 6 * ST;   // b[3], x[3]
           if (P.contact_model == 1) cs[0] = RS(dot(nbv, vel));   // spring-damper: approach speed n_b . v_b
-          else cs[0] = RS((RC(1) + RC(P.restitution)) * dot(nbv, vel) - RC(P.erp) * dist / RC(P.dt));
+          else cs[0] = RS((RC(1) + RC(par_of(par_restitution, P.restitution))) * dot(nbv, vel) - RC(P.erp) * dist / RC(P.dt));
           cs[ST] = RS(dot(f1, vel));
           cs[2 * ST] = RS(dot(f2, vel));
           cs[3 * ST] = RS(0); cs[4 * ST] = RS(0); cs[5 * ST] = RS(0);
@@ -818,7 +896,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
           }
           RS* const cs = A.ptr<RS>(M.x_conS) + c * 6 * ST;   // b[3], x[3]
           if (P.contact_model == 1) cs[0] = RS(dot(nrm, vel));
-          else cs[0] = RS((RC(1) + RC(P.restitution)) * dot(nrm, vel) - RC(P.erp) * dist / RC(P.dt));
+          else cs[0] = RS((RC(1) + RC(par_of(par_restitution, P.restitution))) * dot(nrm, vel) - RC(P.erp) * dist / RC(P.dt));
           cs[ST] = RS(dot(g1, vel));
           cs[2 * ST] = RS(dot(g2, vel));
           cs[3 * ST] = RS(0); cs[4 * ST] = RS(0); cs[5 * ST] = RS(0);
@@ -836,7 +914,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     // matrix-free projected Gauss-Seidel on w = Y p; row order normals | friction-1 | friction-2
     // (solve_pgs, mb_constraint_solver.hpp:101-142; bounds :417-436)
     for (int k = 0; k < n3; ++k) wv[k * ST] = RS(0);
-    const RS cfm = RS(P.cfm), mu = RS(P.friction);
+    const RS cfm = RS(P.cfm), mu = RS(par_of(par_friction, P.friction));
     if (P.contact_model == 1) {
       // Spring-damper law instead of the LCP (DESIGN.md "Spring-damper contacts"; parity unpinned): closed-form impulses
       //   p_n = dt max(0, k x^n + d x^n xdot),  x = -distance, xdot = n_b . v_b
@@ -963,8 +1041,8 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // ---- reward / done / auto-reset, write back ------------------------------------------------------------------------
   if constexpr (AD) {   // the Jacobian column of this lane's direction: rows q' | qd'
     if (live && io.jac) {
-      for (int k = 0; k < M.n_q; ++k) io.jac[((size_t)k * io.jac_n_in + dir) * ns + e] = qv[k * ST].d;
-      for (int k = 0; k < n; ++k) io.jac[((size_t)(M.n_q + k) * io.jac_n_in + dir) * ns + e] = qdv[k * ST].d;
+      for (int k = 0; k < M.n_q; ++k) io.jac[((size_t)k * io.jac_n_in + jcol) * ns + e] = qv[k * ST].d;
+      for (int k = 0; k < n; ++k) io.jac[((size_t)(M.n_q + k) * io.jac_n_in + jcol) * ns + e] = qdv[k * ST].d;
     }
     return;
   }
@@ -1019,7 +1097,7 @@ extern "C" int tds_launch_stepw(const DevModel* M, const SimParams* P, const Env
       if (err == cudaSuccess) smem_set = smem;                                                          \
     }                                                                                                   \
     if (err == cudaSuccess) {                                                                           \
-      k<<<blocks, threads, smem, stream>>>(*M, *P, *E, *io, mode, use_pd, gscratch);                    \
+      k<<<blocks, threads, smem, stream>>>(*M, *P, *E, *io, mode, use_pd, gscratch, NoPar{});           \
       err = cudaGetLastError();                                                                         \
     }                                                                                                   \
   } while (0)
@@ -1038,7 +1116,7 @@ extern "C" int tds_launch_stepw_jacobian(const DevModel* M, const SimParams* P, 
   using namespace tdsw;
   typedef tds::Dual<double> D;
   const dim3 grid((io->n + 31) / 32, n_dirs);
-  tds_stepw_kernel<D, D, D, D, false><<<grid, 32, 0, stream>>>(*M, *P, *E, *io, mode, use_pd, gscratch);
+  tds_stepw_kernel<D, D, D, D, false><<<grid, 32, 0, stream>>>(*M, *P, *E, *io, mode, use_pd, gscratch, NoPar{});
   return (int)cudaGetLastError();
 }
 
@@ -1050,7 +1128,7 @@ extern "C" int tds_launch_stepw_vjp(const DevModel* M, const SimParams* P, const
                                     int use_pd, char* gscratch, cudaStream_t stream) {
   using namespace tdsw;
   typedef tds::Tape<double> T;
-  tds_stepw_kernel<T, T, T, T, false><<<(io->n + 31) / 32, 32, 0, stream>>>(*M, *P, *E, *io, mode, use_pd, gscratch);
+  tds_stepw_kernel<T, T, T, T, false><<<(io->n + 31) / 32, 32, 0, stream>>>(*M, *P, *E, *io, mode, use_pd, gscratch, NoPar{});
   return (int)cudaGetLastError();
 }
 #endif  // TDS_STEPW_KERNEL_ONLY

@@ -145,3 +145,16 @@ struct StepIO {
   const double* g_out; double* g_in;
   void* tape; double* tape_adj; int tape_cap; int* tape_overflow;
 };
+
+// Installed physical parameters (tds_b200_set_physical_params_*): the slot of each model quantity in the lane's value vector,
+// or -1 = the model's value, and the values themselves.  Passed only to the instances of the world-frame kernel that read them
+// (StepIO stays as it is: the other instances keep it on their stack).
+struct ParMap {
+  const double* values;                // [k][n_stride] fp64, offset to the launch's first environment
+  double* grad;                        // [k][n_stride] fp64 cotangents from the taping instance, or null
+  int n;                               // installed parameters k
+  int friction, restitution;           // SimParams::friction / restitution
+  int any_base;                        // some base quantity is installed: the base inertia is packed per lane
+  short body[TDS_MAX_LINKS + 1][10];   // body b (0 = floating base, i + 1 = link i): mass, com x y z, I_com xx xy xz yy yz zz
+  short joint[TDS_MAX_LINKS][2];       // link i: joint stiffness, joint damping
+};

@@ -84,6 +84,82 @@ def merge_models(models):
     return np.concatenate([head, ms[0][HEADER:HEADER + BASE], np.concatenate(links).ravel(), geoms.ravel(), vis.ravel()])
 
 
+_BODY_COMPONENTS = ("mass", "com.x", "com.y", "com.z", "inertia.xx", "inertia.xy", "inertia.xz", "inertia.yy", "inertia.yz", "inertia.zz")
+_INERTIA_SYM = ((0, 0), (0, 1), (0, 2), (1, 1), (1, 2), (2, 2))
+# World::default_friction / default_restitution of the reference (src/world.hpp), the simulator's defaults (BatchSim.set_params)
+DEFAULT_FRICTION, DEFAULT_RESTITUTION = 0.5, 0.0
+
+
+def param_names(model):
+    """Names of the physical parameter ids of a flat model (include/tds_b200.h), index = id: "friction", "restitution",
+    "base.mass", "base.com.x", ..., "link<i>.inertia.zz", then "link<i>.stiffness", "link<i>.damping".  Base ids exist for
+    fixed-base models too (they cannot be installed there).  Host only."""
+    n_links = model_dims(model)["n_links"]
+    names = ["friction", "restitution"]
+    for b in range(n_links + 1):
+        body = "base" if b == 0 else f"link{b - 1}"
+        names += [f"{body}.{c}" for c in _BODY_COMPONENTS]
+    for i in range(n_links):
+        names += [f"link{i}.stiffness", f"link{i}.damping"]
+    return names
+
+
+def param_values(model, friction=DEFAULT_FRICTION, restitution=DEFAULT_RESTITUTION):
+    """The model's value of every parameter id (float64, index = id): friction and restitution are the solver settings given
+    (the simulator's defaults unless stated), off-diagonal inertias the symmetric component 0.5 (I_ab + I_ba) the model compiler
+    uses.  Host only."""
+    m = np.asarray(model, dtype=np.float64)
+    n_links = model_dims(m)["n_links"]
+    out = [float(friction), float(restitution)]
+    for b in range(n_links + 1):
+        rec = m[HEADER:HEADER + BASE] if b == 0 else m[HEADER + BASE + (b - 1) * LINK + 19:HEADER + BASE + (b - 1) * LINK + 32]
+        inertia = rec[4:13].reshape(3, 3)
+        out += list(rec[0:4]) + [0.5 * (inertia[r, c] + inertia[c, r]) for r, c in _INERTIA_SYM]
+    for i in range(n_links):
+        rec = m[HEADER + BASE + i * LINK:HEADER + BASE + (i + 1) * LINK]
+        out += [rec[32], rec[33]]
+    return np.asarray(out, dtype=np.float64)
+
+
+def param_ids(model, names_or_ids):
+    """Parameter names and / or ids -> list of int ids (ValueError for an unknown name)."""
+    names = None
+    ids = []
+    for x in names_or_ids:
+        if isinstance(x, str):
+            names = names or {nm: k for k, nm in enumerate(param_names(model))}
+            if x not in names:
+                raise ValueError(f"unknown physical parameter {x!r}")
+            ids.append(names[x])
+        else:
+            ids.append(int(x))
+    return ids
+
+
+def set_param_values(model, ids, values):
+    """A copy of the flat model with parameter ids (not friction / restitution: those are solver settings) set to values, as
+    the simulator applies them per environment; an off-diagonal inertia id sets both entries."""
+    m = np.array(model, dtype=np.float64)
+    n_links = model_dims(m)["n_links"]
+    j0 = 2 + 10 * (n_links + 1)
+    for i, v in zip(ids, values):
+        if i < 2:
+            raise ValueError("friction / restitution are solver settings, not model entries")
+        if i < j0:
+            b, c = divmod(i - 2, 10)
+            o = HEADER if b == 0 else HEADER + BASE + (b - 1) * LINK + 19
+            if c < 4:
+                m[o + c] = v
+            else:
+                r, cc = _INERTIA_SYM[c - 4]
+                m[o + 4 + 3 * r + cc] = v
+                m[o + 4 + 3 * cc + r] = v
+        else:
+            li, c = divmod(i - j0, 2)
+            m[HEADER + BASE + li * LINK + 32 + c] = v
+    return m
+
+
 def save_model(path, model, meta=None):
     with open(path, "w") as f:
         json.dump({"layout": "tds_b200_model.h", "meta": meta or {}, "model": [float(v) for v in model]}, f)

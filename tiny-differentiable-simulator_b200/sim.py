@@ -40,6 +40,7 @@ class BatchSim:
         (self.n_envs, self.n_stride, self.n_q, self.n_qd, self.n_tau, self.n_links,
          self.n_contact_points, self.n_act) = list(dims)
         self.device = device
+        self.param_ids = []   # installed physical parameters (set_physical_params)
         self.set_params(dt, gravity, friction, restitution, erp, cfm, pgs_iterations, keep_all_points)
         self.set_precision(precision)
 
@@ -186,6 +187,78 @@ class BatchSim:
         st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
         self._check(self._L.tds_b200_step_vjp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), _ptr(g_out),
                                                      _ptr(g_in), st), "step_vjp_device")
+
+    # ---- per-environment physical parameters (DESIGN.md section 7.9) ----
+    def set_physical_params(self, names_or_ids, values=None):
+        """Install physical parameters per environment: names (tds_b200.model.param_names) or ids, and values float64 [n_envs, k]
+        or [k] (every environment), a numpy array or a CUDA tensor.  names_or_ids None (or empty) clears the set.  Every stepping
+        call then uses each environment's values for these parameters and the model's for the rest."""
+        from .model import param_ids
+        ids = [] if names_or_ids is None else param_ids(self.model, names_or_ids)
+        k = len(ids)
+        idv = np.ascontiguousarray(ids, dtype=np.int32)
+        idp = ctypes.c_void_p(idv.ctypes.data) if k else None
+        if k == 0:
+            self._check(self._L.tds_b200_set_physical_params_host(self._h, 0, None, None), "set_physical_params")
+        elif hasattr(values, "is_cuda") and values.is_cuda:
+            import torch
+            v = values.to(torch.float64)
+            if v.dim() == 1:
+                v = v.unsqueeze(0).expand(self.n_envs, k)
+            if tuple(v.shape) != (self.n_envs, k):
+                raise ValueError(f"values: [n_envs, {k}] or [{k}] expected, got {tuple(values.shape)}")
+            soa = torch.zeros((k, self.n_stride), dtype=torch.float64, device=v.device)
+            soa[:, :self.n_envs] = v.t()
+            st = torch.cuda.current_stream(v.device)
+            self._check(self._L.tds_b200_set_physical_params_device(self._h, k, idp, _ptr(soa), ctypes.c_void_p(st.cuda_stream)),
+                        "set_physical_params")
+            st.synchronize()   # the simulator's copy is complete before soa is released
+        else:
+            v = np.asarray(values, dtype=np.float64)
+            if v.ndim == 1:
+                v = np.broadcast_to(v, (self.n_envs, k))
+            if v.shape != (self.n_envs, k):
+                raise ValueError(f"values: [n_envs, {k}] or [{k}] expected, got {v.shape}")
+            v = np.ascontiguousarray(v)
+            self._check(self._L.tds_b200_set_physical_params_host(self._h, k, idp, _dp(v)), "set_physical_params")
+        self.param_ids = ids
+
+    def param_count(self):
+        """Number of physical parameter ids of the model (include/tds_b200.h)."""
+        return self._L.tds_b200_param_count(self._h)
+
+    def step_param_jacobian_host(self, mode, q, qd, tau_or_action=None, use_pd=False):
+        """d(outputs) / d(installed parameters) of one step per environment by dual numbers: [n, rows, k] float64, rows as in
+        step_jacobian_host, columns in the order of set_physical_params."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        qd = np.ascontiguousarray(qd, dtype=np.float64)
+        t = None if tau_or_action is None else np.ascontiguousarray(tau_or_action, dtype=np.float64)
+        rows, _ = self.jacobian_dims(mode, use_pd)
+        jac = np.zeros((self.n_envs, rows, len(self.param_ids)))
+        self._check(self._L.tds_b200_step_param_jacobian_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), _dp(jac)),
+                    "step_param_jacobian_host")
+        return jac
+
+    def step_vjp_params_host(self, mode, q, qd, tau_or_action, g_out, use_pd=False):
+        """step_vjp_host with the installed parameters as further inputs: returns (g_in [n, cols], g_par [n, k])."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        qd = np.ascontiguousarray(qd, dtype=np.float64)
+        t = None if tau_or_action is None else np.ascontiguousarray(tau_or_action, dtype=np.float64)
+        rows, cols = self.jacobian_dims(mode, use_pd)
+        g = np.ascontiguousarray(g_out, dtype=np.float64)
+        assert g.shape == (self.n_envs, rows), (g.shape, rows)
+        g_in = np.zeros((self.n_envs, cols))
+        g_par = np.zeros((self.n_envs, len(self.param_ids)))
+        self._check(self._L.tds_b200_step_vjp_params_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), _dp(g), _dp(g_in),
+                                                          _dp(g_par)), "step_vjp_params_host")
+        return g_in, g_par
+
+    def step_vjp_params_device(self, mode, q, qd, tau_or_action, g_out, g_in, g_par, use_pd=False, stream=None):
+        """step_vjp_device with the installed parameters: g_par [k, n_stride] float64 CUDA tensor; g_in may be None."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_step_vjp_params_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action),
+                                                            _ptr(g_out), _ptr(g_in), _ptr(g_par), st), "step_vjp_params_device")
 
     def vjp_tape_info(self):
         """(tape capacity in nodes per lane, environments per chunk) of the reverse-mode path as it stands."""
