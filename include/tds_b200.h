@@ -174,6 +174,26 @@ int tds_b200_step_vjp_params_device(tds_b200_sim* sim, int mode, int use_pd, con
 int tds_b200_step_vjp_params_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd,
                                   const double* tau_or_action, const double* g_out, double* g_in, double* g_par);
 
+/* ---- Jacobian-vector products (forward mode, DESIGN.md 7.10): t_out = J V for m tangent directions V per environment ----------
+ * J is the step's Jacobian over its inputs (columns as tds_b200_step_jacobian_*, kp, kd, max_force included with use_pd) and, while a
+ * parameter set is installed, over the installed parameters (in the order of tds_b200_set_physical_params_*).  Semantics as the
+ * Jacobian's: the derivative of the fp64 world-frame step at the fp32-rounded inputs, of the branch taken, with each environment's
+ * parameter values.  One lane per (environment, tangent) of the dual-number step; the tangents run in chunks as the Jacobian's
+ * directions, so m = cols costs about one Jacobian.  t_in or t_par may be NULL (zero tangent), not both.  Argument checks: mode WORLD
+ * -> -2, use_pd without tds_b200_set_env -> -3, a NULL required pointer (q, qd, t_out; the action with use_pd), m < 1 or both tangents
+ * NULL -> -1, t_par without an installed set -> -4.
+ *   device: q, qd, tau_or_action as in tds_b200_step_device; t_in [cols * m][n_stride], t_par [k * m][n_stride], t_out [rows * m][n_stride]
+ *           fp64: entry (c, j) of environment e at (c * m + j) * n_stride + e.  Asynchronous on `stream`.
+ *   host:   q [n][n_q], qd [n][n_qd], tau_or_action [n][..] fp64 (rounded to fp32); t_in [n][cols][m], t_par [n][k][m],
+ *           t_out [n][rows][m] fp64.  Synchronous.
+ * tds_b200_jacobian_chunk: the directions (Jacobian columns or tangents) one launch takes; more run in several launches, each with
+ * arena scratch of at most 2 GB. */
+int tds_b200_step_jvp_device(tds_b200_sim* sim, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                             int m, const double* t_in, const double* t_par, double* t_out, void* stream);
+int tds_b200_step_jvp_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                           int m, const double* t_in, const double* t_par, double* t_out);
+int tds_b200_jacobian_chunk(const tds_b200_sim* sim);
+
 /* Stand-alone integration stages of the fine-grained surface (device SoA arrays as above):
  * integrate_euler (src/dynamics/integrator.hpp:10-133): qd += qdd dt (qdd may be NULL = zero), q += qd dt, floating base
  * quaternion increment + normalisation; integrate_euler_qdd (:141-195): qd += qdd dt only. */
@@ -353,6 +373,19 @@ int tds_b200_rigid_vjp_device(tds_b200_rigid* h, const double* state, const doub
                               double* g_state, double* g_force, void* stream);
 int tds_b200_rigid_vjp_host(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
                             double* g_state, double* g_force);
+/* Jacobian-vector products of `steps` World::step calls: t_state_out = d state_out / d (state | force) along m tangents, by the
+ * dual-number kernel seeded with the tangents, one lane per (world, tangent) running the whole rollout in one launch (no
+ * checkpoints).  The force acts in the first step only; a force tangent with force NULL differentiates at zero force.  state_out (the
+ * rollout's end state, written by the lanes of tangent 0) may be NULL and must not alias state.  t_state or t_force may be NULL
+ * (zero tangent), not both; m < 1, m > 65535 or a NULL required pointer -> -1.
+ *   device: state [13 n_bodies][n_stride], force [3 n_bodies][n_stride]; t_state / t_state_out [13 n_bodies * m][n_stride],
+ *           t_force [3 n_bodies * m][n_stride] fp64, entry (r, j) of world e at (r * m + j) * n_stride + e.  Asynchronous.
+ *   host:   state [n_worlds][n_bodies][13], force [n_worlds][n_bodies][3]; t_state / t_state_out [n_worlds][n_bodies][13][m],
+ *           t_force [n_worlds][n_bodies][3][m] fp64.  Synchronous. */
+int tds_b200_rigid_jvp_device(tds_b200_rigid* h, const double* state, const double* force, int steps, int m, const double* t_state,
+                              const double* t_force, double* state_out, double* t_state_out, void* stream);
+int tds_b200_rigid_jvp_host(tds_b200_rigid* h, const double* state, const double* force, int steps, int m, const double* t_state,
+                            const double* t_force, double* state_out, double* t_state_out);
 
 #ifdef __cplusplus
 }

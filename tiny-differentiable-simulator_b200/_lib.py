@@ -104,6 +104,16 @@ def lib():
     L.tds_b200_step_vjp_params_host.restype = ci
     L.tds_b200_step_vjp_params_host.argtypes = [vp, ci, ci, dp, dp, dp, dp, dp, dp]
     L.tds_b200_vjp_tape_info.argtypes = [vp, ctypes.POINTER(ci)]
+    L.tds_b200_step_jvp_device.restype = ci
+    L.tds_b200_step_jvp_device.argtypes = [vp, ci, ci, fp, fp, fp, ci, vp, vp, vp, vp]
+    L.tds_b200_step_jvp_host.restype = ci
+    L.tds_b200_step_jvp_host.argtypes = [vp, ci, ci, dp, dp, dp, ci, dp, dp, dp]
+    L.tds_b200_jacobian_chunk.restype = ci
+    L.tds_b200_jacobian_chunk.argtypes = [vp]
+    L.tds_b200_rigid_jvp_device.restype = ci
+    L.tds_b200_rigid_jvp_device.argtypes = [vp, vp, vp, ci, ci, vp, vp, vp, vp, vp]
+    L.tds_b200_rigid_jvp_host.restype = ci
+    L.tds_b200_rigid_jvp_host.argtypes = [vp, vp, vp, ci, ci, vp, vp, vp, vp]
     L.tds_b200_integrate_euler_device.restype = ci
     L.tds_b200_integrate_euler_device.argtypes = [vp, fp, fp, fp, vp]
     L.tds_b200_integrate_euler_qdd_device.restype = ci
@@ -179,9 +189,10 @@ DECLARED_SYMBOLS = [
     "tds_b200_step_vjp_device", "tds_b200_step_vjp_host", "tds_b200_vjp_tape_info",
     "tds_b200_param_count", "tds_b200_set_physical_params_device", "tds_b200_set_physical_params_host",
     "tds_b200_step_param_jacobian_device", "tds_b200_step_param_jacobian_host", "tds_b200_step_vjp_params_device",
-    "tds_b200_step_vjp_params_host", "tds_b200_integrate_euler_device", "tds_b200_integrate_euler_qdd_device", "tds_b200_contact_pairs", "tds_b200_model_contact_pairs", "tds_b200_contact_tuples", "tds_b200_model_contact_tuples", "tds_b200_contact_list_device", "tds_b200_contact_list_host", "tds_b200_contact_list_candidates_host",
+    "tds_b200_step_vjp_params_host", "tds_b200_step_jvp_device", "tds_b200_step_jvp_host", "tds_b200_jacobian_chunk",
+    "tds_b200_integrate_euler_device", "tds_b200_integrate_euler_qdd_device", "tds_b200_contact_pairs", "tds_b200_model_contact_pairs", "tds_b200_contact_tuples", "tds_b200_model_contact_tuples", "tds_b200_contact_list_device", "tds_b200_contact_list_host", "tds_b200_contact_list_candidates_host",
     "tds_b200_rigid_create", "tds_b200_rigid_destroy", "tds_b200_rigid_set_params", "tds_b200_rigid_step_device", "tds_b200_rigid_step_host", "tds_b200_rigid_jacobian_host",
-    "tds_b200_rigid_vjp_device", "tds_b200_rigid_vjp_host",
+    "tds_b200_rigid_vjp_device", "tds_b200_rigid_vjp_host", "tds_b200_rigid_jvp_device", "tds_b200_rigid_jvp_host",
     "tds_b200_step_device", "tds_b200_step_host", "tds_b200_env_set_state_host",
     "tds_b200_env_get_state_host", "tds_b200_env_step_host", "tds_b200_env_step_device",
     "tds_b200_stream", "tds_b200_env_q", "tds_b200_env_qd", "cuda_model_laikago_forward_zero",

@@ -15,6 +15,11 @@ identification by gradient descent through rollouts.
 
 rigid_step does the same for a batch of rigid-body worlds (RigidWorld) on float64 [n_worlds, n_bodies, 13] / [..., 3] tensors:
 the reverse pass checkpoints the states of the rollout on the device and sweeps one step at a time.
+
+Both functions also have forward-mode rules (DESIGN.md section 7.10), for torch.autograd.forward_ad dual tensors and torch.func.jvp:
+the tangent of the outputs is the Jacobian-vector product of the same derivative (BatchSim.step_jvp_device, RigidWorld.step_jvp_device),
+run with the parameter values of the same call.  Tangents of q, qd, tau_or_action and of the outputs are float32, those of params
+float64; the PD gains have zero tangent.  rigid_step's forward mode runs the whole rollout in one launch.
 """
 import torch
 
@@ -30,9 +35,19 @@ def _soa(x, n_stride, dtype):
     return out
 
 
+def _plain(t):
+    """The tensor under torch.func's wrappers.  Under torch.func.jvp the forward-mode rules below receive the tangents wrapped for the
+    transform's levels; they unwrap them and run with the transforms switched off (torch._C._DisableFuncTorch), so that the tensors
+    handed to the C-ABI have storage."""
+    from torch._C._functorch import get_unwrapped, is_functorch_wrapped_tensor
+    while t is not None and is_functorch_wrapped_tensor(t):
+        t = get_unwrapped(t)
+    return t
+
+
 class _Step(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, sim, mode, use_pd, q, qd, tau, params):
+    def forward(sim, mode, use_pd, q, qd, tau, params):
         n, ns = sim.n_envs, sim.n_stride
         if params is not None:
             sim.set_physical_params(sim.param_ids, params.detach())
@@ -41,11 +56,21 @@ class _Step(torch.autograd.Function):
         q_out, qd_out = torch.empty_like(qs), torch.empty_like(qds)
         qdd_out = torch.empty_like(qds) if mode == MODE_FD else None
         sim.step_device(mode, qs, qds, ts, q_out=q_out, qd_out=qd_out, qdd_out=qdd_out, use_pd=use_pd)
-        ctx.sim, ctx.mode, ctx.use_pd, ctx.has_tau, ctx.has_params = sim, mode, use_pd, tau is not None, params is not None
-        ctx.save_for_backward(qs, qds, ts if ts is not None else qs, params.detach() if params is not None else qs)
         if mode == MODE_FD:
             return qdd_out[:sim.n_qd, :n].t().contiguous()
         return q_out[:sim.n_q, :n].t().contiguous(), qd_out[:sim.n_qd, :n].t().contiguous()
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        # (separate from forward so that torch.func transforms accept the Function; the SoA inputs are rebuilt here, the values
+        # forward stepped)
+        sim, mode, use_pd, q, qd, tau, params = inputs
+        ns = sim.n_stride
+        qs, qds = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32)
+        ts = None if tau is None else _soa(tau, ns, torch.float32)
+        ctx.sim, ctx.mode, ctx.use_pd, ctx.has_tau, ctx.has_params = sim, mode, use_pd, tau is not None, params is not None
+        ctx.save_for_backward(qs, qds, ts if ts is not None else qs, params.detach() if params is not None else qs)
+        ctx.jvp_inputs = (qs, qds, ts, params.detach() if params is not None else None)
 
     @staticmethod
     def backward(ctx, *grads):
@@ -78,6 +103,38 @@ class _Step(torch.autograd.Function):
             gt = g_in[k0:k0 + (sim.n_act if ctx.use_pd else sim.n_tau), :n].t().to(torch.float32)
         return None, None, None, gq, gqd, gt, gp
 
+    @staticmethod
+    def jvp(ctx, _sim, _mode, _use_pd, *tangents):
+        with torch._C._DisableFuncTorch():
+            return _Step._jvp(ctx, *(_plain(t) for t in tangents))
+
+    @staticmethod
+    def _jvp(ctx, tq, tqd, ttau, tpar):
+        # forward mode: the m = 1 Jacobian-vector product of the fp64 world-frame step at the same inputs and parameter values
+        sim, mode, use_pd = ctx.sim, ctx.mode, ctx.use_pd
+        qs, qds, ts, par = (_plain(t) for t in ctx.jvp_inputs)
+        n, ns = sim.n_envs, sim.n_stride
+        rows, cols = sim.jacobian_dims(mode, use_pd)
+        t_in = t_par = None
+        if tq is not None or tqd is not None or (ttau is not None and ctx.has_tau):
+            t_in = torch.zeros((cols, ns), dtype=torch.float64, device=qs.device)
+            k0 = sim.n_q + sim.n_qd
+            for t, r0 in ((tq, 0), (tqd, sim.n_q), (ttau if ctx.has_tau else None, k0)):   # the PD gains: zero tangent
+                if t is not None and t.shape[1]:
+                    t_in[r0:r0 + t.shape[1], :n] = t.to(torch.float64).t()
+        if tpar is not None and ctx.has_params:
+            t_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=qs.device)
+            t_par[:, :n] = tpar.to(torch.float64).t()
+        t_out = torch.zeros((rows, ns), dtype=torch.float64, device=qs.device)
+        if t_in is not None or t_par is not None:
+            if ctx.has_params:
+                sim.set_physical_params(sim.param_ids, par)   # the values of this step
+            sim.step_jvp_device(mode, qs, qds, ts, 1, t_in, t_par, t_out, use_pd=use_pd)
+        if mode == MODE_FD:
+            return t_out[:sim.n_qd, :n].t().to(torch.float32).contiguous()
+        return (t_out[:sim.n_q, :n].t().to(torch.float32).contiguous(),
+                t_out[sim.n_q:sim.n_q + sim.n_qd, :n].t().to(torch.float32).contiguous())
+
 
 def step(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False, params=None):
     """One differentiable step of every environment of `sim` (a BatchSim).  q [n_envs, n_q], qd [n_envs, n_qd], tau_or_action
@@ -109,15 +166,23 @@ def _on_side_stream(dev, fn, tensors):
 
 class _RigidStep(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, world, steps, state, force):
+    def forward(world, steps, state, force):
         n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
         s = _soa(state.reshape(n, 13 * nb), ns, torch.float64)
         f = None if force is None else _soa(force.reshape(n, 3 * nb), ns, torch.float64)
         out = torch.empty_like(s)
         _on_side_stream(state.device, lambda st: world.step_device(s, out, f, steps, stream=st), (s, out, f))
+        return out[:, :n].t().reshape(n, nb, 13).contiguous()
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        world, steps, state, force = inputs
+        n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
+        s = _soa(state.reshape(n, 13 * nb), ns, torch.float64)
+        f = None if force is None else _soa(force.reshape(n, 3 * nb), ns, torch.float64)
         ctx.world, ctx.steps, ctx.has_force = world, steps, force is not None
         ctx.save_for_backward(s, f if f is not None else s)
-        return out[:, :n].t().reshape(n, nb, 13).contiguous()
+        ctx.jvp_inputs = (s, f)
 
     @staticmethod
     def backward(ctx, g):
@@ -132,6 +197,24 @@ class _RigidStep(torch.autograd.Function):
         gs = g_state[:, :n].t().reshape(n, nb, 13)
         gf = g_force[:, :n].t().reshape(n, nb, 3) if ctx.has_force else None
         return None, None, gs, gf
+
+    @staticmethod
+    def jvp(ctx, _world, _steps, t_state, t_force):
+        with torch._C._DisableFuncTorch():
+            return _RigidStep._jvp(ctx, _plain(t_state), _plain(t_force))
+
+    @staticmethod
+    def _jvp(ctx, t_state, t_force):
+        # forward mode: the whole rollout in one launch of the tangent-seeded rigid kernel
+        world = ctx.world
+        s, f = (_plain(t) for t in ctx.jvp_inputs)
+        n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
+        ts = None if t_state is None else _soa(t_state.reshape(n, 13 * nb), ns, torch.float64)
+        tf = None if t_force is None or not ctx.has_force else _soa(t_force.reshape(n, 3 * nb), ns, torch.float64)
+        t_out = torch.zeros_like(s)
+        if ts is not None or tf is not None:
+            _on_side_stream(s.device, lambda st: world.step_jvp_device(s, f, 1, ts, tf, None, t_out, ctx.steps, stream=st), (s, f, ts, tf, t_out))
+        return t_out[:, :n].t().reshape(n, nb, 13).contiguous()
 
 
 def rigid_step(world, state, force=None, steps=1):

@@ -45,6 +45,10 @@ extern "C" int tds_launch_stepw_jacobian_par(const DevModel* M, const SimParams*
                                              int mode, int use_pd, int n_dirs, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_stepw_vjp_par(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
                                         int mode, int use_pd, char* gscratch, cudaStream_t stream);
+// Jacobian-vector products, with or without installed parameters (tds_stepw_jvp.cu)
+extern "C" int tds_launch_stepw_jvp(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
+                                    const double* t_in, const double* t_par, int m, int mode, int use_pd, int n_dirs, char* gscratch,
+                                    cudaStream_t stream);
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
 // (plane candidates first, then - worlds of several multibodies - the candidates between multibodies, list after list)
@@ -392,6 +396,7 @@ struct tds_b200_sim {
   char* vjp_buf = nullptr; size_t vjp_buf_bytes = 0;
   int* vjp_flag = nullptr;
   double* vjp_g = nullptr; size_t vjp_g_bytes = 0;
+  double* jvp_dev = nullptr; size_t jvp_dev_bytes = 0;   // Jacobian-vector product, host path: t_in | t_par | t_out on the device
   // installed physical parameters (tds_b200_set_physical_params_*): slot map (par.n == 0: none) and values [k][ns] fp64
   ParMap par;
   double* par_dev = nullptr; size_t par_dev_bytes = 0;
@@ -635,7 +640,7 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->rq); cudaFree(s->rqd); cudaFree(s->zero_act); cudaFree(s->pol_act); cudaFree(s->sticky); cudaFree(s->r_total);
   cudaFree(s->pol_params); cudaFree(s->act_qidx); cudaFree(s->r_steps);
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
-  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev);
+  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->jvp_dev);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
   if (s->stage_host) cudaFreeHost(s->stage_host);
   if (s->stream) cudaStreamDestroy(s->stream);
@@ -838,13 +843,16 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
   return 0;
 }
 
+// tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null)
+struct JvpTangents { const double* t_in; const double* t_par; int m; };
+
 // Jacobian columns: the step's inputs (params == false) or the installed physical parameters, which are the dual instance's
-// directions dims[1] + s (params == true)
+// directions dims[1] + s (params == true); or, with jv, the m columns J V of the tangent-seeded instance
 static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
-                        double* jac, void* stream, bool params) {
+                        double* jac, void* stream, bool params, const JvpTangents* jv = nullptr) {
   int dims[2];
   tds_b200_jacobian_dims(s, mode, use_pd, dims);
-  const int n_dirs = params ? s->par.n : dims[1], dir_base = params ? dims[1] : 0;
+  const int n_dirs = jv ? jv->m : (params ? s->par.n : dims[1]), dir_base = (params && !jv) ? dims[1] : 0;
   StepIO io;
   memset(&io, 0, sizeof(io));
   io.q_in = q; io.qd_in = qd; io.tau_in = tau_or_action;
@@ -859,6 +867,7 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   int chunk = (int)(cap / per_dir);
   if (chunk < 1) chunk = 1;
   if (chunk > n_dirs) chunk = n_dirs;
+  if (chunk > 65535) chunk = 65535;                          // (gridDim.y)
   if (per_dir * chunk > s->jac_scratch_bytes) {
     if (s->jac_scratch) cudaFree(s->jac_scratch);
     s->jac_scratch = nullptr; s->jac_scratch_bytes = 0;
@@ -868,11 +877,21 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   for (int d0 = 0; d0 < n_dirs; d0 += chunk) {
     io.jac_dir0 = dir_base + d0;
     const int nd = n_dirs - d0 < chunk ? n_dirs - d0 : chunk;
-    int rc = pm ? tds_launch_stepw_jacobian_par(&s->dm_ad, &s->P, &s->E, &io, pm, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream)
+    int rc = jv ? tds_launch_stepw_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch,
+                                       (cudaStream_t)stream)
+           : pm ? tds_launch_stepw_jacobian_par(&s->dm_ad, &s->P, &s->E, &io, pm, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream)
                 : tds_launch_stepw_jacobian(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream);
-    if (rc) { set_err(std::string("jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
+    if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
   }
   return 0;
+}
+
+// diagnostics of the chunking above: how many directions (Jacobian columns or tangents) one launch takes for this simulator
+int tds_b200_jacobian_chunk(const tds_b200_sim* s) {
+  if (!s) return -1;
+  const size_t per_dir = (size_t)(s->n + 31) / 32 * (size_t)s->dm_ad.x_total * 32 * 4;
+  const size_t chunk = ((size_t)2 << 30) / per_dir;
+  return (int)(chunk < 1 ? 1 : (chunk > 65535 ? 65535 : chunk));
 }
 
 static int jacobian_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* jac, bool params) {
@@ -949,6 +968,84 @@ int tds_b200_step_jacobian_host(tds_b200_sim* s, int mode, int use_pd, const dou
 int tds_b200_step_param_jacobian_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
                                       const double* tau_or_action, double* jac) {
   return jacobian_host(s, mode, use_pd, q, qd, tau_or_action, jac, true);
+}
+
+// ---- Jacobian-vector products: t_out = J V for m tangents V by the tangent-seeded dual instance (tds_stepw_jvp.cu), one lane per
+// (environment, tangent), the tangents in chunks as the Jacobian's directions
+static int jvp_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* tau_or_action, int m,
+                     const void* t_in, const void* t_par, const void* t_out) {
+  if (!s || !q || !qd || !t_out || m < 1 || (!t_in && !t_par) || (use_pd && !tau_or_action)) return -1;
+  if (mode == 3) { set_err("jvp: modes FD, NOCONTACT, FULL"); return -2; }
+  if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+  if (t_par && s->par.n == 0) { set_err("jvp: parameter tangents without installed physical parameters"); return -4; }
+  return 0;
+}
+
+int tds_b200_step_jvp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                             int m, const double* t_in, const double* t_par, double* t_out, void* stream) {
+  if (int rc = jvp_check(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out)) return rc;
+  const JvpTangents jv{t_in, t_par, m};
+  return jacobian_run(s, mode, use_pd, q, qd, tau_or_action, t_out, stream, false, &jv);
+}
+
+int tds_b200_step_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                           int m, const double* t_in, const double* t_par, double* t_out) {
+  if (int rc = jvp_check(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out)) return rc;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const DevModel& M = s->dm[0];
+  const int n = s->n, ns = s->ns, k = s->par.n;
+  int dims[2];
+  tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  const int n_in = use_pd ? s->E.n_act : s->n_tau;
+  const size_t maxdim = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + 1;
+  int rc = ensure_stage(s, sizeof(double) * n * maxdim, 0);
+  if (rc) return rc;
+  const size_t ti = (size_t)dims[1] * m * ns, tp = (size_t)(t_par ? k : 0) * m * ns, to = (size_t)dims[0] * m * ns;
+  if (sizeof(double) * (ti + tp + to) > s->jvp_dev_bytes) {
+    if (s->jvp_dev) cudaFree(s->jvp_dev);
+    s->jvp_dev = nullptr; s->jvp_dev_bytes = 0;
+    CUDA_TRY(cudaMalloc((void**)&s->jvp_dev, sizeof(double) * (ti + tp + to)));
+    s->jvp_dev_bytes = sizeof(double) * (ti + tp + to);
+  }
+  double* st = (double*)s->stage_dev;
+  const int T = 128, B = (n + T - 1) / T;
+  cudaStream_t sm = s->stream;
+  auto up = [&](const double* src, int dim, float* dst) -> int {
+    if (dim == 0) return 0;
+    CUDA_TRY(cudaMemcpyAsync(st, src, sizeof(double) * n * dim, cudaMemcpyHostToDevice, sm));
+    aos_to_soa_kernel<double><<<B, T, 0, sm>>>(st, dim, 0, dst, dim, n, ns);
+    return 0;
+  };
+  if ((rc = up(q, M.n_q, s->q))) return rc;
+  if ((rc = up(qd, M.n_qd, s->qd))) return rc;
+  if (tau_or_action) { if ((rc = up(tau_or_action, n_in, s->act))) return rc; }
+  else CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * ns * (n_in > 0 ? n_in : 1), sm));
+  // tangents: host [n][dim][m] -> device [dim * m][ns]
+  std::vector<double> tmp(std::max(std::max(ti, tp), to), 0.0);
+  auto up_t = [&](const double* src, int dim, double* dst) -> int {
+    const size_t w = (size_t)dim * m;
+    std::fill(tmp.begin(), tmp.end(), 0.0);
+    for (int e = 0; e < n; ++e) for (size_t c = 0; c < w; ++c) tmp[c * ns + e] = src[(size_t)e * w + c];
+    CUDA_TRY(cudaMemcpyAsync(dst, tmp.data(), sizeof(double) * w * ns, cudaMemcpyHostToDevice, sm));
+    CUDA_TRY(cudaStreamSynchronize(sm));   // (tmp is reused)
+    return 0;
+  };
+  double* tin_d = t_in ? s->jvp_dev : nullptr;
+  double* tpar_d = t_par ? s->jvp_dev + ti : nullptr;
+  double* tout_d = s->jvp_dev + ti + tp;
+  if (t_in && (rc = up_t(t_in, dims[1], tin_d))) return rc;
+  if (t_par && (rc = up_t(t_par, k, tpar_d))) return rc;
+  CUDA_TRY(cudaMemsetAsync(tout_d, 0, sizeof(double) * to, sm));
+  const JvpTangents jv{tin_d, tpar_d, m};
+  rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, tout_d, sm, false, &jv);
+  if (rc) return rc;
+  CUDA_TRY(cudaMemcpyAsync(tmp.data(), tout_d, sizeof(double) * to, cudaMemcpyDeviceToHost, sm));
+  CUDA_TRY(cudaStreamSynchronize(sm));
+  CUDA_TRY(cudaGetLastError());
+  const size_t w = (size_t)dims[0] * m;
+  for (int e = 0; e < n; ++e)
+    for (size_t c = 0; c < w; ++c) t_out[(size_t)e * w + c] = tmp[c * ns + e];
+  return 0;
 }
 
 // ---- vector-Jacobian product: g_in = g_out^T d(q', qd' | qdd) / d(q | qd | tau or action (| kp, kd, max_force)) by the taping

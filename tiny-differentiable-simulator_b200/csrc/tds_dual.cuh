@@ -40,6 +40,11 @@ template <typename T> struct is_dual<Dual<T>> { static constexpr bool value = tr
 // instance (tds_tape.cuh) makes it leaf idx
 template <typename T> TDS_D T ad_seed(T x, int, int) { return x; }
 template <typename T> TDS_D Dual<T> ad_seed(Dual<T> x, int idx, int dir) { if (idx == dir) x.d = T(1); return x; }
+// the Jacobian-vector product instances: entry idx of tangent j gets the dual part t[(idx * m + j) * ns + e] (t null: zero tangent)
+template <typename T> TDS_D Dual<T> jv_seed(Dual<T> x, const double* t, int idx, int m, int j, int ns, int e) {
+  x.d = t ? T(t[((size_t)idx * m + j) * ns + e]) : T(0);
+  return x;
+}
 
 template <typename T> TDS_D double val_of(Dual<T> a) { return (double)a.v; }
 template <typename T> TDS_D Dual<T> min_t(Dual<T> a, Dual<T> b) { return a.v < b.v ? a : b; }

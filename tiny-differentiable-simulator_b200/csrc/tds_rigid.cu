@@ -72,6 +72,13 @@ struct RigidVjpIO {
   TapeNode* tape; double* adj; int cap; int* overflow;
 };
 
+// buffers of the Jacobian-vector product instance (JV, dual numbers; one lane per (world, tangent j = blockIdx.y + jac_dir0), the
+// whole rollout): state entry r of tangent j is t_state[(r * m + j) * ns + e], force entry r t_force[(r * m + j) * ns + e] (either may
+// be null: zero tangent); t_out [13 nb * m][ns] receives d state_out along tangent j at row r, column j
+struct RigidJvpIO { const double* t_state; const double* t_force; double* t_out; int m; };
+template <bool JV> struct RigidArg { typedef RigidVjpIO type; };
+template <> struct RigidArg<true> { typedef RigidJvpIO type; };
+
 template <typename T> struct Contact { V3<T> n, ra, rb; T dist; int a, b; };   // normal on b, point - position of a / b
 
 // contact_sphere_sphere (contact_point.hpp:44-94) between two spheres given by centre and radius; pa / pb: the bodies' positions
@@ -106,18 +113,21 @@ TDS_D void plane_sphere(const V3<T>& pn, T pc, const V3<T>& c, T r, Contact<T>* 
   else { k.n = pn; k.ra = point_b - pb; k.rb = point_a - pa; k.a = b; k.b = a; }
 }
 
-template <typename T, typename TS>
+template <typename T, typename TS, bool JV = false>
 __global__ void __launch_bounds__(128) tds_rigid_step_kernel(const __grid_constant__ RigidWorld W, const TS* s_in,
                                                              TS* s_out, const TS* __restrict__ force, int steps,
                                                              int n, int ns, double* __restrict__ jac, int jac_dir0,
-                                                             const RigidVjpIO vio = RigidVjpIO{}) {
+                                                             const typename RigidArg<JV>::type vio = {}) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= n) return;
   constexpr bool AD = is_dual<T>::value;
   constexpr bool TP = is_tape<T>::value;                     // taping instance: one lane per world, one step
   const int dir = AD ? (int)blockIdx.y + jac_dir0 : -1;      // differentiable instance: input direction of this lane
   const int nb = W.n_bodies;
-  auto seed = [&](T x, int idx) -> T { return ad_seed(x, idx, dir); };   // d input_idx / d direction, or leaf idx of the tape
+  auto seed = [&](T x, int idx) -> T {   // d input_idx / d direction, or leaf idx of the tape, or the tangent's entry idx
+    if constexpr (JV) return idx < 13 * nb ? jv_seed(x, vio.t_state, idx, vio.m, dir, ns, e) : jv_seed(x, vio.t_force, idx - 13 * nb, vio.m, dir, ns, e);
+    else return ad_seed(x, idx, dir);
+  };
   if constexpr (TP) tape_begin(vio.tape + ((size_t)(e >> 5) * vio.cap * 32 + (e & 31)), vio.g_out ? vio.cap : 0, vio.overflow, 16 * nb);
   V3<T> pos[TDS_RIGID_MAX_BODIES], lin[TDS_RIGID_MAX_BODIES], ang[TDS_RIGID_MAX_BODIES];
   T qx[TDS_RIGID_MAX_BODIES], qy[TDS_RIGID_MAX_BODIES], qz[TDS_RIGID_MAX_BODIES], qw[TDS_RIGID_MAX_BODIES];
@@ -254,7 +264,8 @@ __global__ void __launch_bounds__(128) tds_rigid_step_kernel(const __grid_consta
     const T out[13] = {pos[b].x, pos[b].y, pos[b].z, qx[b], qy[b], qz[b], qw[b], lin[b].x, lin[b].y, lin[b].z, ang[b].x, ang[b].y, ang[b].z};
     for (int k = 0; k < 13; ++k) {
       if constexpr (AD) {
-        if (jac) jac[((size_t)(b * 13 + k) * (16 * nb) + dir) * ns + e] = out[k].d;     // [row][column][world]
+        if constexpr (JV) vio.t_out[((size_t)(b * 13 + k) * vio.m + dir) * ns + e] = out[k].d;   // [row][tangent][world]
+        else if (jac) jac[((size_t)(b * 13 + k) * (16 * nb) + dir) * ns + e] = out[k].d;     // [row][column][world]
         if (blockIdx.y == 0 && s_out) s_out[(size_t)(b * 13 + k) * ns + e] = (TS)val_of(out[k]);
       } else if constexpr (!TP) {
         s_out[(size_t)(b * 13 + k) * ns + e] = (TS)out[k];
@@ -281,6 +292,7 @@ struct tds_b200_rigid {
   char* vjp_buf = nullptr; size_t vjp_buf_bytes = 0;
   int* vjp_flag = nullptr;
   double* vjp_g = nullptr;     // [2 * 13 n_bodies + 3 n_bodies][ns]: g_state | next state cotangent | g_force of the host path
+  double* jvp_buf = nullptr; size_t jvp_buf_bytes = 0;   // Jacobian-vector product, host path: t_state | t_force | t_state_out
   cudaStream_t stream = nullptr;
 };
 
@@ -314,7 +326,7 @@ void tds_b200_rigid_destroy(tds_b200_rigid* h) {
   if (!h) return;
   cudaSetDevice(h->device);
   cudaFree(h->state); cudaFree(h->state2); cudaFree(h->force); cudaFree(h->jac);
-  cudaFree(h->ckpt); cudaFree(h->vjp_buf); cudaFree(h->vjp_flag); cudaFree(h->vjp_g);
+  cudaFree(h->ckpt); cudaFree(h->vjp_buf); cudaFree(h->vjp_flag); cudaFree(h->vjp_g); cudaFree(h->jvp_buf);
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
@@ -503,6 +515,67 @@ int tds_b200_rigid_vjp_host(tds_b200_rigid* h, const double* state, const double
   for (int e = 0; e < n; ++e) {
     for (int k = 0; k < rows; ++k) g_state[(size_t)e * rows + k] = t[(size_t)k * ns + e];
     if (g_force) for (int k = 0; k < 3 * nb; ++k) g_force[(size_t)e * 3 * nb + k] = f[(size_t)k * ns + e];
+  }
+  return 0;
+}
+
+// Jacobian-vector products of `steps` steps: one launch of the tangent-seeded dual instance, one lane per (world, tangent), each lane
+// runs the whole rollout.  A force tangent with a null force acts on a zero force (the handle's force buffer is cleared for it).
+int tds_b200_rigid_jvp_device(tds_b200_rigid* h, const double* state, const double* force, int steps, int m, const double* t_state,
+                              const double* t_force, double* state_out, double* t_state_out, void* stream) {
+  if (!h || !state || !t_state_out || steps < 0 || m < 1 || m > 65535 || (!t_state && !t_force) || state_out == state)
+    return rigid_fail("rigid_jvp_device: bad argument", -1);
+  cudaStream_t sm = stream ? (cudaStream_t)stream : h->stream;
+  const int nb = h->W.n_bodies;
+  if (!force && t_force) {
+    RB_TRY(cudaMemsetAsync(h->force, 0, sizeof(double) * 3 * nb * h->ns, sm));
+    force = h->force;
+  }
+  const int T = 128;
+  const dim3 grid((h->n + T - 1) / T, m);
+  const tdsrb::RigidJvpIO v{t_state, t_force, t_state_out, m};
+  tdsrb::tds_rigid_step_kernel<tds::Dual<double>, double, true><<<grid, T, 0, sm>>>(h->W, state, state_out, force, steps, h->n, h->ns,
+                                                                                   nullptr, 0, v);
+  RB_TRY(cudaGetLastError());
+  return 0;
+}
+
+int tds_b200_rigid_jvp_host(tds_b200_rigid* h, const double* state, const double* force, int steps, int m, const double* t_state,
+                            const double* t_force, double* state_out, double* t_state_out) {
+  if (!h || !state || !t_state_out || steps < 0 || m < 1 || m > 65535 || (!t_state && !t_force)) return rigid_fail("rigid_jvp_host: bad argument", -1);
+  RB_TRY(cudaSetDevice(h->device));
+  int rc = rigid_upload(h, state, force);
+  if (rc) return rc;
+  const int nb = h->W.n_bodies, n = h->n, ns = h->ns, rows = 13 * nb;
+  const size_t ts = (size_t)rows * m * ns, tf = (size_t)3 * nb * m * ns, need = sizeof(double) * (2 * ts + tf);
+  if (need > h->jvp_buf_bytes) {
+    cudaFree(h->jvp_buf);
+    h->jvp_buf = nullptr; h->jvp_buf_bytes = 0;
+    RB_TRY(cudaMalloc((void**)&h->jvp_buf, need));
+    h->jvp_buf_bytes = need;
+  }
+  if (!h->state2) RB_TRY(cudaMalloc((void**)&h->state2, sizeof(double) * (size_t)rows * ns));
+  double *ds = h->jvp_buf, *df = h->jvp_buf + ts, *dout = h->jvp_buf + ts + tf;
+  // host [n][dim][m] -> device [dim * m][ns]
+  auto up = [&](const double* src, int dim, double* dst) -> int {
+    if (!src) return 0;
+    std::vector<double> t((size_t)dim * m * ns, 0.0);
+    for (int e = 0; e < n; ++e) for (int k = 0; k < dim * m; ++k) t[(size_t)k * ns + e] = src[(size_t)e * dim * m + k];
+    RB_TRY(cudaMemcpyAsync(dst, t.data(), sizeof(double) * t.size(), cudaMemcpyHostToDevice, h->stream));
+    RB_TRY(cudaStreamSynchronize(h->stream));
+    return 0;
+  };
+  if ((rc = up(t_state, rows, ds)) || (rc = up(t_force, 3 * nb, df))) return rc;
+  rc = tds_b200_rigid_jvp_device(h, h->state, force ? h->force : nullptr, steps, m, t_state ? ds : nullptr, t_force ? df : nullptr,
+                                 h->state2, dout, h->stream);
+  if (rc) return rc;
+  std::vector<double> t(ts), so((size_t)rows * ns);
+  RB_TRY(cudaMemcpyAsync(t.data(), dout, sizeof(double) * ts, cudaMemcpyDeviceToHost, h->stream));
+  RB_TRY(cudaMemcpyAsync(so.data(), h->state2, sizeof(double) * so.size(), cudaMemcpyDeviceToHost, h->stream));
+  RB_TRY(cudaStreamSynchronize(h->stream));
+  for (int e = 0; e < n; ++e) {
+    for (size_t k = 0; k < (size_t)rows * m; ++k) t_state_out[(size_t)e * rows * m + k] = t[k * ns + e];
+    if (state_out) for (int k = 0; k < rows; ++k) state_out[(size_t)e * rows + k] = so[(size_t)k * ns + e];
   }
   return 0;
 }

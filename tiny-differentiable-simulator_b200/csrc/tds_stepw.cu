@@ -35,8 +35,15 @@ namespace tdsw {
 
 // kernel argument of the instances without installed physical parameters: nothing
 struct NoPar {};
-template <bool PAR> struct ParArg { typedef NoPar type; };
-template <> struct ParArg<true> { typedef ParMap type; };
+// tangents of the Jacobian-vector product instances (JV, DESIGN.md section 7.10): input column c of tangent j is
+// t_in[(c * m + j) * n_stride + e], installed parameter slot s is t_par[(s * m + j) * n_stride + e]; null: zero tangent
+struct JvpTan { const double* t_in; const double* t_par; int m; };
+struct NoParJvp { JvpTan jv; };
+struct ParMapJvp : ParMap { JvpTan jv; };
+template <bool PAR, bool JV = false> struct ParArg { typedef NoPar type; };
+template <> struct ParArg<true, false> { typedef ParMap type; };
+template <> struct ParArg<false, true> { typedef NoParJvp type; };
+template <> struct ParArg<true, true> { typedef ParMapJvp type; };
 
 // joint stiffness and damping enter the step at fp32, as DevModel stores them; the derivative is taken at the rounded value
 TDS_D double f32_round(double x) { return (double)(float)x; }
@@ -51,11 +58,14 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // pm also says which model quantity each slot replaces.  In the dual instance slot s is input direction n_in_ad + s, in the taping
 // instance leaf n_in_ad + s (after the state / control inputs, so g_in keeps its layout).  The values are read where the model
 // values are read (once per step each; the reads of a warp are coalesced), so the arena layout does not change.
-template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false>
+// JV (dual instances only): Jacobian-vector product.  The lane's direction is tangent j = blockIdx.y + io.jac_dir0 of pm.jv; every
+// input and installed parameter is seeded with its entry of that tangent, and the dual parts of the outputs are column j of io.jac
+// (io.jac_n_in = m columns): t_out = J V, row-major per environment as the Jacobian.
+template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
-                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR>::type pm = {}) {
+                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV>::type pm = {}) {
   extern __shared__ __align__(16) char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp_in_blk = threadIdx.x >> 5;
@@ -68,9 +78,12 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   Arena A;
   if (SMEM) { A.blk = smem_raw + (size_t)warp_in_blk * M.x_total * 32 * 4; A.stride = 32; A.col = lane; }
   else { A.blk = gscratch + ((size_t)blockIdx.y * ((size_t)gridDim.x * (blockDim.x >> 5)) + (size_t)(env >> 5)) * M.x_total * 32 * 4; A.stride = 32; A.col = lane; }  // per-warp block, same addressing as shared memory
-  auto seed = [&](RQ x, int idx) -> RQ { return ad_seed(x, idx, dir); };   // d input_idx / d direction, or leaf idx of the tape
   const int ST = A.stride;
   const int ns = io.n_stride;
+  auto seed = [&](RQ x, int idx) -> RQ {   // d input_idx / d direction, or leaf idx of the tape, or the tangent's entry idx
+    if constexpr (JV) return jv_seed(x, pm.jv.t_in, idx, pm.jv.m, dir, ns, e);
+    else return ad_seed(x, idx, dir);
+  };
   const int n_links = M.n_links;
   const int n = M.n_qd;
   const int nb = M.nb;
@@ -96,13 +109,15 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
         for (int k = 0; k < n_in_ad; ++k) io.g_in[(size_t)k * ns + e] = adj[(size_t)k * 32];
     }
   };
-  // Jacobian column of this lane's direction: parameter directions n_in_ad + s are column s of the parameter Jacobian
-  const int jcol = (PAR && dir >= n_in_ad) ? dir - n_in_ad : dir;
+  // Jacobian column of this lane's direction: parameter directions n_in_ad + s are column s of the parameter Jacobian (the JVP
+  // instances: the tangent's column)
+  const int jcol = (PAR && !JV && dir >= n_in_ad) ? dir - n_in_ad : dir;
   // physical quantities: the lane's installed value (the dual / taping instances seed it) or the model's.  RP keeps fp64 in the
   // plain instances, as the model stores these quantities.
   typedef typename std::conditional<AD || TP, RQ, double>::type RP;
   auto par_of = [&](int slot, double model_v) -> RP {
-    if constexpr (PAR) { if (slot >= 0) return ad_seed(RP(pm.values[(size_t)slot * ns + e]), n_in_ad + slot, dir); }
+    if constexpr (PAR && JV) { if (slot >= 0) return jv_seed(RP(pm.values[(size_t)slot * ns + e]), pm.jv.t_par, slot, pm.jv.m, dir, ns, e); }
+    else if constexpr (PAR) { if (slot >= 0) return ad_seed(RP(pm.values[(size_t)slot * ns + e]), n_in_ad + slot, dir); }
     return RP(model_v);
   };
   auto body_slot = [&](int b, int c) -> int {

@@ -111,6 +111,39 @@ class RigidWorld:
         self._check(self._L.tds_b200_rigid_vjp_device(self._h, p(state), p(force), int(steps), p(g_state_out), p(g_state), p(g_force),
                                                       ctypes.c_void_p(stream.cuda_stream) if stream is not None else None), "rigid_vjp_device")
 
+    def step_jvp(self, state, force=None, t_state=None, t_force=None, steps=1):
+        """(state_out, t_state_out): Jacobian-vector products of `steps` World::step calls by forward mode on the GPU, one launch for
+        the whole rollout.  t_state [n_worlds][n_bodies][13][m], t_force [n_worlds][n_bodies][3][m] (either may be None; without the
+        trailing m axis: m = 1, and t_state_out then comes back without it too).  t_state_out [n_worlds][n_bodies][13][m]."""
+        s, f = self._args(state, force)
+        single = np.ndim(t_state if t_state is not None else t_force) == 3
+
+        def prep(x, dim):
+            if x is None:
+                return None
+            x = np.asarray(x, dtype=np.float64)
+            if x.ndim == 3:
+                x = x[..., None]
+            assert x.shape[:3] == (self.n_worlds, self.n_bodies, dim), x.shape
+            return np.ascontiguousarray(x)
+        ts, tf = prep(t_state, 13), prep(t_force, 3)
+        m = (ts if ts is not None else tf).shape[3] if (ts is not None or tf is not None) else 0
+        out = np.zeros_like(s)
+        t_out = np.zeros((self.n_worlds, self.n_bodies, 13, max(m, 1)))
+        v = lambda a: ctypes.c_void_p(a.ctypes.data) if a is not None else None
+        self._check(self._L.tds_b200_rigid_jvp_host(self._h, v(s), v(f), int(steps), m, v(ts), v(tf), v(out), v(t_out)), "rigid_jvp_host")
+        return out, (t_out[..., 0] if single else t_out)
+
+    def step_jvp_device(self, state, force, m, t_state, t_force, state_out, t_state_out, steps=1, stream=None):
+        """Device version of step_jvp: float64 CUDA tensors state [13 * n_bodies][n_stride], force [3 * n_bodies][n_stride] or None,
+        t_state / t_state_out [13 * n_bodies * m][n_stride], t_force [3 * n_bodies * m][n_stride] (entry (r, j) at row r * m + j;
+        t_state or t_force may be None), state_out [13 * n_bodies][n_stride] or None (not state itself).  stream None = the world's
+        own stream.  Asynchronous."""
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+        self._check(self._L.tds_b200_rigid_jvp_device(self._h, p(state), p(force), int(steps), int(m), p(t_state), p(t_force), p(state_out),
+                                                      p(t_state_out), ctypes.c_void_p(stream.cuda_stream) if stream is not None else None),
+                    "rigid_jvp_device")
+
     def step_device(self, state_in, state_out, force=None, steps=1, stream=None):
         """CUDA tensors, fp64: state [13 * n_bodies][n_stride], force [3 * n_bodies][n_stride] or None; in place allowed."""
         p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None

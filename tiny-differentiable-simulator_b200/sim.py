@@ -260,6 +260,49 @@ class BatchSim:
         self._check(self._L.tds_b200_step_vjp_params_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action),
                                                             _ptr(g_out), _ptr(g_in), _ptr(g_par), st), "step_vjp_params_device")
 
+    def step_jvp_host(self, mode, q, qd, tau_or_action, t_in, t_par=None, use_pd=False):
+        """Jacobian-vector products of one step per environment by forward mode on the GPU: t_out [n, rows, m] = J V for the m
+        tangents t_in [n, cols, m] of the inputs (rows / cols as in step_jacobian_host) and t_par [n, k, m] of the installed
+        parameters; either may be None.  A tangent given as [n, cols] (or [n, k]) is m = 1, and the result is then [n, rows].
+        Same derivative as step_jacobian_host: m = cols identity tangents give the Jacobian."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        qd = np.ascontiguousarray(qd, dtype=np.float64)
+        t = None if tau_or_action is None else np.ascontiguousarray(tau_or_action, dtype=np.float64)
+        rows, cols = self.jacobian_dims(mode, use_pd)
+        k = len(self.param_ids)
+        single = (t_in if t_in is not None else t_par) is not None and np.ndim(t_in if t_in is not None else t_par) == 2
+
+        def prep(x, dim):
+            if x is None:
+                return None
+            x = np.asarray(x, dtype=np.float64)
+            if x.ndim == 2:
+                x = x[:, :, None]
+            if x.shape[:2] != (self.n_envs, dim):
+                raise ValueError(f"tangent: [n_envs, {dim}, m] or [n_envs, {dim}] expected, got {x.shape}")
+            return np.ascontiguousarray(x)
+        ti, tp = prep(t_in, cols), prep(t_par, k)
+        if ti is not None and tp is not None and ti.shape[2] != tp.shape[2]:
+            raise ValueError("t_in and t_par: the same number of tangents m expected")
+        m = (ti if ti is not None else tp).shape[2] if (ti is not None or tp is not None) else 0
+        out = np.zeros((self.n_envs, rows, max(m, 1)))
+        self._check(self._L.tds_b200_step_jvp_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), m, _dp(ti), _dp(tp), _dp(out)),
+                    "step_jvp_host")
+        return out[:, :, 0] if single else out
+
+    def step_jvp_device(self, mode, q, qd, tau_or_action, m, t_in, t_par, t_out, use_pd=False, stream=None):
+        """Device version of step_jvp_host on the SoA layout: q, qd, tau_or_action float32 CUDA tensors [dim, n_stride] as for
+        step_device; t_in [cols * m, n_stride], t_par [k * m, n_stride] (either may be None) and t_out [rows * m, n_stride] float64
+        CUDA tensors, entry (c, j) at row c * m + j.  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_step_jvp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), int(m), _ptr(t_in),
+                                                     _ptr(t_par), _ptr(t_out), st), "step_jvp_device")
+
+    def jacobian_chunk(self):
+        """Directions (Jacobian columns or JVP tangents) one launch of the dual-number step takes; more run in several launches."""
+        return self._L.tds_b200_jacobian_chunk(self._h)
+
     def vjp_tape_info(self):
         """(tape capacity in nodes per lane, environments per chunk) of the reverse-mode path as it stands."""
         info = (ctypes.c_int * 2)()
