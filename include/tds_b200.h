@@ -387,6 +387,42 @@ int tds_b200_rigid_jvp_device(tds_b200_rigid* h, const double* state, const doub
 int tds_b200_rigid_jvp_host(tds_b200_rigid* h, const double* state, const double* force, int steps, int m, const double* t_state,
                             const double* t_force, double* state_out, double* t_state_out);
 
+/* ---- per-world physical parameters of the rigid-body world (DESIGN.md 7.11): system identification and domain randomisation ------
+ * Parameter ids, one value per world each:
+ *   0            friction (RigidWorld friction, tds_b200_rigid_set_params)
+ *   1            restitution
+ *   2 + 4 b + c  body b: c = 0 mass; c = 1..3 shape sizes: sphere radius (c = 1); capsule radius, length (c = 1, 2); box extents
+ *                x, y, z (c = 1..3).  The box's corner radius stays 1e-2.
+ * tds_b200_rigid_param_count: 2 + 4 n_bodies.
+ * Refused (-2, reason in tds_b200_last_error): an id out of range, an id given twice, the mass of a static body (model mass 0), a size
+ * component the shape does not have, any id of a plane.  A body's static / dynamic status stays that of the description.
+ *
+ * tds_b200_rigid_set_physical_params_*: install k parameters; the handle copies the values into a buffer it owns (new values for the
+ * same ids keep the buffer).  k = 0 clears the set.  device: values [k][n_stride] fp64 device pointer, copied on `stream` (NULL: the
+ * world's stream) WITHOUT checking the values.  host: values [n_worlds][k] fp64, synchronous; a non-finite value, a mass or size <= 0,
+ * a negative friction or restitution -> -3.  While a set is installed, rigid_step_*, rigid_jacobian_host, rigid_vjp_* and rigid_jvp_*
+ * use each world's values for those ids (and the description's for the rest).
+ *
+ * The derivative entries below return -4 when no set is installed; their other argument checks are those of the entries they extend
+ * (-1).  Columns and slots are in the order of the installed ids.
+ *   tds_b200_rigid_param_jacobian_host: d state_out / d (installed parameters) of `steps` steps, jac [n_worlds][13 n_bodies][k].
+ *   tds_b200_rigid_vjp_params_*: tds_b200_rigid_vjp_* that also writes g_par = g_state_out^T d state_out / d (parameters), summed over
+ *     all `steps` (the force still acts in step 0 only): device [k][n_stride], host [n_worlds][k].  g_par must not be NULL.
+ *   tds_b200_rigid_jvp_params_*: tds_b200_rigid_jvp_* with parameter tangents t_par: device [k * m][n_stride] (entry (s, j) at
+ *     (s * m + j) * n_stride + e), host [n_worlds][k][m].  t_state, t_force and t_par may each be NULL (zero tangent), not all three. */
+int tds_b200_rigid_param_count(const tds_b200_rigid* h);
+int tds_b200_rigid_set_physical_params_device(tds_b200_rigid* h, int k, const int* ids, const double* values, void* stream);
+int tds_b200_rigid_set_physical_params_host(tds_b200_rigid* h, int k, const int* ids, const double* values);
+int tds_b200_rigid_param_jacobian_host(tds_b200_rigid* h, const double* state, const double* force, int steps, double* state_out, double* jac);
+int tds_b200_rigid_vjp_params_device(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
+                                     double* g_state, double* g_force, double* g_par, void* stream);
+int tds_b200_rigid_vjp_params_host(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
+                                   double* g_state, double* g_force, double* g_par);
+int tds_b200_rigid_jvp_params_device(tds_b200_rigid* h, const double* state, const double* force, int steps, int m, const double* t_state,
+                                     const double* t_force, const double* t_par, double* state_out, double* t_state_out, void* stream);
+int tds_b200_rigid_jvp_params_host(tds_b200_rigid* h, const double* state, const double* force, int steps, int m, const double* t_state,
+                                   const double* t_force, const double* t_par, double* state_out, double* t_state_out);
+
 #ifdef __cplusplus
 }
 #endif

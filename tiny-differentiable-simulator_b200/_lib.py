@@ -142,6 +142,22 @@ def lib():
     L.tds_b200_rigid_vjp_device.argtypes = [vp, vp, vp, ci, vp, vp, vp, vp]
     L.tds_b200_rigid_vjp_host.restype = ci
     L.tds_b200_rigid_vjp_host.argtypes = [vp, vp, vp, ci, vp, vp, vp]
+    L.tds_b200_rigid_param_count.restype = ci
+    L.tds_b200_rigid_param_count.argtypes = [vp]
+    L.tds_b200_rigid_set_physical_params_device.restype = ci
+    L.tds_b200_rigid_set_physical_params_device.argtypes = [vp, ci, vp, vp, vp]
+    L.tds_b200_rigid_set_physical_params_host.restype = ci
+    L.tds_b200_rigid_set_physical_params_host.argtypes = [vp, ci, vp, vp]
+    L.tds_b200_rigid_param_jacobian_host.restype = ci
+    L.tds_b200_rigid_param_jacobian_host.argtypes = [vp, vp, vp, ci, vp, vp]
+    L.tds_b200_rigid_vjp_params_device.restype = ci
+    L.tds_b200_rigid_vjp_params_device.argtypes = [vp, vp, vp, ci, vp, vp, vp, vp, vp]
+    L.tds_b200_rigid_vjp_params_host.restype = ci
+    L.tds_b200_rigid_vjp_params_host.argtypes = [vp, vp, vp, ci, vp, vp, vp, vp]
+    L.tds_b200_rigid_jvp_params_device.restype = ci
+    L.tds_b200_rigid_jvp_params_device.argtypes = [vp, vp, vp, ci, ci, vp, vp, vp, vp, vp, vp]
+    L.tds_b200_rigid_jvp_params_host.restype = ci
+    L.tds_b200_rigid_jvp_params_host.argtypes = [vp, vp, vp, ci, ci, vp, vp, vp, vp, vp]
     L.tds_b200_contact_tuples.restype = ci
     L.tds_b200_contact_tuples.argtypes = [vp, vp, ci]
     L.tds_b200_model_contact_tuples.restype = ci
@@ -193,6 +209,9 @@ DECLARED_SYMBOLS = [
     "tds_b200_integrate_euler_device", "tds_b200_integrate_euler_qdd_device", "tds_b200_contact_pairs", "tds_b200_model_contact_pairs", "tds_b200_contact_tuples", "tds_b200_model_contact_tuples", "tds_b200_contact_list_device", "tds_b200_contact_list_host", "tds_b200_contact_list_candidates_host",
     "tds_b200_rigid_create", "tds_b200_rigid_destroy", "tds_b200_rigid_set_params", "tds_b200_rigid_step_device", "tds_b200_rigid_step_host", "tds_b200_rigid_jacobian_host",
     "tds_b200_rigid_vjp_device", "tds_b200_rigid_vjp_host", "tds_b200_rigid_jvp_device", "tds_b200_rigid_jvp_host",
+    "tds_b200_rigid_param_count", "tds_b200_rigid_set_physical_params_device", "tds_b200_rigid_set_physical_params_host",
+    "tds_b200_rigid_param_jacobian_host", "tds_b200_rigid_vjp_params_device", "tds_b200_rigid_vjp_params_host",
+    "tds_b200_rigid_jvp_params_device", "tds_b200_rigid_jvp_params_host",
     "tds_b200_step_device", "tds_b200_step_host", "tds_b200_env_set_state_host",
     "tds_b200_env_get_state_host", "tds_b200_env_step_host", "tds_b200_env_step_device",
     "tds_b200_stream", "tds_b200_env_q", "tds_b200_env_qd", "cuda_model_laikago_forward_zero",

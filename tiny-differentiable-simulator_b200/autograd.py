@@ -14,7 +14,9 @@ DESIGN.md section 7.9) the forward installs those values and steps, and the back
 identification by gradient descent through rollouts.
 
 rigid_step does the same for a batch of rigid-body worlds (RigidWorld) on float64 [n_worlds, n_bodies, 13] / [..., 3] tensors:
-the reverse pass checkpoints the states of the rollout on the device and sweeps one step at a time.
+the reverse pass checkpoints the states of the rollout on the device and sweeps one step at a time.  Its params (float64 [n_worlds,
+k], for the masses, shape sizes, friction and restitution installed by RigidWorld.set_physical_params, DESIGN.md section 7.11) get
+their gradient summed over the rollout's steps.
 
 Both functions also have forward-mode rules (DESIGN.md section 7.10), for torch.autograd.forward_ad dual tensors and torch.func.jvp:
 the tangent of the outputs is the Jacobian-vector product of the same derivative (BatchSim.step_jvp_device, RigidWorld.step_jvp_device),
@@ -166,61 +168,89 @@ def _on_side_stream(dev, fn, tensors):
 
 class _RigidStep(torch.autograd.Function):
     @staticmethod
-    def forward(world, steps, state, force):
+    def forward(world, steps, state, force, params):
         n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
         s = _soa(state.reshape(n, 13 * nb), ns, torch.float64)
         f = None if force is None else _soa(force.reshape(n, 3 * nb), ns, torch.float64)
         out = torch.empty_like(s)
-        _on_side_stream(state.device, lambda st: world.step_device(s, out, f, steps, stream=st), (s, out, f))
+
+        def run(st):
+            if params is not None:
+                world.set_physical_params(world.param_ids, params.detach(), stream=st)
+            world.step_device(s, out, f, steps, stream=st)
+        _on_side_stream(state.device, run, (s, out, f))
         return out[:, :n].t().reshape(n, nb, 13).contiguous()
 
     @staticmethod
     def setup_context(ctx, inputs, output):
-        world, steps, state, force = inputs
+        world, steps, state, force, params = inputs
         n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
         s = _soa(state.reshape(n, 13 * nb), ns, torch.float64)
         f = None if force is None else _soa(force.reshape(n, 3 * nb), ns, torch.float64)
-        ctx.world, ctx.steps, ctx.has_force = world, steps, force is not None
-        ctx.save_for_backward(s, f if f is not None else s)
-        ctx.jvp_inputs = (s, f)
+        par = params.detach() if params is not None else None
+        ctx.world, ctx.steps, ctx.has_force, ctx.has_params = world, steps, force is not None, params is not None
+        ctx.save_for_backward(s, f if f is not None else s, par if par is not None else s)
+        ctx.jvp_inputs = (s, f, par)
 
     @staticmethod
     def backward(ctx, g):
         world = ctx.world
-        s, f = ctx.saved_tensors
+        s, f, par = ctx.saved_tensors
         n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
         g_out = _soa(g.reshape(n, 13 * nb), ns, torch.float64)
         g_state = torch.zeros_like(g_out)
         g_force = torch.zeros((3 * nb, ns), dtype=torch.float64, device=g.device) if ctx.has_force else None
-        _on_side_stream(g.device, lambda st: world.step_vjp_device(s, f if ctx.has_force else None, g_out, g_state, g_force,
-                                                                   ctx.steps, stream=st), (s, f, g_out, g_state, g_force))
+        fs = f if ctx.has_force else None
+        g_par = None
+        if ctx.has_params:
+            g_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=g.device)
+
+            def run(st):
+                # the values of this call (a later call of the graph may have installed others)
+                world.set_physical_params(world.param_ids, par, stream=st)
+                world.step_vjp_params_device(s, fs, g_out, g_state, g_force, g_par, ctx.steps, stream=st)
+        else:
+            def run(st):
+                world.step_vjp_device(s, fs, g_out, g_state, g_force, ctx.steps, stream=st)
+        _on_side_stream(g.device, run, (s, f, g_out, g_state, g_force, g_par))
         gs = g_state[:, :n].t().reshape(n, nb, 13)
         gf = g_force[:, :n].t().reshape(n, nb, 3) if ctx.has_force else None
-        return None, None, gs, gf
+        gp = g_par[:, :n].t().contiguous() if ctx.has_params else None
+        return None, None, gs, gf, gp
 
     @staticmethod
-    def jvp(ctx, _world, _steps, t_state, t_force):
+    def jvp(ctx, _world, _steps, t_state, t_force, t_params):
         with torch._C._DisableFuncTorch():
-            return _RigidStep._jvp(ctx, _plain(t_state), _plain(t_force))
+            return _RigidStep._jvp(ctx, _plain(t_state), _plain(t_force), _plain(t_params))
 
     @staticmethod
-    def _jvp(ctx, t_state, t_force):
-        # forward mode: the whole rollout in one launch of the tangent-seeded rigid kernel
+    def _jvp(ctx, t_state, t_force, t_params):
+        # forward mode: the whole rollout in one launch of the tangent-seeded rigid kernel, with the parameter values of this call
         world = ctx.world
-        s, f = (_plain(t) for t in ctx.jvp_inputs)
+        s, f, par = (_plain(t) for t in ctx.jvp_inputs)
         n, nb, ns = world.n_worlds, world.n_bodies, world.n_stride
         ts = None if t_state is None else _soa(t_state.reshape(n, 13 * nb), ns, torch.float64)
         tf = None if t_force is None or not ctx.has_force else _soa(t_force.reshape(n, 3 * nb), ns, torch.float64)
+        tp = None if t_params is None or not ctx.has_params else _soa(t_params, ns, torch.float64)
         t_out = torch.zeros_like(s)
-        if ts is not None or tf is not None:
-            _on_side_stream(s.device, lambda st: world.step_jvp_device(s, f, 1, ts, tf, None, t_out, ctx.steps, stream=st), (s, f, ts, tf, t_out))
+        if ts is not None or tf is not None or tp is not None:
+            def run(st):
+                if ctx.has_params:
+                    world.set_physical_params(world.param_ids, par, stream=st)
+                world.step_jvp_device(s, f, 1, ts, tf, None, t_out, ctx.steps, stream=st, t_par=tp)
+            _on_side_stream(s.device, run, (s, f, ts, tf, tp, t_out))
         return t_out[:, :n].t().reshape(n, nb, 13).contiguous()
 
 
-def rigid_step(world, state, force=None, steps=1):
+def rigid_step(world, state, force=None, steps=1, params=None):
     """`steps` differentiable World::step calls of every world of `world` (a RigidWorld).  state [n_worlds, n_bodies, 13], force
-    [n_worlds, n_bodies, 3] (applied before the first step) float64 CUDA tensors.  Returns the new state."""
+    [n_worlds, n_bodies, 3] (applied before the first step) float64 CUDA tensors.  Returns the new state.  params: None, or a float64
+    CUDA tensor [n_worlds, k] of values for the parameters installed by world.set_physical_params (then also differentiated; a [k]
+    leaf expanded to [n_worlds, k] gets the gradient summed over the worlds)."""
     for name, t in (("state", state), ("force", force)):
         if t is not None and (t.dtype != torch.float64 or not t.is_cuda or t.shape[:2] != (world.n_worlds, world.n_bodies)):
             raise ValueError(f"{name}: a float64 CUDA tensor [n_worlds, n_bodies, dim] is expected")
-    return _RigidStep.apply(world, int(steps), state, force)
+    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or not world.param_ids or
+                               tuple(params.shape) != (world.n_worlds, len(world.param_ids))):
+        raise ValueError("params: a float64 CUDA tensor [n_worlds, k] for the k parameters installed by set_physical_params is expected")
+    return _RigidStep.apply(world, int(steps), state, force, params)
