@@ -194,6 +194,31 @@ int tds_b200_step_jvp_host(tds_b200_sim* sim, int mode, int use_pd, const double
                            int m, const double* t_in, const double* t_par, double* t_out);
 int tds_b200_jacobian_chunk(const tds_b200_sim* sim);
 
+/* ---- joint-space mass matrix M(q) (DESIGN.md 7.12; mass_matrix in python/pytinydiffsim.inl) ----------------------------------------
+ * The dense symmetric n_qd x n_qd matrix of every environment, both triangles, by the CRBA of the world-frame step (the matrix its
+ * contact solve factors), in fp64 at the fp32-rounded q; qd plays no part (the reference calls forward_kinematics with an empty qd).
+ * A world of several multibodies gives the block-diagonal matrix.  While a parameter set is installed, each environment's masses,
+ * centres of mass and inertias are used; stiffness, damping, friction and restitution do not enter M (their derivative is zero).
+ * Argument checks: a NULL required pointer, m < 1 or both tangents NULL -> -1; t_par / g_par without an installed set -> -4.
+ *   device: q [n_q][n_stride] fp32 as tds_b200_step_device; M [n_qd * n_qd][n_stride] fp64, entry (r, c) at (r * n_qd + c) * n_stride + e.
+ *           Asynchronous on `stream`.
+ *   host:   q [n][n_q] fp64 (rounded to fp32); M [n][n_qd][n_qd] fp64.  Synchronous.
+ * _jvp: dM = sum_c dM/dq_c t_q[c] + sum_s dM/dp_s t_par[s] for m tangents, one lane per (environment, tangent) of the dual-number
+ *   instance, in chunks as tds_b200_step_jvp_*.  M (may be NULL) receives the value.  Layouts as tds_b200_step_jvp_*: device t_q
+ *   [n_q * m][n_stride], t_par [k * m][n_stride], t_M [n_qd * n_qd * m][n_stride] (entry ((r n_qd + c), j) at ((r n_qd + c) m + j) n_stride + e);
+ *   host t_q [n][n_q][m], t_par [n][k][m], t_M [n][n_qd][n_qd][m].
+ * _vjp: g_q[c] = sum_rs G[r][s] dM[r][s]/dq_c and, while a set is installed, g_par[s] = sum G dM/dp_s, for a cotangent G in M's
+ *   layout: the JVP along the n_q + k identity tangents contracted with G on the device.  g_q or g_par may be NULL, not both.  Device
+ *   g_q [n_q][n_stride], g_par [k][n_stride] fp64 (asynchronous); host g_q [n][n_q], g_par [n][k] (synchronous). */
+int tds_b200_mass_matrix_device(tds_b200_sim* sim, const float* q, double* M, void* stream);
+int tds_b200_mass_matrix_host(tds_b200_sim* sim, const double* q, double* M);
+int tds_b200_mass_matrix_jvp_device(tds_b200_sim* sim, const float* q, int m, const double* t_q, const double* t_par, double* M,
+                                    double* t_M, void* stream);
+int tds_b200_mass_matrix_jvp_host(tds_b200_sim* sim, const double* q, int m, const double* t_q, const double* t_par, double* M,
+                                  double* t_M);
+int tds_b200_mass_matrix_vjp_device(tds_b200_sim* sim, const float* q, const double* G, double* g_q, double* g_par, void* stream);
+int tds_b200_mass_matrix_vjp_host(tds_b200_sim* sim, const double* q, const double* G, double* g_q, double* g_par);
+
 /* Stand-alone integration stages of the fine-grained surface (device SoA arrays as above):
  * integrate_euler (src/dynamics/integrator.hpp:10-133): qd += qdd dt (qdd may be NULL = zero), q += qd dt, floating base
  * quaternion increment + normalisation; integrate_euler_qdd (:141-195): qd += qdd dt only. */

@@ -110,6 +110,18 @@ def lib():
     L.tds_b200_step_jvp_host.argtypes = [vp, ci, ci, dp, dp, dp, ci, dp, dp, dp]
     L.tds_b200_jacobian_chunk.restype = ci
     L.tds_b200_jacobian_chunk.argtypes = [vp]
+    L.tds_b200_mass_matrix_device.restype = ci
+    L.tds_b200_mass_matrix_device.argtypes = [vp, fp, vp, vp]
+    L.tds_b200_mass_matrix_host.restype = ci
+    L.tds_b200_mass_matrix_host.argtypes = [vp, dp, dp]
+    L.tds_b200_mass_matrix_jvp_device.restype = ci
+    L.tds_b200_mass_matrix_jvp_device.argtypes = [vp, fp, ci, vp, vp, vp, vp, vp]
+    L.tds_b200_mass_matrix_jvp_host.restype = ci
+    L.tds_b200_mass_matrix_jvp_host.argtypes = [vp, dp, ci, dp, dp, dp, dp]
+    L.tds_b200_mass_matrix_vjp_device.restype = ci
+    L.tds_b200_mass_matrix_vjp_device.argtypes = [vp, fp, vp, vp, vp, vp]
+    L.tds_b200_mass_matrix_vjp_host.restype = ci
+    L.tds_b200_mass_matrix_vjp_host.argtypes = [vp, dp, dp, dp, dp]
     L.tds_b200_rigid_jvp_device.restype = ci
     L.tds_b200_rigid_jvp_device.argtypes = [vp, vp, vp, ci, ci, vp, vp, vp, vp, vp]
     L.tds_b200_rigid_jvp_host.restype = ci
@@ -206,6 +218,8 @@ DECLARED_SYMBOLS = [
     "tds_b200_param_count", "tds_b200_set_physical_params_device", "tds_b200_set_physical_params_host",
     "tds_b200_step_param_jacobian_device", "tds_b200_step_param_jacobian_host", "tds_b200_step_vjp_params_device",
     "tds_b200_step_vjp_params_host", "tds_b200_step_jvp_device", "tds_b200_step_jvp_host", "tds_b200_jacobian_chunk",
+    "tds_b200_mass_matrix_device", "tds_b200_mass_matrix_host", "tds_b200_mass_matrix_jvp_device", "tds_b200_mass_matrix_jvp_host",
+    "tds_b200_mass_matrix_vjp_device", "tds_b200_mass_matrix_vjp_host",
     "tds_b200_integrate_euler_device", "tds_b200_integrate_euler_qdd_device", "tds_b200_contact_pairs", "tds_b200_model_contact_pairs", "tds_b200_contact_tuples", "tds_b200_model_contact_tuples", "tds_b200_contact_list_device", "tds_b200_contact_list_host", "tds_b200_contact_list_candidates_host",
     "tds_b200_rigid_create", "tds_b200_rigid_destroy", "tds_b200_rigid_set_params", "tds_b200_rigid_step_device", "tds_b200_rigid_step_host", "tds_b200_rigid_jacobian_host",
     "tds_b200_rigid_vjp_device", "tds_b200_rigid_vjp_host", "tds_b200_rigid_jvp_device", "tds_b200_rigid_jvp_host",

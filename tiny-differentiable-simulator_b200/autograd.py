@@ -22,6 +22,10 @@ Both functions also have forward-mode rules (DESIGN.md section 7.10), for torch.
 the tangent of the outputs is the Jacobian-vector product of the same derivative (BatchSim.step_jvp_device, RigidWorld.step_jvp_device),
 run with the parameter values of the same call.  Tangents of q, qd, tau_or_action and of the outputs are float32, those of params
 float64; the PD gains have zero tangent.  rigid_step's forward mode runs the whole rollout in one launch.
+
+mass_matrix(sim, q, params=None) is the joint-space mass matrix M(q) [n_envs, n_qd, n_qd] (float64, DESIGN.md section 7.12) with a
+backward rule (BatchSim.mass_matrix_vjp_device: float32 q.grad, float64 params.grad) and a forward-mode rule
+(BatchSim.mass_matrix_jvp_device).
 """
 import torch
 
@@ -254,3 +258,70 @@ def rigid_step(world, state, force=None, steps=1, params=None):
                                tuple(params.shape) != (world.n_worlds, len(world.param_ids))):
         raise ValueError("params: a float64 CUDA tensor [n_worlds, k] for the k parameters installed by set_physical_params is expected")
     return _RigidStep.apply(world, int(steps), state, force, params)
+
+
+class _MassMatrix(torch.autograd.Function):
+    @staticmethod
+    def forward(sim, q, params):
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        if params is not None:
+            sim.set_physical_params(sim.param_ids, params.detach())
+        qs = _soa(q, ns, torch.float32)
+        M = torch.zeros((max(nd * nd, 1), ns), dtype=torch.float64, device=q.device)
+        _on_side_stream(q.device, lambda st: sim.mass_matrix_device(qs, M, stream=st), (qs, M))
+        return M[:nd * nd, :n].t().reshape(n, nd, nd).contiguous()
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        sim, q, params = inputs
+        qs = _soa(q, sim.n_stride, torch.float32)
+        par = params.detach() if params is not None else None
+        ctx.sim, ctx.has_params = sim, params is not None
+        ctx.save_for_backward(qs, par if par is not None else qs)
+        ctx.jvp_inputs = (qs, par)
+
+    @staticmethod
+    def backward(ctx, g):
+        sim = ctx.sim
+        qs, par = ctx.saved_tensors
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        G = _soa(g.reshape(n, nd * nd), ns, torch.float64)
+        g_q = torch.zeros((max(sim.n_q, 1), ns), dtype=torch.float64, device=g.device)
+        g_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=g.device) if ctx.has_params else None
+        if ctx.has_params:
+            sim.set_physical_params(sim.param_ids, par)   # the values of this call
+        _on_side_stream(g.device, lambda st: sim.mass_matrix_vjp_device(qs, G, g_q, g_par, stream=st), (qs, G, g_q, g_par))
+        gq = g_q[:sim.n_q, :n].t().to(torch.float32)
+        gp = g_par[:, :n].t().contiguous() if ctx.has_params else None
+        return None, gq, gp
+
+    @staticmethod
+    def jvp(ctx, _sim, t_q, t_params):
+        with torch._C._DisableFuncTorch():
+            return _MassMatrix._jvp(ctx, _plain(t_q), _plain(t_params))
+
+    @staticmethod
+    def _jvp(ctx, t_q, t_params):
+        sim = ctx.sim
+        qs, par = (_plain(t) for t in ctx.jvp_inputs)
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        tq = None if t_q is None else _soa(t_q, ns, torch.float64)
+        tp = None if t_params is None or not ctx.has_params else _soa(t_params, ns, torch.float64)
+        t_M = torch.zeros((max(nd * nd, 1), ns), dtype=torch.float64, device=qs.device)
+        if tq is not None or tp is not None:
+            if ctx.has_params:
+                sim.set_physical_params(sim.param_ids, par)   # the values of this call
+            _on_side_stream(qs.device, lambda st: sim.mass_matrix_jvp_device(qs, 1, tq, tp, t_M, stream=st), (qs, tq, tp, t_M))
+        return t_M[:nd * nd, :n].t().reshape(n, nd, nd).contiguous()
+
+
+def mass_matrix(sim, q, params=None):
+    """The joint-space mass matrix M(q) of every environment of `sim` (a BatchSim): [n_envs, n_qd, n_qd] float64, from q [n_envs, n_q]
+    float32 CUDA tensor (fp64 CRBA at the fp32-rounded q).  params: None, or a float64 CUDA tensor [n_envs, k] of values for the
+    parameters installed by sim.set_physical_params (then also differentiated).  Differentiable in reverse and forward mode."""
+    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
+        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
+    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
+                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
+        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    return _MassMatrix.apply(sim, q, params)

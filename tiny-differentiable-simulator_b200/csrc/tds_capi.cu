@@ -49,6 +49,13 @@ extern "C" int tds_launch_stepw_vjp_par(const DevModel* M, const SimParams* P, c
 extern "C" int tds_launch_stepw_jvp(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
                                     const double* t_in, const double* t_par, int m, int mode, int use_pd, int n_dirs, char* gscratch,
                                     cudaStream_t stream);
+// mass matrix M(q), its Jacobian-vector products and the two helper kernels of its vector-Jacobian product (tds_mass.cu)
+extern "C" int tds_launch_mass(const DevModel* M, const StepIO* io, const ParMap* pm, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_mass_jvp(const DevModel* M, const StepIO* io, const ParMap* pm, const double* t_q, const double* t_par, int m,
+                                   int n_dirs, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_mass_eye(double* t_q, double* t_par, int n_q, int k, int d0, int m, int ns, cudaStream_t stream);
+extern "C" int tds_launch_mass_contract(const double* G, const double* dM, int nn, int m, int d0, int n_q, double* g_q, double* g_par, int n,
+                                        int ns, cudaStream_t stream);
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
 // (plane candidates first, then - worlds of several multibodies - the candidates between multibodies, list after list)
@@ -397,6 +404,8 @@ struct tds_b200_sim {
   int* vjp_flag = nullptr;
   double* vjp_g = nullptr; size_t vjp_g_bytes = 0;
   double* jvp_dev = nullptr; size_t jvp_dev_bytes = 0;   // Jacobian-vector product, host path: t_in | t_par | t_out on the device
+  DevModel dm_m;          // layout of the fp64 mass-matrix instance (8-byte scalars)
+  double* mass_dev = nullptr; size_t mass_dev_bytes = 0; // mass matrix: identity tangents | dM of the VJP, host-path staging
   // installed physical parameters (tds_b200_set_physical_params_*): slot map (par.n == 0: none) and values [k][ns] fp64
   ParMap par;
   double* par_dev = nullptr; size_t par_dev_bytes = 0;
@@ -589,6 +598,8 @@ tds_b200_sim* tds_b200_create(const double* model, int n_model, int n_envs, int 
   }
   s->dm_ad = base;
   tds_build_layout_w(&s->dm_ad, 16, 16, 16, -1, 16);
+  s->dm_m = base;
+  tds_build_layout_w(&s->dm_m, 8, 8, 8, -1, 8);
   s->model.assign(model, model + n_model);
   { const char* e = nullptr; tds_build_par_map(&base, 0, nullptr, &s->par, &e); }
   if (const char* kv = getenv("TDS_B200_KERNEL"))
@@ -640,7 +651,7 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->rq); cudaFree(s->rqd); cudaFree(s->zero_act); cudaFree(s->pol_act); cudaFree(s->sticky); cudaFree(s->r_total);
   cudaFree(s->pol_params); cudaFree(s->act_qidx); cudaFree(s->r_steps);
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
-  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->jvp_dev);
+  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->jvp_dev); cudaFree(s->mass_dev);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
   if (s->stage_host) cudaFreeHost(s->stage_host);
   if (s->stream) cudaStreamDestroy(s->stream);
@@ -843,8 +854,9 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
   return 0;
 }
 
-// tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null)
-struct JvpTangents { const double* t_in; const double* t_par; int m; };
+// tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null); mass: of the mass matrix
+// (t_in = the q tangents; the step's arguments are not read)
+struct JvpTangents { const double* t_in; const double* t_par; int m; bool mass = false; };
 
 // Jacobian columns: the step's inputs (params == false) or the installed physical parameters, which are the dual instance's
 // directions dims[1] + s (params == true); or, with jv, the m columns J V of the tangent-seeded instance
@@ -877,7 +889,8 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   for (int d0 = 0; d0 < n_dirs; d0 += chunk) {
     io.jac_dir0 = dir_base + d0;
     const int nd = n_dirs - d0 < chunk ? n_dirs - d0 : chunk;
-    int rc = jv ? tds_launch_stepw_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch,
+    int rc = (jv && jv->mass) ? tds_launch_mass_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
+           : jv ? tds_launch_stepw_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch,
                                        (cudaStream_t)stream)
            : pm ? tds_launch_stepw_jacobian_par(&s->dm_ad, &s->P, &s->E, &io, pm, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream)
                 : tds_launch_stepw_jacobian(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream);
@@ -1045,6 +1058,179 @@ int tds_b200_step_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* 
   const size_t w = (size_t)dims[0] * m;
   for (int e = 0; e < n; ++e)
     for (size_t c = 0; c < w; ++c) t_out[(size_t)e * w + c] = tmp[c * ns + e];
+  return 0;
+}
+
+// ---- joint-space mass matrix M(q) (DESIGN.md section 7.12): the MASS instances of the world-frame kernel (tds_mass.cu) ------------------
+static int grow_dev(double** p, size_t* have, size_t bytes) {
+  if (bytes <= *have) return 0;
+  if (*p) cudaFree(*p);
+  *p = nullptr; *have = 0;
+  CUDA_TRY(cudaMalloc((void**)p, bytes));
+  *have = bytes;
+  return 0;
+}
+
+// M [n_qd * n_qd][ns] from q [n_q][ns] fp32, one lane per environment on the 8-byte layout
+static int mass_run(tds_b200_sim* s, const float* q, double* Mo, cudaStream_t sm) {
+  StepIO io;
+  memset(&io, 0, sizeof(io));
+  io.q_in = q; io.jac = Mo; io.jac_n_in = 1;
+  io.n = s->n; io.n_stride = s->ns;
+  ParMap pmv = s->par;
+  pmv.values = s->par_dev; pmv.grad = nullptr;
+  const size_t need = (size_t)(s->n + 31) / 32 * (size_t)s->dm_m.x_total * 32 * 4;
+  if (need > s->jac_scratch_bytes) {
+    if (s->jac_scratch) cudaFree(s->jac_scratch);
+    s->jac_scratch = nullptr; s->jac_scratch_bytes = 0;
+    CUDA_TRY(cudaMalloc((void**)&s->jac_scratch, need));
+    s->jac_scratch_bytes = need;
+  }
+  const int rc = tds_launch_mass(&s->dm_m, &io, s->par.n > 0 ? &pmv : nullptr, s->jac_scratch, sm);
+  if (rc) set_err(std::string("mass matrix launch: ") + cudaGetErrorString((cudaError_t)rc));
+  return rc;
+}
+
+static int mass_jvp_run(tds_b200_sim* s, const float* q, int m, const double* t_q, const double* t_par, double* Mo, double* t_M,
+                        cudaStream_t sm) {
+  if (Mo) { if (int rc = mass_run(s, q, Mo, sm)) return rc; }
+  JvpTangents jv{t_q, t_par, m};
+  jv.mass = true;
+  return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, nullptr, nullptr, t_M, sm, false, &jv);
+}
+
+// g = G : dM along the n_q + k identity tangents, in chunks of directions whose dM stays within 1 GB
+static int mass_vjp_run(tds_b200_sim* s, const float* q, const double* G, double* g_q, double* g_par, cudaStream_t sm) {
+  const int n_q = s->dm[0].n_q, nn = s->dm[0].n_qd * s->dm[0].n_qd, k = s->par.n, ns = s->ns;
+  const int total = n_q + k;
+  const size_t per_dir = sizeof(double) * (size_t)(nn + total) * ns;   // dM + identity tangents of one direction
+  int chunk = (int)(((size_t)1 << 30) / per_dir);
+  if (chunk < 1) chunk = 1;
+  if (chunk > total) chunk = total;
+  if (int rc = grow_dev(&s->mass_dev, &s->mass_dev_bytes, per_dir * chunk)) return rc;
+  for (int d0 = 0; d0 < total; d0 += chunk) {
+    const int nd = total - d0 < chunk ? total - d0 : chunk;
+    double* tq = s->mass_dev;
+    double* tp = k > 0 ? tq + (size_t)n_q * nd * ns : nullptr;
+    double* dM = tq + (size_t)total * nd * ns;
+    int rc = tds_launch_mass_eye(tq, tp, n_q, k, d0, nd, ns, sm);
+    if (!rc) rc = mass_jvp_run(s, q, nd, tq, tp, nullptr, dM, sm);
+    if (!rc) rc = tds_launch_mass_contract(G, dM, nn, nd, d0, n_q, g_q, g_par, s->n, ns, sm);
+    if (rc) { set_err(std::string("mass matrix vjp: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
+  }
+  return 0;
+}
+
+// q [n][n_q] fp64 host -> s->q [n_q][ns] fp32 on the simulator's stream
+static int mass_upload_q(tds_b200_sim* s, const double* q) {
+  const int n = s->n, n_q = s->dm[0].n_q;
+  if (int rc = ensure_stage(s, sizeof(double) * n * (n_q + 1), 0)) return rc;
+  if (n_q == 0) return 0;
+  CUDA_TRY(cudaMemcpyAsync(s->stage_dev, q, sizeof(double) * n * n_q, cudaMemcpyHostToDevice, s->stream));
+  aos_to_soa_kernel<double><<<(n + 127) / 128, 128, 0, s->stream>>>((double*)s->stage_dev, n_q, 0, s->q, n_q, n, s->ns);
+  return 0;
+}
+
+// device [rows][ns] -> host [n][rows]
+static int mass_download(tds_b200_sim* s, const double* src, size_t rows, double* dst) {
+  std::vector<double> tmp(rows * s->ns);
+  CUDA_TRY(cudaMemcpyAsync(tmp.data(), src, sizeof(double) * rows * s->ns, cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  CUDA_TRY(cudaGetLastError());
+  for (int e = 0; e < s->n; ++e)
+    for (size_t r = 0; r < rows; ++r) dst[(size_t)e * rows + r] = tmp[r * s->ns + e];
+  return 0;
+}
+
+int tds_b200_mass_matrix_device(tds_b200_sim* s, const float* q, double* M, void* stream) {
+  if (!s || !q || !M) return -1;
+  return mass_run(s, q, M, (cudaStream_t)stream);
+}
+
+int tds_b200_mass_matrix_host(tds_b200_sim* s, const double* q, double* M) {
+  if (!s || !q || !M) return -1;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
+  int rc = mass_upload_q(s, q);
+  if (!rc) rc = grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * nn * s->ns);
+  if (!rc) rc = mass_run(s, s->q, s->jac_dev, s->stream);
+  if (!rc) rc = mass_download(s, s->jac_dev, nn, M);
+  return rc;
+}
+
+static int mass_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_par, const void* t_M) {
+  if (!s || !q || !t_M || m < 1 || (!t_q && !t_par)) return -1;
+  if (t_par && s->par.n == 0) { set_err("mass matrix jvp: parameter tangents without installed physical parameters"); return -4; }
+  return 0;
+}
+
+int tds_b200_mass_matrix_jvp_device(tds_b200_sim* s, const float* q, int m, const double* t_q, const double* t_par, double* M,
+                                    double* t_M, void* stream) {
+  if (int rc = mass_jvp_check(s, q, m, t_q, t_par, t_M)) return rc;
+  return mass_jvp_run(s, q, m, t_q, t_par, M, t_M, (cudaStream_t)stream);
+}
+
+int tds_b200_mass_matrix_jvp_host(tds_b200_sim* s, const double* q, int m, const double* t_q, const double* t_par, double* M,
+                                  double* t_M) {
+  if (int rc = mass_jvp_check(s, q, m, t_q, t_par, t_M)) return rc;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, k = s->par.n;
+  const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
+  const size_t tq = (size_t)n_q * m * ns, tp = (size_t)(t_par ? k : 0) * m * ns, to = nn * m * ns;
+  int rc = mass_upload_q(s, q);
+  if (!rc) rc = grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (tq + tp + to + nn * ns));
+  if (rc) return rc;
+  double* tq_d = t_q ? s->jvp_dev : nullptr;
+  double* tp_d = t_par ? s->jvp_dev + tq : nullptr;
+  double* to_d = s->jvp_dev + tq + tp;
+  double* M_d = M ? to_d + to : nullptr;
+  // tangents: host [n][dim][m] -> device [dim * m][ns]
+  auto up_t = [&](const double* src, int dim, double* dst) -> int {
+    const size_t w = (size_t)dim * m;
+    std::vector<double> tmp(w * ns, 0.0);
+    for (int e = 0; e < n; ++e) for (size_t c = 0; c < w; ++c) tmp[c * ns + e] = src[(size_t)e * w + c];
+    CUDA_TRY(cudaMemcpyAsync(dst, tmp.data(), sizeof(double) * w * ns, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));   // (tmp is released)
+    return 0;
+  };
+  if (t_q && n_q && (rc = up_t(t_q, n_q, tq_d))) return rc;
+  if (t_par && (rc = up_t(t_par, k, tp_d))) return rc;
+  if ((rc = mass_jvp_run(s, s->q, m, tq_d, tp_d, M_d, to_d, s->stream))) return rc;
+  if ((rc = mass_download(s, to_d, nn * m, t_M))) return rc;
+  return M ? mass_download(s, M_d, nn, M) : 0;
+}
+
+static int mass_vjp_check(tds_b200_sim* s, const void* q, const void* G, const void* g_q, const void* g_par) {
+  if (!s || !q || !G || (!g_q && !g_par)) return -1;
+  if (g_par && s->par.n == 0) { set_err("mass matrix vjp: parameter cotangents without installed physical parameters"); return -4; }
+  return 0;
+}
+
+int tds_b200_mass_matrix_vjp_device(tds_b200_sim* s, const float* q, const double* G, double* g_q, double* g_par, void* stream) {
+  if (int rc = mass_vjp_check(s, q, G, g_q, g_par)) return rc;
+  return mass_vjp_run(s, q, G, g_q, g_par, (cudaStream_t)stream);
+}
+
+int tds_b200_mass_matrix_vjp_host(tds_b200_sim* s, const double* q, const double* G, double* g_q, double* g_par) {
+  if (int rc = mass_vjp_check(s, q, G, g_q, g_par)) return rc;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, k = s->par.n;
+  const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
+  int rc = mass_upload_q(s, q);
+  if (!rc) rc = grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (nn + n_q + k + 1) * ns);
+  if (rc) return rc;
+  double* G_d = s->vjp_g;
+  double* gq_d = G_d + nn * ns;
+  double* gp_d = gq_d + (size_t)n_q * ns;
+  {
+    std::vector<double> tmp(nn * ns, 0.0);
+    for (int e = 0; e < n; ++e) for (size_t r = 0; r < nn; ++r) tmp[r * ns + e] = G[(size_t)e * nn + r];
+    CUDA_TRY(cudaMemcpyAsync(G_d, tmp.data(), sizeof(double) * nn * ns, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));
+  }
+  if ((rc = mass_vjp_run(s, s->q, G_d, g_q ? gq_d : nullptr, g_par ? gp_d : nullptr, s->stream))) return rc;
+  if (g_q && n_q && (rc = mass_download(s, gq_d, n_q, g_q))) return rc;
+  if (g_par && (rc = mass_download(s, gp_d, k, g_par))) return rc;
   return 0;
 }
 

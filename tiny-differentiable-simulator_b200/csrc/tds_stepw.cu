@@ -61,7 +61,12 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // JV (dual instances only): Jacobian-vector product.  The lane's direction is tangent j = blockIdx.y + io.jac_dir0 of pm.jv; every
 // input and installed parameter is seeded with its entry of that tangent, and the dual parts of the outputs are column j of io.jac
 // (io.jac_n_in = m columns): t_out = J V, row-major per environment as the Jacobian.
-template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false>
+// MASS: the joint-space mass matrix M(q) (DESIGN.md section 7.12), launched in MODE_NOCONTACT.  Pass 1 from q alone (qd = 0, no PD, tau or
+// contact detection: mass_matrix.hpp:36),
+// the CRBA of pass 2 and the floating-base block as if a contact were active, then the dense symmetric n_qd x n_qd matrix in place of
+// the solve: entry (r, c) at io.jac[(r * n_qd + c) * ns + e] (fp64 instance), or its dual part as column j of an m-column Jacobian,
+// io.jac[((r * n_qd + c) * m + j) * ns + e] (JV instance, t_in = the q tangents).  ABA, integration and reward are not compiled in.
+template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
@@ -160,9 +165,9 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // input directions of the differentiable instance: q | qd | tau or action | kp, kd, max_force (with PD)
   const int in0 = M.n_q + n;
   for (int k = 0; k < M.n_q; ++k) qv[k * ST] = seed(RQ(io.q_in[(size_t)k * ns + e]), k);
-  for (int k = 0; k < n; ++k) qdv[k * ST] = seed(RQ(io.qd_in[(size_t)k * ns + e]), M.n_q + k);
+  for (int k = 0; k < n; ++k) qdv[k * ST] = MASS ? RQ(0.f) : seed(RQ(io.qd_in[(size_t)k * ns + e]), M.n_q + k);
   for (int k = 0; k < n; ++k) tauv[k * ST] = RQ(0.f);
-  if (use_pd) {
+  if (!MASS && use_pd) {
     const RQ kp = seed(RQ(E.kp), in0 + E.n_act), kd = seed(RQ(E.kd), in0 + E.n_act + 1), fmax_ = seed(RQ(E.max_force), in0 + E.n_act + 2);
     for (int k = 0; k < E.n_act; ++k) {
       const int li = E.act_link[k];
@@ -173,7 +178,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       f = min_t(max_t(f, -fmax_), fmax_);
       tauv[M.qd_idx[li] * ST] = f;
     }
-  } else if (io.tau_in) {
+  } else if (!MASS && io.tau_in) {
     const int off = M.floating ? 6 : 0;
     for (int k = off; k < n; ++k) tauv[k * ST] = seed(RQ(io.tau_in[(size_t)(k - off) * ns + e]), in0 + k - off);
   }
@@ -451,7 +456,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       pgc[g] = cnt;
     }
   }
-  const bool any_contact = __any_sync(0xffffffffu, n_active > 0 || n_pair_active > 0);
+  const bool any_contact = MASS || __any_sync(0xffffffffu, n_active > 0 || n_pair_active > 0);   // MASS: the CRBA always runs
   TDSW_PHASE();  // 2
 
   // ---- pass 2: leaf -> root.  ABA (forward_dynamics.hpp:50-216) + CRBA (mass_matrix.hpp:39-125) ----------
@@ -495,11 +500,13 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     const Sv<RA> v = ld6<RA>(vrec, ST);
     Abi<RA> Ia = abi_from_rbi(rb);
     Sv<RA> pA = cross_mf(v, rbi_mul(rb, v));                 // kinematics.hpp:132
-    if (fl & TDS_LF_CHILD_ADJ) { abi_add(Ia, cA); pA = pA + cP; rbi_add(Ic, cC); }
+    if (fl & TDS_LF_CHILD_ADJ) { if constexpr (!MASS) { abi_add(Ia, cA); pA = pA + cP; } rbi_add(Ic, cC); }
     if (M.acc_slot[i] >= 0) {
-      Abi<RA> sa; Sv<RA> sp;
-      acc_ld27<RA>(A.ptr<RA>(M.x_acc + M.acc_slot[i] * M.x_acc_words), ST, sa, sp);
-      abi_add(Ia, sa); pA = pA + sp;
+      if constexpr (!MASS) {
+        Abi<RA> sa; Sv<RA> sp;
+        acc_ld27<RA>(A.ptr<RA>(M.x_acc + M.acc_slot[i] * M.x_acc_words), ST, sa, sp);
+        abi_add(Ia, sa); pA = pA + sp;
+      }
       rbi_add(Ic, ld_rbi<RC>(A.ptr<RC>(M.x_acc + M.acc_slot[i] * M.x_acc_words + M.x_acc_ic_word), ST));
     }
     Sv<RA> pa = pA;
@@ -507,7 +514,14 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     // every lane must have finished reading its RC record before any lane writes the RA view.
     __syncwarp();
     RA* const urec = A.ptr<RA>(M.x_link + i * LWD);
-    if (fl & TDS_LF_FIXED) {
+    if constexpr (MASS) {   // the CRBA columns of the two branches below (mass_matrix.hpp:58-111), without the ABA
+      const int d0 = M.qd_idx[i];
+      for (int a = 0; a < n_cols(i); ++a) {
+        const Sv<RC> F = rbi_mul(Ic, S_col(i, a));
+        for (int b = 0; b <= a; ++b) Mset(d0 + a, d0 + b, RS(dot(S_col(i, b), F)));
+        crba_ancestors(i, d0 + a, F);
+      }
+    } else if (fl & TDS_LF_FIXED) {
       Sv<RA> z; z.top = v3<RA>(RA(0), RA(0), RA(0)); z.bot = z.top;
       st6<RA>(vrec, ST, z);
       st6<RA>(urec, ST, z);
@@ -619,7 +633,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     else {
       const int slot = (p >= 0) ? M.acc_slot[p] : M.base_acc;
       if (slot >= 0) {
-        acc_add27<RA>(A.ptr<RA>(M.x_acc + slot * M.x_acc_words), ST, Ia, pa);
+        if constexpr (!MASS) acc_add27<RA>(A.ptr<RA>(M.x_acc + slot * M.x_acc_words), ST, Ia, pa);
         rbi_acc<RC>(A.ptr<RC>(M.x_acc + slot * M.x_acc_words + M.x_acc_ic_word), ST, Ic);
       }
     }
@@ -666,7 +680,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     }
     const M3<RA> Rt = cvt<RA>(transpose(Rb));
     Abi<RA> Ab;
-    {
+    if constexpr (!MASS) {
       Rbi<RA> rbb = base_par ? cvt_rbi<RA>(bp) : model_rbi_of<RA>(M.base_rbi);
       Ab = abi_from_rbi(rbb);
       Abi<RA> Arot;
@@ -674,7 +688,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       abi_add(Ab, Arot);
     }
     Sv<RA> pb;
-    {
+    if constexpr (!MASS) {
       // gyroscopic bias, kinematics.hpp:54-61 (reference mixes frames here; reproduced as written)
       const M3<RA> RbA = cvt<RA>(Rb);
       M3<RA> Ic0;
@@ -707,7 +721,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       b11[0] = RS(Ib.m); b11[3 * ST] = z; b11[4 * ST] = RS(Ib.m); b11[6 * ST] = z; b11[7 * ST] = z; b11[8 * ST] = RS(Ib.m);
     }
     // -base_abi.inv_mul(bias) with the reference's block inverse (C = -H), inertia.hpp:302-328
-    {
+    if constexpr (!MASS) {
       M3<RC> I3, H3, M3m;
       I3.xx = Ab.I.xx; I3.xy = Ab.I.xy; I3.xz = Ab.I.xz; I3.yx = Ab.I.xy; I3.yy = Ab.I.yy; I3.yz = Ab.I.yz; I3.zx = Ab.I.xz; I3.zy = Ab.I.yz; I3.zz = Ab.I.zz;
       H3 = cvt<RC>(Ab.H);
@@ -741,6 +755,21 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   } else {
     a_prev.top = v3<RA>(RA(0), RA(0), RA(0));
     a_prev.bot = v3<RA>(RA(-P.gravity[0]), RA(-P.gravity[1]), RA(-P.gravity[2]));
+  }
+  if constexpr (MASS) {   // dense symmetric M from the blocked lower triangle (the padding dofs are not written)
+    if (live && io.jac) {
+      auto put = [&](int k, RS x) {
+        if constexpr (AD) io.jac[((size_t)k * io.jac_n_in + jcol) * ns + e] = x.d;
+        else io.jac[(size_t)k * ns + e] = x;
+      };
+      for (int r = 0; r < n; ++r)
+        for (int c = 0; c <= r; ++c) {
+          const RS x = Mb[(btri(r / 3, c / 3) + (r % 3) * 3 + (c % 3)) * ST];
+          put(r * n + c, x);
+          if (c < r) put(c * n + r, x);
+        }
+    }
+    return;
   }
   const Sv<RA> a_base = a_prev;
   const RA dtA = RA(P.dt);

@@ -4,6 +4,7 @@
     TinyMultiBody (.q .qd .qdd .tau, is_floating, num_dofs, clear_forces)     :611-655
     TinyUrdfParser.load_urdf, UrdfToMultiBody2.convert2                       :1013-1034
     forward_dynamics(mb, gravity), integrate_euler(mb, dt), integrate_euler_qdd(mb, dt)   :659-663
+    mass_matrix(mb[, q])                                                      :659-663 (mass_matrix.hpp)
     VectorizedLaikagoEnv, VectorizedAntEnv (pytinydiffsim_includes.h:58-227), CartpoleEnv (:1123)
 
 The fine-grained calls operate on one MultiBody like the reference's; each is one stage of the GPU path (forward dynamics =
@@ -157,6 +158,15 @@ def integrate_euler(mb, dt):
 
 def integrate_euler_qdd(mb, dt):
     mb._integrate(dt, False)
+
+
+def mass_matrix(mb, q=None):
+    """The joint-space mass matrix M(q) of the multibody: a NumPy float64 [num_dofs, num_dofs] array (qd-dimension, both triangles),
+    by the CRBA of the GPU step in fp64 at the fp32-rounded q.  The reference's C++ call mass_matrix(mb, &M) reads the multibody's
+    own q (mass_matrix.hpp:36, forward kinematics with an empty qd); its binding is served here in both forms: mass_matrix(mb) at
+    mb.q, and mass_matrix(mb, q) at a q given explicitly (mb.q is left as it is)."""
+    qv = np.asarray(mb.q if q is None else q, dtype=np.float64).reshape(1, -1)
+    return mb._sim.mass_matrix_host(qv)[0]
 
 
 # ---- rigid bodies (python/pytinydiffsim.inl:336-385, 448-455; examples/billiard_optimization.py) --------------------------------

@@ -299,6 +299,78 @@ class BatchSim:
         self._check(self._L.tds_b200_step_jvp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), int(m), _ptr(t_in),
                                                      _ptr(t_par), _ptr(t_out), st), "step_jvp_device")
 
+    # ---- joint-space mass matrix M(q) (DESIGN.md section 7.12) ----
+    def mass_matrix_host(self, q):
+        """M(q) of every environment: [n, n_qd, n_qd] float64, symmetric, by the CRBA of the world-frame step in fp64 at the
+        fp32-rounded q [n, n_q] (qd plays no part).  Installed physical parameters give each environment its own masses, centres of
+        mass and inertias.  A world of several multibodies gives the block-diagonal matrix."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        assert q.shape == (self.n_envs, self.n_q), q.shape
+        M = np.zeros((self.n_envs, self.n_qd, self.n_qd))
+        self._check(self._L.tds_b200_mass_matrix_host(self._h, _dp(q), _dp(M)), "mass_matrix_host")
+        return M
+
+    def mass_matrix_device(self, q, M, stream=None):
+        """Device version of mass_matrix_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride] as for step_device, M float64
+        CUDA tensor [n_qd * n_qd, n_stride], entry (r, c) at row r * n_qd + c.  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_mass_matrix_device(self._h, _ptr(q), _ptr(M), st), "mass_matrix_device")
+
+    def mass_matrix_jvp_host(self, q, t_q, t_par=None):
+        """Directional derivatives of M: dM [n, n_qd, n_qd, m] = sum_c dM/dq_c t_q[c] + sum_s dM/dp_s t_par[s] for the m tangents
+        t_q [n, n_q, m] of q and t_par [n, k, m] of the installed parameters (either may be None); a tangent given as [n, n_q] (or
+        [n, k]) is m = 1 and the result is then [n, n_qd, n_qd].  Returns (M, dM)."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        k = len(self.param_ids)
+        lead = t_q if t_q is not None else t_par
+        single = lead is not None and np.ndim(lead) == 2
+
+        def prep(x, dim):
+            if x is None:
+                return None
+            x = np.asarray(x, dtype=np.float64)
+            if x.ndim == 2:
+                x = x[:, :, None]
+            if x.shape[:2] != (self.n_envs, dim):
+                raise ValueError(f"tangent: [n_envs, {dim}, m] or [n_envs, {dim}] expected, got {x.shape}")
+            return np.ascontiguousarray(x)
+        tq, tp = prep(t_q, self.n_q), prep(t_par, k)
+        if tq is not None and tp is not None and tq.shape[2] != tp.shape[2]:
+            raise ValueError("t_q and t_par: the same number of tangents m expected")
+        m = (tq if tq is not None else tp).shape[2] if lead is not None else 0
+        M = np.zeros((self.n_envs, self.n_qd, self.n_qd))
+        dM = np.zeros((self.n_envs, self.n_qd, self.n_qd, max(m, 1)))
+        self._check(self._L.tds_b200_mass_matrix_jvp_host(self._h, _dp(q), m, _dp(tq), _dp(tp), _dp(M), _dp(dM)), "mass_matrix_jvp_host")
+        return M, (dM[..., 0] if single else dM)
+
+    def mass_matrix_jvp_device(self, q, m, t_q, t_par, t_M, M=None, stream=None):
+        """Device version of mass_matrix_jvp_host: q float32 [n_q, n_stride]; t_q [n_q * m, n_stride], t_par [k * m, n_stride] (either
+        may be None), t_M [n_qd * n_qd * m, n_stride] and M [n_qd * n_qd, n_stride] (or None) float64 CUDA tensors, entry (c, j) at row
+        c * m + j.  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_mass_matrix_jvp_device(self._h, _ptr(q), int(m), _ptr(t_q), _ptr(t_par), _ptr(M), _ptr(t_M), st),
+                    "mass_matrix_jvp_device")
+
+    def mass_matrix_vjp_host(self, q, G):
+        """Cotangent G [n, n_qd, n_qd] of M -> (g_q [n, n_q], g_par [n, k] or None without installed parameters): g = sum G * dM/dx."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        G = np.ascontiguousarray(G, dtype=np.float64)
+        assert G.shape == (self.n_envs, self.n_qd, self.n_qd), G.shape
+        k = len(self.param_ids)
+        g_q = np.zeros((self.n_envs, self.n_q))
+        g_par = np.zeros((self.n_envs, k)) if k else None
+        self._check(self._L.tds_b200_mass_matrix_vjp_host(self._h, _dp(q), _dp(G), _dp(g_q), _dp(g_par)), "mass_matrix_vjp_host")
+        return g_q, g_par
+
+    def mass_matrix_vjp_device(self, q, G, g_q, g_par=None, stream=None):
+        """Device version of mass_matrix_vjp_host: q float32 [n_q, n_stride], G float64 [n_qd * n_qd, n_stride] in M's layout, g_q
+        [n_q, n_stride] and g_par [k, n_stride] float64 CUDA tensors (either may be None, not both).  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_mass_matrix_vjp_device(self._h, _ptr(q), _ptr(G), _ptr(g_q), _ptr(g_par), st), "mass_matrix_vjp_device")
+
     def jacobian_chunk(self):
         """Directions (Jacobian columns or JVP tangents) one launch of the dual-number step takes; more run in several launches."""
         return self._L.tds_b200_jacobian_chunk(self._h)
