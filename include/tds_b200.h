@@ -219,6 +219,40 @@ int tds_b200_mass_matrix_jvp_host(tds_b200_sim* sim, const double* q, int m, con
 int tds_b200_mass_matrix_vjp_device(tds_b200_sim* sim, const float* q, const double* G, double* g_q, double* g_par, void* stream);
 int tds_b200_mass_matrix_vjp_host(tds_b200_sim* sim, const double* q, const double* G, double* g_q, double* g_par);
 
+/* ---- forward kinematics and linear point Jacobians (DESIGN.md 7.13; forward_kinematics_q, point_jacobian: jacobian.hpp:13-83) ------
+ * From q alone (rounded to fp32; qd plays no part) and a point table of K points (0 <= K <= TDS_B200_MAX_KIN_POINTS), the same for all
+ * environments and passed with each call in host memory: point k sits on link links[k] (-1: the base) at local[3k .. 3k+2] in that
+ * link's frame.  Outputs, fp64, world coordinates, each may be NULL but not all three:
+ *   xf: every link's world transform, 12 per link (R row-major, then the position: the layout of tds_b200_step's link transforms);
+ *   x:  every point's world position;
+ *   J:  every point's 3 x n_qd linear Jacobian, the reference's convention: a floating base gives the columns [-[x - r0]x^T | I3]
+ *       with the base's rotation ignored; fixed links have no columns; a spherical joint has 3; in a world of several multibodies a
+ *       point has entries in its own multibody's dofs only.
+ * Installed physical parameters do not enter kinematics.  Argument checks -> -1: NULL q; K out of range, a link index out of range,
+ * or NULL links / local with K > 0; no output (no cotangent); m < 1 or NULL t_q; NULL g_q.
+ *   device: q [n_q][n_stride] fp32 as tds_b200_step_device; xf [n_links * 12][n_stride], x [3K][n_stride], J [3K * n_qd][n_stride] fp64
+ *           with entry (point k, row r, column c) of J at row (3k + r) * n_qd + c.  Asynchronous on `stream`.
+ *   host:   q [n][n_q] fp64; xf [n][n_links][12], x [n][K][3], J [n][K][3][n_qd].  Synchronous.
+ * _jvp: the directional derivatives along m tangents t_q of q, one lane per (environment, tangent) of the dual-number instance, in
+ *   chunks as tds_b200_step_jvp_*.  Device t_q [n_q * m][n_stride] and t_xf / t_x / t_J [rows * m][n_stride] (entry (r, j) at
+ *   (r * m + j) * n_stride + e); host t_q [n][n_q][m], t_xf [n][n_links * 12][m], t_x [n][3K][m], t_J [n][3K * n_qd][m].
+ * _vjp: g_q[c] = <G_xf, dxf/dq_c> + <G_x, dx/dq_c> + <G_J, dJ/dq_c> for cotangents in the outputs' layouts (a NULL one is zero): the
+ *   JVP along the n_q identity tangents contracted with the cotangent on the device.  Device g_q [n_q][n_stride] fp64 (asynchronous);
+ *   host g_q [n][n_q] (synchronous). */
+#define TDS_B200_MAX_KIN_POINTS 64
+int tds_b200_kinematics_device(tds_b200_sim* sim, const float* q, int K, const int* links, const double* local, double* xf, double* x,
+                               double* J, void* stream);
+int tds_b200_kinematics_host(tds_b200_sim* sim, const double* q, int K, const int* links, const double* local, double* xf, double* x,
+                             double* J);
+int tds_b200_kinematics_jvp_device(tds_b200_sim* sim, const float* q, int K, const int* links, const double* local, int m,
+                                   const double* t_q, double* t_xf, double* t_x, double* t_J, void* stream);
+int tds_b200_kinematics_jvp_host(tds_b200_sim* sim, const double* q, int K, const int* links, const double* local, int m,
+                                 const double* t_q, double* t_xf, double* t_x, double* t_J);
+int tds_b200_kinematics_vjp_device(tds_b200_sim* sim, const float* q, int K, const int* links, const double* local, const double* G_xf,
+                                   const double* G_x, const double* G_J, double* g_q, void* stream);
+int tds_b200_kinematics_vjp_host(tds_b200_sim* sim, const double* q, int K, const int* links, const double* local, const double* G_xf,
+                                 const double* G_x, const double* G_J, double* g_q);
+
 /* Stand-alone integration stages of the fine-grained surface (device SoA arrays as above):
  * integrate_euler (src/dynamics/integrator.hpp:10-133): qd += qdd dt (qdd may be NULL = zero), q += qd dt, floating base
  * quaternion increment + normalisation; integrate_euler_qdd (:141-195): qd += qdd dt only. */

@@ -26,6 +26,10 @@ float64; the PD gains have zero tangent.  rigid_step's forward mode runs the who
 mass_matrix(sim, q, params=None) is the joint-space mass matrix M(q) [n_envs, n_qd, n_qd] (float64, DESIGN.md section 7.12) with a
 backward rule (BatchSim.mass_matrix_vjp_device: float32 q.grad, float64 params.grad) and a forward-mode rule
 (BatchSim.mass_matrix_jvp_device).
+
+forward_kinematics(sim, q, links, local) is every link's world transform and every point's world position and linear Jacobian (float64,
+DESIGN.md section 7.13) with a backward rule (BatchSim.kinematics_vjp_device: float32 q.grad) and a forward-mode rule
+(BatchSim.kinematics_jvp_device).
 """
 import torch
 
@@ -325,3 +329,83 @@ def mass_matrix(sim, q, params=None):
                                tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
         raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
     return _MassMatrix.apply(sim, q, params)
+
+
+def _kin_outputs(sim, K, xf, x, J):
+    """Device outputs [rows, n_stride] of the kinematics entries -> (R [n, n_links, 3, 3], p [n, n_links, 3], x [n, K, 3],
+    J [n, K, 3, n_qd])."""
+    n, nl, nd = sim.n_envs, sim.n_links, sim.n_qd
+    xf = xf[:nl * 12, :n].t().reshape(n, nl, 12)
+    return (xf[..., :9].reshape(n, nl, 3, 3).contiguous(), xf[..., 9:].contiguous(), x[:3 * K, :n].t().reshape(n, K, 3).contiguous(),
+            J[:3 * K * nd, :n].t().reshape(n, K, 3, nd).contiguous())
+
+
+def _kin_buffers(sim, K, device):
+    ns, nl, nd = sim.n_stride, sim.n_links, sim.n_qd
+    z = dict(dtype=torch.float64, device=device)
+    return torch.zeros((max(nl * 12, 1), ns), **z), torch.zeros((max(3 * K, 1), ns), **z), torch.zeros((max(3 * K * nd, 1), ns), **z)
+
+
+class _ForwardKinematics(torch.autograd.Function):
+    @staticmethod
+    def forward(sim, q, links, local):
+        lk, lc, K = sim._points(links, local)
+        qs = _soa(q, sim.n_stride, torch.float32)
+        xf, x, J = _kin_buffers(sim, K, q.device)
+        xo, Jo = (x, J) if K else (None, None)
+        _on_side_stream(q.device, lambda st: sim.kinematics_device(qs, lk, lc, xf, xo, Jo, stream=st), (qs, xf, x, J))
+        return _kin_outputs(sim, K, xf, x, J)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        sim, q, links, local = inputs
+        lk, lc, K = sim._points(links, local)
+        qs = _soa(q, sim.n_stride, torch.float32)
+        ctx.sim, ctx.points = sim, (lk, lc, K)
+        ctx.save_for_backward(qs)
+        ctx.jvp_q = qs
+
+    @staticmethod
+    def backward(ctx, gR, gp, gx, gJ):
+        sim = ctx.sim
+        (qs,) = ctx.saved_tensors
+        lk, lc, K = ctx.points
+        n, ns, nl, nd = sim.n_envs, sim.n_stride, sim.n_links, sim.n_qd
+        dev = qs.device
+
+        def zero_if_none(g, shape):
+            return torch.zeros(shape, dtype=torch.float64, device=dev) if g is None else g.to(torch.float64)
+        gxf = torch.cat([zero_if_none(gR, (n, nl, 3, 3)).reshape(n, nl, 9), zero_if_none(gp, (n, nl, 3))], dim=2).reshape(n, nl * 12)
+        G_xf = _soa(gxf, ns, torch.float64)
+        G_x = _soa(zero_if_none(gx, (n, K, 3)).reshape(n, 3 * K), ns, torch.float64) if K else None
+        G_J = _soa(zero_if_none(gJ, (n, K, 3, nd)).reshape(n, 3 * K * nd), ns, torch.float64) if K and nd else None
+        g_q = torch.zeros((max(sim.n_q, 1), ns), dtype=torch.float64, device=dev)
+        _on_side_stream(dev, lambda st: sim.kinematics_vjp_device(qs, lk, lc, G_xf, G_x, G_J, g_q, stream=st), (qs, G_xf, G_x, G_J, g_q))
+        return None, g_q[:sim.n_q, :n].t().to(torch.float32), None, None
+
+    @staticmethod
+    def jvp(ctx, _sim, t_q, _links, _local):
+        with torch._C._DisableFuncTorch():
+            return _ForwardKinematics._jvp(ctx, _plain(t_q))
+
+    @staticmethod
+    def _jvp(ctx, t_q):
+        sim = ctx.sim
+        qs = _plain(ctx.jvp_q)
+        lk, lc, K = ctx.points
+        t_xf, t_x, t_J = _kin_buffers(sim, K, qs.device)
+        if t_q is not None:
+            tq = _soa(t_q, sim.n_stride, torch.float64)
+            xo, Jo = (t_x, t_J) if K else (None, None)
+            _on_side_stream(qs.device, lambda st: sim.kinematics_jvp_device(qs, lk, lc, 1, tq, t_xf, xo, Jo, stream=st), (qs, tq, t_xf, t_x, t_J))
+        return _kin_outputs(sim, K, t_xf, t_x, t_J)
+
+
+def forward_kinematics(sim, q, links, local):
+    """Forward kinematics and linear point Jacobians of every environment of `sim` (a BatchSim) at q [n_envs, n_q] float32 CUDA tensor
+    (fp64 at the fp32-rounded q), for the point table links [K] (-1: the base) / local [K, 3] (coordinates in the link's frame; both
+    constants of the call): (R [n_envs, n_links, 3, 3], p [n_envs, n_links, 3], x [n_envs, K, 3], J [n_envs, K, 3, n_qd]), float64 world
+    coordinates.  Differentiable along q in reverse mode (float32 q.grad from the cotangents of all four outputs) and forward mode."""
+    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
+        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
+    return _ForwardKinematics.apply(sim, q, links, local)

@@ -56,6 +56,11 @@ extern "C" int tds_launch_mass_jvp(const DevModel* M, const StepIO* io, const Pa
 extern "C" int tds_launch_mass_eye(double* t_q, double* t_par, int n_q, int k, int d0, int m, int ns, cudaStream_t stream);
 extern "C" int tds_launch_mass_contract(const double* G, const double* dM, int nn, int m, int d0, int n_q, double* g_q, double* g_par, int n,
                                         int ns, cudaStream_t stream);
+// forward kinematics and point Jacobians, and their Jacobian-vector products (tds_kin.cu)
+extern "C" int tds_launch_kin(const DevModel* M, const StepIO* io, const TdsKinCall* kc, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_kin_jvp(const DevModel* M, const StepIO* io, const TdsKinCall* kc, const double* t_q, int m, int n_dirs,
+                                  char* gscratch, cudaStream_t stream);
+static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
 // (plane candidates first, then - worlds of several multibodies - the candidates between multibodies, list after list)
@@ -761,6 +766,8 @@ static int set_physical_params(tds_b200_sim* s, int k, const int* ids, const dou
     // steps run on non-blocking streams, which a plain cudaMemcpy does not wait for
     CUDA_TRY(cudaDeviceSynchronize());
     CUDA_TRY(cudaMemcpy(s->par_dev, tmp.data(), bytes, cudaMemcpyHostToDevice));
+    // a copy from pageable memory may return before its DMA has landed, and the non-blocking streams do not wait for it either
+    CUDA_TRY(cudaDeviceSynchronize());
   }
   s->par = pm;
   return 0;
@@ -855,8 +862,9 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
 }
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null); mass: of the mass matrix
-// (t_in = the q tangents; the step's arguments are not read)
-struct JvpTangents { const double* t_in; const double* t_par; int m; bool mass = false; };
+// (t_in = the q tangents; the step's arguments are not read); kin: of the kinematics of this point table and these outputs (t_in =
+// the q tangents, t_par unused)
+struct JvpTangents { const double* t_in; const double* t_par; int m; bool mass = false; const TdsKinCall* kin = nullptr; };
 
 // Jacobian columns: the step's inputs (params == false) or the installed physical parameters, which are the dual instance's
 // directions dims[1] + s (params == true); or, with jv, the m columns J V of the tangent-seeded instance
@@ -889,7 +897,8 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   for (int d0 = 0; d0 < n_dirs; d0 += chunk) {
     io.jac_dir0 = dir_base + d0;
     const int nd = n_dirs - d0 < chunk ? n_dirs - d0 : chunk;
-    int rc = (jv && jv->mass) ? tds_launch_mass_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
+    int rc = (jv && jv->kin) ? tds_launch_kin_jvp(&s->dm_ad, &io, jv->kin, jv->t_in, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
+           : (jv && jv->mass) ? tds_launch_mass_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
            : jv ? tds_launch_stepw_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch,
                                        (cudaStream_t)stream)
            : pm ? tds_launch_stepw_jacobian_par(&s->dm_ad, &s->P, &s->E, &io, pm, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream)
@@ -1232,6 +1241,201 @@ int tds_b200_mass_matrix_vjp_host(tds_b200_sim* s, const double* q, const double
   if (g_q && n_q && (rc = mass_download(s, gq_d, n_q, g_q))) return rc;
   if (g_par && (rc = mass_download(s, gp_d, k, g_par))) return rc;
   return 0;
+}
+
+// ---- forward kinematics and point Jacobians (DESIGN.md section 7.13): the KIN instances of the world-frame kernel (tds_kin.cu) ---------
+// rows of the outputs xf | x | J
+struct KinRows { size_t xf, x, J; size_t all() const { return xf + x + J; } };
+static KinRows kin_rows(const tds_b200_sim* s, int K) {
+  return KinRows{(size_t)s->dm[0].n_links * 12, (size_t)3 * K, (size_t)3 * K * s->dm[0].n_qd};
+}
+
+static int kin_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local) {
+  if (!s || !q) return -1;
+  if (K < 0 || K > TDS_B200_MAX_KIN_POINTS) { set_err("kinematics: K out of [0, TDS_B200_MAX_KIN_POINTS]"); return -1; }
+  if (K > 0 && (!links || !local)) return -1;
+  for (int k = 0; k < K; ++k)
+    if (links[k] < -1 || links[k] >= s->dm[0].n_links) { set_err("kinematics: a link index out of [-1, n_links)"); return -1; }
+  return 0;
+}
+
+// fp64 outputs from q [n_q][ns] fp32, one lane per environment on the 8-byte layout of the mass matrix
+static int kin_run(tds_b200_sim* s, const float* q, const TdsKinCall* kc, cudaStream_t sm) {
+  StepIO io;
+  memset(&io, 0, sizeof(io));
+  io.q_in = q; io.jac_n_in = 1;
+  io.n = s->n; io.n_stride = s->ns;
+  const size_t need = (size_t)(s->n + 31) / 32 * (size_t)s->dm_m.x_total * 32 * 4;
+  if (need > s->jac_scratch_bytes) {
+    if (s->jac_scratch) cudaFree(s->jac_scratch);
+    s->jac_scratch = nullptr; s->jac_scratch_bytes = 0;
+    CUDA_TRY(cudaMalloc((void**)&s->jac_scratch, need));
+    s->jac_scratch_bytes = need;
+  }
+  const int rc = tds_launch_kin(&s->dm_m, &io, kc, s->jac_scratch, sm);
+  if (rc) set_err(std::string("kinematics launch: ") + cudaGetErrorString((cudaError_t)rc));
+  return rc;
+}
+
+// m tangents t_q [n_q * m][ns] -> the outputs' columns [rows * m][ns], through the Jacobian's chunk loop
+static int kin_jvp_run(tds_b200_sim* s, const float* q, const TdsKinCall* kc, int m, const double* t_q, cudaStream_t sm) {
+  JvpTangents jv{t_q, nullptr, m};
+  jv.kin = kc;
+  return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, nullptr, nullptr, nullptr, sm, false, &jv);
+}
+
+// g_q = <G, d(xf | x | J)> along the n_q identity tangents, G [rows][ns] concatenated, in chunks of directions within 1 GB
+static int kin_vjp_run(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, const double* G, double* g_q,
+                       double* buf, int chunk, cudaStream_t sm) {
+  const int n_q = s->dm[0].n_q, ns = s->ns;
+  const KinRows R = kin_rows(s, K);
+  for (int d0 = 0; d0 < n_q; d0 += chunk) {
+    const int nd = n_q - d0 < chunk ? n_q - d0 : chunk;
+    double* tq = buf;
+    double* dO = tq + (size_t)n_q * nd * ns;
+    TdsKinCall kc{K, links, local, dO, dO + R.xf * nd * ns, dO + (R.xf + R.x) * nd * ns};
+    int rc = tds_launch_mass_eye(tq, nullptr, n_q, 0, d0, nd, ns, sm);
+    if (!rc) rc = kin_jvp_run(s, q, &kc, nd, tq, sm);
+    if (!rc) rc = tds_launch_mass_contract(G, dO, (int)R.all(), nd, d0, n_q, g_q, nullptr, s->n, ns, sm);
+    if (rc) { set_err(std::string("kinematics vjp: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
+  }
+  return 0;
+}
+
+// device buffer of the VJP: the concatenated cotangent [rows][ns], then identity tangents + output columns of `chunk` directions
+static int kin_vjp_buffers(tds_b200_sim* s, int K, double** G, double** buf, int* chunk) {
+  const int n_q = s->dm[0].n_q, ns = s->ns;
+  const size_t rows = kin_rows(s, K).all();
+  const size_t per_dir = sizeof(double) * (rows + n_q) * ns;
+  int c = (int)(((size_t)1 << 30) / per_dir);
+  if (c < 1) c = 1;
+  if (c > n_q) c = n_q;
+  if (c < 1) c = 1;
+  if (int rc = grow_dev(&s->mass_dev, &s->mass_dev_bytes, sizeof(double) * rows * ns + per_dir * c)) return rc;
+  *G = s->mass_dev;
+  *buf = s->mass_dev + rows * ns;
+  *chunk = c;
+  return 0;
+}
+
+int tds_b200_kinematics_device(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, double* xf, double* x,
+                               double* J, void* stream) {
+  if (int rc = kin_check(s, q, K, links, local)) return rc;
+  if (!xf && !x && !J) return -1;
+  const TdsKinCall kc{K, links, local, xf, x, J};
+  return kin_run(s, q, &kc, (cudaStream_t)stream);
+}
+
+int tds_b200_kinematics_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, double* xf, double* x,
+                             double* J) {
+  if (int rc = kin_check(s, q, K, links, local)) return rc;
+  if (!xf && !x && !J) return -1;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const KinRows R = kin_rows(s, K);
+  const size_t ns = s->ns;
+  int rc = mass_upload_q(s, q);
+  if (!rc) rc = grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (R.all() + 1) * ns);
+  if (rc) return rc;
+  double* d = s->jac_dev;
+  const TdsKinCall kc{K, links, local, xf ? d : nullptr, x ? d + R.xf * ns : nullptr, J ? d + (R.xf + R.x) * ns : nullptr};
+  if ((rc = kin_run(s, s->q, &kc, s->stream))) return rc;
+  if (xf && (rc = mass_download(s, kc.xf, R.xf, xf))) return rc;
+  if (x && R.x && (rc = mass_download(s, kc.x, R.x, x))) return rc;
+  if (J && R.J && (rc = mass_download(s, kc.J, R.J, J))) return rc;
+  return 0;
+}
+
+static int kin_jvp_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local, int m, const void* t_q,
+                         const void* t_xf, const void* t_x, const void* t_J) {
+  if (int rc = kin_check(s, q, K, links, local)) return rc;
+  if (m < 1 || !t_q || (!t_xf && !t_x && !t_J)) return -1;
+  return 0;
+}
+
+int tds_b200_kinematics_jvp_device(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, int m,
+                                   const double* t_q, double* t_xf, double* t_x, double* t_J, void* stream) {
+  if (int rc = kin_jvp_check(s, q, K, links, local, m, t_q, t_xf, t_x, t_J)) return rc;
+  const TdsKinCall kc{K, links, local, t_xf, t_x, t_J};
+  return kin_jvp_run(s, q, &kc, m, t_q, (cudaStream_t)stream);
+}
+
+int tds_b200_kinematics_jvp_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, int m,
+                                 const double* t_q, double* t_xf, double* t_x, double* t_J) {
+  if (int rc = kin_jvp_check(s, q, K, links, local, m, t_q, t_xf, t_x, t_J)) return rc;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q;
+  const KinRows R = kin_rows(s, K);
+  const size_t tq = (size_t)n_q * m * ns, to = R.all() * m * ns;
+  int rc = mass_upload_q(s, q);
+  if (!rc) rc = grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (tq + to + 1));
+  if (rc) return rc;
+  double* tq_d = s->jvp_dev;
+  double* to_d = s->jvp_dev + tq;
+  if (n_q) {   // tangents: host [n][n_q][m] -> device [n_q * m][ns]
+    const size_t w = (size_t)n_q * m;
+    std::vector<double> tmp(w * ns, 0.0);
+    for (int e = 0; e < n; ++e) for (size_t c = 0; c < w; ++c) tmp[c * ns + e] = t_q[(size_t)e * w + c];
+    CUDA_TRY(cudaMemcpyAsync(tq_d, tmp.data(), sizeof(double) * w * ns, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));
+  }
+  const TdsKinCall kc{K, links, local, t_xf ? to_d : nullptr, t_x ? to_d + R.xf * m * ns : nullptr,
+                      t_J ? to_d + (R.xf + R.x) * m * ns : nullptr};
+  if ((rc = kin_jvp_run(s, s->q, &kc, m, tq_d, s->stream))) return rc;
+  if (t_xf && (rc = mass_download(s, kc.xf, R.xf * m, t_xf))) return rc;
+  if (t_x && R.x && (rc = mass_download(s, kc.x, R.x * m, t_x))) return rc;
+  if (t_J && R.J && (rc = mass_download(s, kc.J, R.J * m, t_J))) return rc;
+  return 0;
+}
+
+static int kin_vjp_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local, const void* G_xf, const void* G_x,
+                         const void* G_J, const void* g_q) {
+  if (int rc = kin_check(s, q, K, links, local)) return rc;
+  if (!g_q || (!G_xf && !G_x && !G_J)) return -1;
+  return 0;
+}
+
+int tds_b200_kinematics_vjp_device(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, const double* G_xf,
+                                   const double* G_x, const double* G_J, double* g_q, void* stream) {
+  if (int rc = kin_vjp_check(s, q, K, links, local, G_xf, G_x, G_J, g_q)) return rc;
+  if (s->dm[0].n_q == 0) return 0;
+  const cudaStream_t sm = (cudaStream_t)stream;
+  const KinRows R = kin_rows(s, K);
+  const size_t ns = s->ns;
+  double *G, *buf;
+  int chunk;
+  if (int rc = kin_vjp_buffers(s, K, &G, &buf, &chunk)) return rc;
+  // the concatenated cotangent xf | x | J, zero where a part is NULL
+  CUDA_TRY(cudaMemsetAsync(G, 0, sizeof(double) * R.all() * ns, sm));
+  if (G_xf) CUDA_TRY(cudaMemcpyAsync(G, G_xf, sizeof(double) * R.xf * ns, cudaMemcpyDeviceToDevice, sm));
+  if (G_x && R.x) CUDA_TRY(cudaMemcpyAsync(G + R.xf * ns, G_x, sizeof(double) * R.x * ns, cudaMemcpyDeviceToDevice, sm));
+  if (G_J && R.J) CUDA_TRY(cudaMemcpyAsync(G + (R.xf + R.x) * ns, G_J, sizeof(double) * R.J * ns, cudaMemcpyDeviceToDevice, sm));
+  return kin_vjp_run(s, q, K, links, local, G, g_q, buf, chunk, sm);
+}
+
+int tds_b200_kinematics_vjp_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, const double* G_xf,
+                                 const double* G_x, const double* G_J, double* g_q) {
+  if (int rc = kin_vjp_check(s, q, K, links, local, G_xf, G_x, G_J, g_q)) return rc;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q;
+  if (n_q == 0) return 0;
+  const KinRows R = kin_rows(s, K);
+  double *G, *buf;
+  int chunk;
+  int rc = mass_upload_q(s, q);
+  if (!rc) rc = kin_vjp_buffers(s, K, &G, &buf, &chunk);
+  if (!rc) rc = grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)n_q * ns);
+  if (rc) return rc;
+  {  // cotangents: host [n][rows of the part] -> device [rows][ns], concatenated
+    std::vector<double> tmp(R.all() * ns, 0.0);
+    auto put = [&](const double* src, size_t rows, size_t r0) {
+      if (src) for (int e = 0; e < n; ++e) for (size_t r = 0; r < rows; ++r) tmp[(r0 + r) * ns + e] = src[(size_t)e * rows + r];
+    };
+    put(G_xf, R.xf, 0); put(G_x, R.x, R.xf); put(G_J, R.J, R.xf + R.x);
+    CUDA_TRY(cudaMemcpyAsync(G, tmp.data(), sizeof(double) * R.all() * ns, cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));
+  }
+  if ((rc = kin_vjp_run(s, s->q, K, links, local, G, s->vjp_g, buf, chunk, s->stream))) return rc;
+  return mass_download(s, s->vjp_g, n_q, g_q);
 }
 
 // ---- vector-Jacobian product: g_in = g_out^T d(q', qd' | qdd) / d(q | qd | tau or action (| kp, kd, max_force)) by the taping

@@ -498,6 +498,8 @@ static int rigid_set_physical_params(tds_b200_rigid* h, int k, const int* ids, c
     // steps run on non-blocking streams, which a plain cudaMemcpy does not wait for
     RB_TRY(cudaDeviceSynchronize());
     RB_TRY(cudaMemcpy(h->par_dev, t.data(), sizeof(double) * sec, cudaMemcpyHostToDevice));
+    // a copy from pageable memory may return before its DMA has landed, and the non-blocking streams do not wait for it either
+    RB_TRY(cudaDeviceSynchronize());
   }
   h->par = pm;
   return 0;

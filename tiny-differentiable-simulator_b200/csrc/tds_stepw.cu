@@ -40,10 +40,21 @@ struct NoPar {};
 struct JvpTan { const double* t_in; const double* t_par; int m; };
 struct NoParJvp { JvpTan jv; };
 struct ParMapJvp : ParMap { JvpTan jv; };
-template <bool PAR, bool JV = false> struct ParArg { typedef NoPar type; };
+// kernel argument of the kinematics instances (KIN, DESIGN.md section 7.13): the outputs (each may be null) and the point table, the
+// same for every environment: point k sits on link link[k] (-1: the base) at local[3k..3k+2] in that link's frame
+struct KinArg {
+  double* xf; double* x; double* J;
+  int K;
+  int link[TDS_MAX_KIN_POINTS];
+  double local[3 * TDS_MAX_KIN_POINTS];
+};
+struct KinArgJvp : KinArg { JvpTan jv; };
+template <bool PAR, bool JV = false, bool KIN = false> struct ParArg { typedef NoPar type; };
 template <> struct ParArg<true, false> { typedef ParMap type; };
 template <> struct ParArg<false, true> { typedef NoParJvp type; };
 template <> struct ParArg<true, true> { typedef ParMapJvp type; };
+template <> struct ParArg<false, false, true> { typedef KinArg type; };
+template <> struct ParArg<false, true, true> { typedef KinArgJvp type; };
 
 // joint stiffness and damping enter the step at fp32, as DevModel stores them; the derivative is taken at the rounded value
 TDS_D double f32_round(double x) { return (double)(float)x; }
@@ -66,11 +77,17 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // the CRBA of pass 2 and the floating-base block as if a contact were active, then the dense symmetric n_qd x n_qd matrix in place of
 // the solve: entry (r, c) at io.jac[(r * n_qd + c) * ns + e] (fp64 instance), or its dual part as column j of an m-column Jacobian,
 // io.jac[((r * n_qd + c) * m + j) * ns + e] (JV instance, t_in = the q tangents).  ABA, integration and reward are not compiled in.
-template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false>
+// KIN: forward kinematics and linear point Jacobians (DESIGN.md section 7.13), launched in MODE_NOCONTACT with the point table as pm.
+// Pass 1 from q alone (qd = 0, no PD, tau or contact detection: forward_kinematics_q), without the inertias pass 2 needs; as pass 1
+// reaches link l it writes l's world transform (pm.xf, the layout of io.link_xf), and the world position p_l + R_l local + O
+// (pm.x) and the 3 x n_qd Jacobian (pm.J, jacobian.hpp:13-83) of every point on l.  Returns before pass 2.  Row r of a output at
+// out[r * ns + e] (fp64 instance), or its dual part as column j of an m-column Jacobian, out[(r * m + j) * ns + e] (JV instance).
+template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
+          bool KIN = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
-                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV>::type pm = {}) {
+                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN>::type pm = {}) {
   extern __shared__ __align__(16) char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp_in_blk = threadIdx.x >> 5;
@@ -165,7 +182,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // input directions of the differentiable instance: q | qd | tau or action | kp, kd, max_force (with PD)
   const int in0 = M.n_q + n;
   for (int k = 0; k < M.n_q; ++k) qv[k * ST] = seed(RQ(io.q_in[(size_t)k * ns + e]), k);
-  for (int k = 0; k < n; ++k) qdv[k * ST] = MASS ? RQ(0.f) : seed(RQ(io.qd_in[(size_t)k * ns + e]), M.n_q + k);
+  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(io.qd_in[(size_t)k * ns + e]), M.n_q + k);
   for (int k = 0; k < n; ++k) tauv[k * ST] = RQ(0.f);
   if (!MASS && use_pd) {
     const RQ kp = seed(RQ(E.kp), in0 + E.n_act), kd = seed(RQ(E.kd), in0 + E.n_act + 1), fmax_ = seed(RQ(E.max_force), in0 + E.n_act + 2);
@@ -182,11 +199,13 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     const int off = M.floating ? 6 : 0;
     for (int k = off; k < n; ++k) tauv[k * ST] = seed(RQ(io.tau_in[(size_t)(k - off) * ns + e]), in0 + k - off);
   }
-  for (int s = 0; s < M.n_acc; ++s) {
-    RA* pa = A.ptr<RA>(M.x_acc + s * M.x_acc_words);
-    for (int k = 0; k < 27; ++k) pa[k * ST] = RA(0);
-    RC* pc = A.ptr<RC>(M.x_acc + s * M.x_acc_words + M.x_acc_ic_word);
-    for (int k = 0; k < 10; ++k) pc[k * ST] = RC(0);
+  if constexpr (!KIN) {   // (the KIN lanes return before pass 2 reads the accumulators)
+    for (int s = 0; s < M.n_acc; ++s) {
+      RA* pa = A.ptr<RA>(M.x_acc + s * M.x_acc_words);
+      for (int k = 0; k < 27; ++k) pa[k * ST] = RA(0);
+      RC* pc = A.ptr<RC>(M.x_acc + s * M.x_acc_words + M.x_acc_ic_word);
+      for (int k = 0; k < 10; ++k) pc[k * ST] = RC(0);
+    }
   }
   const bool world_step = mode == MODE_WORLD;   // World::step(dt) on its own (src/world.hpp:302-363): q, qd in -> qd out
   const bool want_contacts = (mode == MODE_FULL || world_step) && (M.has_plane || M.n_pair_points > 0);
@@ -270,6 +289,46 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       }
     }
   };
+  // KIN: the outputs of link l (-1: the base) at its world rotation R and position p (relative to O).  The Jacobian of a point on l
+  // reads the stored S of l and of its ancestors, all written by the time pass 1 reaches l (links are ordered parent first), so it is
+  // written here too and the points' positions need no storage.
+  auto kin_link = [&](int l, const M3<RC>& R, const V3<RC>& p) {
+    if constexpr (KIN) {
+      if (!live) return;
+      auto put = [&](double* o, size_t r, const RC& x) {
+        if constexpr (AD) o[(r * io.jac_n_in + jcol) * ns + e] = x.d;
+        else o[r * ns + e] = x;
+      };
+      if (pm.xf && l >= 0) {   // the layout of io.link_xf: R row-major, then the position
+        const size_t r0 = (size_t)l * 12;
+        put(pm.xf, r0, R.xx); put(pm.xf, r0 + 1, R.xy); put(pm.xf, r0 + 2, R.xz);
+        put(pm.xf, r0 + 3, R.yx); put(pm.xf, r0 + 4, R.yy); put(pm.xf, r0 + 5, R.yz);
+        put(pm.xf, r0 + 6, R.zx); put(pm.xf, r0 + 7, R.zy); put(pm.xf, r0 + 8, R.zz);
+        put(pm.xf, r0 + 9, p.x + O.x); put(pm.xf, r0 + 10, p.y + O.y); put(pm.xf, r0 + 11, p.z + O.z);
+      }
+      for (int k = 0; k < pm.K; ++k) {
+        if (pm.link[k] != l) continue;
+        const V3<RC> xr = p + mul(R, v3<RC>(RC(pm.local[3 * k]), RC(pm.local[3 * k + 1]), RC(pm.local[3 * k + 2])));
+        if (pm.x) { put(pm.x, 3 * k, xr.x + O.x); put(pm.x, 3 * k + 1, xr.y + O.y); put(pm.x, 3 * k + 2, xr.z + O.z); }
+        if (!pm.J) continue;
+        // rows 3k .. 3k + 2 of n_qd columns: zero outside the point's chain (and outside its multibody)
+        const size_t r0 = (size_t)3 * k * n;
+        auto put_col = [&](int c, const V3<RC>& col) { put(pm.J, r0 + c, col.x); put(pm.J, r0 + n + c, col.y); put(pm.J, r0 + 2 * n + c, col.z); };
+        const V3<RC> z = v3<RC>(RC(0), RC(0), RC(0));
+        for (int c = 0; c < n; ++c) put_col(c, z);
+        if (M.floating) {   // jacobian.hpp:39-58: [-[x - r0]x^T | I3] with the base rotation ignored (O is the base origin r0)
+          put_col(0, v3<RC>(RC(0), -xr.z, xr.y)); put_col(1, v3<RC>(xr.z, RC(0), -xr.x)); put_col(2, v3<RC>(-xr.y, xr.x, RC(0)));
+          put_col(3, v3<RC>(RC(1), RC(0), RC(0))); put_col(4, v3<RC>(RC(0), RC(1), RC(0))); put_col(5, v3<RC>(RC(0), RC(0), RC(1)));
+        }
+        for (int j = l; j >= 0; j = M.parent[j]) {   // jacobian.hpp:63-80: column = S_j evaluated at the point (fixed links: none)
+          for (int cj = 0; cj < n_cols(j); ++cj) {
+            const Sv<RC> S = S_col(j, cj);
+            put_col(M.qd_idx[j] + cj, S.bot + cross(S.top, xr));
+          }
+        }
+      }
+    }
+  };
   M3<RC> R_prev = Rb;
   V3<RC> p_prev = M.floating ? v3<RC>(RC(0), RC(0), RC(0)) : v3<RC>(-O.x, -O.y, -O.z);
   Sv<RA> v_prev;
@@ -285,6 +344,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   const Sv<RA> v_base = v_prev;
   { RC* px = A.ptr<RC>(M.x_xw); st9<RC>(px, ST, R_base); st3<RC>(px + 9 * ST, ST, p_base); }
   if (want_contacts) emit_geoms(-1, R_base, p_base);
+  if constexpr (KIN) kin_link(-1, R_base, p_base);
   for (int i = 0; i < n_links; ++i) {
     const int p = M.parent[i];
     const int fl = M.flags[i];
@@ -344,7 +404,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     st6<RC>(Sw + i * 6 * ST, ST, S);
     if (M.xw_slot[i] >= 0) { RC* px = A.ptr<RC>(M.x_xw + (M.xw_slot[i] + 1) * 12 * RCW); st9<RC>(px, ST, Ri); st3<RC>(px + 9 * ST, ST, pi); }
     // rigid-body inertia about O in world axes: com c = p_i + R_i com_l, I = R Icom R^T + m (|c|^2 1 - c c^T)
-    {
+    if constexpr (!KIN) {
       const double* rb = M.rbic[i];
       auto rbc = [&](int c) -> RP { return par_of(body_slot(i + 1, c), rb[c]); };
       Rbi<RC> r;
@@ -384,8 +444,10 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       o[(size_t)6 * ns] = (float)val_of(Ri.zx); o[(size_t)7 * ns] = (float)val_of(Ri.zy); o[(size_t)8 * ns] = (float)val_of(Ri.zz);
       o[(size_t)9 * ns] = (float)val_of(pi.x + O.x); o[(size_t)10 * ns] = (float)val_of(pi.y + O.y); o[(size_t)11 * ns] = (float)val_of(pi.z + O.z);
     }
+    if constexpr (KIN) kin_link(i, Ri, pi);
     R_prev = Ri; p_prev = pi; v_prev = v;
   }
+  if constexpr (KIN) return;
   // ---- contacts between the multibodies of the world (world.hpp:206-282), group = ordered pair of multibodies -----------------------
   // contact_sphere_sphere (contact_point.hpp:44-94) on sphere centres / capsule end spheres (contact_capsule_sphere, :406-438);
   // sphere A x capsule B goes through the dispatcher's swapped call (:478-492): points exchanged, normal negated.

@@ -9,6 +9,7 @@
 #define TDS_MAX_POINTS 64   // candidate contact points of a model (sphere 1, capsule 2, box 8 per geom)
 #define TDS_MAX_PAIR_POINTS 64   // candidate contact points between geoms of DIFFERENT multibodies of one world
 #define TDS_MAX_PAIR_GROUPS 10   // ordered multibody pairs (a < b) that have such candidates (5 multibodies: 10 pairs)
+#define TDS_MAX_KIN_POINTS 64    // points of one forward-kinematics call (TDS_B200_MAX_KIN_POINTS)
 
 // link flags
 #define TDS_LF_PARENT_ADJ 1   // parent == i-1  -> deltas are carried in registers
@@ -144,6 +145,15 @@ struct StepIO {
   // tape_cap entries per lane and interleaved by lane within a warp; tape_overflow: set when a lane ran out of capacity
   const double* g_out; double* g_in;
   void* tape; double* tape_adj; int tape_cap; int* tape_overflow;
+};
+
+// One call of the kinematics instances (tds_kin.cu, DESIGN.md section 7.13), as the C-ABI hands it to the launchers: the point table
+// (host memory, copied into the kernel argument) and the outputs xf [n_links * 12][ns], x [3K][ns], J [3K * n_qd][ns] (each may be null)
+struct TdsKinCall {
+  int K;
+  const int* link;       // [K], -1 = the base
+  const double* local;   // [3K]
+  double* xf; double* x; double* J;
 };
 
 // Installed physical parameters (tds_b200_set_physical_params_*): the slot of each model quantity in the lane's value vector,

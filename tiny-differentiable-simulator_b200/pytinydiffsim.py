@@ -5,6 +5,7 @@
     TinyUrdfParser.load_urdf, UrdfToMultiBody2.convert2                       :1013-1034
     forward_dynamics(mb, gravity), integrate_euler(mb, dt), integrate_euler_qdd(mb, dt)   :659-663
     mass_matrix(mb[, q])                                                      :659-663 (mass_matrix.hpp)
+    point_jacobian(mb, link_index, point, is_local_point=False)               (jacobian.hpp:85-90)
     VectorizedLaikagoEnv, VectorizedAntEnv (pytinydiffsim_includes.h:58-227), CartpoleEnv (:1123)
 
 The fine-grained calls operate on one MultiBody like the reference's; each is one stage of the GPU path (forward dynamics =
@@ -167,6 +168,30 @@ def mass_matrix(mb, q=None):
     mb.q, and mass_matrix(mb, q) at a q given explicitly (mb.q is left as it is)."""
     qv = np.asarray(mb.q if q is None else q, dtype=np.float64).reshape(1, -1)
     return mb._sim.mass_matrix_host(qv)[0]
+
+
+def point_jacobian(mb, link_index, point, is_local_point=False):
+    """The 3 x num_dofs linear Jacobian of a point on link `link_index` (-1: the base) at mb.q: a NumPy float64 array, the reference's
+    point_jacobian2(mb, link_index, point, is_local_point) (jacobian.hpp:85-90), computed by the kinematics of the GPU step in fp64 at the
+    fp32-rounded q.  The reference's Python binding of it is not pinned here; this follows the C++ signature.  `point` is in the link's
+    frame when is_local_point, else in world coordinates; a world point is mapped into the link's frame with the link's transform from
+    the same kernel.  A floating base gives the reference's columns [-[x - r0]x^T | I3] (its rotation ignored)."""
+    qv = np.asarray(mb.q, dtype=np.float64).reshape(1, -1)
+    sim = mb._sim
+    link = int(link_index)
+    if not -1 <= link < sim.n_links:
+        raise IndexError(f"link_index {link} out of [-1, {sim.n_links})")
+    pt = np.asarray(point, dtype=np.float64).reshape(3)
+    if not is_local_point:
+        if link >= 0:
+            R, p, _, _ = sim.kinematics_host(qv, [], np.zeros((0, 3)))
+            R, p = R[0, link], p[0, link]
+        else:   # the base's transform: its origin and axes as points of the base
+            _, _, x, _ = sim.kinematics_host(qv, [-1] * 4, np.vstack([np.zeros(3), np.eye(3)]))
+            p = x[0, 0]
+            R = (x[0, 1:] - p).T
+        pt = R.T @ (pt - p)
+    return sim.kinematics_host(qv, [link], pt.reshape(1, 3))[3][0, 0]
 
 
 # ---- rigid bodies (python/pytinydiffsim.inl:336-385, 448-455; examples/billiard_optimization.py) --------------------------------

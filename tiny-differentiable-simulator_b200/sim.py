@@ -371,6 +371,100 @@ class BatchSim:
         st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
         self._check(self._L.tds_b200_mass_matrix_vjp_device(self._h, _ptr(q), _ptr(G), _ptr(g_q), _ptr(g_par), st), "mass_matrix_vjp_device")
 
+    # ---- forward kinematics and linear point Jacobians (DESIGN.md section 7.13) ----
+    @staticmethod
+    def _points(links, local):
+        """The point table as the C-ABI takes it: (links int32 [K], local float64 [K, 3], K)."""
+        lk = np.ascontiguousarray(np.asarray(links, dtype=np.int64).ravel(), dtype=np.int32)
+        lc = np.ascontiguousarray(np.asarray(local, dtype=np.float64).reshape(-1, 3))
+        if lc.shape[0] != lk.size:
+            raise ValueError(f"links [K] and local [K, 3] expected, got {lk.shape} and {lc.shape}")
+        return lk, lc, lk.size
+
+    def _kin_args(self, links, local):
+        lk, lc, K = self._points(links, local)
+        return (lk, lc), K, ctypes.c_void_p(lk.ctypes.data) if K else None, _dp(lc) if K else None
+
+    def kinematics_host(self, q, links, local):
+        """Forward kinematics and linear point Jacobians at the fp32-rounded q [n, n_q] (qd plays no part) for the point table links [K]
+        (-1: the base) / local [K, 3] (coordinates in the link's frame): (R [n, n_links, 3, 3], p [n, n_links, 3], x [n, K, 3],
+        J [n, K, 3, n_qd]), float64, world coordinates.  J follows the reference's point_jacobian (a floating base gives
+        [-[x - r0]x^T | I3] with the base's rotation ignored).  Installed physical parameters do not enter."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        assert q.shape == (self.n_envs, self.n_q), q.shape
+        keep, K, lp, cp = self._kin_args(links, local)
+        xf = np.zeros((self.n_envs, self.n_links, 12))
+        x = np.zeros((self.n_envs, K, 3))
+        J = np.zeros((self.n_envs, K, 3, self.n_qd))
+        self._check(self._L.tds_b200_kinematics_host(self._h, _dp(q), K, lp, cp, _dp(xf), _dp(x), _dp(J)), "kinematics_host")
+        return xf[:, :, :9].reshape(self.n_envs, self.n_links, 3, 3), xf[:, :, 9:].copy(), x, J
+
+    def kinematics_device(self, q, links, local, xf=None, x=None, J=None, stream=None):
+        """Device version of kinematics_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride]; xf [n_links * 12, n_stride], x [3K,
+        n_stride] and J [3K * n_qd, n_stride] float64 CUDA tensors (any may be None, not all three), entry (point k, row r, column c) of J
+        at row (3k + r) * n_qd + c.  The point table is host data.  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_kinematics_device(self._h, _ptr(q), K, lp, cp, _ptr(xf), _ptr(x), _ptr(J), st), "kinematics_device")
+
+    def kinematics_jvp_host(self, q, links, local, t_q):
+        """Directional derivatives along m tangents t_q [n, n_q, m] of q: (dxf [n, n_links, 12, m], dx [n, K, 3, m], dJ [n, K, 3, n_qd, m])
+        (xf in the layout R row-major | p); a tangent given as [n, n_q] is m = 1 and the trailing axis is dropped."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        tq = np.asarray(t_q, dtype=np.float64)
+        single = tq.ndim == 2
+        if single:
+            tq = tq[:, :, None]
+        if tq.shape[:2] != (self.n_envs, self.n_q):
+            raise ValueError(f"t_q: [n_envs, {self.n_q}, m] or [n_envs, {self.n_q}] expected, got {tq.shape}")
+        tq = np.ascontiguousarray(tq)
+        m = tq.shape[2]
+        keep, K, lp, cp = self._kin_args(links, local)
+        n = self.n_envs
+        dxf, dx, dJ = np.zeros((n, self.n_links, 12, m)), np.zeros((n, K, 3, m)), np.zeros((n, K, 3, self.n_qd, m))
+        self._check(self._L.tds_b200_kinematics_jvp_host(self._h, _dp(q), K, lp, cp, m, _dp(tq), _dp(dxf), _dp(dx), _dp(dJ)),
+                    "kinematics_jvp_host")
+        return (dxf[..., 0], dx[..., 0], dJ[..., 0]) if single else (dxf, dx, dJ)
+
+    def kinematics_jvp_device(self, q, links, local, m, t_q, t_xf=None, t_x=None, t_J=None, stream=None):
+        """Device version of kinematics_jvp_host: q float32 [n_q, n_stride]; t_q [n_q * m, n_stride] and t_xf [n_links * 12 * m, n_stride],
+        t_x [3K * m, n_stride], t_J [3K * n_qd * m, n_stride] (any may be None, not all three) float64 CUDA tensors, entry (r, j) at row
+        r * m + j.  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_kinematics_jvp_device(self._h, _ptr(q), K, lp, cp, int(m), _ptr(t_q), _ptr(t_xf), _ptr(t_x), _ptr(t_J),
+                                                           st), "kinematics_jvp_device")
+
+    def kinematics_vjp_host(self, q, links, local, G_xf=None, G_x=None, G_J=None):
+        """Cotangents G_xf [n, n_links, 12], G_x [n, K, 3], G_J [n, K, 3, n_qd] (None: zero, not all three) -> g_q [n, n_q] =
+        sum G * d(outputs)/dq."""
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        keep, K, lp, cp = self._kin_args(links, local)
+        n = self.n_envs
+
+        def prep(G, shape):
+            if G is None:
+                return None
+            G = np.ascontiguousarray(G, dtype=np.float64)
+            assert G.size == int(np.prod(shape)), (G.shape, shape)
+            return G
+        gxf, gx, gJ = prep(G_xf, (n, self.n_links, 12)), prep(G_x, (n, K, 3)), prep(G_J, (n, K, 3, self.n_qd))
+        g_q = np.zeros((n, self.n_q))
+        self._check(self._L.tds_b200_kinematics_vjp_host(self._h, _dp(q), K, lp, cp, _dp(gxf), _dp(gx), _dp(gJ), _dp(g_q)),
+                    "kinematics_vjp_host")
+        return g_q
+
+    def kinematics_vjp_device(self, q, links, local, G_xf, G_x, G_J, g_q, stream=None):
+        """Device version of kinematics_vjp_host: q float32 [n_q, n_stride], cotangents float64 in the layouts of kinematics_device (None:
+        zero, not all three), g_q float64 [n_q, n_stride] CUDA tensors.  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_kinematics_vjp_device(self._h, _ptr(q), K, lp, cp, _ptr(G_xf), _ptr(G_x), _ptr(G_J), _ptr(g_q), st),
+                    "kinematics_vjp_device")
+
     def jacobian_chunk(self):
         """Directions (Jacobian columns or JVP tangents) one launch of the dual-number step takes; more run in several launches."""
         return self._L.tds_b200_jacobian_chunk(self._h)
