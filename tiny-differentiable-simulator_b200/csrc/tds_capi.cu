@@ -16,6 +16,7 @@
 #include "tds_types.h"
 #include "tds_team.h"
 #include "tds_tape.cuh"
+#include "tds_host_io.h"
 
 extern "C" int tds_launch_stept(const TeamModel* TM, const TeamLink* tl_dev, const DevModel* M, const SimParams* P,
                                 const EnvParams* E, const StepIO* io, int mode, int use_pd, int precision,
@@ -442,6 +443,7 @@ struct tds_b200_sim {
   int n_tau = 0, n_points = 0;
   ContactCandTable cand;              // static candidate table (reference enumeration order)
   int *c_count = nullptr, *c_links = nullptr, *c_cand = nullptr;   // device: per-environment contact list of the last tds_b200_contact_list_* call
+  size_t c_count_bytes = 0, c_links_bytes = 0, c_cand_bytes = 0;
   // resident state + staging
   float *q = nullptr, *qd = nullptr, *act = nullptr, *qdd = nullptr, *reward = nullptr, *done = nullptr;
   float *cdist = nullptr, *link_xf = nullptr;
@@ -449,8 +451,6 @@ struct tds_b200_sim {
   size_t scratch_bytes = 0;
   void* stage_dev = nullptr;   // device staging for AoS host buffers
   size_t stage_dev_bytes = 0;
-  void* stage_host = nullptr;  // pinned host staging
-  size_t stage_host_bytes = 0;
   cudaStream_t stream = nullptr;
   int max_smem_optin = 0;
   long long* phase_clk = nullptr;  // profiling only (tds_b200_debug_phase_clocks)
@@ -461,7 +461,7 @@ struct tds_b200_sim {
   int *act_qidx = nullptr, *r_steps = nullptr;
   float* obs_stats = nullptr;      // caller-owned [3 * n_obs][ns] running statistics of the observation filter, or null
   bool act_qidx_valid = false;
-  size_t pol_params_rows = 0;
+  size_t pol_params_bytes = 0;
   // set around the step launch of tds_b200_env_step_host when the specialised kernel serves the host layouts itself
   const float* io_act_aos = nullptr; float* io_obs_aos = nullptr; float* io_obs_tail = nullptr;
   const void* zc_key[4] = {nullptr, nullptr, nullptr, nullptr};   // zero-copy path: last buffer set and its device aliases
@@ -486,33 +486,67 @@ static bool is_pinned(const void* p) {
   return a.type == cudaMemoryTypeHost;
 }
 
-static int ensure_stage(tds_b200_sim* s, size_t dev_bytes, size_t host_bytes) {
-  if (dev_bytes > s->stage_dev_bytes) {
+static int ensure_stage(tds_b200_sim* s, size_t bytes) {
+  if (bytes > s->stage_dev_bytes) {
     // the graph of tds_b200_env_step_host holds addresses inside the staging buffer: it dies with the buffer
     drop_host_graph(s);
-    if (s->stage_dev) cudaFree(s->stage_dev);
-    s->stage_dev = nullptr; s->stage_dev_bytes = 0;
-    CUDA_TRY(cudaMalloc(&s->stage_dev, dev_bytes));
-    s->stage_dev_bytes = dev_bytes;
-  }
-  if (host_bytes > s->stage_host_bytes) {
-    if (s->stage_host) cudaFreeHost(s->stage_host);
-    s->stage_host = nullptr; s->stage_host_bytes = 0;
-    CUDA_TRY(cudaMallocHost(&s->stage_host, host_bytes));
-    s->stage_host_bytes = host_bytes;
+    CUDA_TRY(grow_dev(&s->stage_dev, &s->stage_dev_bytes, bytes));
   }
   return 0;
 }
 
 static int ensure_scratch(tds_b200_sim* s, int prec) {
   const int words = s->dm[prec].w_total > s->dm[prec].x_total ? s->dm[prec].w_total : s->dm[prec].x_total;
-  size_t need = (size_t)words * 4 * s->ns;
-  if (need > s->scratch_bytes) {
-    if (s->scratch) cudaFree(s->scratch);
-    s->scratch = nullptr; s->scratch_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->scratch, need));
-    s->scratch_bytes = need;
-  }
+  CUDA_TRY(grow_dev(&s->scratch, &s->scratch_bytes, (size_t)words * 4 * s->ns));
+  return 0;
+}
+
+// Entry of a host path that reuses the simulator's derivative buffers (jac_scratch, jac_dev, jvp_dev, vjp_g, mass_dev): selects the
+// device and waits for device work already queued.  A device entry point of this simulator may still be running on a caller's
+// stream with these buffers, and the simulator's own stream, which the host path runs on, is not ordered against that stream.
+static int enter_derivative_host(tds_b200_sim* s) {
+  CUDA_TRY(cudaSetDevice(s->device));
+  CUDA_TRY(cudaDeviceSynchronize());
+  return 0;
+}
+
+// ---- fp32 state of the host paths: fp64 host [n][dim] <-> the resident fp32 [dim][ns] buffers, through stage_dev on the
+// simulator's stream
+
+// src [n][dim] -> dst [dim][ns]; stage_dev holds n * dim doubles
+static int put_state(tds_b200_sim* s, const double* src, int dim, float* dst) {
+  if (dim == 0) return 0;
+  CUDA_TRY(cudaMemcpyAsync(s->stage_dev, src, sizeof(double) * s->n * dim, cudaMemcpyHostToDevice, s->stream));
+  aos_to_soa_kernel<double><<<(s->n + 127) / 128, 128, 0, s->stream>>>((const double*)s->stage_dev, dim, 0, dst, dim, s->n, s->ns);
+  return 0;
+}
+
+// q -> s->q, with stage_dev sized for any one state array of the host paths (q, qd, the step's inputs, the contact distances)
+static int put_q(tds_b200_sim* s, const double* q) {
+  const DevModel& M = s->dm[0];
+  const size_t rows = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + s->n_points + 1;
+  if (int rc = ensure_stage(s, sizeof(double) * s->n * rows)) return rc;
+  return put_state(s, q, M.n_q, s->q);
+}
+
+// q, qd and the step's inputs (NULL: zero) -> s->q, s->qd, s->act
+static int put_step_inputs(tds_b200_sim* s, int use_pd, const double* q, const double* qd, const double* tau_or_action) {
+  const int n_in = use_pd ? s->E.n_act : s->n_tau;
+  int rc = put_q(s, q);
+  if (!rc) rc = put_state(s, qd, s->dm[0].n_qd, s->qd);
+  if (rc) return rc;
+  if (tau_or_action) return put_state(s, tau_or_action, n_in, s->act);
+  CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * s->ns * (n_in > 0 ? n_in : 1), s->stream));
+  return 0;
+}
+
+// src [dim][ns] -> dst [n][dim] (dst NULL: nothing); returns with dst written
+static int get_state(tds_b200_sim* s, const float* src, int dim, double* dst) {
+  if (dim == 0 || !dst) return 0;
+  if (int rc = ensure_stage(s, sizeof(double) * s->n * dim)) return rc;
+  soa_to_aos_kernel<double><<<(s->n + 127) / 128, 128, 0, s->stream>>>(src, (double*)s->stage_dev, dim, 0, dim, s->n, s->ns);
+  CUDA_TRY(cudaMemcpyAsync(dst, s->stage_dev, sizeof(double) * s->n * dim, cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
   return 0;
 }
 
@@ -658,7 +692,6 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
   cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->jvp_dev); cudaFree(s->mass_dev);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
-  if (s->stage_host) cudaFreeHost(s->stage_host);
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
 }
@@ -751,21 +784,15 @@ static int set_physical_params(tds_b200_sim* s, int k, const int* ids, const dou
   const size_t bytes = sizeof(double) * (size_t)k * s->ns;
   if (bytes > s->par_dev_bytes) {
     drop_host_graph(s);
-    cudaFree(s->par_dev);
-    s->par_dev = nullptr; s->par_dev_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->par_dev, bytes));
+    CUDA_TRY(grow_dev(&s->par_dev, &s->par_dev_bytes, bytes));
     CUDA_TRY(cudaMemset(s->par_dev, 0, bytes));
-    s->par_dev_bytes = bytes;
   }
   if (device) {
     CUDA_TRY(cudaMemcpyAsync(s->par_dev, values, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   } else {
-    std::vector<double> tmp((size_t)k * s->ns, 0.0);
-    for (int e = 0; e < s->n; ++e)
-      for (int j = 0; j < k; ++j) tmp[(size_t)j * s->ns + e] = values[(size_t)e * k + j];
-    // steps run on non-blocking streams, which a plain cudaMemcpy does not wait for
+    // steps run on non-blocking streams, which this copy does not wait for
     CUDA_TRY(cudaDeviceSynchronize());
-    CUDA_TRY(cudaMemcpy(s->par_dev, tmp.data(), bytes, cudaMemcpyHostToDevice));
+    CUDA_TRY(put_rows(s->par_dev, values, k, s->n, s->ns, s->stream));
     // a copy from pageable memory may return before its DMA has landed, and the non-blocking streams do not wait for it either
     CUDA_TRY(cudaDeviceSynchronize());
   }
@@ -826,13 +853,7 @@ int tds_b200_step_device(tds_b200_sim* s, int mode, int use_pd, const float* q_i
     const int use_smem_t = s->smem_ok_t[p] ? 1 : 0;
     if (!use_smem_t) {
       const size_t warp_bytes = ((size_t)s->tm[p].t_total * (32 / TDS_TEAM_T) + (size_t)s->tm[p].l_total * 32) * 4;
-      const size_t need = warp_bytes * ((s->n + (32 / TDS_TEAM_T) - 1) / (32 / TDS_TEAM_T));
-      if (need > s->scratch_bytes) {
-        if (s->scratch) cudaFree(s->scratch);
-        s->scratch = nullptr; s->scratch_bytes = 0;
-        CUDA_TRY(cudaMalloc((void**)&s->scratch, need));
-        s->scratch_bytes = need;
-      }
+      CUDA_TRY(grow_dev(&s->scratch, &s->scratch_bytes, warp_bytes * ((s->n + (32 / TDS_TEAM_T) - 1) / (32 / TDS_TEAM_T))));
     }
     int rct = tds_launch_stept(&s->tm[p], s->team_dev, &s->dm[p], &s->P, &s->E, &io, mode, use_pd, p, s->scratch, use_smem_t,
                                (cudaStream_t)stream);
@@ -866,6 +887,17 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
 // the q tangents, t_par unused)
 struct JvpTangents { const double* t_in; const double* t_par; int m; bool mass = false; const TdsKinCall* kin = nullptr; };
 
+// scratch of one launch of a world-frame instance of layout M over every environment: x_total words per lane
+static size_t lane_arena_bytes(const tds_b200_sim* s, const DevModel& M) {
+  return (size_t)(s->n + 31) / 32 * (size_t)M.x_total * 32 * 4;
+}
+
+// directions (Jacobian columns or tangents) one launch of the dual instance takes: the scratch stays within 2 GB
+static int dir_chunk(const tds_b200_sim* s) {
+  const size_t chunk = ((size_t)2 << 30) / lane_arena_bytes(s, s->dm_ad);
+  return (int)(chunk < 1 ? 1 : (chunk > 65535 ? 65535 : chunk));   // (gridDim.y)
+}
+
 // Jacobian columns: the step's inputs (params == false) or the installed physical parameters, which are the dual instance's
 // directions dims[1] + s (params == true); or, with jv, the m columns J V of the tangent-seeded instance
 static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
@@ -881,19 +913,8 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   ParMap pmv = s->par;
   pmv.values = s->par_dev; pmv.grad = nullptr;
   const ParMap* pm = s->par.n > 0 ? &pmv : nullptr;
-  const size_t warps = (size_t)(s->n + 31) / 32;
-  const size_t per_dir = warps * (size_t)s->dm_ad.x_total * 32 * 4;
-  const size_t cap = (size_t)2 << 30;                       // scratch bound: directions are processed in chunks
-  int chunk = (int)(cap / per_dir);
-  if (chunk < 1) chunk = 1;
-  if (chunk > n_dirs) chunk = n_dirs;
-  if (chunk > 65535) chunk = 65535;                          // (gridDim.y)
-  if (per_dir * chunk > s->jac_scratch_bytes) {
-    if (s->jac_scratch) cudaFree(s->jac_scratch);
-    s->jac_scratch = nullptr; s->jac_scratch_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->jac_scratch, per_dir * chunk));
-    s->jac_scratch_bytes = per_dir * chunk;
-  }
+  const int chunk = std::min(dir_chunk(s), n_dirs);
+  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_ad) * chunk));
   for (int d0 = 0; d0 < n_dirs; d0 += chunk) {
     io.jac_dir0 = dir_base + d0;
     const int nd = n_dirs - d0 < chunk ? n_dirs - d0 : chunk;
@@ -909,12 +930,7 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
 }
 
 // diagnostics of the chunking above: how many directions (Jacobian columns or tangents) one launch takes for this simulator
-int tds_b200_jacobian_chunk(const tds_b200_sim* s) {
-  if (!s) return -1;
-  const size_t per_dir = (size_t)(s->n + 31) / 32 * (size_t)s->dm_ad.x_total * 32 * 4;
-  const size_t chunk = ((size_t)2 << 30) / per_dir;
-  return (int)(chunk < 1 ? 1 : (chunk > 65535 ? 65535 : chunk));
-}
+int tds_b200_jacobian_chunk(const tds_b200_sim* s) { return s ? dir_chunk(s) : -1; }
 
 static int jacobian_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* jac, bool params) {
   if (!s || !q || !qd || !jac) return -1;
@@ -939,46 +955,16 @@ int tds_b200_step_param_jacobian_device(tds_b200_sim* s, int mode, int use_pd, c
 static int jacobian_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
                          const double* tau_or_action, double* jac, bool params) {
   if (int rc = jacobian_check(s, mode, use_pd, q, qd, jac, params)) return rc;
-  CUDA_TRY(cudaSetDevice(s->device));
-  const DevModel& M = s->dm[0];
-  const int n = s->n, ns = s->ns;
+  if (int rc = enter_derivative_host(s)) return rc;
   int dims[2];
   tds_b200_jacobian_dims(s, mode, use_pd, dims);
   if (params) dims[1] = s->par.n;
-  const int n_in = use_pd ? s->E.n_act : s->n_tau;
-  const size_t maxdim = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + 1;
-  int rc = ensure_stage(s, sizeof(double) * n * maxdim, 0);
-  if (rc) return rc;
-  const size_t jb = sizeof(double) * (size_t)dims[0] * dims[1] * ns;
-  if (jb > s->jac_dev_bytes) {
-    if (s->jac_dev) cudaFree(s->jac_dev);
-    s->jac_dev = nullptr; s->jac_dev_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->jac_dev, jb));
-    s->jac_dev_bytes = jb;
-  }
-  double* st = (double*)s->stage_dev;
-  const int T = 128, B = (n + T - 1) / T;
-  cudaStream_t sm = s->stream;
-  auto up = [&](const double* src, int dim, float* dst) -> int {
-    if (dim == 0) return 0;
-    CUDA_TRY(cudaMemcpyAsync(st, src, sizeof(double) * n * dim, cudaMemcpyHostToDevice, sm));
-    aos_to_soa_kernel<double><<<B, T, 0, sm>>>(st, dim, 0, dst, dim, n, ns);
-    return 0;
-  };
-  if ((rc = up(q, M.n_q, s->q))) return rc;
-  if ((rc = up(qd, M.n_qd, s->qd))) return rc;
-  if (tau_or_action) { if ((rc = up(tau_or_action, n_in, s->act))) return rc; }
-  else CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * ns * (n_in > 0 ? n_in : 1), sm));
-  CUDA_TRY(cudaMemsetAsync(s->jac_dev, 0, jb, sm));
-  rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, s->jac_dev, sm, params);
-  if (rc) return rc;
-  std::vector<double> tmp((size_t)dims[0] * dims[1] * ns);
-  CUDA_TRY(cudaMemcpyAsync(tmp.data(), s->jac_dev, jb, cudaMemcpyDeviceToHost, sm));
-  CUDA_TRY(cudaStreamSynchronize(sm));
-  CUDA_TRY(cudaGetLastError());
-  const size_t rc_n = (size_t)dims[0] * dims[1];
-  for (int e = 0; e < n; ++e)
-    for (size_t k = 0; k < rc_n; ++k) jac[(size_t)e * rc_n + k] = tmp[k * ns + e];
+  const size_t rows = (size_t)dims[0] * dims[1];
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * rows * s->ns));
+  if (int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action)) return rc;
+  CUDA_TRY(cudaMemsetAsync(s->jac_dev, 0, sizeof(double) * rows * s->ns, s->stream));
+  if (int rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, s->jac_dev, s->stream, params)) return rc;
+  CUDA_TRY(get_rows(jac, s->jac_dev, rows, s->n, s->ns, s->stream));
   return 0;
 }
 
@@ -1013,73 +999,27 @@ int tds_b200_step_jvp_device(tds_b200_sim* s, int mode, int use_pd, const float*
 int tds_b200_step_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
                            int m, const double* t_in, const double* t_par, double* t_out) {
   if (int rc = jvp_check(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out)) return rc;
-  CUDA_TRY(cudaSetDevice(s->device));
-  const DevModel& M = s->dm[0];
+  if (int rc = enter_derivative_host(s)) return rc;
   const int n = s->n, ns = s->ns, k = s->par.n;
   int dims[2];
   tds_b200_jacobian_dims(s, mode, use_pd, dims);
-  const int n_in = use_pd ? s->E.n_act : s->n_tau;
-  const size_t maxdim = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + 1;
-  int rc = ensure_stage(s, sizeof(double) * n * maxdim, 0);
-  if (rc) return rc;
-  const size_t ti = (size_t)dims[1] * m * ns, tp = (size_t)(t_par ? k : 0) * m * ns, to = (size_t)dims[0] * m * ns;
-  if (sizeof(double) * (ti + tp + to) > s->jvp_dev_bytes) {
-    if (s->jvp_dev) cudaFree(s->jvp_dev);
-    s->jvp_dev = nullptr; s->jvp_dev_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->jvp_dev, sizeof(double) * (ti + tp + to)));
-    s->jvp_dev_bytes = sizeof(double) * (ti + tp + to);
-  }
-  double* st = (double*)s->stage_dev;
-  const int T = 128, B = (n + T - 1) / T;
-  cudaStream_t sm = s->stream;
-  auto up = [&](const double* src, int dim, float* dst) -> int {
-    if (dim == 0) return 0;
-    CUDA_TRY(cudaMemcpyAsync(st, src, sizeof(double) * n * dim, cudaMemcpyHostToDevice, sm));
-    aos_to_soa_kernel<double><<<B, T, 0, sm>>>(st, dim, 0, dst, dim, n, ns);
-    return 0;
-  };
-  if ((rc = up(q, M.n_q, s->q))) return rc;
-  if ((rc = up(qd, M.n_qd, s->qd))) return rc;
-  if (tau_or_action) { if ((rc = up(tau_or_action, n_in, s->act))) return rc; }
-  else CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * ns * (n_in > 0 ? n_in : 1), sm));
-  // tangents: host [n][dim][m] -> device [dim * m][ns]
-  std::vector<double> tmp(std::max(std::max(ti, tp), to), 0.0);
-  auto up_t = [&](const double* src, int dim, double* dst) -> int {
-    const size_t w = (size_t)dim * m;
-    std::fill(tmp.begin(), tmp.end(), 0.0);
-    for (int e = 0; e < n; ++e) for (size_t c = 0; c < w; ++c) tmp[c * ns + e] = src[(size_t)e * w + c];
-    CUDA_TRY(cudaMemcpyAsync(dst, tmp.data(), sizeof(double) * w * ns, cudaMemcpyHostToDevice, sm));
-    CUDA_TRY(cudaStreamSynchronize(sm));   // (tmp is reused)
-    return 0;
-  };
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]
+  const size_t ti = (size_t)dims[1] * m, tp = (size_t)(t_par ? k : 0) * m, to = (size_t)dims[0] * m;
+  CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (ti + tp + to) * ns));
+  if (int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action)) return rc;
   double* tin_d = t_in ? s->jvp_dev : nullptr;
-  double* tpar_d = t_par ? s->jvp_dev + ti : nullptr;
-  double* tout_d = s->jvp_dev + ti + tp;
-  if (t_in && (rc = up_t(t_in, dims[1], tin_d))) return rc;
-  if (t_par && (rc = up_t(t_par, k, tpar_d))) return rc;
-  CUDA_TRY(cudaMemsetAsync(tout_d, 0, sizeof(double) * to, sm));
+  double* tpar_d = t_par ? s->jvp_dev + ti * ns : nullptr;
+  double* tout_d = s->jvp_dev + (ti + tp) * ns;
+  if (t_in) CUDA_TRY(put_rows(tin_d, t_in, ti, n, ns, s->stream));
+  if (t_par) CUDA_TRY(put_rows(tpar_d, t_par, tp, n, ns, s->stream));
+  CUDA_TRY(cudaMemsetAsync(tout_d, 0, sizeof(double) * to * ns, s->stream));
   const JvpTangents jv{tin_d, tpar_d, m};
-  rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, tout_d, sm, false, &jv);
-  if (rc) return rc;
-  CUDA_TRY(cudaMemcpyAsync(tmp.data(), tout_d, sizeof(double) * to, cudaMemcpyDeviceToHost, sm));
-  CUDA_TRY(cudaStreamSynchronize(sm));
-  CUDA_TRY(cudaGetLastError());
-  const size_t w = (size_t)dims[0] * m;
-  for (int e = 0; e < n; ++e)
-    for (size_t c = 0; c < w; ++c) t_out[(size_t)e * w + c] = tmp[c * ns + e];
+  if (int rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, tout_d, s->stream, false, &jv)) return rc;
+  CUDA_TRY(get_rows(t_out, tout_d, to, n, ns, s->stream));
   return 0;
 }
 
 // ---- joint-space mass matrix M(q) (DESIGN.md section 7.12): the MASS instances of the world-frame kernel (tds_mass.cu) ------------------
-static int grow_dev(double** p, size_t* have, size_t bytes) {
-  if (bytes <= *have) return 0;
-  if (*p) cudaFree(*p);
-  *p = nullptr; *have = 0;
-  CUDA_TRY(cudaMalloc((void**)p, bytes));
-  *have = bytes;
-  return 0;
-}
-
 // M [n_qd * n_qd][ns] from q [n_q][ns] fp32, one lane per environment on the 8-byte layout
 static int mass_run(tds_b200_sim* s, const float* q, double* Mo, cudaStream_t sm) {
   StepIO io;
@@ -1088,13 +1028,7 @@ static int mass_run(tds_b200_sim* s, const float* q, double* Mo, cudaStream_t sm
   io.n = s->n; io.n_stride = s->ns;
   ParMap pmv = s->par;
   pmv.values = s->par_dev; pmv.grad = nullptr;
-  const size_t need = (size_t)(s->n + 31) / 32 * (size_t)s->dm_m.x_total * 32 * 4;
-  if (need > s->jac_scratch_bytes) {
-    if (s->jac_scratch) cudaFree(s->jac_scratch);
-    s->jac_scratch = nullptr; s->jac_scratch_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->jac_scratch, need));
-    s->jac_scratch_bytes = need;
-  }
+  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_m)));
   const int rc = tds_launch_mass(&s->dm_m, &io, s->par.n > 0 ? &pmv : nullptr, s->jac_scratch, sm);
   if (rc) set_err(std::string("mass matrix launch: ") + cudaGetErrorString((cudaError_t)rc));
   return rc;
@@ -1116,7 +1050,7 @@ static int mass_vjp_run(tds_b200_sim* s, const float* q, const double* G, double
   int chunk = (int)(((size_t)1 << 30) / per_dir);
   if (chunk < 1) chunk = 1;
   if (chunk > total) chunk = total;
-  if (int rc = grow_dev(&s->mass_dev, &s->mass_dev_bytes, per_dir * chunk)) return rc;
+  CUDA_TRY(grow_dev(&s->mass_dev, &s->mass_dev_bytes, per_dir * chunk));
   for (int d0 = 0; d0 < total; d0 += chunk) {
     const int nd = total - d0 < chunk ? total - d0 : chunk;
     double* tq = s->mass_dev;
@@ -1130,27 +1064,6 @@ static int mass_vjp_run(tds_b200_sim* s, const float* q, const double* G, double
   return 0;
 }
 
-// q [n][n_q] fp64 host -> s->q [n_q][ns] fp32 on the simulator's stream
-static int mass_upload_q(tds_b200_sim* s, const double* q) {
-  const int n = s->n, n_q = s->dm[0].n_q;
-  if (int rc = ensure_stage(s, sizeof(double) * n * (n_q + 1), 0)) return rc;
-  if (n_q == 0) return 0;
-  CUDA_TRY(cudaMemcpyAsync(s->stage_dev, q, sizeof(double) * n * n_q, cudaMemcpyHostToDevice, s->stream));
-  aos_to_soa_kernel<double><<<(n + 127) / 128, 128, 0, s->stream>>>((double*)s->stage_dev, n_q, 0, s->q, n_q, n, s->ns);
-  return 0;
-}
-
-// device [rows][ns] -> host [n][rows]
-static int mass_download(tds_b200_sim* s, const double* src, size_t rows, double* dst) {
-  std::vector<double> tmp(rows * s->ns);
-  CUDA_TRY(cudaMemcpyAsync(tmp.data(), src, sizeof(double) * rows * s->ns, cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  CUDA_TRY(cudaGetLastError());
-  for (int e = 0; e < s->n; ++e)
-    for (size_t r = 0; r < rows; ++r) dst[(size_t)e * rows + r] = tmp[r * s->ns + e];
-  return 0;
-}
-
 int tds_b200_mass_matrix_device(tds_b200_sim* s, const float* q, double* M, void* stream) {
   if (!s || !q || !M) return -1;
   return mass_run(s, q, M, (cudaStream_t)stream);
@@ -1158,13 +1071,13 @@ int tds_b200_mass_matrix_device(tds_b200_sim* s, const float* q, double* M, void
 
 int tds_b200_mass_matrix_host(tds_b200_sim* s, const double* q, double* M) {
   if (!s || !q || !M) return -1;
-  CUDA_TRY(cudaSetDevice(s->device));
+  if (int rc = enter_derivative_host(s)) return rc;
   const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
-  int rc = mass_upload_q(s, q);
-  if (!rc) rc = grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * nn * s->ns);
-  if (!rc) rc = mass_run(s, s->q, s->jac_dev, s->stream);
-  if (!rc) rc = mass_download(s, s->jac_dev, nn, M);
-  return rc;
+  if (int rc = put_q(s, q)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * nn * s->ns));
+  if (int rc = mass_run(s, s->q, s->jac_dev, s->stream)) return rc;
+  CUDA_TRY(get_rows(M, s->jac_dev, nn, s->n, s->ns, s->stream));
+  return 0;
 }
 
 static int mass_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_par, const void* t_M) {
@@ -1182,31 +1095,23 @@ int tds_b200_mass_matrix_jvp_device(tds_b200_sim* s, const float* q, int m, cons
 int tds_b200_mass_matrix_jvp_host(tds_b200_sim* s, const double* q, int m, const double* t_q, const double* t_par, double* M,
                                   double* t_M) {
   if (int rc = mass_jvp_check(s, q, m, t_q, t_par, t_M)) return rc;
-  CUDA_TRY(cudaSetDevice(s->device));
+  if (int rc = enter_derivative_host(s)) return rc;
   const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, k = s->par.n;
   const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
-  const size_t tq = (size_t)n_q * m * ns, tp = (size_t)(t_par ? k : 0) * m * ns, to = nn * m * ns;
-  int rc = mass_upload_q(s, q);
-  if (!rc) rc = grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (tq + tp + to + nn * ns));
-  if (rc) return rc;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]
+  const size_t tq = (size_t)n_q * m, tp = (size_t)(t_par ? k : 0) * m, to = nn * m;
+  if (int rc = put_q(s, q)) return rc;
+  CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (tq + tp + to + nn) * ns));
   double* tq_d = t_q ? s->jvp_dev : nullptr;
-  double* tp_d = t_par ? s->jvp_dev + tq : nullptr;
-  double* to_d = s->jvp_dev + tq + tp;
-  double* M_d = M ? to_d + to : nullptr;
-  // tangents: host [n][dim][m] -> device [dim * m][ns]
-  auto up_t = [&](const double* src, int dim, double* dst) -> int {
-    const size_t w = (size_t)dim * m;
-    std::vector<double> tmp(w * ns, 0.0);
-    for (int e = 0; e < n; ++e) for (size_t c = 0; c < w; ++c) tmp[c * ns + e] = src[(size_t)e * w + c];
-    CUDA_TRY(cudaMemcpyAsync(dst, tmp.data(), sizeof(double) * w * ns, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaStreamSynchronize(s->stream));   // (tmp is released)
-    return 0;
-  };
-  if (t_q && n_q && (rc = up_t(t_q, n_q, tq_d))) return rc;
-  if (t_par && (rc = up_t(t_par, k, tp_d))) return rc;
-  if ((rc = mass_jvp_run(s, s->q, m, tq_d, tp_d, M_d, to_d, s->stream))) return rc;
-  if ((rc = mass_download(s, to_d, nn * m, t_M))) return rc;
-  return M ? mass_download(s, M_d, nn, M) : 0;
+  double* tp_d = t_par ? s->jvp_dev + tq * ns : nullptr;
+  double* to_d = s->jvp_dev + (tq + tp) * ns;
+  double* M_d = M ? to_d + to * ns : nullptr;
+  if (t_q) CUDA_TRY(put_rows(tq_d, t_q, tq, n, ns, s->stream));
+  if (t_par) CUDA_TRY(put_rows(tp_d, t_par, tp, n, ns, s->stream));
+  if (int rc = mass_jvp_run(s, s->q, m, tq_d, tp_d, M_d, to_d, s->stream)) return rc;
+  CUDA_TRY(get_rows(t_M, to_d, to, n, ns, s->stream));
+  if (M) CUDA_TRY(get_rows(M, M_d, nn, n, ns, s->stream));
+  return 0;
 }
 
 static int mass_vjp_check(tds_b200_sim* s, const void* q, const void* G, const void* g_q, const void* g_par) {
@@ -1222,24 +1127,18 @@ int tds_b200_mass_matrix_vjp_device(tds_b200_sim* s, const float* q, const doubl
 
 int tds_b200_mass_matrix_vjp_host(tds_b200_sim* s, const double* q, const double* G, double* g_q, double* g_par) {
   if (int rc = mass_vjp_check(s, q, G, g_q, g_par)) return rc;
-  CUDA_TRY(cudaSetDevice(s->device));
+  if (int rc = enter_derivative_host(s)) return rc;
   const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, k = s->par.n;
   const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
-  int rc = mass_upload_q(s, q);
-  if (!rc) rc = grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (nn + n_q + k + 1) * ns);
-  if (rc) return rc;
+  if (int rc = put_q(s, q)) return rc;
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (nn + n_q + k + 1) * ns));
   double* G_d = s->vjp_g;
   double* gq_d = G_d + nn * ns;
   double* gp_d = gq_d + (size_t)n_q * ns;
-  {
-    std::vector<double> tmp(nn * ns, 0.0);
-    for (int e = 0; e < n; ++e) for (size_t r = 0; r < nn; ++r) tmp[r * ns + e] = G[(size_t)e * nn + r];
-    CUDA_TRY(cudaMemcpyAsync(G_d, tmp.data(), sizeof(double) * nn * ns, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaStreamSynchronize(s->stream));
-  }
-  if ((rc = mass_vjp_run(s, s->q, G_d, g_q ? gq_d : nullptr, g_par ? gp_d : nullptr, s->stream))) return rc;
-  if (g_q && n_q && (rc = mass_download(s, gq_d, n_q, g_q))) return rc;
-  if (g_par && (rc = mass_download(s, gp_d, k, g_par))) return rc;
+  CUDA_TRY(put_rows(G_d, G, nn, n, ns, s->stream));
+  if (int rc = mass_vjp_run(s, s->q, G_d, g_q ? gq_d : nullptr, g_par ? gp_d : nullptr, s->stream)) return rc;
+  if (g_q) CUDA_TRY(get_rows(g_q, gq_d, n_q, n, ns, s->stream));
+  if (g_par) CUDA_TRY(get_rows(g_par, gp_d, k, n, ns, s->stream));
   return 0;
 }
 
@@ -1265,13 +1164,7 @@ static int kin_run(tds_b200_sim* s, const float* q, const TdsKinCall* kc, cudaSt
   memset(&io, 0, sizeof(io));
   io.q_in = q; io.jac_n_in = 1;
   io.n = s->n; io.n_stride = s->ns;
-  const size_t need = (size_t)(s->n + 31) / 32 * (size_t)s->dm_m.x_total * 32 * 4;
-  if (need > s->jac_scratch_bytes) {
-    if (s->jac_scratch) cudaFree(s->jac_scratch);
-    s->jac_scratch = nullptr; s->jac_scratch_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->jac_scratch, need));
-    s->jac_scratch_bytes = need;
-  }
+  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_m)));
   const int rc = tds_launch_kin(&s->dm_m, &io, kc, s->jac_scratch, sm);
   if (rc) set_err(std::string("kinematics launch: ") + cudaGetErrorString((cudaError_t)rc));
   return rc;
@@ -1311,7 +1204,7 @@ static int kin_vjp_buffers(tds_b200_sim* s, int K, double** G, double** buf, int
   if (c < 1) c = 1;
   if (c > n_q) c = n_q;
   if (c < 1) c = 1;
-  if (int rc = grow_dev(&s->mass_dev, &s->mass_dev_bytes, sizeof(double) * rows * ns + per_dir * c)) return rc;
+  CUDA_TRY(grow_dev(&s->mass_dev, &s->mass_dev_bytes, sizeof(double) * rows * ns + per_dir * c));
   *G = s->mass_dev;
   *buf = s->mass_dev + rows * ns;
   *chunk = c;
@@ -1330,18 +1223,17 @@ int tds_b200_kinematics_host(tds_b200_sim* s, const double* q, int K, const int*
                              double* J) {
   if (int rc = kin_check(s, q, K, links, local)) return rc;
   if (!xf && !x && !J) return -1;
-  CUDA_TRY(cudaSetDevice(s->device));
+  if (int rc = enter_derivative_host(s)) return rc;
   const KinRows R = kin_rows(s, K);
-  const size_t ns = s->ns;
-  int rc = mass_upload_q(s, q);
-  if (!rc) rc = grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (R.all() + 1) * ns);
-  if (rc) return rc;
+  const int n = s->n, ns = s->ns;
+  if (int rc = put_q(s, q)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (R.all() + 1) * ns));
   double* d = s->jac_dev;
   const TdsKinCall kc{K, links, local, xf ? d : nullptr, x ? d + R.xf * ns : nullptr, J ? d + (R.xf + R.x) * ns : nullptr};
-  if ((rc = kin_run(s, s->q, &kc, s->stream))) return rc;
-  if (xf && (rc = mass_download(s, kc.xf, R.xf, xf))) return rc;
-  if (x && R.x && (rc = mass_download(s, kc.x, R.x, x))) return rc;
-  if (J && R.J && (rc = mass_download(s, kc.J, R.J, J))) return rc;
+  if (int rc = kin_run(s, s->q, &kc, s->stream)) return rc;
+  if (xf) CUDA_TRY(get_rows(xf, kc.xf, R.xf, n, ns, s->stream));
+  if (x) CUDA_TRY(get_rows(x, kc.x, R.x, n, ns, s->stream));
+  if (J) CUDA_TRY(get_rows(J, kc.J, R.J, n, ns, s->stream));
   return 0;
 }
 
@@ -1362,28 +1254,22 @@ int tds_b200_kinematics_jvp_device(tds_b200_sim* s, const float* q, int K, const
 int tds_b200_kinematics_jvp_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, int m,
                                  const double* t_q, double* t_xf, double* t_x, double* t_J) {
   if (int rc = kin_jvp_check(s, q, K, links, local, m, t_q, t_xf, t_x, t_J)) return rc;
-  CUDA_TRY(cudaSetDevice(s->device));
+  if (int rc = enter_derivative_host(s)) return rc;
   const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q;
   const KinRows R = kin_rows(s, K);
+  // tangents: host [n][rows][m] <-> device [rows * m][ns]
   const size_t tq = (size_t)n_q * m * ns, to = R.all() * m * ns;
-  int rc = mass_upload_q(s, q);
-  if (!rc) rc = grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (tq + to + 1));
-  if (rc) return rc;
+  if (int rc = put_q(s, q)) return rc;
+  CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (tq + to + 1)));
   double* tq_d = s->jvp_dev;
   double* to_d = s->jvp_dev + tq;
-  if (n_q) {   // tangents: host [n][n_q][m] -> device [n_q * m][ns]
-    const size_t w = (size_t)n_q * m;
-    std::vector<double> tmp(w * ns, 0.0);
-    for (int e = 0; e < n; ++e) for (size_t c = 0; c < w; ++c) tmp[c * ns + e] = t_q[(size_t)e * w + c];
-    CUDA_TRY(cudaMemcpyAsync(tq_d, tmp.data(), sizeof(double) * w * ns, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaStreamSynchronize(s->stream));
-  }
+  CUDA_TRY(put_rows(tq_d, t_q, (size_t)n_q * m, n, ns, s->stream));
   const TdsKinCall kc{K, links, local, t_xf ? to_d : nullptr, t_x ? to_d + R.xf * m * ns : nullptr,
                       t_J ? to_d + (R.xf + R.x) * m * ns : nullptr};
-  if ((rc = kin_jvp_run(s, s->q, &kc, m, tq_d, s->stream))) return rc;
-  if (t_xf && (rc = mass_download(s, kc.xf, R.xf * m, t_xf))) return rc;
-  if (t_x && R.x && (rc = mass_download(s, kc.x, R.x * m, t_x))) return rc;
-  if (t_J && R.J && (rc = mass_download(s, kc.J, R.J * m, t_J))) return rc;
+  if (int rc = kin_jvp_run(s, s->q, &kc, m, tq_d, s->stream)) return rc;
+  if (t_xf) CUDA_TRY(get_rows(t_xf, kc.xf, R.xf * m, n, ns, s->stream));
+  if (t_x) CUDA_TRY(get_rows(t_x, kc.x, R.x * m, n, ns, s->stream));
+  if (t_J) CUDA_TRY(get_rows(t_J, kc.J, R.J * m, n, ns, s->stream));
   return 0;
 }
 
@@ -1415,27 +1301,24 @@ int tds_b200_kinematics_vjp_device(tds_b200_sim* s, const float* q, int K, const
 int tds_b200_kinematics_vjp_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, const double* G_xf,
                                  const double* G_x, const double* G_J, double* g_q) {
   if (int rc = kin_vjp_check(s, q, K, links, local, G_xf, G_x, G_J, g_q)) return rc;
-  CUDA_TRY(cudaSetDevice(s->device));
+  if (int rc = enter_derivative_host(s)) return rc;
   const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q;
   if (n_q == 0) return 0;
   const KinRows R = kin_rows(s, K);
   double *G, *buf;
   int chunk;
-  int rc = mass_upload_q(s, q);
-  if (!rc) rc = kin_vjp_buffers(s, K, &G, &buf, &chunk);
-  if (!rc) rc = grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)n_q * ns);
-  if (rc) return rc;
-  {  // cotangents: host [n][rows of the part] -> device [rows][ns], concatenated
-    std::vector<double> tmp(R.all() * ns, 0.0);
-    auto put = [&](const double* src, size_t rows, size_t r0) {
-      if (src) for (int e = 0; e < n; ++e) for (size_t r = 0; r < rows; ++r) tmp[(r0 + r) * ns + e] = src[(size_t)e * rows + r];
-    };
-    put(G_xf, R.xf, 0); put(G_x, R.x, R.xf); put(G_J, R.J, R.xf + R.x);
-    CUDA_TRY(cudaMemcpyAsync(G, tmp.data(), sizeof(double) * R.all() * ns, cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaStreamSynchronize(s->stream));
-  }
-  if ((rc = kin_vjp_run(s, s->q, K, links, local, G, s->vjp_g, buf, chunk, s->stream))) return rc;
-  return mass_download(s, s->vjp_g, n_q, g_q);
+  if (int rc = put_q(s, q)) return rc;
+  if (int rc = kin_vjp_buffers(s, K, &G, &buf, &chunk)) return rc;
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)n_q * ns));
+  // the concatenated cotangent xf | x | J, zero where a part is NULL; every row is written once, with its final value
+  const double* parts[3] = {G_xf, G_x, G_J};
+  const size_t rows[3] = {R.xf, R.x, R.J};
+  double* d = G;
+  for (int i = 0; i < 3; d += rows[i] * ns, ++i)
+    CUDA_TRY(parts[i] ? put_rows(d, parts[i], rows[i], n, ns, s->stream) : cudaMemsetAsync(d, 0, sizeof(double) * rows[i] * ns, s->stream));
+  if (int rc = kin_vjp_run(s, s->q, K, links, local, G, s->vjp_g, buf, chunk, s->stream)) return rc;
+  CUDA_TRY(get_rows(g_q, s->vjp_g, n_q, n, ns, s->stream));
+  return 0;
 }
 
 // ---- vector-Jacobian product: g_in = g_out^T d(q', qd' | qdd) / d(q | qd | tau or action (| kp, kd, max_force)) by the taping
@@ -1449,6 +1332,14 @@ static int vjp_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const
   return 0;
 }
 
+// warps of environments one launch of the taping instance takes at the current tape capacity: arena + tape + adjoints within 2 GB
+static size_t tape_warps(const tds_b200_sim* s) {
+  const size_t arena_warp = (size_t)s->dm_ad.x_total * 32 * 4;
+  const size_t lane_bytes = (size_t)s->tape_cap * (sizeof(tds::TapeNode) + sizeof(double));
+  const size_t warps = ((size_t)2 << 30) / (arena_warp + 32 * lane_bytes);
+  return warps < 1 ? 1 : warps;
+}
+
 // g_in (may be null while parameters are installed) and g_par [k][ns] (or null); every pointer is offset per chunk of environments
 static int vjp_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
                    const double* g_out, double* g_in, double* g_par, void* stream) {
@@ -1456,25 +1347,17 @@ static int vjp_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const 
   const ParMap* pm = s->par.n > 0 ? &pmv : nullptr;
   cudaStream_t sm = (cudaStream_t)stream;
   const size_t arena_warp = (size_t)s->dm_ad.x_total * 32 * 4;
-  const size_t cap_bytes = (size_t)2 << 30;
   if (!s->vjp_flag) CUDA_TRY(cudaMalloc((void**)&s->vjp_flag, sizeof(int)));
   const int n = s->n, ns = s->ns;
   for (int e0 = 0; e0 < n;) {
-    const size_t lane_bytes = (size_t)s->tape_cap * (sizeof(tds::TapeNode) + sizeof(double));
-    size_t warps = cap_bytes / (arena_warp + 32 * lane_bytes);
-    if (warps < 1) warps = 1;
+    size_t warps = tape_warps(s);
     const size_t left = (size_t)(n - e0 + 31) / 32;
     if (warps > left) warps = left;
     const int chunk = (int)(warps * 32 < (size_t)(n - e0) ? warps * 32 : (size_t)(n - e0));
     const size_t tape_b = warps * 32 * s->tape_cap * sizeof(tds::TapeNode), adj_b = warps * 32 * s->tape_cap * sizeof(double);
     const size_t need = warps * arena_warp + tape_b + adj_b;
-    if (need > s->vjp_buf_bytes) {
-      CUDA_TRY(cudaStreamSynchronize(sm));
-      if (s->vjp_buf) cudaFree(s->vjp_buf);
-      s->vjp_buf = nullptr; s->vjp_buf_bytes = 0;
-      CUDA_TRY(cudaMalloc((void**)&s->vjp_buf, need));
-      s->vjp_buf_bytes = need;
-    }
+    if (need > s->vjp_buf_bytes) CUDA_TRY(cudaStreamSynchronize(sm));   // (earlier chunks still use the buffer)
+    CUDA_TRY(grow_dev(&s->vjp_buf, &s->vjp_buf_bytes, need));
     StepIO io;
     memset(&io, 0, sizeof(io));
     io.q_in = q + e0; io.qd_in = qd + e0; io.tau_in = tau_or_action ? tau_or_action + e0 : nullptr;   // [dim][ns]: column offset
@@ -1516,57 +1399,20 @@ int tds_b200_step_vjp_params_device(tds_b200_sim* s, int mode, int use_pd, const
 
 static int vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd,
                     const double* tau_or_action, const double* g_out, double* g_in, double* g_par) {
-  CUDA_TRY(cudaSetDevice(s->device));
-  const DevModel& M = s->dm[0];
-  const int n = s->n, ns = s->ns;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, n_par = g_par ? s->par.n : 0;
   int dims[2];
   tds_b200_jacobian_dims(s, mode, use_pd, dims);
-  const int n_in = use_pd ? s->E.n_act : s->n_tau;
-  const size_t maxdim = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + 1;
-  int rc = ensure_stage(s, sizeof(double) * n * maxdim, 0);
-  if (rc) return rc;
-  const int n_par = g_par ? s->par.n : 0;
-  const size_t gb = sizeof(double) * (size_t)(dims[0] + dims[1] + n_par) * ns;
-  if (gb > s->vjp_g_bytes) {
-    if (s->vjp_g) cudaFree(s->vjp_g);
-    s->vjp_g = nullptr; s->vjp_g_bytes = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->vjp_g, gb));
-    s->vjp_g_bytes = gb;
-  }
-  double* st = (double*)s->stage_dev;
-  const int T = 128, B = (n + T - 1) / T;
-  cudaStream_t sm = s->stream;
-  auto up = [&](const double* src, int dim, float* dst) -> int {
-    if (dim == 0) return 0;
-    CUDA_TRY(cudaMemcpyAsync(st, src, sizeof(double) * n * dim, cudaMemcpyHostToDevice, sm));
-    aos_to_soa_kernel<double><<<B, T, 0, sm>>>(st, dim, 0, dst, dim, n, ns);
-    return 0;
-  };
-  if ((rc = up(q, M.n_q, s->q))) return rc;
-  if ((rc = up(qd, M.n_qd, s->qd))) return rc;
-  if (tau_or_action) { if ((rc = up(tau_or_action, n_in, s->act))) return rc; }
-  else CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * ns * (n_in > 0 ? n_in : 1), sm));
-  std::vector<double> tmp((size_t)std::max(std::max(dims[0], dims[1]), n_par) * ns, 0.0);
-  for (int e = 0; e < n; ++e)
-    for (int k = 0; k < dims[0]; ++k) tmp[(size_t)k * ns + e] = g_out[(size_t)e * dims[0] + k];
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)(dims[0] + dims[1] + n_par) * ns));
+  if (int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action)) return rc;
   double* gout_d = s->vjp_g;
   double* gin_d = s->vjp_g + (size_t)dims[0] * ns;
   double* gpar_d = g_par ? s->vjp_g + (size_t)(dims[0] + dims[1]) * ns : nullptr;
-  CUDA_TRY(cudaMemcpyAsync(gout_d, tmp.data(), sizeof(double) * dims[0] * ns, cudaMemcpyHostToDevice, sm));
-  CUDA_TRY(cudaMemsetAsync(gin_d, 0, sizeof(double) * (dims[1] + n_par) * ns, sm));
-  rc = vjp_run(s, mode, use_pd, s->q, s->qd, s->act, gout_d, g_in ? gin_d : nullptr, gpar_d, sm);
-  if (rc) return rc;
-  auto down = [&](const double* src, int dim, double* dst) -> int {
-    if (!dst) return 0;
-    CUDA_TRY(cudaMemcpyAsync(tmp.data(), src, sizeof(double) * dim * ns, cudaMemcpyDeviceToHost, sm));
-    CUDA_TRY(cudaStreamSynchronize(sm));
-    for (int e = 0; e < n; ++e)
-      for (int j = 0; j < dim; ++j) dst[(size_t)e * dim + j] = tmp[(size_t)j * ns + e];
-    return 0;
-  };
-  if ((rc = down(gin_d, dims[1], g_in))) return rc;
-  if ((rc = down(gpar_d, n_par, g_par))) return rc;
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(put_rows(gout_d, g_out, dims[0], n, ns, s->stream));
+  CUDA_TRY(cudaMemsetAsync(gin_d, 0, sizeof(double) * (dims[1] + n_par) * ns, s->stream));
+  if (int rc = vjp_run(s, mode, use_pd, s->q, s->qd, s->act, gout_d, g_in ? gin_d : nullptr, gpar_d, s->stream)) return rc;
+  if (g_in) CUDA_TRY(get_rows(g_in, gin_d, dims[1], n, ns, s->stream));
+  if (g_par) CUDA_TRY(get_rows(g_par, gpar_d, n_par, n, ns, s->stream));
   return 0;
 }
 
@@ -1587,10 +1433,7 @@ int tds_b200_step_vjp_params_host(tds_b200_sim* s, int mode, int use_pd, const d
 // (a batch larger than that runs in several chunks)
 int tds_b200_vjp_tape_info(const tds_b200_sim* s, int info[2]) {
   if (!s || !info) return -1;
-  const size_t arena_warp = (size_t)s->dm_ad.x_total * 32 * 4;
-  const size_t lane_bytes = (size_t)s->tape_cap * (sizeof(tds::TapeNode) + sizeof(double));
-  size_t warps = ((size_t)2 << 30) / (arena_warp + 32 * lane_bytes);
-  if (warps < 1) warps = 1;
+  const size_t warps = tape_warps(s);
   info[0] = s->tape_cap;
   info[1] = (int)(warps * 32 < (size_t)1 << 30 ? warps * 32 : (size_t)1 << 30);
   return 0;
@@ -1602,39 +1445,15 @@ int tds_b200_step_host(tds_b200_sim* s, int mode, int use_pd, const double* q, c
   if (!s || !q || !qd) return -1;
   CUDA_TRY(cudaSetDevice(s->device));
   const DevModel& M = s->dm[0];
-  const int n = s->n, ns = s->ns;
-  const int n_in = use_pd ? s->E.n_act : s->n_tau;
-  const size_t maxdim = (size_t)(M.n_q > M.n_qd ? M.n_q : M.n_qd) + s->n_points + 1;
-  int rc = ensure_stage(s, sizeof(double) * n * maxdim, 0);
+  int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action);
+  if (!rc) rc = tds_b200_step_device(s, mode, use_pd, s->q, s->qd, s->act, s->q, s->qd, s->qdd, nullptr, nullptr,
+                                     contact_dist ? s->cdist : nullptr, nullptr, s->stream);
+  if (!rc) rc = get_state(s, s->q, M.n_q, q_out);
+  if (!rc) rc = get_state(s, s->qd, M.n_qd, qd_out);
+  if (!rc && mode == TDS_B200_MODE_FD) rc = get_state(s, s->qdd, M.n_qd, qdd_out);
+  if (!rc) rc = get_state(s, s->cdist, s->n_points, contact_dist);
   if (rc) return rc;
-  double* st = (double*)s->stage_dev;
-  const int T = 128, B = (n + T - 1) / T;
-  cudaStream_t sm = s->stream;
-  auto up = [&](const double* src, int dim, float* dst) -> int {
-    if (dim == 0) return 0;
-    CUDA_TRY(cudaMemcpyAsync(st, src, sizeof(double) * n * dim, cudaMemcpyHostToDevice, sm));
-    aos_to_soa_kernel<double><<<B, T, 0, sm>>>(st, dim, 0, dst, dim, n, ns);
-    return 0;
-  };
-  if ((rc = up(q, M.n_q, s->q))) return rc;
-  if ((rc = up(qd, M.n_qd, s->qd))) return rc;
-  if (tau_or_action) { if ((rc = up(tau_or_action, n_in, s->act))) return rc; }
-  else CUDA_TRY(cudaMemsetAsync(s->act, 0, sizeof(float) * ns * (n_in > 0 ? n_in : 1), sm));
-  rc = tds_b200_step_device(s, mode, use_pd, s->q, s->qd, s->act, s->q, s->qd, s->qdd, nullptr, nullptr,
-                            contact_dist ? s->cdist : nullptr, nullptr, sm);
-  if (rc) return rc;
-  auto down = [&](const float* src, int dim, double* dst) -> int {
-    if (dim == 0 || !dst) return 0;
-    soa_to_aos_kernel<double><<<B, T, 0, sm>>>(src, st, dim, 0, dim, n, ns);
-    CUDA_TRY(cudaMemcpyAsync(dst, st, sizeof(double) * n * dim, cudaMemcpyDeviceToHost, sm));
-    CUDA_TRY(cudaStreamSynchronize(sm));
-    return 0;
-  };
-  if ((rc = down(s->q, M.n_q, q_out))) return rc;
-  if ((rc = down(s->qd, M.n_qd, qd_out))) return rc;
-  if (mode == TDS_B200_MODE_FD && (rc = down(s->qdd, M.n_qd, qdd_out))) return rc;
-  if ((rc = down(s->cdist, s->n_points, contact_dist))) return rc;
-  CUDA_TRY(cudaStreamSynchronize(sm));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -1733,19 +1552,11 @@ int tds_b200_contact_list_host(tds_b200_sim* s, int* count, int* links) {
   CUDA_TRY(cudaSetDevice(s->device));
   const int n = s->n, ns = s->ns, np = s->cand.n_points;
   if (np == 0) { for (int e = 0; e < n; ++e) count[e] = 0; return 0; }
-  if (!s->c_count) {
-    CUDA_TRY(cudaMalloc((void**)&s->c_count, sizeof(int) * ns));
-    CUDA_TRY(cudaMalloc((void**)&s->c_links, sizeof(int) * (size_t)ns * 2 * np));
-  }
-  int rc = tds_b200_contact_list_device(s, s->cdist, s->c_count, s->c_links, s->stream);
-  if (rc) return rc;
-  std::vector<int> tmp((size_t)ns * 2 * np);
-  CUDA_TRY(cudaMemcpyAsync(count, s->c_count, sizeof(int) * n, cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(tmp.data(), s->c_links, sizeof(int) * tmp.size(), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  if (links)
-    for (int e = 0; e < n; ++e)
-      for (int k = 0; k < 2 * np; ++k) links[(size_t)e * 2 * np + k] = tmp[(size_t)k * ns + e];
+  CUDA_TRY(grow_dev(&s->c_count, &s->c_count_bytes, sizeof(int) * ns));
+  CUDA_TRY(grow_dev(&s->c_links, &s->c_links_bytes, sizeof(int) * (size_t)ns * 2 * np));
+  if (int rc = tds_b200_contact_list_device(s, s->cdist, s->c_count, s->c_links, s->stream)) return rc;
+  CUDA_TRY(get_rows(count, s->c_count, 1, n, ns, s->stream));
+  if (links) CUDA_TRY(get_rows(links, s->c_links, 2 * np, n, ns, s->stream));
   return 0;
 }
 
@@ -1754,37 +1565,23 @@ int tds_b200_contact_list_candidates_host(tds_b200_sim* s, int* count, int* cand
   CUDA_TRY(cudaSetDevice(s->device));
   const int n = s->n, ns = s->ns, np = s->cand.n_points;
   if (np == 0) { for (int e = 0; e < n; ++e) count[e] = 0; return 0; }
-  if (!s->c_count) {
-    CUDA_TRY(cudaMalloc((void**)&s->c_count, sizeof(int) * ns));
-    CUDA_TRY(cudaMalloc((void**)&s->c_links, sizeof(int) * (size_t)ns * 2 * np));
-  }
-  if (!s->c_cand) CUDA_TRY(cudaMalloc((void**)&s->c_cand, sizeof(int) * (size_t)ns * np));
+  CUDA_TRY(grow_dev(&s->c_count, &s->c_count_bytes, sizeof(int) * ns));
+  CUDA_TRY(grow_dev(&s->c_links, &s->c_links_bytes, sizeof(int) * (size_t)ns * 2 * np));
+  CUDA_TRY(grow_dev(&s->c_cand, &s->c_cand_bytes, sizeof(int) * (size_t)ns * np));
   const int T = 128, B = (n + T - 1) / T;
   contact_list_kernel<<<B, T, 0, s->stream>>>(s->cdist, s->cand, s->P.keep_all_points, s->c_count, s->c_links, s->c_cand, n, ns);
   CUDA_TRY(cudaGetLastError());
-  std::vector<int> tmp((size_t)ns * np);
-  CUDA_TRY(cudaMemcpyAsync(count, s->c_count, sizeof(int) * n, cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(tmp.data(), s->c_cand, sizeof(int) * tmp.size(), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  for (int e = 0; e < n; ++e)
-    for (int k = 0; k < np; ++k) cand[(size_t)e * np + k] = tmp[(size_t)k * ns + e];
+  CUDA_TRY(get_rows(count, s->c_count, 1, n, ns, s->stream));
+  CUDA_TRY(get_rows(cand, s->c_cand, np, n, ns, s->stream));
   return 0;
 }
 
 int tds_b200_env_set_state_host(tds_b200_sim* s, const double* q, const double* qd) {
   if (!s) return -1;
   CUDA_TRY(cudaSetDevice(s->device));
-  const DevModel& M = s->dm[0];
-  const int n = s->n, ns = s->ns;
-  int rc = ensure_stage(s, sizeof(double) * n * (size_t)(M.n_q + M.n_qd), 0);
+  int rc = put_q(s, q);
+  if (!rc) rc = put_state(s, qd, s->dm[0].n_qd, s->qd);
   if (rc) return rc;
-  double* st = (double*)s->stage_dev;
-  const int T = 128, B = (n + T - 1) / T;
-  CUDA_TRY(cudaMemcpyAsync(st, q, sizeof(double) * n * M.n_q, cudaMemcpyHostToDevice, s->stream));
-  aos_to_soa_kernel<double><<<B, T, 0, s->stream>>>(st, M.n_q, 0, s->q, M.n_q, n, ns);
-  double* st2 = st + (size_t)n * M.n_q;
-  CUDA_TRY(cudaMemcpyAsync(st2, qd, sizeof(double) * n * M.n_qd, cudaMemcpyHostToDevice, s->stream));
-  aos_to_soa_kernel<double><<<B, T, 0, s->stream>>>(st2, M.n_qd, 0, s->qd, M.n_qd, n, ns);
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   return 0;
 }
@@ -1792,18 +1589,8 @@ int tds_b200_env_set_state_host(tds_b200_sim* s, const double* q, const double* 
 int tds_b200_env_get_state_host(tds_b200_sim* s, double* q, double* qd) {
   if (!s) return -1;
   CUDA_TRY(cudaSetDevice(s->device));
-  const DevModel& M = s->dm[0];
-  const int n = s->n, ns = s->ns;
-  int rc = ensure_stage(s, sizeof(double) * n * (size_t)(M.n_q + M.n_qd), 0);
-  if (rc) return rc;
-  double* st = (double*)s->stage_dev;
-  const int T = 128, B = (n + T - 1) / T;
-  soa_to_aos_kernel<double><<<B, T, 0, s->stream>>>(s->q, st, M.n_q, 0, M.n_q, n, ns);
-  soa_to_aos_kernel<double><<<B, T, 0, s->stream>>>(s->qd, st + (size_t)n * M.n_q, M.n_qd, 0, M.n_qd, n, ns);
-  if (q) CUDA_TRY(cudaMemcpyAsync(q, st, sizeof(double) * n * M.n_q, cudaMemcpyDeviceToHost, s->stream));
-  if (qd) CUDA_TRY(cudaMemcpyAsync(qd, st + (size_t)n * M.n_q, sizeof(double) * n * M.n_qd, cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  return 0;
+  const int rc = get_state(s, s->q, s->dm[0].n_q, q);
+  return rc ? rc : get_state(s, s->qd, s->dm[0].n_qd, qd);
 }
 
 int tds_b200_env_step_device(tds_b200_sim* s, const float* actions, float* reward, float* done, void* stream) {
@@ -1933,27 +1720,13 @@ int tds_b200_env_rollout_host(tds_b200_sim* s, const double* policy, int n_param
   if (rc) return rc;
   const int n = s->n, ns = s->ns, na = s->E.n_act;
   cudaStream_t sm = s->stream;
-  const int T = 128, B = (n + T - 1) / T;
   const size_t rows = (size_t)n_params > (size_t)na ? (size_t)n_params : (size_t)na;
-  if (rows > s->pol_params_rows) {
-    cudaFree(s->pol_params); s->pol_params = nullptr; s->pol_params_rows = 0;
-    CUDA_TRY(cudaMalloc((void**)&s->pol_params, sizeof(float) * rows * ns));
-    s->pol_params_rows = rows;
-  }
-  rc = ensure_stage(s, sizeof(double) * (size_t)n * rows, 0);
-  if (rc) return rc;
-  double* st = (double*)s->stage_dev;
-  const float* d_noise = nullptr;
-  if (noise) {   // [n][n_act] -> [n_act][ns]
-    CUDA_TRY(cudaMemcpyAsync(st, noise, sizeof(double) * n * na, cudaMemcpyHostToDevice, sm));
-    aos_to_soa_kernel<double><<<B, T, 0, sm>>>(st, na, 0, s->pol_params, na, n, ns);
-    d_noise = s->pol_params;
-  }
-  rc = tds_b200_env_reset_device(s, nullptr, d_noise, (float)noise_amp, seed, settle_steps, sm);
-  if (rc) return rc;
-  CUDA_TRY(cudaMemcpyAsync(st, policy, sizeof(double) * n * n_params, cudaMemcpyHostToDevice, sm));
-  aos_to_soa_kernel<double><<<B, T, 0, sm>>>(st, n_params, 0, s->pol_params, n_params, n, ns);
-  rc = tds_b200_env_rollout_device(s, s->pol_params, n_params, rollout_length, (float)shift, s->r_total, s->r_steps, sm);
+  CUDA_TRY(grow_dev(&s->pol_params, &s->pol_params_bytes, sizeof(float) * rows * ns));
+  rc = ensure_stage(s, sizeof(double) * (size_t)n * rows);
+  if (!rc && noise) rc = put_state(s, noise, na, s->pol_params);   // [n][n_act] -> [n_act][ns]
+  if (!rc) rc = tds_b200_env_reset_device(s, nullptr, noise ? s->pol_params : nullptr, (float)noise_amp, seed, settle_steps, sm);
+  if (!rc) rc = put_state(s, policy, n_params, s->pol_params);
+  if (!rc) rc = tds_b200_env_rollout_device(s, s->pol_params, n_params, rollout_length, (float)shift, s->r_total, s->r_steps, sm);
   if (rc) return rc;
   std::vector<float> tot(n);
   CUDA_TRY(cudaMemcpyAsync(tot.data(), s->r_total, sizeof(float) * n, cudaMemcpyDeviceToHost, sm));
@@ -2002,7 +1775,7 @@ int tds_b200_env_step_host(tds_b200_sim* s, const float* actions, float* obs, fl
   const size_t in_b = sizeof(float) * (size_t)n * na, obs_b = sizeof(float) * (size_t)n * nobs;
   // obs | rewards | dones adjacent in the caller's memory: pack them on the device and copy once
   const bool packed = obs && rewards == obs + (size_t)n * nobs && dones == rewards + n;
-  int rc = ensure_stage(s, in_b + obs_b + sizeof(float) * 2 * (size_t)n, 0);
+  int rc = ensure_stage(s, in_b + obs_b + sizeof(float) * 2 * (size_t)n);
   if (rc) return rc;
   float* d_in = (float*)s->stage_dev;
   float* d_obs = (float*)((char*)s->stage_dev + in_b);

@@ -392,6 +392,8 @@ __global__ void __launch_bounds__(128) tds_rigid_step_kernel(const __grid_consta
 #include <string>
 #include <vector>
 
+#include "tds_host_io.h"
+
 extern "C" void tds_b200_set_error(const char* msg);
 // the PAR instances (csrc/tds_rigid_par.cu)
 extern "C" int tds_launch_rigid_step_par(const RigidWorld* W, const RigidParMap* pm, const double* s_in, double* s_out, const double* force,
@@ -412,13 +414,14 @@ struct tds_b200_rigid {
   double* par_dev = nullptr; size_t par_bytes = 0;
   int n = 0, ns = 0, device = 0;
   double *state = nullptr, *state2 = nullptr, *force = nullptr, *jac = nullptr;   // state2: output of the differentiable instance
+  size_t state2_bytes = 0, jac_bytes = 0;
   // vector-Jacobian product: checkpointed states, tape capacity (nodes per lane; doubles on overflow and stays grown), tape +
   // adjoint buffer, overflow flag, device staging of the host path
   double* ckpt = nullptr; size_t ckpt_bytes = 0;
   int tape_cap = 4096;
   char* vjp_buf = nullptr; size_t vjp_buf_bytes = 0;
   int* vjp_flag = nullptr;
-  double* vjp_g = nullptr;     // [2 * 13 n_bodies + 3 n_bodies][ns]: g_state | next state cotangent | g_force of the host path
+  double* vjp_g = nullptr; size_t vjp_g_bytes = 0;   // [2 * 13 n_bodies + 3 n_bodies][ns]: g_state | next state cotangent | g_force of the host path
   double* jvp_buf = nullptr; size_t jvp_buf_bytes = 0;   // Jacobian-vector product, host path: t_state | t_force | t_state_out
   cudaStream_t stream = nullptr;
 };
@@ -484,20 +487,16 @@ static int rigid_set_physical_params(tds_b200_rigid* h, int k, const int* ids, c
   const size_t sec = (size_t)k * h->ns, bytes = sizeof(double) * 3 * sec;
   if (bytes > h->par_bytes) {
     RB_TRY(cudaDeviceSynchronize());
-    cudaFree(h->par_dev);
-    h->par_dev = nullptr; h->par_bytes = 0; h->par.n = 0;
-    RB_TRY(cudaMalloc((void**)&h->par_dev, bytes));
+    h->par.n = 0;
+    RB_TRY(grow_dev(&h->par_dev, &h->par_bytes, bytes));
     RB_TRY(cudaMemset(h->par_dev, 0, bytes));
-    h->par_bytes = bytes;
   }
   if (device) {
     RB_TRY(cudaMemcpyAsync(h->par_dev, values, sizeof(double) * sec, cudaMemcpyDeviceToDevice, stream ? (cudaStream_t)stream : h->stream));
   } else {
-    std::vector<double> t(sec, 0.0);
-    for (int e = 0; e < h->n; ++e) for (int s = 0; s < k; ++s) t[(size_t)s * h->ns + e] = values[(size_t)e * k + s];
-    // steps run on non-blocking streams, which a plain cudaMemcpy does not wait for
+    // steps run on non-blocking streams, which this copy does not wait for
     RB_TRY(cudaDeviceSynchronize());
-    RB_TRY(cudaMemcpy(h->par_dev, t.data(), sizeof(double) * sec, cudaMemcpyHostToDevice));
+    RB_TRY(put_rows(h->par_dev, values, k, h->n, h->ns, h->stream));
     // a copy from pageable memory may return before its DMA has landed, and the non-blocking streams do not wait for it either
     RB_TRY(cudaDeviceSynchronize());
   }
@@ -539,19 +538,17 @@ int tds_b200_rigid_step_device(tds_b200_rigid* h, const double* state_in, double
   return 0;
 }
 
+// host state [n][13 nb] and force [n][3 nb] (or NULL) -> h->state, h->force
 static int rigid_upload(tds_b200_rigid* h, const double* state, const double* force) {
   const int nb = h->W.n_bodies, n = h->n, ns = h->ns;
-  std::vector<double> t((size_t)13 * nb * ns, 0.0);
-  for (int e = 0; e < n; ++e) for (int k = 0; k < 13 * nb; ++k) t[(size_t)k * ns + e] = state[(size_t)e * 13 * nb + k];
-  for (int e = n; e < ns; ++e) for (int b = 0; b < nb; ++b) t[(size_t)(b * 13 + 6) * ns + e] = 1.0;
-  RB_TRY(cudaMemcpyAsync(h->state, t.data(), sizeof(double) * t.size(), cudaMemcpyHostToDevice, h->stream));
-  if (force) {
-    std::vector<double> f((size_t)3 * nb * ns, 0.0);
-    for (int e = 0; e < n; ++e) for (int k = 0; k < 3 * nb; ++k) f[(size_t)k * ns + e] = force[(size_t)e * 3 * nb + k];
-    RB_TRY(cudaMemcpyAsync(h->force, f.data(), sizeof(double) * f.size(), cudaMemcpyHostToDevice, h->stream));
+  RB_TRY(put_rows(h->state, state, 13 * nb, n, ns, h->stream));
+  if (ns > n) {   // padding worlds hold the identity orientation: w (row 13 b + 6) = 1
+    const std::vector<double> one((size_t)nb * (ns - n), 1.0);
+    RB_TRY(cudaMemcpy2DAsync(h->state + (size_t)6 * ns + n, sizeof(double) * 13 * ns, one.data(), sizeof(double) * (ns - n),
+                             sizeof(double) * (ns - n), nb, cudaMemcpyHostToDevice, h->stream));
     RB_TRY(cudaStreamSynchronize(h->stream));
   }
-  RB_TRY(cudaStreamSynchronize(h->stream));
+  if (force) RB_TRY(put_rows(h->force, force, 3 * nb, n, ns, h->stream));
   return 0;
 }
 
@@ -560,14 +557,9 @@ int tds_b200_rigid_step_host(tds_b200_rigid* h, const double* state, const doubl
   if (!h || !state || !state_out) return rigid_fail("rigid_step_host: bad argument", -1);
   RB_TRY(cudaSetDevice(h->device));
   int rc = rigid_upload(h, state, force);
+  if (!rc) rc = tds_b200_rigid_step_device(h, h->state, h->state, force ? h->force : nullptr, steps, h->stream);
   if (rc) return rc;
-  rc = tds_b200_rigid_step_device(h, h->state, h->state, force ? h->force : nullptr, steps, h->stream);
-  if (rc) return rc;
-  const int nb = h->W.n_bodies, n = h->n, ns = h->ns;
-  std::vector<double> t((size_t)13 * nb * ns);
-  RB_TRY(cudaMemcpyAsync(t.data(), h->state, sizeof(double) * t.size(), cudaMemcpyDeviceToHost, h->stream));
-  RB_TRY(cudaStreamSynchronize(h->stream));
-  for (int e = 0; e < n; ++e) for (int k = 0; k < 13 * nb; ++k) state_out[(size_t)e * 13 * nb + k] = t[(size_t)k * ns + e];
+  RB_TRY(get_rows(state_out, h->state, 13 * h->W.n_bodies, h->n, h->ns, h->stream));
   return 0;
 }
 
@@ -576,14 +568,15 @@ int tds_b200_rigid_step_host(tds_b200_rigid* h, const double* state, const doubl
 // params: over the installed parameters instead (jac [n_worlds][13 n_bodies][k])
 static int rigid_jacobian(tds_b200_rigid* h, const double* state, const double* force, int steps, double* state_out, double* jac, bool params) {
   RB_TRY(cudaSetDevice(h->device));
+  RB_TRY(cudaDeviceSynchronize());   // (device calls of this world on other streams may still use its derivative buffers)
   const int nb = h->W.n_bodies, n = h->n, ns = h->ns, rows = 13 * nb, cols = params ? h->par.n : 16 * nb;
   std::vector<double> zero_f;
   if (!force) { zero_f.assign((size_t)n * 3 * nb, 0.0); force = zero_f.data(); }
   int rc = rigid_upload(h, state, force);
   if (rc) return rc;
   // (sized for the 16 n_bodies input columns, which bound the k <= 2 + 4 n_bodies parameter columns)
-  if (!h->jac) RB_TRY(cudaMalloc((void**)&h->jac, sizeof(double) * (size_t)rows * 16 * nb * ns));
-  if (!h->state2) RB_TRY(cudaMalloc((void**)&h->state2, sizeof(double) * (size_t)rows * ns));   // (the lanes of other directions still read the input)
+  RB_TRY(grow_dev(&h->jac, &h->jac_bytes, sizeof(double) * (size_t)rows * 16 * nb * ns));
+  RB_TRY(grow_dev(&h->state2, &h->state2_bytes, sizeof(double) * (size_t)rows * ns));   // (the lanes of other directions still read the input)
   if (h->par.n) {
     const RigidParMap pm = rigid_launch_map(h);
     rc = rigid_launch_rc(tds_launch_rigid_jacobian_par(&h->W, &pm, h->state, h->state2, h->force, steps, n, ns, h->jac, params ? 16 * nb : 0, cols,
@@ -595,14 +588,8 @@ static int rigid_jacobian(tds_b200_rigid* h, const double* state, const double* 
     tdsrb::tds_rigid_step_kernel<tds::Dual<double>, double><<<grid, T, 0, h->stream>>>(h->W, h->state, h->state2, h->force, steps, n, ns, h->jac, 0);
     RB_TRY(cudaGetLastError());
   }
-  std::vector<double> t((size_t)rows * cols * ns), so((size_t)rows * ns);
-  RB_TRY(cudaMemcpyAsync(t.data(), h->jac, sizeof(double) * t.size(), cudaMemcpyDeviceToHost, h->stream));
-  RB_TRY(cudaMemcpyAsync(so.data(), h->state2, sizeof(double) * so.size(), cudaMemcpyDeviceToHost, h->stream));
-  RB_TRY(cudaStreamSynchronize(h->stream));
-  for (int e = 0; e < n; ++e) {
-    for (int k = 0; k < rows * cols; ++k) jac[(size_t)e * rows * cols + k] = t[(size_t)k * ns + e];
-    if (state_out) for (int k = 0; k < rows; ++k) state_out[(size_t)e * rows + k] = so[(size_t)k * ns + e];
-  }
+  RB_TRY(get_rows(jac, h->jac, (size_t)rows * cols, n, ns, h->stream));
+  if (state_out) RB_TRY(get_rows(state_out, h->state2, rows, n, ns, h->stream));
   return 0;
 }
 
@@ -639,13 +626,8 @@ static int rigid_tape_pass(tds_b200_rigid* h, const double* s_in, double* s_out,
     if (warps > left) warps = left;
     const int chunk = (int)(warps * 32 < (size_t)(n - e0) ? warps * 32 : (size_t)(n - e0));
     const size_t tape_b = warps * 32 * h->tape_cap * sizeof(TapeNode), need = record ? warps * 32 * lane_bytes : 0;
-    if (need > h->vjp_buf_bytes) {
-      RB_TRY(cudaStreamSynchronize(sm));
-      cudaFree(h->vjp_buf);
-      h->vjp_buf = nullptr; h->vjp_buf_bytes = 0;
-      RB_TRY(cudaMalloc((void**)&h->vjp_buf, need));
-      h->vjp_buf_bytes = need;
-    }
+    if (need > h->vjp_buf_bytes) RB_TRY(cudaStreamSynchronize(sm));   // (earlier chunks still use the buffer)
+    RB_TRY(grow_dev(&h->vjp_buf, &h->vjp_buf_bytes, need));
     RigidVjpIO v = vio;
     if (record) {
       v.g_out += e0; v.g_state += e0; if (v.g_force) v.g_force += e0;
@@ -685,6 +667,11 @@ static int rigid_tape_pass(tds_b200_rigid* h, const double* s_in, double* s_out,
   return 0;
 }
 
+// vjp_g, the state and force cotangents of the VJP: [2 * 13 n_bodies + 3 n_bodies][ns]
+static cudaError_t grow_vjp_g(tds_b200_rigid* h) {
+  return grow_dev(&h->vjp_g, &h->vjp_g_bytes, sizeof(double) * (size_t)(2 * 13 + 3) * h->W.n_bodies * h->ns);
+}
+
 // g_par: [k][ns] sum over the steps of the installed parameters' cotangents, or null
 static int rigid_vjp(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
                      double* g_state, double* g_force, double* g_par, cudaStream_t sm) {
@@ -695,15 +682,10 @@ static int rigid_vjp(tds_b200_rigid* h, const double* state, const double* force
   if (g_par) RB_TRY(cudaMemsetAsync(g_par, 0, sizeof(double) * h->par.n * ns, sm));
   if (steps == 0) return 0;
   // forward, one step at a time, by the same instance without recording: states 0 .. steps - 1 are kept
-  if (sb * steps > h->ckpt_bytes) {
-    RB_TRY(cudaStreamSynchronize(sm));
-    cudaFree(h->ckpt);
-    h->ckpt = nullptr; h->ckpt_bytes = 0;
-    RB_TRY(cudaMalloc((void**)&h->ckpt, sb * steps));
-    h->ckpt_bytes = sb * steps;
-  }
+  if (sb * steps > h->ckpt_bytes) RB_TRY(cudaStreamSynchronize(sm));   // (the last call's work may still read the checkpoints)
+  RB_TRY(grow_dev(&h->ckpt, &h->ckpt_bytes, sb * steps));
   RB_TRY(cudaMemcpyAsync(h->ckpt, state, sb, cudaMemcpyDeviceToDevice, sm));
-  if (!h->vjp_g) RB_TRY(cudaMalloc((void**)&h->vjp_g, sizeof(double) * (size_t)(2 * rows + 3 * nb) * ns));
+  RB_TRY(grow_vjp_g(h));
   const size_t st = (size_t)rows * ns;
   for (int k = 0; k + 1 < steps; ++k) {
     int rc = rigid_tape_pass(h, h->ckpt + k * st, h->ckpt + (k + 1) * st, k == 0 ? force : nullptr, RigidVjpIO{}, sm);
@@ -738,28 +720,19 @@ int tds_b200_rigid_vjp_params_device(tds_b200_rigid* h, const double* state, con
 static int rigid_vjp_host(tds_b200_rigid* h, const double* state, const double* force, int steps, const double* g_state_out,
                           double* g_state, double* g_force, double* g_par) {
   RB_TRY(cudaSetDevice(h->device));
+  RB_TRY(cudaDeviceSynchronize());   // (device calls of this world on other streams may still use its derivative buffers)
+  const int nb = h->W.n_bodies, n = h->n, ns = h->ns, rows = 13 * nb;
   int rc = rigid_upload(h, state, force);
   if (rc) return rc;
-  const int nb = h->W.n_bodies, n = h->n, ns = h->ns, rows = 13 * nb;
-  if (!h->vjp_g) RB_TRY(cudaMalloc((void**)&h->vjp_g, sizeof(double) * (size_t)(2 * rows + 3 * nb) * ns));
-  std::vector<double> t((size_t)rows * ns, 0.0), f((size_t)3 * nb * ns, 0.0);
-  for (int e = 0; e < n; ++e) for (int k = 0; k < rows; ++k) t[(size_t)k * ns + e] = g_state_out[(size_t)e * rows + k];
+  RB_TRY(grow_vjp_g(h));
   double* gs = h->vjp_g;
   double* gf = h->vjp_g + (size_t)2 * rows * ns;
-  RB_TRY(cudaMemcpyAsync(gs, t.data(), sizeof(double) * t.size(), cudaMemcpyHostToDevice, h->stream));
   double* gp = g_par ? h->par_dev + (size_t)2 * h->par.n * ns : nullptr;
-  rc = rigid_vjp(h, h->state, force ? h->force : nullptr, steps, gs, gs, gf, gp, h->stream);
-  if (rc) return rc;
-  std::vector<double> p(gp ? (size_t)h->par.n * ns : 0);
-  RB_TRY(cudaMemcpyAsync(t.data(), gs, sizeof(double) * t.size(), cudaMemcpyDeviceToHost, h->stream));
-  RB_TRY(cudaMemcpyAsync(f.data(), gf, sizeof(double) * f.size(), cudaMemcpyDeviceToHost, h->stream));
-  if (gp) RB_TRY(cudaMemcpyAsync(p.data(), gp, sizeof(double) * p.size(), cudaMemcpyDeviceToHost, h->stream));
-  RB_TRY(cudaStreamSynchronize(h->stream));
-  for (int e = 0; e < n; ++e) {
-    for (int k = 0; k < rows; ++k) g_state[(size_t)e * rows + k] = t[(size_t)k * ns + e];
-    if (g_force) for (int k = 0; k < 3 * nb; ++k) g_force[(size_t)e * 3 * nb + k] = f[(size_t)k * ns + e];
-    if (gp) for (int s = 0; s < h->par.n; ++s) g_par[(size_t)e * h->par.n + s] = p[(size_t)s * ns + e];
-  }
+  RB_TRY(put_rows(gs, g_state_out, rows, n, ns, h->stream));
+  if ((rc = rigid_vjp(h, h->state, force ? h->force : nullptr, steps, gs, gs, gf, gp, h->stream))) return rc;
+  RB_TRY(get_rows(g_state, gs, rows, n, ns, h->stream));
+  if (g_force) RB_TRY(get_rows(g_force, gf, 3 * nb, n, ns, h->stream));
+  if (gp) RB_TRY(get_rows(g_par, gp, h->par.n, n, ns, h->stream));
   return 0;
 }
 
@@ -819,41 +792,23 @@ int tds_b200_rigid_jvp_params_device(tds_b200_rigid* h, const double* state, con
 static int rigid_jvp_host(tds_b200_rigid* h, const double* state, const double* force, int steps, int m, const double* t_state,
                           const double* t_force, const double* t_par, double* state_out, double* t_state_out) {
   RB_TRY(cudaSetDevice(h->device));
+  RB_TRY(cudaDeviceSynchronize());   // (device calls of this world on other streams may still use its derivative buffers)
+  const int nb = h->W.n_bodies, n = h->n, ns = h->ns, rows = 13 * nb;
   int rc = rigid_upload(h, state, force);
   if (rc) return rc;
-  const int nb = h->W.n_bodies, n = h->n, ns = h->ns, rows = 13 * nb;
-  const size_t ts = (size_t)rows * m * ns, tf = (size_t)3 * nb * m * ns, tp = t_par ? (size_t)h->par.n * m * ns : 0;
-  const size_t need = sizeof(double) * (2 * ts + tf + tp);
-  if (need > h->jvp_buf_bytes) {
-    cudaFree(h->jvp_buf);
-    h->jvp_buf = nullptr; h->jvp_buf_bytes = 0;
-    RB_TRY(cudaMalloc((void**)&h->jvp_buf, need));
-    h->jvp_buf_bytes = need;
-  }
-  if (!h->state2) RB_TRY(cudaMalloc((void**)&h->state2, sizeof(double) * (size_t)rows * ns));
-  double *ds = h->jvp_buf, *df = h->jvp_buf + ts, *dout = h->jvp_buf + ts + tf;
-  // host [n][dim][m] -> device [dim * m][ns]
-  auto up = [&](const double* src, int dim, double* dst) -> int {
-    if (!src) return 0;
-    std::vector<double> t((size_t)dim * m * ns, 0.0);
-    for (int e = 0; e < n; ++e) for (int k = 0; k < dim * m; ++k) t[(size_t)k * ns + e] = src[(size_t)e * dim * m + k];
-    RB_TRY(cudaMemcpyAsync(dst, t.data(), sizeof(double) * t.size(), cudaMemcpyHostToDevice, h->stream));
-    RB_TRY(cudaStreamSynchronize(h->stream));
-    return 0;
-  };
-  double* dp = dout + ts;
-  if ((rc = up(t_state, rows, ds)) || (rc = up(t_force, 3 * nb, df)) || (rc = up(t_par, h->par.n, dp))) return rc;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; t_state | t_force | t_state_out | t_par
+  const size_t ts = (size_t)rows * m, tf = (size_t)3 * nb * m, tp = t_par ? (size_t)h->par.n * m : 0;
+  RB_TRY(grow_dev(&h->jvp_buf, &h->jvp_buf_bytes, sizeof(double) * (2 * ts + tf + tp) * ns));
+  RB_TRY(grow_dev(&h->state2, &h->state2_bytes, sizeof(double) * (size_t)rows * ns));
+  double *ds = h->jvp_buf, *df = ds + ts * ns, *dout = df + tf * ns, *dp = dout + ts * ns;
+  if (t_state) RB_TRY(put_rows(ds, t_state, ts, n, ns, h->stream));
+  if (t_force) RB_TRY(put_rows(df, t_force, tf, n, ns, h->stream));
+  if (t_par) RB_TRY(put_rows(dp, t_par, tp, n, ns, h->stream));
   rc = rigid_jvp(h, h->state, force ? h->force : nullptr, steps, m, t_state ? ds : nullptr, t_force ? df : nullptr, t_par ? dp : nullptr,
                  h->state2, dout, h->stream);
   if (rc) return rc;
-  std::vector<double> t(ts), so((size_t)rows * ns);
-  RB_TRY(cudaMemcpyAsync(t.data(), dout, sizeof(double) * ts, cudaMemcpyDeviceToHost, h->stream));
-  RB_TRY(cudaMemcpyAsync(so.data(), h->state2, sizeof(double) * so.size(), cudaMemcpyDeviceToHost, h->stream));
-  RB_TRY(cudaStreamSynchronize(h->stream));
-  for (int e = 0; e < n; ++e) {
-    for (size_t k = 0; k < (size_t)rows * m; ++k) t_state_out[(size_t)e * rows * m + k] = t[k * ns + e];
-    if (state_out) for (int k = 0; k < rows; ++k) state_out[(size_t)e * rows + k] = so[(size_t)k * ns + e];
-  }
+  RB_TRY(get_rows(t_state_out, dout, ts, n, ns, h->stream));
+  if (state_out) RB_TRY(get_rows(state_out, h->state2, rows, n, ns, h->stream));
   return 0;
 }
 
