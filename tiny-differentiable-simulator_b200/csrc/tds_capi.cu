@@ -21,6 +21,7 @@
 extern "C" int tds_launch_stept(const TeamModel* TM, const TeamLink* tl_dev, const DevModel* M, const SimParams* P,
                                 const EnvParams* E, const StepIO* io, int mode, int use_pd, int precision,
                                 char* gscratch, int use_smem, cudaStream_t stream);
+extern "C" size_t tds_stept_tile_bytes(const TeamModel* TM);
 extern "C" unsigned long long tds_stepr_table_owner(int dev);
 extern "C" int tds_launch_stepr(const TeamModel* TM, const TeamLink* tl_host, unsigned long long token, const DevModel* M,
                                 const SimParams* P, const EnvParams* E, const StepIO* io, int mode, int use_pd,
@@ -563,8 +564,7 @@ static int rebuild_team(tds_b200_sim* s) {
   for (int p = 0; p < 3; ++p) {
     s->tm[p] = base;
     tds_build_team_layout(&s->tm[p], sizes[p][0], sizes[p][1], sizes[p][2]);
-    const size_t warp_bytes = ((size_t)s->tm[p].t_total * (32 / TDS_TEAM_T) + (size_t)s->tm[p].l_total * 32) * 4;
-    s->smem_ok_t[p] = warp_bytes <= (size_t)s->max_smem_optin;
+    s->smem_ok_t[p] = tds_stept_tile_bytes(&s->tm[p]) <= (size_t)s->max_smem_optin;
     s->smem_ok_r[p] = tds_stepr_tile_bytes(&s->tm[p]) <= (size_t)s->max_smem_optin;
   }
   static unsigned long long next_token = 1;
@@ -851,10 +851,8 @@ int tds_b200_step_device(tds_b200_sim* s, int mode, int use_pd, const float* q_i
   }
   if (kern == 2) {
     const int use_smem_t = s->smem_ok_t[p] ? 1 : 0;
-    if (!use_smem_t) {
-      const size_t warp_bytes = ((size_t)s->tm[p].t_total * (32 / TDS_TEAM_T) + (size_t)s->tm[p].l_total * 32) * 4;
-      CUDA_TRY(grow_dev(&s->scratch, &s->scratch_bytes, warp_bytes * ((s->n + (32 / TDS_TEAM_T) - 1) / (32 / TDS_TEAM_T))));
-    }
+    if (!use_smem_t)   // one tile per warp of 32 / TDS_TEAM_T environments
+      CUDA_TRY(grow_dev(&s->scratch, &s->scratch_bytes, tds_stept_tile_bytes(&s->tm[p]) * ((s->n + (32 / TDS_TEAM_T) - 1) / (32 / TDS_TEAM_T))));
     int rct = tds_launch_stept(&s->tm[p], s->team_dev, &s->dm[p], &s->P, &s->E, &io, mode, use_pd, p, s->scratch, use_smem_t,
                                (cudaStream_t)stream);
     if (rct) set_err(std::string("team step launch: ") + cudaGetErrorString((cudaError_t)rct));

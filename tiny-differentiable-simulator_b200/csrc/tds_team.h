@@ -1,7 +1,7 @@
 // Team ("sub-warp") decomposition of one environment over T lanes: the kinematic tree is cut into a TRUNK
 // (ancestor-closed set of links at the root, processed by lane 0 of the team) and SUBTREES hanging off the
 // trunk, distributed over the T lanes.  Host side: partition + per-role link tables + scratch layout.
-// Device side: tds_stept.cu.
+// Device side: tds_team_step.cuh (step body), run by tds_stept.cu (lane teams) and tds_stepr.cu (role warps).
 #pragma once
 #include <string.h>
 

@@ -1,6 +1,6 @@
 // Shared device helpers of the world-frame kernels (tds_stepw.cu: one lane per environment,
-// tds_stept.cu: a team of lanes per environment): strided shared-memory accessors, accumulator
-// records, 3x3 register blocks for the blocked dense solves.
+// tds_team_step.cuh: four roles per environment, on lanes or warps): strided shared-memory accessors,
+// accumulator records, 3x3 register blocks for the blocked dense solves.
 #pragma once
 #include <cuda_runtime.h>
 
