@@ -455,6 +455,7 @@ struct tds_b200_sim {
   cudaStream_t stream = nullptr;
   int max_smem_optin = 0;
   long long* phase_clk = nullptr;  // profiling only (tds_b200_debug_phase_clocks)
+  long long* phase_clk_dev = nullptr;   // profiling only: caller-owned record that replaces phase_clk (tds_b200_debug_phase_clocks_device)
   // tds_b200_env_step_host with pinned caller buffers: the copy / transpose / step / copy sequence is captured once
   // per buffer set and replayed (one graph launch instead of nine stream operations)
   // environment layer scratch: reset staging, zero actions, actuated coordinate map, rollout bookkeeping
@@ -825,7 +826,7 @@ int tds_b200_step_device(tds_b200_sim* s, int mode, int use_pd, const float* q_i
   io.q_in = q_in; io.qd_in = qd_in; io.tau_in = tau_or_action;
   io.q_out = q_out; io.qd_out = qd_out; io.qdd_out = qdd_out;
   io.reward = reward; io.done = done; io.contact_dist = contact_dist; io.link_xf = link_xf;
-  io.phase_clk = s->phase_clk;
+  io.phase_clk = s->phase_clk_dev ? s->phase_clk_dev : s->phase_clk;
   io.act_aos = s->io_act_aos; io.obs_aos = s->io_obs_aos; io.obs_tail = s->io_obs_tail;
   io.jac = nullptr; io.jac_n_in = 0; io.jac_dir0 = 0;
   io.n = s->n; io.n_stride = s->ns;
@@ -1758,6 +1759,15 @@ int tds_b200_debug_phase_clocks(tds_b200_sim* s, int enable, long long* out_host
   }
   if (!enable && s->phase_clk) { cudaFree(s->phase_clk); s->phase_clk = nullptr; }
   return nw;
+}
+
+// Profiling aid: the launches enqueued from now on write their stamps to the caller's device buffer ([n_warps][16], see
+// tds_b200_debug_phase_clocks for n_warps) instead; null returns to the library's own record.  One buffer per launch
+// keeps the stamps of every step of a captured sequence (scripts/step_gaps.py).
+int tds_b200_debug_phase_clocks_device(tds_b200_sim* s, long long* dev) {
+  if (!s) return -1;
+  s->phase_clk_dev = dev;
+  return 0;
 }
 
 void* tds_b200_stream(tds_b200_sim* s) { return s ? (void*)s->stream : nullptr; }

@@ -292,6 +292,17 @@ template <typename T> TDS_D Abi<T> abi_nz() {
 template <typename T> TDS_D Sv<T> sv_nz() { Sv<T> s; const T z = negz<T>(); s.top = v3<T>(z, z, z); s.bot = s.top; return s; }
 template <typename T> TDS_D Rbi<T> rbi_nz() { Rbi<T> r; const T z = negz<T>(); r.m = z; r.h = v3<T>(z, z, z); r.I = {z, z, z, z, z, z}; return r; }
 
+// %globaltimer (ns, one clock for the whole device: the gaps between consecutive grids are measured across SMs)
+TDS_D long long global_ns() {
+#ifdef TDS_STEPS_KERNEL_ONLY   // (the host-compiled copy of the kernel source in tests/cpp has no PTX)
+  return 0;
+#else
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return (long long)t;
+#endif
+}
+
 // VAR selects what the instance carries besides the step itself (code bytes are paid at the instruction-fetch rate):
 //   0 general: forward-dynamics-only mode, per-link world transforms and contact distances as outputs
 //   1 lean: full / no-contact step on the device layout only      2 lean + host layouts (tds_b200_env_step_host)
@@ -1645,8 +1656,28 @@ TDS_D void tile_body(char* const smem, const SimParams& P, const EnvParams& E, c
     }
   }
   TDSS_PHASE();  // 9
+  // %globaltimer after the role's last store (slot 15; slot 14 is stamped by the kernel around griddepcontrol.wait)
+  if (io.phase_clk && lane == 0 && tile * 32 < io.n_stride) io.phase_clk[((size_t)tile * TT + role) * 16 + 15] = global_ns();
 #undef TDSS_PHASE
 #undef TDSS_STAMP
+}
+
+// Warms L2 with the rows of global memory the tile reads first: q, qd and the device-layout actions / torques, 128 B
+// (32 environments) per row, one row per thread.  Runs BEFORE griddepcontrol.wait, i.e. possibly while the previous
+// kernel of the stream (the previous step, a policy kernel) still writes these rows: a prefetch only moves lines into
+// L2, the GPU's point of coherence, and returns nothing to the SM; the loads that feed the arithmetic stay after the
+// wait.  The host-layout actions may be mapped host memory and are not prefetched.
+template <class SP, int VAR> TDS_D void prefetch_tile_rows(const StepIO& io, const int use_pd, const int tile, const int tid) {
+  constexpr int NA = VAR == 2 ? 0 : SP::N_ACT, NTAU = VAR == 2 ? 0 : SP::N_QD - (SP::FLOATING ? 6 : 0);
+  const int n_in = io.tau_in ? (use_pd ? NA : NTAU) : 0;
+  const size_t col = (size_t)tile * 32;
+  const float* row = nullptr;
+  if (tid < SP::N_Q) row = io.q_in + (size_t)tid * io.n_stride;
+  else if (tid < SP::N_Q + SP::N_QD) row = io.qd_in + (size_t)(tid - SP::N_Q) * io.n_stride;
+  else if (tid < SP::N_Q + SP::N_QD + n_in) row = io.tau_in + (size_t)(tid - SP::N_Q - SP::N_QD) * io.n_stride;
+#ifndef TDS_STEPS_KERNEL_ONLY
+  if (row) asm volatile("prefetch.global.L2 [%0];" :: "l"(row + col));
+#endif
 }
 
 // TPC tiles per CTA.  1 (shipped): one tile per CTA, two CTAs may share an SM.
@@ -1662,16 +1693,25 @@ tds_step_spec_kernel(const __grid_constant__ SimParams P, const __grid_constant_
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp index, known uniform to the compiler
   const int role = warp % TDS_TEAM_T, sub = warp / TDS_TEAM_T;
   if ((mode_flags & 256) && role != 0) return;   // profiling aid (TDS_B200_DEBUG_SOLO): role 0 alone, results are garbage
-  // Programmatic dependent launch (back-to-back steps of one stream / graph): let the next step's grid be scheduled now
-  // (single-wave batches: its CTAs take the second slot of every SM and park at their own wait), then wait for the
-  // previous step's grid to complete and flush before the first read of the state.  Both are no-ops without the attribute.
-#ifndef TDS_STEPS_KERNEL_ONLY   // (the host-compiled copy of the kernel source in tests/cpp has no PTX)
+  const int tile = (int)blockIdx.x * TPC + sub, tid = (int)threadIdx.x - sub * 32 * TDS_TEAM_T;
+  char* const smem = smem_raw + (size_t)sub * ((size_t)Lay<SP, RA, RC, RS>::TOTAL * 32 * 4);
+  // profiling: %globaltimer stamps in the free slots of the (tile, role) record: slot 14 = kernel entry (role 0) or the
+  // return from griddepcontrol.wait (roles 1..), slot 15 = after the role's last store (end of tile_body)
+  long long* const gstamp = (io.phase_clk && (tid & 31) == 0 && tile * 32 < io.n_stride) ? io.phase_clk + ((size_t)tile * TDS_TEAM_T + role) * 16 : nullptr;
+  if (gstamp && role == 0) gstamp[14] = global_ns();
+  // Programmatic dependent launch (launched with cudaLaunchAttributeProgrammaticStreamSerialization, SpecHost::launch):
+  // with mode bit 512 (a single-wave grid) the next step's grid may be scheduled from now on; its CTAs take the SMs this
+  // grid leaves idle or vacates and run up to their own wait.  Everything above the wait reads nothing that earlier work in the
+  // stream writes; griddepcontrol.wait returns once the previous grid has completed and its memory is visible.
+#ifndef TDS_STEPS_KERNEL_ONLY
   if (mode_flags & 512) asm volatile("griddepcontrol.launch_dependents;");
+#endif
+  prefetch_tile_rows<SP, VAR>(io, use_pd, tile, tid);
+#ifndef TDS_STEPS_KERNEL_ONLY
   asm volatile("griddepcontrol.wait;" ::: "memory");
 #endif
-  char* const smem = smem_raw + (size_t)sub * ((size_t)Lay<SP, RA, RC, RS>::TOTAL * 32 * 4);
-  tile_body<SP, RA, RC, RS, VAR>(smem, P, E, io, mode_flags & 255, use_pd, role, (int)blockIdx.x * TPC + sub,
-                                 (int)threadIdx.x - sub * 32 * TDS_TEAM_T);
+  if (gstamp && role != 0) gstamp[14] = global_ns();
+  tile_body<SP, RA, RC, RS, VAR>(smem, P, E, io, mode_flags & 255, use_pd, role, tile, tid);
 #ifndef TDS_STEPS_KERNEL_ONLY
   if (!(mode_flags & 512)) asm volatile("griddepcontrol.launch_dependents;");
 #endif
@@ -1713,33 +1753,55 @@ template <class SP> struct SpecHost {
     int dev_ = 0; cudaGetDevice(&dev_);
     static int sm_count[64] = {0};
     if (!sm_count[dev_ & 63]) cudaDeviceGetAttribute(&sm_count[dev_ & 63], cudaDevAttrMultiProcessorCount, dev_);
+    static int smem_per_sm[64] = {0};
+    if (!smem_per_sm[dev_ & 63]) cudaDeviceGetAttribute(&smem_per_sm[dev_ & 63], cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev_);
     // throughput mode: more tiles than two waves of single-tile CTAs and two tiles fit one CTA's shared memory
     static const int tpc_env = getenv("TDS_B200_TPC") ? atoi(getenv("TDS_B200_TPC")) : 0;
-    static const bool pdl = getenv("TDS_B200_PDL") ? atoi(getenv("TDS_B200_PDL")) != 0 : false;
     // (opt-in until measured on the target: TDS_B200_TPC=2; TDS_B200_TPC=-1 = automatic for batches of more than two waves)
     int tpc = 1;
     if (tpc_env == -1) tpc = (tiles > 2 * sm_count[dev_ & 63] && 2 * smem1 <= 227 * 1024) ? 2 : 1;
     if (tpc_env == 2) tpc = 2 * smem1 <= 227 * 1024 ? 2 : 1;
+    // Every step is a programmatic dependent launch: its grid may be scheduled before the previous kernel of the stream
+    // (or the previous kernel node of a captured graph) has completed; the kernel does its step-independent prologue
+    // and waits in griddepcontrol.wait for that kernel's completion and memory flush.  After a kernel that never
+    // triggers (a policy kernel, the reset kernels, a kernel of another library) the dependency resolves when its
+    // CTAs exit, as without the attribute.
+    // When the grid is one wave (the tiles fit the device's co-resident CTA slots), the kernel triggers at entry (mode
+    // bit 512): the next step's grid is scheduled while this one runs, and its CTAs take the SMs this one leaves idle and
+    // each SM as soon as this step's CTA there exits, so only the wait separates the two steps.  This cannot starve the
+    // running grid: a dependent grid is scheduled only after EVERY CTA of its primary has triggered or exited, i.e. when
+    // all of the primary's CTAs are already resident, so a dependent CTA never holds a slot that the primary still needs.
+    // Larger batches trigger after the tile's last store.
+    // A grid of at most one CTA per SM asks for more than half of the SM's shared memory (smem_one), so that the
+    // scheduler cannot put two of them on one SM.  Measured on the H100 (scripts/step_gaps.py, DESIGN.md section 4.3):
+    // with two slots per SM, the next step's CTAs were placed next to running tiles, and the grid's span grew by as much
+    // as the overlap saved.
 #define TDSS_LAUNCH(RA, RC, RS, VAR, TPC)                                                               \
   do {                                                                                                  \
     auto k = tds_step_spec_kernel<SP, RA, RC, RS, VAR, TPC>;                                            \
     const size_t smem = smem1 * TPC;                                                                    \
     static bool attr_set_dev[64] = {false}; bool& attr_set = attr_set_dev[dev_ & 63]; /* the attribute is per device */ \
-    if (!attr_set && smem > 48 * 1024) {                                                                \
-      err = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);            \
+    static int ctas_per_sm_dev[64] = {0}; int& ctas_per_sm = ctas_per_sm_dev[dev_ & 63];              \
+    const size_t smem_one = smem > (size_t)smem_per_sm[dev_ & 63] / 2 ? smem : (size_t)smem_per_sm[dev_ & 63] / 2; \
+    if (!attr_set && smem_one > 48 * 1024) {                                                            \
+      err = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_one);        \
       /* two tiles per SM when the batch has more tiles than SMs: ask for the largest shared-memory carveout */ \
       if (err == cudaSuccess) err = cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared); \
       if (err == cudaSuccess) attr_set = true;                                                          \
     }                                                                                                   \
+    if (err == cudaSuccess && !ctas_per_sm)                                                             \
+      err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, k, 32 * TDS_TEAM_T * TPC, smem); \
     if (err == cudaSuccess) {                                                                           \
+      const int ctas = (tiles + TPC - 1) / TPC;                                                         \
+      const bool one_per_sm = ctas <= sm_count[dev_ & 63];                                              \
       cudaLaunchConfig_t cfg = {};                                                                      \
-      cfg.gridDim = dim3((tiles + TPC - 1) / TPC); cfg.blockDim = dim3(32 * TDS_TEAM_T * TPC);          \
-      cfg.dynamicSmemBytes = smem; cfg.stream = stream;                                                 \
+      cfg.gridDim = dim3(ctas); cfg.blockDim = dim3(32 * TDS_TEAM_T * TPC);                             \
+      cfg.dynamicSmemBytes = one_per_sm ? smem_one : smem; cfg.stream = stream;                         \
       cudaLaunchAttribute at[1];                                                                        \
       at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                    \
       at[0].val.programmaticStreamSerializationAllowed = 1;                                             \
-      cfg.attrs = at; cfg.numAttrs = pdl ? 1 : 0;                                                       \
-      const int mode_k = mode | ((pdl && tiles <= sm_count[dev_ & 63]) ? 512 : 0);                      \
+      cfg.attrs = at; cfg.numAttrs = 1;                                                                 \
+      const int mode_k = mode | (one_per_sm || ctas <= ctas_per_sm * sm_count[dev_ & 63] ? 512 : 0);   \
       err = cudaLaunchKernelEx(&cfg, k, *P, *E, *io, mode_k, use_pd);                                   \
     }                                                                                                   \
   } while (0)
