@@ -253,6 +253,42 @@ int tds_b200_kinematics_vjp_device(tds_b200_sim* sim, const float* q, int K, con
 int tds_b200_kinematics_vjp_host(tds_b200_sim* sim, const double* q, int K, const int* links, const double* local, const double* G_xf,
                                  const double* G_x, const double* G_J, double* g_q);
 
+/* ---- inverse dynamics tau = ID(q, qd, qdd) and bias forces (DESIGN.md 7.14; inverse_dynamics.hpp) ------------------------------------
+ * The joint forces tau [n_qd] (fp64, one row per dof, a floating base's 6 rows included) for which the multibody has the accelerations
+ * qdd, by the recursive Newton-Euler algorithm at the fp32-rounded q, qd, qdd and the simulator's gravity (tds_b200_set_params).  qd or
+ * qdd may be NULL, meaning zero; bias forces h(q, qd) are ID(q, qd, 0): pass a NULL qdd.
+ *   Fixed base (worlds of several multibodies included): the exact inverse of this library's forward dynamics (MODE_FD), so tau
+ *   contains the terms the ABA subtracts: stiffness q + damping qd of 1-dof joints, the quaternion axis-angle stiffness term and per-dof
+ *   damping of spherical joints.  While a parameter set is installed, each environment's masses, centres of mass, inertias, stiffness
+ *   and damping are used.
+ *   Floating base: the textbook RNEA in the coordinates of tds_b200_mass_matrix: qdd[0:6] is the base-frame spatial acceleration
+ *   [angular; linear], gravity is rotated into the base frame, and rows 0..5 are the wrench on the base in the base frame [moment
+ *   about the base origin; force].  This is NOT the inverse of the reference's floating-base forward dynamics, which adds gravity
+ *   un-rotated, has a frame-mixing gyroscopic term and does not invert its own mass matrix.
+ * Argument checks: NULL q, no output (tau, t_tau; G, or every cotangent output), m < 1 or every tangent NULL -> -1; t_par / g_par
+ * without an installed set -> -4.
+ *   device: q [n_q][n_stride], qd and qdd [n_qd][n_stride] fp32 as tds_b200_step_device; tau [n_qd][n_stride] fp64.  Asynchronous.
+ *   host:   q [n][n_q], qd and qdd [n][n_qd] fp64 (rounded to fp32); tau [n][n_qd] fp64.  Synchronous.
+ * _jvp: dtau along m tangents of q, qd, qdd and the installed parameters (each may be NULL: zero, not all), one lane per (environment,
+ *   tangent) of the dual-number instance, in chunks as tds_b200_step_jvp_*.  tau (may be NULL) receives the value.  Device t_q
+ *   [n_q * m][n_stride], t_qd and t_qdd [n_qd * m][n_stride], t_par [k * m][n_stride], t_tau [n_qd * m][n_stride] (entry (r, j) at
+ *   (r * m + j) * n_stride + e); host t_q [n][n_q][m], t_qd and t_qdd [n][n_qd][m], t_par [n][k][m], t_tau [n][n_qd][m].
+ * _vjp: g_x[c] = sum_r G[r] dtau[r]/dx_c for x = q, qd, qdd and, while a set is installed, the parameters, for a cotangent G in tau's
+ *   layout: the JVP along the n_q + 2 n_qd (+ k) identity tangents contracted with G on the device.  Any of g_q, g_qd, g_qdd, g_par may
+ *   be NULL, not all.  Device g_q [n_q][n_stride], g_qd and g_qdd [n_qd][n_stride], g_par [k][n_stride] fp64 (asynchronous); host
+ *   g_q [n][n_q], g_qd and g_qdd [n][n_qd], g_par [n][k] (synchronous). */
+int tds_b200_inverse_dynamics_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, double* tau, void* stream);
+int tds_b200_inverse_dynamics_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, double* tau);
+int tds_b200_inverse_dynamics_jvp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, int m, const double* t_q,
+                                         const double* t_qd, const double* t_qdd, const double* t_par, double* tau, double* t_tau,
+                                         void* stream);
+int tds_b200_inverse_dynamics_jvp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, int m, const double* t_q,
+                                       const double* t_qd, const double* t_qdd, const double* t_par, double* tau, double* t_tau);
+int tds_b200_inverse_dynamics_vjp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, const double* G, double* g_q,
+                                         double* g_qd, double* g_qdd, double* g_par, void* stream);
+int tds_b200_inverse_dynamics_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, const double* G, double* g_q,
+                                       double* g_qd, double* g_qdd, double* g_par);
+
 /* Stand-alone integration stages of the fine-grained surface (device SoA arrays as above):
  * integrate_euler (src/dynamics/integrator.hpp:10-133): qd += qdd dt (qdd may be NULL = zero), q += qd dt, floating base
  * quaternion increment + normalisation; integrate_euler_qdd (:141-195): qd += qdd dt only. */

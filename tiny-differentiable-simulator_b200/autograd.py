@@ -27,6 +27,10 @@ mass_matrix(sim, q, params=None) is the joint-space mass matrix M(q) [n_envs, n_
 backward rule (BatchSim.mass_matrix_vjp_device: float32 q.grad, float64 params.grad) and a forward-mode rule
 (BatchSim.mass_matrix_jvp_device).
 
+inverse_dynamics(sim, q, qd, qdd=None, params=None) is tau = ID(q, qd, qdd) [n_envs, n_qd] (float64, DESIGN.md section 7.14) with a
+backward rule (BatchSim.inverse_dynamics_vjp_device: float32 q.grad, qd.grad, qdd.grad, float64 params.grad) and a forward-mode rule
+(BatchSim.inverse_dynamics_jvp_device).
+
 forward_kinematics(sim, q, links, local) is every link's world transform and every point's world position and linear Jacobian (float64,
 DESIGN.md section 7.13) with a backward rule (BatchSim.kinematics_vjp_device: float32 q.grad) and a forward-mode rule
 (BatchSim.kinematics_jvp_device).
@@ -329,6 +333,94 @@ def mass_matrix(sim, q, params=None):
                                tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
         raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
     return _MassMatrix.apply(sim, q, params)
+
+
+class _InverseDynamics(torch.autograd.Function):
+    @staticmethod
+    def forward(sim, q, qd, qdd, params):
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        if params is not None:
+            sim.set_physical_params(sim.param_ids, params.detach())
+        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
+        tau = torch.zeros((max(nd, 1), ns), dtype=torch.float64, device=q.device)
+        _on_side_stream(q.device, lambda st: sim.inverse_dynamics_device(qs, qds, qdds, tau, stream=st), (qs, qds, qdds, tau))
+        return tau[:nd, :n].t().contiguous()
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        sim, q, qd, qdd, params = inputs
+        ns = sim.n_stride
+        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
+        par = params.detach() if params is not None else None
+        ctx.sim, ctx.has = sim, (qd is not None, qdd is not None, params is not None)
+        ctx.save_for_backward(qs, *(t if t is not None else qs for t in (qds, qdds, par)))
+        ctx.jvp_inputs = (qs, qds, qdds, par)
+
+    @staticmethod
+    def backward(ctx, g):
+        sim = ctx.sim
+        has_qd, has_qdd, has_par = ctx.has
+        qs, qds, qdds, par = ctx.saved_tensors
+        qds, qdds = (qds if has_qd else None), (qdds if has_qdd else None)
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        G = _soa(g, ns, torch.float64)
+        z = lambda rows: torch.zeros((max(rows, 1), ns), dtype=torch.float64, device=g.device)
+        g_q, g_qd, g_qdd = z(sim.n_q), (z(nd) if has_qd else None), (z(nd) if has_qdd else None)
+        g_par = z(par.shape[1]) if has_par else None
+        if has_par:
+            sim.set_physical_params(sim.param_ids, par)   # the values of this call
+        _on_side_stream(g.device, lambda st: sim.inverse_dynamics_vjp_device(qs, qds, qdds, G, g_q, g_qd, g_qdd, g_par, stream=st),
+                        (qs, qds, qdds, G, g_q, g_qd, g_qdd, g_par))
+        out = lambda t, rows, dt: None if t is None else t[:rows, :n].t().to(dt).contiguous()
+        return None, out(g_q, sim.n_q, torch.float32), out(g_qd, nd, torch.float32), out(g_qdd, nd, torch.float32), \
+            out(g_par, par.shape[1], torch.float64)
+
+    @staticmethod
+    def jvp(ctx, _sim, t_q, t_qd, t_qdd, t_params):
+        with torch._C._DisableFuncTorch():
+            return _InverseDynamics._jvp(ctx, _plain(t_q), _plain(t_qd), _plain(t_qdd), _plain(t_params))
+
+    @staticmethod
+    def _jvp(ctx, t_q, t_qd, t_qdd, t_params):
+        sim = ctx.sim
+        has_qd, has_qdd, has_par = ctx.has
+        qs, qds, qdds, par = (_plain(t) for t in ctx.jvp_inputs)
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        tq = _soa_opt(t_q, ns, torch.float64)
+        tqd = _soa_opt(t_qd if has_qd else None, ns, torch.float64)
+        tqdd = _soa_opt(t_qdd if has_qdd else None, ns, torch.float64)
+        tp = _soa_opt(t_params if has_par else None, ns, torch.float64)
+        t_tau = torch.zeros((max(nd, 1), ns), dtype=torch.float64, device=qs.device)
+        if any(t is not None for t in (tq, tqd, tqdd, tp)):
+            if has_par:
+                sim.set_physical_params(sim.param_ids, par)   # the values of this call
+            _on_side_stream(qs.device, lambda st: sim.inverse_dynamics_jvp_device(qs, qds, qdds, 1, tq, tqd, tqdd, tp, t_tau, stream=st),
+                            (qs, qds, qdds, tq, tqd, tqdd, tp, t_tau))
+        return t_tau[:nd, :n].t().contiguous()
+
+
+def _soa_opt(x, n_stride, dtype):
+    return None if x is None else _soa(x, n_stride, dtype)
+
+
+def inverse_dynamics(sim, q, qd, qdd=None, params=None):
+    """Inverse dynamics of every environment of `sim` (a BatchSim): tau [n_envs, n_qd] float64, the joint forces for which the
+    multibodies have the accelerations qdd at (q, qd) under the simulator's gravity (DESIGN.md section 7.14), by the recursive
+    Newton-Euler algorithm in fp64 at the fp32-rounded inputs.  q [n_envs, n_q], qd and qdd [n_envs, n_qd] float32 CUDA tensors; qd or
+    qdd None: zero (the bias forces h(q, qd) are inverse_dynamics(sim, q, qd)).  Fixed base: the inverse of the MODE_FD step, stiffness
+    and damping terms included.  Floating base: rows 0..5 are the wrench on the base in the base frame for the base-frame spatial
+    acceleration qdd[0:6], with gravity rotated into the base frame - the textbook RNEA in the coordinates of mass_matrix, not the
+    inverse of the reference's floating-base forward dynamics.  params: None, or a float64 CUDA tensor [n_envs, k] of values for the
+    parameters installed by sim.set_physical_params (then also differentiated).  Differentiable in reverse and forward mode."""
+    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
+        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
+    for name, t in (("qd", qd), ("qdd", qdd)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or tuple(t.shape) != (sim.n_envs, sim.n_qd)):
+            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, n_qd] is expected")
+    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
+                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
+        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    return _InverseDynamics.apply(sim, q, qd, qdd, params)
 
 
 def _kin_outputs(sim, K, xf, x, J):

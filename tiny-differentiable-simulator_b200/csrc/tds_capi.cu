@@ -62,6 +62,10 @@ extern "C" int tds_launch_mass_contract(const double* G, const double* dM, int n
 extern "C" int tds_launch_kin(const DevModel* M, const StepIO* io, const TdsKinCall* kc, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_kin_jvp(const DevModel* M, const StepIO* io, const TdsKinCall* kc, const double* t_q, int m, int n_dirs,
                                   char* gscratch, cudaStream_t stream);
+// inverse dynamics tau = ID(q, qd, qdd) and its Jacobian-vector products (tds_invdyn.cu)
+extern "C" int tds_launch_inv(const DevModel* M, const SimParams* P, const StepIO* io, const ParMap* pm, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_inv_jvp(const DevModel* M, const SimParams* P, const StepIO* io, const ParMap* pm, const double* t_in,
+                                  const double* t_par, int m, int n_dirs, char* gscratch, cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
@@ -883,8 +887,9 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null); mass: of the mass matrix
 // (t_in = the q tangents; the step's arguments are not read); kin: of the kinematics of this point table and these outputs (t_in =
-// the q tangents, t_par unused)
-struct JvpTangents { const double* t_in; const double* t_par; int m; bool mass = false; const TdsKinCall* kin = nullptr; };
+// the q tangents, t_par unused); inv: of the inverse dynamics (t_in = the q | qd | qdd tangents; qd and qdd in the step's qd and
+// tau_or_action)
+struct JvpTangents { const double* t_in; const double* t_par; int m; bool mass = false; const TdsKinCall* kin = nullptr; bool inv = false; };
 
 // scratch of one launch of a world-frame instance of layout M over every environment: x_total words per lane
 static size_t lane_arena_bytes(const tds_b200_sim* s, const DevModel& M) {
@@ -917,7 +922,8 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   for (int d0 = 0; d0 < n_dirs; d0 += chunk) {
     io.jac_dir0 = dir_base + d0;
     const int nd = n_dirs - d0 < chunk ? n_dirs - d0 : chunk;
-    int rc = (jv && jv->kin) ? tds_launch_kin_jvp(&s->dm_ad, &io, jv->kin, jv->t_in, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
+    int rc = (jv && jv->inv) ? tds_launch_inv_jvp(&s->dm_ad, &s->P, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
+           : (jv && jv->kin) ? tds_launch_kin_jvp(&s->dm_ad, &io, jv->kin, jv->t_in, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
            : (jv && jv->mass) ? tds_launch_mass_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
            : jv ? tds_launch_stepw_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch,
                                        (cudaStream_t)stream)
@@ -1317,6 +1323,188 @@ int tds_b200_kinematics_vjp_host(tds_b200_sim* s, const double* q, int K, const 
     CUDA_TRY(parts[i] ? put_rows(d, parts[i], rows[i], n, ns, s->stream) : cudaMemsetAsync(d, 0, sizeof(double) * rows[i] * ns, s->stream));
   if (int rc = kin_vjp_run(s, s->q, K, links, local, G, s->vjp_g, buf, chunk, s->stream)) return rc;
   CUDA_TRY(get_rows(g_q, s->vjp_g, n_q, n, ns, s->stream));
+  return 0;
+}
+
+// ---- inverse dynamics tau = ID(q, qd, qdd) (DESIGN.md section 7.14): the INV instances of the world-frame kernel (tds_invdyn.cu) -------
+// tau [n_qd][ns] from q [n_q][ns], qd and qdd [n_qd][ns] fp32 (either NULL: zero), one lane per environment on the 8-byte layout
+static int inv_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* tau, cudaStream_t sm) {
+  StepIO io;
+  memset(&io, 0, sizeof(io));
+  io.q_in = q; io.qd_in = qd; io.tau_in = qdd; io.jac = tau; io.jac_n_in = 1;
+  io.n = s->n; io.n_stride = s->ns;
+  ParMap pmv = s->par;
+  pmv.values = s->par_dev; pmv.grad = nullptr;
+  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_m)));
+  const int rc = tds_launch_inv(&s->dm_m, &s->P, &io, s->par.n > 0 ? &pmv : nullptr, s->jac_scratch, sm);
+  if (rc) set_err(std::string("inverse dynamics launch: ") + cudaGetErrorString((cudaError_t)rc));
+  return rc;
+}
+
+// inputs of the inverse dynamics' derivatives: q | qd | qdd
+static int inv_n_in(const tds_b200_sim* s) { return s->dm[0].n_q + 2 * s->dm[0].n_qd; }
+
+// t_tau [n_qd * m][ns] along t_in [(n_q + 2 n_qd) * m][ns] (q | qd | qdd tangents, contiguous) and t_par (either may be NULL); tau, if
+// not NULL, receives the value
+static int inv_jvp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int m, const double* t_in, const double* t_par,
+                       double* tau, double* t_tau, cudaStream_t sm) {
+  if (tau) { if (int rc = inv_run(s, q, qd, qdd, tau, sm)) return rc; }
+  JvpTangents jv{t_in, t_par, m};
+  jv.inv = true;
+  return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, qdd, t_tau, sm, false, &jv);
+}
+
+// g_in [(n_q + 2 n_qd)][ns] (q | qd | qdd, contiguous) and g_par [k][ns] (NULL: not wanted) = G . dtau along the identity tangents, in
+// chunks of directions whose dtau and tangents stay within 1 GB (s->mass_dev)
+static int inv_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const double* G, double* g_in, double* g_par,
+                       cudaStream_t sm) {
+  const int n_in = inv_n_in(s), nd_ = s->dm[0].n_qd, k = g_par ? s->par.n : 0, ns = s->ns;
+  const int total = n_in + k;
+  const size_t per_dir = sizeof(double) * (size_t)(nd_ + total) * ns;   // dtau + identity tangents of one direction
+  int chunk = (int)(((size_t)1 << 30) / per_dir);
+  if (chunk < 1) chunk = 1;
+  if (chunk > total) chunk = total;
+  CUDA_TRY(grow_dev(&s->mass_dev, &s->mass_dev_bytes, per_dir * chunk));
+  for (int d0 = 0; d0 < total; d0 += chunk) {
+    const int nd = total - d0 < chunk ? total - d0 : chunk;
+    double* tin = s->mass_dev;
+    double* tp = k > 0 ? tin + (size_t)n_in * nd * ns : nullptr;
+    double* dtau = tin + (size_t)total * nd * ns;
+    int rc = tds_launch_mass_eye(tin, tp, n_in, k, d0, nd, ns, sm);
+    if (!rc) rc = inv_jvp_run(s, q, qd, qdd, nd, tin, tp, nullptr, dtau, sm);
+    if (!rc) rc = tds_launch_mass_contract(G, dtau, nd_, nd, d0, n_in, g_in, g_par, s->n, ns, sm);
+    if (rc) { set_err(std::string("inverse dynamics vjp: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
+  }
+  return 0;
+}
+
+// [rows][ns] fp64, device to device (dst NULL: nothing; src NULL: zeros)
+static int rows_d2d(double* dst, const double* src, int rows, int ns, cudaStream_t sm) {
+  if (!dst || rows == 0) return 0;
+  CUDA_TRY(src ? cudaMemcpyAsync(dst, src, sizeof(double) * rows * ns, cudaMemcpyDeviceToDevice, sm)
+               : cudaMemsetAsync(dst, 0, sizeof(double) * rows * ns, sm));
+  return 0;
+}
+
+// host q [n][n_q], qd and qdd [n][n_qd] (either NULL: zero) -> s->q, s->qd, s->act; the device pointers of qd and qdd (NULL for NULL)
+static int put_inv_inputs(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, const float** qd_d, const float** qdd_d) {
+  const int nd = s->dm[0].n_qd;
+  int rc = put_q(s, q);
+  if (!rc && qd) rc = put_state(s, qd, nd, s->qd);
+  if (!rc && qdd) rc = put_state(s, qdd, nd, s->act);
+  *qd_d = qd ? s->qd : nullptr;
+  *qdd_d = qdd ? s->act : nullptr;
+  return rc;
+}
+
+int tds_b200_inverse_dynamics_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* tau, void* stream) {
+  if (!s || !q || !tau) return -1;
+  return inv_run(s, q, qd, qdd, tau, (cudaStream_t)stream);
+}
+
+int tds_b200_inverse_dynamics_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, double* tau) {
+  if (!s || !q || !tau) return -1;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int nd = s->dm[0].n_qd;
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (nd > 0 ? nd : 1) * s->ns));
+  if (int rc = inv_run(s, s->q, qd_d, qdd_d, s->jac_dev, s->stream)) return rc;
+  CUDA_TRY(get_rows(tau, s->jac_dev, nd, s->n, s->ns, s->stream));
+  return 0;
+}
+
+static int inv_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_qd, const void* t_qdd, const void* t_par,
+                         const void* t_tau) {
+  if (!s || !q || !t_tau || m < 1 || (!t_q && !t_qd && !t_qdd && !t_par)) return -1;
+  if (t_par && s->par.n == 0) { set_err("inverse dynamics jvp: parameter tangents without installed physical parameters"); return -4; }
+  return 0;
+}
+
+int tds_b200_inverse_dynamics_jvp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int m, const double* t_q,
+                                         const double* t_qd, const double* t_qdd, const double* t_par, double* tau, double* t_tau,
+                                         void* stream) {
+  if (int rc = inv_jvp_check(s, q, m, t_q, t_qd, t_qdd, t_par, t_tau)) return rc;
+  const int n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, ns = s->ns;
+  cudaStream_t sm = (cudaStream_t)stream;
+  double* tin = nullptr;
+  if (t_q || t_qd || t_qdd) {   // the kernel reads the q | qd | qdd tangents as one array
+    CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (size_t)inv_n_in(s) * m * ns));
+    tin = s->jvp_dev;
+    if (int rc = rows_d2d(tin, t_q, n_q * m, ns, sm)) return rc;
+    if (int rc = rows_d2d(tin + (size_t)n_q * m * ns, t_qd, nd * m, ns, sm)) return rc;
+    if (int rc = rows_d2d(tin + (size_t)(n_q + nd) * m * ns, t_qdd, nd * m, ns, sm)) return rc;
+  }
+  return inv_jvp_run(s, q, qd, qdd, m, tin, t_par, tau, t_tau, sm);
+}
+
+int tds_b200_inverse_dynamics_jvp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, int m, const double* t_q,
+                                       const double* t_qd, const double* t_qdd, const double* t_par, double* tau, double* t_tau) {
+  if (int rc = inv_jvp_check(s, q, m, t_q, t_qd, t_qdd, t_par, t_tau)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, k = s->par.n;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; q | qd | qdd contiguous, then the parameters, dtau and tau
+  const size_t ti = (size_t)inv_n_in(s) * m, tp = (size_t)(t_par ? k : 0) * m, to = (size_t)nd * m;
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (ti + tp + to + nd + 1) * ns));
+  double* tin_d = (t_q || t_qd || t_qdd) ? s->jvp_dev : nullptr;
+  double* tp_d = t_par ? s->jvp_dev + ti * ns : nullptr;
+  double* to_d = s->jvp_dev + (ti + tp) * ns;
+  double* tau_d = tau ? to_d + to * ns : nullptr;
+  if (tin_d) {
+    const double* parts[3] = {t_q, t_qd, t_qdd};
+    const size_t rows[3] = {(size_t)n_q * m, (size_t)nd * m, (size_t)nd * m};
+    double* d = tin_d;
+    for (int i = 0; i < 3; d += rows[i] * ns, ++i)
+      CUDA_TRY(parts[i] ? put_rows(d, parts[i], rows[i], n, ns, s->stream) : cudaMemsetAsync(d, 0, sizeof(double) * rows[i] * ns, s->stream));
+  }
+  if (t_par) CUDA_TRY(put_rows(tp_d, t_par, tp, n, ns, s->stream));
+  if (int rc = inv_jvp_run(s, s->q, qd_d, qdd_d, m, tin_d, tp_d, tau_d, to_d, s->stream)) return rc;
+  CUDA_TRY(get_rows(t_tau, to_d, to, n, ns, s->stream));
+  if (tau) CUDA_TRY(get_rows(tau, tau_d, nd, n, ns, s->stream));
+  return 0;
+}
+
+static int inv_vjp_check(tds_b200_sim* s, const void* q, const void* G, const void* g_q, const void* g_qd, const void* g_qdd,
+                         const void* g_par) {
+  if (!s || !q || !G || (!g_q && !g_qd && !g_qdd && !g_par)) return -1;
+  if (g_par && s->par.n == 0) { set_err("inverse dynamics vjp: parameter cotangents without installed physical parameters"); return -4; }
+  return 0;
+}
+
+int tds_b200_inverse_dynamics_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const double* G, double* g_q,
+                                         double* g_qd, double* g_qdd, double* g_par, void* stream) {
+  if (int rc = inv_vjp_check(s, q, G, g_q, g_qd, g_qdd, g_par)) return rc;
+  const int n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, ns = s->ns;
+  cudaStream_t sm = (cudaStream_t)stream;
+  // g_q | g_qd | g_qdd are one array for the contraction: computed in s->vjp_g, then copied out
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)inv_n_in(s) * ns));
+  double* g_in = s->vjp_g;
+  if (int rc = inv_vjp_run(s, q, qd, qdd, G, g_in, g_par, sm)) return rc;
+  if (int rc = rows_d2d(g_q, g_in, n_q, ns, sm)) return rc;
+  if (int rc = rows_d2d(g_qd, g_in + (size_t)n_q * ns, nd, ns, sm)) return rc;
+  return rows_d2d(g_qdd, g_in + (size_t)(n_q + nd) * ns, nd, ns, sm);
+}
+
+int tds_b200_inverse_dynamics_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, const double* G, double* g_q,
+                                       double* g_qd, double* g_qdd, double* g_par) {
+  if (int rc = inv_vjp_check(s, q, G, g_q, g_qd, g_qdd, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, k = s->par.n;
+  const int n_in = inv_n_in(s);
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)(nd + n_in + k + 1) * ns));
+  double* G_d = s->vjp_g;
+  double* gin_d = G_d + (size_t)nd * ns;
+  double* gp_d = gin_d + (size_t)n_in * ns;
+  CUDA_TRY(put_rows(G_d, G, nd, n, ns, s->stream));
+  if (int rc = inv_vjp_run(s, s->q, qd_d, qdd_d, G_d, gin_d, g_par ? gp_d : nullptr, s->stream)) return rc;
+  if (g_q) CUDA_TRY(get_rows(g_q, gin_d, n_q, n, ns, s->stream));
+  if (g_qd) CUDA_TRY(get_rows(g_qd, gin_d + (size_t)n_q * ns, nd, n, ns, s->stream));
+  if (g_qdd) CUDA_TRY(get_rows(g_qdd, gin_d + (size_t)(n_q + nd) * ns, nd, n, ns, s->stream));
+  if (g_par) CUDA_TRY(get_rows(g_par, gp_d, k, n, ns, s->stream));
   return 0;
 }
 

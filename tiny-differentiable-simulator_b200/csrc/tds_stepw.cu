@@ -82,8 +82,15 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // reaches link l it writes l's world transform (pm.xf, the layout of io.link_xf), and the world position p_l + R_l local + O
 // (pm.x) and the 3 x n_qd Jacobian (pm.J, jacobian.hpp:13-83) of every point on l.  Returns before pass 2.  Row r of a output at
 // out[r * ns + e] (fp64 instance), or its dual part as column j of an m-column Jacobian, out[(r * m + j) * ns + e] (JV instance).
+// INV: inverse dynamics tau = ID(q, qd, qdd) by the recursive Newton-Euler algorithm (DESIGN.md section 7.14), launched in MODE_NOCONTACT
+// with the simulator's gravity.  qdd arrives in io.tau_in [n_qd][ns] (null: zero; so does a null io.qd_in), tangent input index
+// n_q + n_qd + k.  Pass 1 carries the accelerations a_i = a_parent + S_i qdd_i + v_i x (S_i qd_i) along with v (a_base = -g, or the
+// floating base's R_b qdd[0:6] - g), forms f_i = r_i a_i + v_i x* (r_i v_i) from the rigid inertia about O and adds S_j . f_i to tau_j
+// for i and its moving ancestors j (all in the common frame: no transforms); a branch point's a_i is kept over its rigid-inertia words,
+// which nothing else reads.  Then the stiffness and damping terms the ABA subtracts, the floating base's wrench in the base frame, and
+// tau [n_qd] at io.jac[r * ns + e] (fp64 instance) or its dual part at io.jac[(r * m + j) * ns + e] (JV instance).  Returns before pass 2.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
-          bool KIN = false>
+          bool KIN = false, bool INV = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
@@ -177,12 +184,36 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   RS* const Mb = A.ptr<RS>(M.x_M);
   RS* const dinv = A.ptr<RS>(M.x_dinv);
   RS* const wv = A.ptr<RS>(M.x_w);
+  // INV only (the step's own statements of these two stay inline: its code must not change).  quaternion_axis_angle(q) of spherical
+  // joint i, the vector its stiffness multiplies (forward_dynamics.hpp:69-74, tiny_algebra.hpp:509-527)
+  auto axis_angle = [&](int i) -> V3<RC> {
+    const int q0 = M.q_idx[i];
+    const RC qx = RC(qv[q0 * ST]), qy = RC(qv[(q0 + 1) * ST]), qz = RC(qv[(q0 + 2) * ST]), qw = RC(qv[(q0 + 3) * ST]);
+    const RC nrm = sqrt_t(qx * qx + qy * qy + qz * qz);
+    const RC theta = RC(2) * atan2_t(nrm, qw);
+    const RC scaling = nrm < RC(1.220703125e-4) ? RC(1) / (RC(0.5) + theta * theta * RC(1.0 / 48.0)) : theta / nrm;   // eps^(1/4)
+    return v3<RC>(scaling * qx, scaling * qy, scaling * qz);
+  };
+  // installed base quantities: (m, h, I about the origin) packed per lane as tds_rbi_pack does on the host (the block after pass 2)
+  auto installed_base = [&](Rbi<RP>& bp) {
+    RP b[10];
+    for (int c = 0; c < 10; ++c) b[c] = par_of(body_slot(0, c), M.base_rbic[c]);
+    const RP cc = b[1] * b[1] + b[2] * b[2] + b[3] * b[3];
+    bp.m = b[0];
+    bp.h = v3<RP>(b[0] * b[1], b[0] * b[2], b[0] * b[3]);
+    bp.I.xx = b[4] + b[0] * (cc - b[1] * b[1]);
+    bp.I.xy = b[5] - b[0] * b[1] * b[2];
+    bp.I.xz = b[6] - b[0] * b[1] * b[3];
+    bp.I.yy = b[7] + b[0] * (cc - b[2] * b[2]);
+    bp.I.yz = b[8] - b[0] * b[2] * b[3];
+    bp.I.zz = b[9] + b[0] * (cc - b[3] * b[3]);
+  };
 
   // ---- load state, PD torques (locomotion_contact_simulation.h:168-258) ---------------------------
   // input directions of the differentiable instance: q | qd | tau or action | kp, kd, max_force (with PD)
   const int in0 = M.n_q + n;
   for (int k = 0; k < M.n_q; ++k) qv[k * ST] = seed(RQ(io.q_in[(size_t)k * ns + e]), k);
-  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(io.qd_in[(size_t)k * ns + e]), M.n_q + k);
+  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ((INV && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
   for (int k = 0; k < n; ++k) tauv[k * ST] = RQ(0.f);
   if (!MASS && use_pd) {
     const RQ kp = seed(RQ(E.kp), in0 + E.n_act), kd = seed(RQ(E.kd), in0 + E.n_act + 1), fmax_ = seed(RQ(E.max_force), in0 + E.n_act + 2);
@@ -195,11 +226,11 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       f = min_t(max_t(f, -fmax_), fmax_);
       tauv[M.qd_idx[li] * ST] = f;
     }
-  } else if (!MASS && io.tau_in) {
+  } else if (!MASS && !INV && io.tau_in) {
     const int off = M.floating ? 6 : 0;
     for (int k = off; k < n; ++k) tauv[k * ST] = seed(RQ(io.tau_in[(size_t)(k - off) * ns + e]), in0 + k - off);
   }
-  if constexpr (!KIN) {   // (the KIN lanes return before pass 2 reads the accumulators)
+  if constexpr (!KIN && !INV) {   // (the KIN and INV lanes return before pass 2 reads the accumulators)
     for (int s = 0; s < M.n_acc; ++s) {
       RA* pa = A.ptr<RA>(M.x_acc + s * M.x_acc_words);
       for (int k = 0; k < 27; ++k) pa[k * ST] = RA(0);
@@ -345,6 +376,28 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   { RC* px = A.ptr<RC>(M.x_xw); st9<RC>(px, ST, R_base); st3<RC>(px + 9 * ST, ST, p_base); }
   if (want_contacts) emit_geoms(-1, R_base, p_base);
   if constexpr (KIN) kin_link(-1, R_base, p_base);
+  // INV: qdd of dof k (seeded at input n_q + n_qd + k); the acceleration of the previous link, of the base; the sum of the link forces
+  auto qdd_in = [&](int k) -> RQ { return seed(RQ(io.tau_in ? io.tau_in[(size_t)k * ns + e] : 0.f), M.n_q + n + k); };
+  // (empty placeholders in the other instances, whose code must not change)
+  typedef typename std::conditional<INV, Sv<RC>, NoPar>::type SvInv;
+  const SvInv a_base_inv = [&]() -> SvInv {
+    if constexpr (INV) {
+      static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the INV instances run in one scalar type");
+      const V3<RC> g = v3<RC>(RC(P.gravity[0]), RC(P.gravity[1]), RC(P.gravity[2]));
+      Sv<RC> a;
+      a.top = v3<RC>(RC(0), RC(0), RC(0));
+      a.bot = v3<RC>(-g.x, -g.y, -g.z);
+      if (M.floating) {   // the base-frame spatial acceleration qdd[0:6] in the common frame (O is the base origin)
+        a.top = mul(Rb, v3<RC>(qdd_in(0), qdd_in(1), qdd_in(2)));
+        a.bot = mul(Rb, v3<RC>(qdd_in(3), qdd_in(4), qdd_in(5))) - g;
+      }
+      return a;
+    } else {
+      return SvInv{};
+    }
+  }();
+  SvInv a_prev_inv = a_base_inv, f_links = SvInv{};
+  if constexpr (INV) { f_links.top = v3<RC>(RC(0), RC(0), RC(0)); f_links.bot = f_links.top; }
   for (int i = 0; i < n_links; ++i) {
     const int p = M.parent[i];
     const int fl = M.flags[i];
@@ -404,6 +457,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     st6<RC>(Sw + i * 6 * ST, ST, S);
     if (M.xw_slot[i] >= 0) { RC* px = A.ptr<RC>(M.x_xw + (M.xw_slot[i] + 1) * 12 * RCW); st9<RC>(px, ST, Ri); st3<RC>(px + 9 * ST, ST, pi); }
     // rigid-body inertia about O in world axes: com c = p_i + R_i com_l, I = R Icom R^T + m (|c|^2 1 - c c^T)
+    typename std::conditional<INV, Rbi<RC>, NoPar>::type r_inv;   // (INV: kept for f_i below)
     if constexpr (!KIN) {
       const double* rb = M.rbic[i];
       auto rbc = [&](int c) -> RP { return par_of(body_slot(i + 1, c), rb[c]); };
@@ -419,7 +473,8 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       const RC cc = dot(c, c);
       r.I.xx += r.m * (cc - c.x * c.x); r.I.yy += r.m * (cc - c.y * c.y); r.I.zz += r.m * (cc - c.z * c.z);
       r.I.xy -= r.m * c.x * c.y; r.I.xz -= r.m * c.x * c.z; r.I.yz -= r.m * c.y * c.z;
-      st_rbi<RC>(A.ptr<RC>(M.x_link + i * LWD), ST, r);
+      if constexpr (INV) r_inv = r;
+      else st_rbi<RC>(A.ptr<RC>(M.x_link + i * LWD), ST, r);
     }
     Sv<RA> v = vp;
     if (fl & TDS_LF_SPHERICAL) {
@@ -445,9 +500,64 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       o[(size_t)9 * ns] = (float)val_of(pi.x + O.x); o[(size_t)10 * ns] = (float)val_of(pi.y + O.y); o[(size_t)11 * ns] = (float)val_of(pi.z + O.z);
     }
     if constexpr (KIN) kin_link(i, Ri, pi);
+    if constexpr (INV) {
+      Sv<RC> a;
+      if (fl & TDS_LF_PARENT_ADJ) a = a_prev_inv;
+      else if (p >= 0) a = ld6<RC>(A.ptr<RC>(M.x_link + p * LWD), ST);
+      else a = a_base_inv;
+      Sv<RC> vJ; vJ.top = v3<RC>(RC(0), RC(0), RC(0)); vJ.bot = vJ.top;
+      for (int c = 0; c < n_cols(i); ++c) {
+        const Sv<RC> Sc = (fl & TDS_LF_SPHERICAL) ? S_col(i, c) : S;
+        const RC qdc = qdv[(M.qd_idx[i] + c) * ST], qddc = qdd_in(M.qd_idx[i] + c);
+        vJ.top = axpy(Sc.top, qdc, vJ.top); vJ.bot = axpy(Sc.bot, qdc, vJ.bot);
+        a.top = axpy(Sc.top, qddc, a.top); a.bot = axpy(Sc.bot, qddc, a.bot);
+      }
+      a = a + cross_mm(v, vJ);                               // kinematics.hpp:96-97
+      const Sv<RC> f = rbi_mul(r_inv, a) + cross_mf(v, rbi_mul(r_inv, v));
+      for (int j = i; j >= 0; j = M.parent[j])               // the chain walk of crba_ancestors, from i itself
+        for (int c = 0; c < n_cols(j); ++c) tauv[(M.qd_idx[j] + c) * ST] += dot(S_col(j, c), f);
+      f_links = f_links + f;
+      st6<RC>(A.ptr<RC>(M.x_link + i * LWD), ST, a);
+      a_prev_inv = a;
+    }
     R_prev = Ri; p_prev = pi; v_prev = v;
   }
   if constexpr (KIN) return;
+  if constexpr (INV) {
+    for (int i = 0; i < n_links; ++i) {   // the stiffness and damping terms the ABA subtracts from tau
+      const int fl = M.flags[i];
+      if (fl & TDS_LF_FIXED) continue;
+      const int d0 = M.qd_idx[i];
+      if (fl & TDS_LF_SPHERICAL) {
+        const RC d = joint_par(i, 1, M.damping[i]);
+        for (int c = 0; c < 3; ++c) tauv[(d0 + c) * ST] += d * qdv[(d0 + c) * ST];
+        if (M.stiffness[i] != 0.f || joint_slot(i, 0) >= 0) {
+          const V3<RC> aa = axis_angle(i);
+          const RC k = joint_par(i, 0, M.stiffness[i]);
+          tauv[d0 * ST] += k * aa.x; tauv[(d0 + 1) * ST] += k * aa.y; tauv[(d0 + 2) * ST] += k * aa.z;
+        }
+      } else {
+        tauv[d0 * ST] += joint_par(i, 0, M.stiffness[i]) * qv[M.q_idx[i] * ST] + joint_par(i, 1, M.damping[i]) * qdv[d0 * ST];
+      }
+    }
+    if (M.floating) {   // the base's wrench [moment about the base origin; force] in the base frame
+      Rbi<RC> Ib = model_rbi_of<RC>(M.base_rbi);
+      if constexpr (PAR) { if (pm.any_base) installed_base(Ib); }
+      Sv<RC> vb, ab;
+      vb.top = v3<RC>(qdv[0], qdv[ST], qdv[2 * ST]); vb.bot = v3<RC>(qdv[3 * ST], qdv[4 * ST], qdv[5 * ST]);
+      ab.top = mulT(Rb, a_base_inv.top); ab.bot = mulT(Rb, a_base_inv.bot);
+      Sv<RC> fb = rbi_mul(Ib, ab) + cross_mf(vb, rbi_mul(Ib, vb));
+      fb.top = fb.top + mulT(Rb, f_links.top); fb.bot = fb.bot + mulT(Rb, f_links.bot);
+      tauv[0] += fb.top.x; tauv[ST] += fb.top.y; tauv[2 * ST] += fb.top.z;
+      tauv[3 * ST] += fb.bot.x; tauv[4 * ST] += fb.bot.y; tauv[5 * ST] += fb.bot.z;
+    }
+    if (live && io.jac)
+      for (int k = 0; k < n; ++k) {
+        if constexpr (AD) io.jac[((size_t)k * io.jac_n_in + jcol) * ns + e] = tauv[k * ST].d;
+        else io.jac[(size_t)k * ns + e] = tauv[k * ST];
+      }
+    return;
+  }
   // ---- contacts between the multibodies of the world (world.hpp:206-282), group = ordered pair of multibodies -----------------------
   // contact_sphere_sphere (contact_point.hpp:44-94) on sphere centres / capsule end spheres (contact_capsule_sphere, :406-438);
   // sphere A x capsule B goes through the dispatcher's swapped call (:478-492): points exchanged, normal negated.

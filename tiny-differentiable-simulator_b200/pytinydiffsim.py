@@ -6,6 +6,7 @@
     forward_dynamics(mb, gravity), integrate_euler(mb, dt), integrate_euler_qdd(mb, dt)   :659-663
     mass_matrix(mb[, q])                                                      :659-663 (mass_matrix.hpp)
     point_jacobian(mb, link_index, point, is_local_point=False)               (jacobian.hpp:85-90)
+    inverse_dynamics(mb, q, qd, qdd, gravity), bias_forces(mb, q, qd, gravity)   (inverse_dynamics.hpp)
     VectorizedLaikagoEnv, VectorizedAntEnv (pytinydiffsim_includes.h:58-227), CartpoleEnv (:1123)
 
 The fine-grained calls operate on one MultiBody like the reference's; each is one stage of the GPU path (forward dynamics =
@@ -168,6 +169,25 @@ def mass_matrix(mb, q=None):
     mb.q, and mass_matrix(mb, q) at a q given explicitly (mb.q is left as it is)."""
     qv = np.asarray(mb.q if q is None else q, dtype=np.float64).reshape(1, -1)
     return mb._sim.mass_matrix_host(qv)[0]
+
+
+def inverse_dynamics(mb, q, qd, qdd, gravity):
+    """The joint forces tau for which the multibody has the accelerations qdd at (q, qd) under `gravity`: a NumPy float64 [num_dofs]
+    array, by the recursive Newton-Euler algorithm of the GPU path in fp64 at the fp32-rounded inputs (DESIGN.md section 7.14).  A
+    floating base's 6 rows are the wrench on the base in the base frame for the base-frame acceleration qdd[0:6], gravity rotated into
+    the base frame.  The reference's Python binding of it is not pinned here; this follows the C++ free function
+    inverse_dynamics(mb, q, qd, qdd, gravity) of inverse_dynamics.hpp.  mb is left as it is."""
+    mb._params(gravity=tuple(np.asarray(gravity, dtype=np.float64)))
+    row = lambda x: np.asarray(x, dtype=np.float64).reshape(1, -1)
+    return mb._sim.inverse_dynamics_host(row(q), row(qd), row(qdd))[0]
+
+
+def bias_forces(mb, q, qd, gravity):
+    """The bias forces h(q, qd) = inverse_dynamics(mb, q, qd, 0, gravity): a NumPy float64 [num_dofs] array.  Follows the C++ free
+    function bias_forces(mb, q, qd, gravity) of inverse_dynamics.hpp.  mb is left as it is."""
+    mb._params(gravity=tuple(np.asarray(gravity, dtype=np.float64)))
+    row = lambda x: np.asarray(x, dtype=np.float64).reshape(1, -1)
+    return mb._sim.inverse_dynamics_host(row(q), row(qd), None)[0]
 
 
 def point_jacobian(mb, link_index, point, is_local_point=False):

@@ -371,6 +371,98 @@ class BatchSim:
         st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
         self._check(self._L.tds_b200_mass_matrix_vjp_device(self._h, _ptr(q), _ptr(G), _ptr(g_q), _ptr(g_par), st), "mass_matrix_vjp_device")
 
+    # ---- inverse dynamics tau = ID(q, qd, qdd) (DESIGN.md section 7.14) ----
+    def _inv_in(self, x, dim, what):
+        if x is None:
+            return None
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        if x.shape != (self.n_envs, dim):
+            raise ValueError(f"{what}: [n_envs, {dim}] expected, got {x.shape}")
+        return x
+
+    def inverse_dynamics_host(self, q, qd=None, qdd=None):
+        """tau [n, n_qd] float64: the joint forces for which every environment has the accelerations qdd at (q, qd) under the
+        simulator's gravity, by the recursive Newton-Euler algorithm in fp64 at the fp32-rounded q [n, n_q], qd, qdd [n, n_qd] (None:
+        zero; the bias forces are inverse_dynamics_host(q, qd)).  Fixed base: the inverse of MODE_FD, stiffness and damping terms
+        included; floating base: rows 0..5 are the base wrench in the base frame for the base-frame acceleration qdd[0:6] (include/tds_b200.h).
+        Installed physical parameters give each environment its own masses, inertias, stiffness and damping."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        tau = np.zeros((self.n_envs, self.n_qd))
+        self._check(self._L.tds_b200_inverse_dynamics_host(self._h, _dp(q), _dp(qd), _dp(qdd), _dp(tau)), "inverse_dynamics_host")
+        return tau
+
+    def inverse_dynamics_device(self, q, qd, qdd, tau, stream=None):
+        """Device version of inverse_dynamics_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd and qdd [n_qd, n_stride]
+        (either may be None), tau float64 [n_qd, n_stride].  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_inverse_dynamics_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(tau), st), "inverse_dynamics_device")
+
+    def inverse_dynamics_jvp_host(self, q, qd, qdd, t_q=None, t_qd=None, t_qdd=None, t_par=None):
+        """Directional derivatives of tau: dtau [n, n_qd, m] along the m tangents t_q [n, n_q, m], t_qd and t_qdd [n, n_qd, m] and t_par
+        [n, k, m] of the installed parameters (each may be None, not all); tangents given as [n, dim] are m = 1 and the result is then
+        [n, n_qd].  Returns (tau, dtau)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        k = len(self.param_ids)
+        given = [t for t in (t_q, t_qd, t_qdd, t_par) if t is not None]
+        if not given:
+            raise ValueError("at least one tangent is expected")
+        single = np.ndim(given[0]) == 2
+
+        def prep(x, dim):
+            if x is None:
+                return None
+            x = np.asarray(x, dtype=np.float64)
+            if x.ndim == 2:
+                x = x[:, :, None]
+            if x.shape[:2] != (self.n_envs, dim):
+                raise ValueError(f"tangent: [n_envs, {dim}, m] or [n_envs, {dim}] expected, got {x.shape}")
+            return np.ascontiguousarray(x)
+        ts = [prep(t_q, self.n_q), prep(t_qd, self.n_qd), prep(t_qdd, self.n_qd), prep(t_par, k)]
+        ms = {t.shape[2] for t in ts if t is not None}
+        if len(ms) != 1:
+            raise ValueError("tangents: the same number of tangents m expected")
+        m = ms.pop()
+        tau = np.zeros((self.n_envs, self.n_qd))
+        dtau = np.zeros((self.n_envs, self.n_qd, m))
+        self._check(self._L.tds_b200_inverse_dynamics_jvp_host(self._h, _dp(q), _dp(qd), _dp(qdd), m, *(_dp(t) for t in ts), _dp(tau),
+                                                               _dp(dtau)), "inverse_dynamics_jvp_host")
+        return tau, (dtau[..., 0] if single else dtau)
+
+    def inverse_dynamics_jvp_device(self, q, qd, qdd, m, t_q, t_qd, t_qdd, t_par, t_tau, tau=None, stream=None):
+        """Device version of inverse_dynamics_jvp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None); t_q
+        [n_q * m, n_stride], t_qd and t_qdd [n_qd * m, n_stride], t_par [k * m, n_stride] (each may be None, not all), t_tau
+        [n_qd * m, n_stride] and tau [n_qd, n_stride] (or None) float64 CUDA tensors, entry (c, j) at row c * m + j.  Asynchronous."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_inverse_dynamics_jvp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), int(m), _ptr(t_q), _ptr(t_qd),
+                                                                 _ptr(t_qdd), _ptr(t_par), _ptr(tau), _ptr(t_tau), st),
+                    "inverse_dynamics_jvp_device")
+
+    def inverse_dynamics_vjp_host(self, q, qd, qdd, G):
+        """Cotangent G [n, n_qd] of tau -> (g_q [n, n_q], g_qd [n, n_qd], g_qdd [n, n_qd], g_par [n, k] or None without installed
+        parameters): g_x = sum_r G[r] dtau[r]/dx."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        G = self._inv_in(G, self.n_qd, "G")
+        k = len(self.param_ids)
+        g_q, g_qd, g_qdd = np.zeros((self.n_envs, self.n_q)), np.zeros((self.n_envs, self.n_qd)), np.zeros((self.n_envs, self.n_qd))
+        g_par = np.zeros((self.n_envs, k)) if k else None
+        self._check(self._L.tds_b200_inverse_dynamics_vjp_host(self._h, _dp(q), _dp(qd), _dp(qdd), _dp(G), _dp(g_q), _dp(g_qd), _dp(g_qdd),
+                                                               _dp(g_par)), "inverse_dynamics_vjp_host")
+        return g_q, g_qd, g_qdd, g_par
+
+    def inverse_dynamics_vjp_device(self, q, qd, qdd, G, g_q, g_qd, g_qdd, g_par=None, stream=None):
+        """Device version of inverse_dynamics_vjp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None), G float64
+        [n_qd, n_stride], g_q [n_q, n_stride], g_qd and g_qdd [n_qd, n_stride], g_par [k, n_stride] float64 CUDA tensors (each may be
+        None, not all).  Asynchronous on the stream."""
+        import torch
+        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        self._check(self._L.tds_b200_inverse_dynamics_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(G), _ptr(g_q), _ptr(g_qd),
+                                                                 _ptr(g_qdd), _ptr(g_par), st), "inverse_dynamics_vjp_device")
+
     # ---- forward kinematics and linear point Jacobians (DESIGN.md section 7.13) ----
     @staticmethod
     def _points(links, local):
