@@ -407,16 +407,15 @@ struct tds_b200_sim {
   DevModel dm[3];         // one layout per precision mode
   DevModel dm_ad;         // layout of the differentiable instance (dual numbers, 16-byte scalars)
   char* jac_scratch = nullptr; size_t jac_scratch_bytes = 0;
-  double* jac_dev = nullptr; size_t jac_dev_bytes = 0;
+  double* jac_dev = nullptr; size_t jac_dev_bytes = 0;   // host paths' Jacobians, tangents and values; the ID device JVP's tangents
   // vector-Jacobian product: tape capacity in nodes per lane (grows by doubling when a run overflows, and stays grown),
   // its node / adjoint / arena buffers, the overflow flag, device staging of the host path
   int tape_cap = 4096;
   char* vjp_buf = nullptr; size_t vjp_buf_bytes = 0;
   int* vjp_flag = nullptr;
-  double* vjp_g = nullptr; size_t vjp_g_bytes = 0;
-  double* jvp_dev = nullptr; size_t jvp_dev_bytes = 0;   // Jacobian-vector product, host path: t_in | t_par | t_out on the device
+  double* vjp_g = nullptr; size_t vjp_g_bytes = 0;   // (also the cotangents G | g of the dynamics queries' VJPs)
   DevModel dm_m;          // layout of the fp64 mass-matrix instance (8-byte scalars)
-  double* mass_dev = nullptr; size_t mass_dev_bytes = 0; // mass matrix: identity tangents | dM of the VJP, host-path staging
+  double* mass_dev = nullptr; size_t mass_dev_bytes = 0; // dynamics queries' VJPs: identity tangents | output columns of a chunk
   // installed physical parameters (tds_b200_set_physical_params_*): slot map (par.n == 0: none) and values [k][ns] fp64
   ParMap par;
   double* par_dev = nullptr; size_t par_dev_bytes = 0;
@@ -507,7 +506,7 @@ static int ensure_scratch(tds_b200_sim* s, int prec) {
   return 0;
 }
 
-// Entry of a host path that reuses the simulator's derivative buffers (jac_scratch, jac_dev, jvp_dev, vjp_g, mass_dev): selects the
+// Entry of a host path that reuses the simulator's derivative buffers (jac_scratch, jac_dev, vjp_g, mass_dev): selects the
 // device and waits for device work already queued.  A device entry point of this simulator may still be running on a caller's
 // stream with these buffers, and the simulator's own stream, which the host path runs on, is not ordered against that stream.
 static int enter_derivative_host(tds_b200_sim* s) {
@@ -695,7 +694,7 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->rq); cudaFree(s->rqd); cudaFree(s->zero_act); cudaFree(s->pol_act); cudaFree(s->sticky); cudaFree(s->r_total);
   cudaFree(s->pol_params); cudaFree(s->act_qidx); cudaFree(s->r_steps);
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
-  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->jvp_dev); cudaFree(s->mass_dev);
+  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->mass_dev);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
@@ -885,11 +884,27 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
   return 0;
 }
 
-// tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null); mass: of the mass matrix
-// (t_in = the q tangents; the step's arguments are not read); kin: of the kinematics of this point table and these outputs (t_in =
-// the q tangents, t_par unused); inv: of the inverse dynamics (t_in = the q | qd | qdd tangents; qd and qdd in the step's qd and
-// tau_or_action)
-struct JvpTangents { const double* t_in; const double* t_par; int m; bool mass = false; const TdsKinCall* kin = nullptr; bool inv = false; };
+// what a Jacobian-vector product differentiates: the step, or one of the dynamics queries of DESIGN.md sections 7.12-7.14
+enum class Query { step, mass, kin, inv };
+
+// tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
+// inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
+// (t_in = the q tangents, t_par unused); inv: t_in = the q | qd | qdd tangents (qd and qdd in the step's qd and tau_or_action)
+struct JvpTangents { const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr; };
+
+// the installed physical parameters as a launch argument in *pmv, or NULL without any
+static const ParMap* installed_par(const tds_b200_sim* s, ParMap* pmv) {
+  *pmv = s->par;
+  pmv->values = s->par_dev; pmv->grad = nullptr;
+  return s->par.n > 0 ? pmv : nullptr;
+}
+
+// -4 with "<what> without installed physical parameters" when parameter tangents or cotangents `par` come without any installed
+static int par_without_installed(const tds_b200_sim* s, const void* par, const char* what) {
+  if (!par || s->par.n > 0) return 0;
+  set_err(std::string(what) + " without installed physical parameters");
+  return -4;
+}
 
 // scratch of one launch of a world-frame instance of layout M over every environment: x_total words per lane
 static size_t lane_arena_bytes(const tds_b200_sim* s, const DevModel& M) {
@@ -914,21 +929,28 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   io.q_in = q; io.qd_in = qd; io.tau_in = tau_or_action;
   io.jac = jac; io.jac_n_in = n_dirs;
   io.n = s->n; io.n_stride = s->ns;
-  ParMap pmv = s->par;
-  pmv.values = s->par_dev; pmv.grad = nullptr;
-  const ParMap* pm = s->par.n > 0 ? &pmv : nullptr;
+  ParMap pmv;
+  const ParMap* pm = installed_par(s, &pmv);
   const int chunk = std::min(dir_chunk(s), n_dirs);
   CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_ad) * chunk));
+  const cudaStream_t sm = (cudaStream_t)stream;
   for (int d0 = 0; d0 < n_dirs; d0 += chunk) {
     io.jac_dir0 = dir_base + d0;
     const int nd = n_dirs - d0 < chunk ? n_dirs - d0 : chunk;
-    int rc = (jv && jv->inv) ? tds_launch_inv_jvp(&s->dm_ad, &s->P, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
-           : (jv && jv->kin) ? tds_launch_kin_jvp(&s->dm_ad, &io, jv->kin, jv->t_in, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
-           : (jv && jv->mass) ? tds_launch_mass_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, (cudaStream_t)stream)
-           : jv ? tds_launch_stepw_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch,
-                                       (cudaStream_t)stream)
-           : pm ? tds_launch_stepw_jacobian_par(&s->dm_ad, &s->P, &s->E, &io, pm, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream)
-                : tds_launch_stepw_jacobian(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, nd, s->jac_scratch, (cudaStream_t)stream);
+    int rc = 0;
+    if (!jv) {
+      rc = pm ? tds_launch_stepw_jacobian_par(&s->dm_ad, &s->P, &s->E, &io, pm, mode, use_pd, nd, s->jac_scratch, sm)
+              : tds_launch_stepw_jacobian(&s->dm_ad, &s->P, &s->E, &io, mode, use_pd, nd, s->jac_scratch, sm);
+    } else {
+      switch (jv->query) {
+        case Query::step:
+          rc = tds_launch_stepw_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch, sm);
+          break;
+        case Query::mass: rc = tds_launch_mass_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
+        case Query::kin: rc = tds_launch_kin_jvp(&s->dm_ad, &io, jv->kin, jv->t_in, jv->m, nd, s->jac_scratch, sm); break;
+        case Query::inv: rc = tds_launch_inv_jvp(&s->dm_ad, &s->P, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
+      }
+    }
     if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
   }
   return 0;
@@ -990,8 +1012,7 @@ static int jvp_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const
   if (!s || !q || !qd || !t_out || m < 1 || (!t_in && !t_par) || (use_pd && !tau_or_action)) return -1;
   if (mode == 3) { set_err("jvp: modes FD, NOCONTACT, FULL"); return -2; }
   if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
-  if (t_par && s->par.n == 0) { set_err("jvp: parameter tangents without installed physical parameters"); return -4; }
-  return 0;
+  return par_without_installed(s, t_par, "jvp: parameter tangents");
 }
 
 int tds_b200_step_jvp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
@@ -1008,65 +1029,83 @@ int tds_b200_step_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* 
   const int n = s->n, ns = s->ns, k = s->par.n;
   int dims[2];
   tds_b200_jacobian_dims(s, mode, use_pd, dims);
-  // tangents: host [n][dim][m] <-> device [dim * m][ns]
-  const size_t ti = (size_t)dims[1] * m, tp = (size_t)(t_par ? k : 0) * m, to = (size_t)dims[0] * m;
-  CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (ti + tp + to) * ns));
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; t_in | t_par | t_out
+  const size_t ti = (size_t)(t_in ? dims[1] : 0) * m, tp = (size_t)(t_par ? k : 0) * m, to = (size_t)dims[0] * m;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + tp + to) * ns));
   if (int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action)) return rc;
-  double* tin_d = t_in ? s->jvp_dev : nullptr;
-  double* tpar_d = t_par ? s->jvp_dev + ti * ns : nullptr;
-  double* tout_d = s->jvp_dev + (ti + tp) * ns;
-  if (t_in) CUDA_TRY(put_rows(tin_d, t_in, ti, n, ns, s->stream));
-  if (t_par) CUDA_TRY(put_rows(tpar_d, t_par, tp, n, ns, s->stream));
-  CUDA_TRY(cudaMemsetAsync(tout_d, 0, sizeof(double) * to * ns, s->stream));
-  const JvpTangents jv{tin_d, tpar_d, m};
+  double* tout_d = s->jac_dev + (ti + tp) * ns;
+  CUDA_TRY(put_parts<double>(s->jac_dev, {{t_in, ti}, {t_par, tp}, {nullptr, to}}, n, ns, s->stream));
+  const JvpTangents jv{t_in ? s->jac_dev : nullptr, t_par ? s->jac_dev + ti * ns : nullptr, m};
   if (int rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, tout_d, s->stream, false, &jv)) return rc;
   CUDA_TRY(get_rows(t_out, tout_d, to, n, ns, s->stream));
   return 0;
 }
 
-// ---- joint-space mass matrix M(q) (DESIGN.md section 7.12): the MASS instances of the world-frame kernel (tds_mass.cu) ------------------
-// M [n_qd * n_qd][ns] from q [n_q][ns] fp32, one lane per environment on the 8-byte layout
-static int mass_run(tds_b200_sim* s, const float* q, double* Mo, cudaStream_t sm) {
+// ---- dynamics queries (DESIGN.md sections 7.12-7.14): the mass matrix, forward kinematics and inverse dynamics by the MASS, KIN and
+// INV instances of the world-frame kernel.  Each query has one value launch (value_run), its JVP through the Jacobian's chunk loop
+// (jacobian_run) and its VJP by identity tangents (vjp_by_eye).
+
+extern "C++" {   // (templates)
+// Value of a dynamics query, one lane per environment on the 8-byte layout: launch(io, installed parameters or NULL) with the inputs
+// q [n_q][ns] and qd, qdd [n_qd][ns] fp32 (NULL: zero) and the output rows `out` in io
+template <typename Launch>
+static int value_run(tds_b200_sim* s, const char* what, const float* q, const float* qd, const float* qdd, double* out, Launch launch) {
   StepIO io;
   memset(&io, 0, sizeof(io));
-  io.q_in = q; io.jac = Mo; io.jac_n_in = 1;
+  io.q_in = q; io.qd_in = qd; io.tau_in = qdd; io.jac = out; io.jac_n_in = 1;
   io.n = s->n; io.n_stride = s->ns;
-  ParMap pmv = s->par;
-  pmv.values = s->par_dev; pmv.grad = nullptr;
+  ParMap pmv;
   CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_m)));
-  const int rc = tds_launch_mass(&s->dm_m, &io, s->par.n > 0 ? &pmv : nullptr, s->jac_scratch, sm);
-  if (rc) set_err(std::string("mass matrix launch: ") + cudaGetErrorString((cudaError_t)rc));
+  const int rc = launch(&io, installed_par(s, &pmv));
+  if (rc) set_err(std::string(what) + " launch: " + cudaGetErrorString((cudaError_t)rc));
   return rc;
+}
+
+// VJP of a dynamics query with `rows` output rows: g_in [n_in][ns] and g_par [k][ns] = <G, dO> for the cotangent G [rows][ns], along
+// the identity tangents of the n_in inputs and, only when g_par is wanted (not NULL), of the k installed parameters.  jvp(nd, t_in,
+// t_par, dO) runs the query's JVP of nd directions into dO [rows * nd][ns]; the directions run in chunks whose tangents and dO stay
+// within 1 GB (s->mass_dev).  A direction's dual lane and its contraction do not depend on the other directions or the chunking.
+template <typename Jvp>
+static int vjp_by_eye(tds_b200_sim* s, const char* what, int n_in, size_t rows, const double* G, double* g_in, double* g_par,
+                      cudaStream_t sm, Jvp jvp) {
+  const int k = g_par ? s->par.n : 0, ns = s->ns, total = n_in + k;
+  const size_t per_dir = sizeof(double) * (rows + total) * ns;   // dO + identity tangents of one direction
+  const int chunk = std::min(total, std::max(1, (int)(((size_t)1 << 30) / per_dir)));
+  CUDA_TRY(grow_dev(&s->mass_dev, &s->mass_dev_bytes, per_dir * chunk));
+  for (int d0 = 0; d0 < total; d0 += chunk) {
+    const int nd = std::min(chunk, total - d0);
+    double* t_in = s->mass_dev;
+    double* t_par = k > 0 ? t_in + (size_t)n_in * nd * ns : nullptr;
+    double* dO = t_in + (size_t)total * nd * ns;
+    int rc = tds_launch_mass_eye(t_in, t_par, n_in, k, d0, nd, ns, sm);
+    if (!rc) rc = jvp(nd, t_in, t_par, dO);
+    if (!rc) rc = tds_launch_mass_contract(G, dO, (int)rows, nd, d0, n_in, g_in, g_par, s->n, ns, sm);
+    if (rc) { set_err(std::string(what) + " vjp: " + cudaGetErrorString((cudaError_t)rc)); return rc; }
+  }
+  return 0;
+}
+}  // extern "C++"
+
+// ---- joint-space mass matrix M(q) (DESIGN.md section 7.12): the MASS instances of the world-frame kernel (tds_mass.cu) ------------------
+// M [n_qd * n_qd][ns] from q [n_q][ns] fp32
+static int mass_run(tds_b200_sim* s, const float* q, double* Mo, cudaStream_t sm) {
+  return value_run(s, "mass matrix", q, nullptr, nullptr, Mo, [&](const StepIO* io, const ParMap* pm) {
+    return tds_launch_mass(&s->dm_m, io, pm, s->jac_scratch, sm);
+  });
 }
 
 static int mass_jvp_run(tds_b200_sim* s, const float* q, int m, const double* t_q, const double* t_par, double* Mo, double* t_M,
                         cudaStream_t sm) {
   if (Mo) { if (int rc = mass_run(s, q, Mo, sm)) return rc; }
-  JvpTangents jv{t_q, t_par, m};
-  jv.mass = true;
+  const JvpTangents jv{t_q, t_par, m, Query::mass};
   return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, nullptr, nullptr, t_M, sm, false, &jv);
 }
 
-// g = G : dM along the n_q + k identity tangents, in chunks of directions whose dM stays within 1 GB
 static int mass_vjp_run(tds_b200_sim* s, const float* q, const double* G, double* g_q, double* g_par, cudaStream_t sm) {
-  const int n_q = s->dm[0].n_q, nn = s->dm[0].n_qd * s->dm[0].n_qd, k = s->par.n, ns = s->ns;
-  const int total = n_q + k;
-  const size_t per_dir = sizeof(double) * (size_t)(nn + total) * ns;   // dM + identity tangents of one direction
-  int chunk = (int)(((size_t)1 << 30) / per_dir);
-  if (chunk < 1) chunk = 1;
-  if (chunk > total) chunk = total;
-  CUDA_TRY(grow_dev(&s->mass_dev, &s->mass_dev_bytes, per_dir * chunk));
-  for (int d0 = 0; d0 < total; d0 += chunk) {
-    const int nd = total - d0 < chunk ? total - d0 : chunk;
-    double* tq = s->mass_dev;
-    double* tp = k > 0 ? tq + (size_t)n_q * nd * ns : nullptr;
-    double* dM = tq + (size_t)total * nd * ns;
-    int rc = tds_launch_mass_eye(tq, tp, n_q, k, d0, nd, ns, sm);
-    if (!rc) rc = mass_jvp_run(s, q, nd, tq, tp, nullptr, dM, sm);
-    if (!rc) rc = tds_launch_mass_contract(G, dM, nn, nd, d0, n_q, g_q, g_par, s->n, ns, sm);
-    if (rc) { set_err(std::string("mass matrix vjp: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
-  }
-  return 0;
+  const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
+  return vjp_by_eye(s, "mass matrix", s->dm[0].n_q, nn, G, g_q, g_par, sm, [&](int nd, const double* t_q, const double* t_par, double* dM) {
+    return mass_jvp_run(s, q, nd, t_q, t_par, nullptr, dM, sm);
+  });
 }
 
 int tds_b200_mass_matrix_device(tds_b200_sim* s, const float* q, double* M, void* stream) {
@@ -1087,8 +1126,7 @@ int tds_b200_mass_matrix_host(tds_b200_sim* s, const double* q, double* M) {
 
 static int mass_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_par, const void* t_M) {
   if (!s || !q || !t_M || m < 1 || (!t_q && !t_par)) return -1;
-  if (t_par && s->par.n == 0) { set_err("mass matrix jvp: parameter tangents without installed physical parameters"); return -4; }
-  return 0;
+  return par_without_installed(s, t_par, "mass matrix jvp: parameter tangents");
 }
 
 int tds_b200_mass_matrix_jvp_device(tds_b200_sim* s, const float* q, int m, const double* t_q, const double* t_par, double* M,
@@ -1101,28 +1139,24 @@ int tds_b200_mass_matrix_jvp_host(tds_b200_sim* s, const double* q, int m, const
                                   double* t_M) {
   if (int rc = mass_jvp_check(s, q, m, t_q, t_par, t_M)) return rc;
   if (int rc = enter_derivative_host(s)) return rc;
-  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, k = s->par.n;
+  const int n = s->n, ns = s->ns;
   const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
-  // tangents: host [n][dim][m] <-> device [dim * m][ns]
-  const size_t tq = (size_t)n_q * m, tp = (size_t)(t_par ? k : 0) * m, to = nn * m;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; t_q | t_par | t_M | M
+  const size_t tq = (size_t)(t_q ? s->dm[0].n_q : 0) * m, tp = (size_t)(t_par ? s->par.n : 0) * m, to = nn * m;
   if (int rc = put_q(s, q)) return rc;
-  CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (tq + tp + to + nn) * ns));
-  double* tq_d = t_q ? s->jvp_dev : nullptr;
-  double* tp_d = t_par ? s->jvp_dev + tq * ns : nullptr;
-  double* to_d = s->jvp_dev + (tq + tp) * ns;
-  double* M_d = M ? to_d + to * ns : nullptr;
-  if (t_q) CUDA_TRY(put_rows(tq_d, t_q, tq, n, ns, s->stream));
-  if (t_par) CUDA_TRY(put_rows(tp_d, t_par, tp, n, ns, s->stream));
-  if (int rc = mass_jvp_run(s, s->q, m, tq_d, tp_d, M_d, to_d, s->stream)) return rc;
-  CUDA_TRY(get_rows(t_M, to_d, to, n, ns, s->stream));
-  if (M) CUDA_TRY(get_rows(M, M_d, nn, n, ns, s->stream));
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (tq + tp + to + nn) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + (tq + tp) * ns;
+  CUDA_TRY(put_parts<double>(d, {{t_q, tq}, {t_par, tp}}, n, ns, s->stream));
+  if (int rc = mass_jvp_run(s, s->q, m, t_q ? d : nullptr, t_par ? d + tq * ns : nullptr, M ? to_d + to * ns : nullptr, to_d, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{t_M, to}, {M, nn}}, to_d, n, ns, s->stream));
   return 0;
 }
 
 static int mass_vjp_check(tds_b200_sim* s, const void* q, const void* G, const void* g_q, const void* g_par) {
   if (!s || !q || !G || (!g_q && !g_par)) return -1;
-  if (g_par && s->par.n == 0) { set_err("mass matrix vjp: parameter cotangents without installed physical parameters"); return -4; }
-  return 0;
+  return par_without_installed(s, g_par, "mass matrix vjp: parameter cotangents");
 }
 
 int tds_b200_mass_matrix_vjp_device(tds_b200_sim* s, const float* q, const double* G, double* g_q, double* g_par, void* stream) {
@@ -1136,14 +1170,12 @@ int tds_b200_mass_matrix_vjp_host(tds_b200_sim* s, const double* q, const double
   const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, k = s->par.n;
   const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
   if (int rc = put_q(s, q)) return rc;
+  // G | g_q | g_par
   CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (nn + n_q + k + 1) * ns));
-  double* G_d = s->vjp_g;
-  double* gq_d = G_d + nn * ns;
-  double* gp_d = gq_d + (size_t)n_q * ns;
-  CUDA_TRY(put_rows(G_d, G, nn, n, ns, s->stream));
-  if (int rc = mass_vjp_run(s, s->q, G_d, g_q ? gq_d : nullptr, g_par ? gp_d : nullptr, s->stream)) return rc;
-  if (g_q) CUDA_TRY(get_rows(g_q, gq_d, n_q, n, ns, s->stream));
-  if (g_par) CUDA_TRY(get_rows(g_par, gp_d, k, n, ns, s->stream));
+  double* g_d = s->vjp_g + nn * ns;
+  CUDA_TRY(put_rows(s->vjp_g, G, nn, n, ns, s->stream));
+  if (int rc = mass_vjp_run(s, s->q, s->vjp_g, g_q ? g_d : nullptr, g_par ? g_d + (size_t)n_q * ns : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, (size_t)n_q}, {g_par, (size_t)k}}, g_d, n, ns, s->stream));
   return 0;
 }
 
@@ -1163,57 +1195,28 @@ static int kin_check(tds_b200_sim* s, const void* q, int K, const int* links, co
   return 0;
 }
 
-// fp64 outputs from q [n_q][ns] fp32, one lane per environment on the 8-byte layout of the mass matrix
+// fp64 outputs from q [n_q][ns] fp32 (installed parameters do not enter)
 static int kin_run(tds_b200_sim* s, const float* q, const TdsKinCall* kc, cudaStream_t sm) {
-  StepIO io;
-  memset(&io, 0, sizeof(io));
-  io.q_in = q; io.jac_n_in = 1;
-  io.n = s->n; io.n_stride = s->ns;
-  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_m)));
-  const int rc = tds_launch_kin(&s->dm_m, &io, kc, s->jac_scratch, sm);
-  if (rc) set_err(std::string("kinematics launch: ") + cudaGetErrorString((cudaError_t)rc));
-  return rc;
+  return value_run(s, "kinematics", q, nullptr, nullptr, nullptr, [&](const StepIO* io, const ParMap*) {
+    return tds_launch_kin(&s->dm_m, io, kc, s->jac_scratch, sm);
+  });
 }
 
 // m tangents t_q [n_q * m][ns] -> the outputs' columns [rows * m][ns], through the Jacobian's chunk loop
 static int kin_jvp_run(tds_b200_sim* s, const float* q, const TdsKinCall* kc, int m, const double* t_q, cudaStream_t sm) {
-  JvpTangents jv{t_q, nullptr, m};
-  jv.kin = kc;
+  const JvpTangents jv{t_q, nullptr, m, Query::kin, kc};
   return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, nullptr, nullptr, nullptr, sm, false, &jv);
 }
 
-// g_q = <G, d(xf | x | J)> along the n_q identity tangents, G [rows][ns] concatenated, in chunks of directions within 1 GB
+// g_q = <G, d(xf | x | J)>, G [rows][ns] concatenated
 static int kin_vjp_run(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, const double* G, double* g_q,
-                       double* buf, int chunk, cudaStream_t sm) {
-  const int n_q = s->dm[0].n_q, ns = s->ns;
+                       cudaStream_t sm) {
   const KinRows R = kin_rows(s, K);
-  for (int d0 = 0; d0 < n_q; d0 += chunk) {
-    const int nd = n_q - d0 < chunk ? n_q - d0 : chunk;
-    double* tq = buf;
-    double* dO = tq + (size_t)n_q * nd * ns;
-    TdsKinCall kc{K, links, local, dO, dO + R.xf * nd * ns, dO + (R.xf + R.x) * nd * ns};
-    int rc = tds_launch_mass_eye(tq, nullptr, n_q, 0, d0, nd, ns, sm);
-    if (!rc) rc = kin_jvp_run(s, q, &kc, nd, tq, sm);
-    if (!rc) rc = tds_launch_mass_contract(G, dO, (int)R.all(), nd, d0, n_q, g_q, nullptr, s->n, ns, sm);
-    if (rc) { set_err(std::string("kinematics vjp: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
-  }
-  return 0;
-}
-
-// device buffer of the VJP: the concatenated cotangent [rows][ns], then identity tangents + output columns of `chunk` directions
-static int kin_vjp_buffers(tds_b200_sim* s, int K, double** G, double** buf, int* chunk) {
-  const int n_q = s->dm[0].n_q, ns = s->ns;
-  const size_t rows = kin_rows(s, K).all();
-  const size_t per_dir = sizeof(double) * (rows + n_q) * ns;
-  int c = (int)(((size_t)1 << 30) / per_dir);
-  if (c < 1) c = 1;
-  if (c > n_q) c = n_q;
-  if (c < 1) c = 1;
-  CUDA_TRY(grow_dev(&s->mass_dev, &s->mass_dev_bytes, sizeof(double) * rows * ns + per_dir * c));
-  *G = s->mass_dev;
-  *buf = s->mass_dev + rows * ns;
-  *chunk = c;
-  return 0;
+  const size_t ns = s->ns;
+  return vjp_by_eye(s, "kinematics", s->dm[0].n_q, R.all(), G, g_q, nullptr, sm, [&](int nd, const double* t_q, const double*, double* dO) {
+    const TdsKinCall kc{K, links, local, dO, dO + R.xf * nd * ns, dO + (R.xf + R.x) * nd * ns};
+    return kin_jvp_run(s, q, &kc, nd, t_q, sm);
+  });
 }
 
 int tds_b200_kinematics_device(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, double* xf, double* x,
@@ -1236,9 +1239,7 @@ int tds_b200_kinematics_host(tds_b200_sim* s, const double* q, int K, const int*
   double* d = s->jac_dev;
   const TdsKinCall kc{K, links, local, xf ? d : nullptr, x ? d + R.xf * ns : nullptr, J ? d + (R.xf + R.x) * ns : nullptr};
   if (int rc = kin_run(s, s->q, &kc, s->stream)) return rc;
-  if (xf) CUDA_TRY(get_rows(xf, kc.xf, R.xf, n, ns, s->stream));
-  if (x) CUDA_TRY(get_rows(x, kc.x, R.x, n, ns, s->stream));
-  if (J) CUDA_TRY(get_rows(J, kc.J, R.J, n, ns, s->stream));
+  CUDA_TRY(get_parts<double>({{xf, R.xf}, {x, R.x}, {J, R.J}}, d, n, ns, s->stream));
   return 0;
 }
 
@@ -1260,21 +1261,18 @@ int tds_b200_kinematics_jvp_host(tds_b200_sim* s, const double* q, int K, const 
                                  const double* t_q, double* t_xf, double* t_x, double* t_J) {
   if (int rc = kin_jvp_check(s, q, K, links, local, m, t_q, t_xf, t_x, t_J)) return rc;
   if (int rc = enter_derivative_host(s)) return rc;
-  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q;
+  const int n = s->n, ns = s->ns;
   const KinRows R = kin_rows(s, K);
-  // tangents: host [n][rows][m] <-> device [rows * m][ns]
-  const size_t tq = (size_t)n_q * m * ns, to = R.all() * m * ns;
+  // tangents: host [n][rows][m] <-> device [rows * m][ns]; t_q | t_xf | t_x | t_J
+  const size_t tq = (size_t)s->dm[0].n_q * m;
   if (int rc = put_q(s, q)) return rc;
-  CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (tq + to + 1)));
-  double* tq_d = s->jvp_dev;
-  double* to_d = s->jvp_dev + tq;
-  CUDA_TRY(put_rows(tq_d, t_q, (size_t)n_q * m, n, ns, s->stream));
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (tq + R.all() * m + 1) * ns));
+  double* to_d = s->jac_dev + tq * ns;
+  CUDA_TRY(put_rows(s->jac_dev, t_q, tq, n, ns, s->stream));
   const TdsKinCall kc{K, links, local, t_xf ? to_d : nullptr, t_x ? to_d + R.xf * m * ns : nullptr,
                       t_J ? to_d + (R.xf + R.x) * m * ns : nullptr};
-  if (int rc = kin_jvp_run(s, s->q, &kc, m, tq_d, s->stream)) return rc;
-  if (t_xf) CUDA_TRY(get_rows(t_xf, kc.xf, R.xf * m, n, ns, s->stream));
-  if (t_x) CUDA_TRY(get_rows(t_x, kc.x, R.x * m, n, ns, s->stream));
-  if (t_J) CUDA_TRY(get_rows(t_J, kc.J, R.J * m, n, ns, s->stream));
+  if (int rc = kin_jvp_run(s, s->q, &kc, m, s->jac_dev, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{t_xf, R.xf * m}, {t_x, R.x * m}, {t_J, R.J * m}}, to_d, n, ns, s->stream));
   return 0;
 }
 
@@ -1288,19 +1286,12 @@ static int kin_vjp_check(tds_b200_sim* s, const void* q, int K, const int* links
 int tds_b200_kinematics_vjp_device(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, const double* G_xf,
                                    const double* G_x, const double* G_J, double* g_q, void* stream) {
   if (int rc = kin_vjp_check(s, q, K, links, local, G_xf, G_x, G_J, g_q)) return rc;
-  if (s->dm[0].n_q == 0) return 0;
   const cudaStream_t sm = (cudaStream_t)stream;
   const KinRows R = kin_rows(s, K);
-  const size_t ns = s->ns;
-  double *G, *buf;
-  int chunk;
-  if (int rc = kin_vjp_buffers(s, K, &G, &buf, &chunk)) return rc;
   // the concatenated cotangent xf | x | J, zero where a part is NULL
-  CUDA_TRY(cudaMemsetAsync(G, 0, sizeof(double) * R.all() * ns, sm));
-  if (G_xf) CUDA_TRY(cudaMemcpyAsync(G, G_xf, sizeof(double) * R.xf * ns, cudaMemcpyDeviceToDevice, sm));
-  if (G_x && R.x) CUDA_TRY(cudaMemcpyAsync(G + R.xf * ns, G_x, sizeof(double) * R.x * ns, cudaMemcpyDeviceToDevice, sm));
-  if (G_J && R.J) CUDA_TRY(cudaMemcpyAsync(G + (R.xf + R.x) * ns, G_J, sizeof(double) * R.J * ns, cudaMemcpyDeviceToDevice, sm));
-  return kin_vjp_run(s, q, K, links, local, G, g_q, buf, chunk, sm);
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * R.all() * s->ns));
+  CUDA_TRY(put_parts_d2d<double>(s->vjp_g, {{G_xf, R.xf}, {G_x, R.x}, {G_J, R.J}}, s->ns, sm));
+  return kin_vjp_run(s, q, K, links, local, s->vjp_g, g_q, sm);
 }
 
 int tds_b200_kinematics_vjp_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, const double* G_xf,
@@ -1308,37 +1299,23 @@ int tds_b200_kinematics_vjp_host(tds_b200_sim* s, const double* q, int K, const 
   if (int rc = kin_vjp_check(s, q, K, links, local, G_xf, G_x, G_J, g_q)) return rc;
   if (int rc = enter_derivative_host(s)) return rc;
   const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q;
-  if (n_q == 0) return 0;
   const KinRows R = kin_rows(s, K);
-  double *G, *buf;
-  int chunk;
   if (int rc = put_q(s, q)) return rc;
-  if (int rc = kin_vjp_buffers(s, K, &G, &buf, &chunk)) return rc;
-  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)n_q * ns));
-  // the concatenated cotangent xf | x | J, zero where a part is NULL; every row is written once, with its final value
-  const double* parts[3] = {G_xf, G_x, G_J};
-  const size_t rows[3] = {R.xf, R.x, R.J};
-  double* d = G;
-  for (int i = 0; i < 3; d += rows[i] * ns, ++i)
-    CUDA_TRY(parts[i] ? put_rows(d, parts[i], rows[i], n, ns, s->stream) : cudaMemsetAsync(d, 0, sizeof(double) * rows[i] * ns, s->stream));
-  if (int rc = kin_vjp_run(s, s->q, K, links, local, G, s->vjp_g, buf, chunk, s->stream)) return rc;
-  CUDA_TRY(get_rows(g_q, s->vjp_g, n_q, n, ns, s->stream));
+  // G (xf | x | J, zero where a part is NULL) | g_q
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (R.all() + n_q) * ns));
+  double* g_d = s->vjp_g + R.all() * ns;
+  CUDA_TRY(put_parts<double>(s->vjp_g, {{G_xf, R.xf}, {G_x, R.x}, {G_J, R.J}}, n, ns, s->stream));
+  if (int rc = kin_vjp_run(s, s->q, K, links, local, s->vjp_g, g_d, s->stream)) return rc;
+  CUDA_TRY(get_rows(g_q, g_d, n_q, n, ns, s->stream));
   return 0;
 }
 
 // ---- inverse dynamics tau = ID(q, qd, qdd) (DESIGN.md section 7.14): the INV instances of the world-frame kernel (tds_invdyn.cu) -------
-// tau [n_qd][ns] from q [n_q][ns], qd and qdd [n_qd][ns] fp32 (either NULL: zero), one lane per environment on the 8-byte layout
+// tau [n_qd][ns] from q [n_q][ns], qd and qdd [n_qd][ns] fp32 (either NULL: zero)
 static int inv_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* tau, cudaStream_t sm) {
-  StepIO io;
-  memset(&io, 0, sizeof(io));
-  io.q_in = q; io.qd_in = qd; io.tau_in = qdd; io.jac = tau; io.jac_n_in = 1;
-  io.n = s->n; io.n_stride = s->ns;
-  ParMap pmv = s->par;
-  pmv.values = s->par_dev; pmv.grad = nullptr;
-  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_m)));
-  const int rc = tds_launch_inv(&s->dm_m, &s->P, &io, s->par.n > 0 ? &pmv : nullptr, s->jac_scratch, sm);
-  if (rc) set_err(std::string("inverse dynamics launch: ") + cudaGetErrorString((cudaError_t)rc));
-  return rc;
+  return value_run(s, "inverse dynamics", q, qd, qdd, tau, [&](const StepIO* io, const ParMap* pm) {
+    return tds_launch_inv(&s->dm_m, &s->P, io, pm, s->jac_scratch, sm);
+  });
 }
 
 // inputs of the inverse dynamics' derivatives: q | qd | qdd
@@ -1349,41 +1326,17 @@ static int inv_n_in(const tds_b200_sim* s) { return s->dm[0].n_q + 2 * s->dm[0].
 static int inv_jvp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int m, const double* t_in, const double* t_par,
                        double* tau, double* t_tau, cudaStream_t sm) {
   if (tau) { if (int rc = inv_run(s, q, qd, qdd, tau, sm)) return rc; }
-  JvpTangents jv{t_in, t_par, m};
-  jv.inv = true;
+  const JvpTangents jv{t_in, t_par, m, Query::inv};
   return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, qdd, t_tau, sm, false, &jv);
 }
 
-// g_in [(n_q + 2 n_qd)][ns] (q | qd | qdd, contiguous) and g_par [k][ns] (NULL: not wanted) = G . dtau along the identity tangents, in
-// chunks of directions whose dtau and tangents stay within 1 GB (s->mass_dev)
+// g_in [(n_q + 2 n_qd)][ns] (q | qd | qdd, contiguous) and g_par [k][ns] (NULL: not wanted) = G . dtau
 static int inv_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const double* G, double* g_in, double* g_par,
                        cudaStream_t sm) {
-  const int n_in = inv_n_in(s), nd_ = s->dm[0].n_qd, k = g_par ? s->par.n : 0, ns = s->ns;
-  const int total = n_in + k;
-  const size_t per_dir = sizeof(double) * (size_t)(nd_ + total) * ns;   // dtau + identity tangents of one direction
-  int chunk = (int)(((size_t)1 << 30) / per_dir);
-  if (chunk < 1) chunk = 1;
-  if (chunk > total) chunk = total;
-  CUDA_TRY(grow_dev(&s->mass_dev, &s->mass_dev_bytes, per_dir * chunk));
-  for (int d0 = 0; d0 < total; d0 += chunk) {
-    const int nd = total - d0 < chunk ? total - d0 : chunk;
-    double* tin = s->mass_dev;
-    double* tp = k > 0 ? tin + (size_t)n_in * nd * ns : nullptr;
-    double* dtau = tin + (size_t)total * nd * ns;
-    int rc = tds_launch_mass_eye(tin, tp, n_in, k, d0, nd, ns, sm);
-    if (!rc) rc = inv_jvp_run(s, q, qd, qdd, nd, tin, tp, nullptr, dtau, sm);
-    if (!rc) rc = tds_launch_mass_contract(G, dtau, nd_, nd, d0, n_in, g_in, g_par, s->n, ns, sm);
-    if (rc) { set_err(std::string("inverse dynamics vjp: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
-  }
-  return 0;
-}
-
-// [rows][ns] fp64, device to device (dst NULL: nothing; src NULL: zeros)
-static int rows_d2d(double* dst, const double* src, int rows, int ns, cudaStream_t sm) {
-  if (!dst || rows == 0) return 0;
-  CUDA_TRY(src ? cudaMemcpyAsync(dst, src, sizeof(double) * rows * ns, cudaMemcpyDeviceToDevice, sm)
-               : cudaMemsetAsync(dst, 0, sizeof(double) * rows * ns, sm));
-  return 0;
+  return vjp_by_eye(s, "inverse dynamics", inv_n_in(s), s->dm[0].n_qd, G, g_in, g_par, sm,
+                    [&](int nd, const double* t_in, const double* t_par, double* dtau) {
+                      return inv_jvp_run(s, q, qd, qdd, nd, t_in, t_par, nullptr, dtau, sm);
+                    });
 }
 
 // host q [n][n_q], qd and qdd [n][n_qd] (either NULL: zero) -> s->q, s->qd, s->act; the device pointers of qd and qdd (NULL for NULL)
@@ -1408,7 +1361,7 @@ int tds_b200_inverse_dynamics_host(tds_b200_sim* s, const double* q, const doubl
   const int nd = s->dm[0].n_qd;
   const float *qd_d, *qdd_d;
   if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
-  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (nd > 0 ? nd : 1) * s->ns));
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (nd + 1) * s->ns));
   if (int rc = inv_run(s, s->q, qd_d, qdd_d, s->jac_dev, s->stream)) return rc;
   CUDA_TRY(get_rows(tau, s->jac_dev, nd, s->n, s->ns, s->stream));
   return 0;
@@ -1417,23 +1370,20 @@ int tds_b200_inverse_dynamics_host(tds_b200_sim* s, const double* q, const doubl
 static int inv_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_qd, const void* t_qdd, const void* t_par,
                          const void* t_tau) {
   if (!s || !q || !t_tau || m < 1 || (!t_q && !t_qd && !t_qdd && !t_par)) return -1;
-  if (t_par && s->par.n == 0) { set_err("inverse dynamics jvp: parameter tangents without installed physical parameters"); return -4; }
-  return 0;
+  return par_without_installed(s, t_par, "inverse dynamics jvp: parameter tangents");
 }
 
 int tds_b200_inverse_dynamics_jvp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int m, const double* t_q,
                                          const double* t_qd, const double* t_qdd, const double* t_par, double* tau, double* t_tau,
                                          void* stream) {
   if (int rc = inv_jvp_check(s, q, m, t_q, t_qd, t_qdd, t_par, t_tau)) return rc;
-  const int n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
   cudaStream_t sm = (cudaStream_t)stream;
   double* tin = nullptr;
   if (t_q || t_qd || t_qdd) {   // the kernel reads the q | qd | qdd tangents as one array
-    CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (size_t)inv_n_in(s) * m * ns));
-    tin = s->jvp_dev;
-    if (int rc = rows_d2d(tin, t_q, n_q * m, ns, sm)) return rc;
-    if (int rc = rows_d2d(tin + (size_t)n_q * m * ns, t_qd, nd * m, ns, sm)) return rc;
-    if (int rc = rows_d2d(tin + (size_t)(n_q + nd) * m * ns, t_qdd, nd * m, ns, sm)) return rc;
+    CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (size_t)inv_n_in(s) * m * s->ns));
+    tin = s->jac_dev;
+    CUDA_TRY(put_parts_d2d<double>(tin, {{t_q, n_q * m}, {t_qd, nd * m}, {t_qdd, nd * m}}, s->ns, sm));
   }
   return inv_jvp_run(s, q, qd, qdd, m, tin, t_par, tau, t_tau, sm);
 }
@@ -1442,69 +1392,56 @@ int tds_b200_inverse_dynamics_jvp_host(tds_b200_sim* s, const double* q, const d
                                        const double* t_qd, const double* t_qdd, const double* t_par, double* tau, double* t_tau) {
   if (int rc = inv_jvp_check(s, q, m, t_q, t_qd, t_qdd, t_par, t_tau)) return rc;
   if (int rc = enter_derivative_host(s)) return rc;
-  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, k = s->par.n;
-  // tangents: host [n][dim][m] <-> device [dim * m][ns]; q | qd | qdd contiguous, then the parameters, dtau and tau
-  const size_t ti = (size_t)inv_n_in(s) * m, tp = (size_t)(t_par ? k : 0) * m, to = (size_t)nd * m;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; q | qd | qdd (contiguous, zero where NULL, none if all are), t_par, dtau, tau
+  const size_t ti = (t_q || t_qd || t_qdd) ? (size_t)inv_n_in(s) * m : 0, tp = (size_t)(t_par ? s->par.n : 0) * m, to = nd * m;
   const float *qd_d, *qdd_d;
   if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
-  CUDA_TRY(grow_dev(&s->jvp_dev, &s->jvp_dev_bytes, sizeof(double) * (ti + tp + to + nd + 1) * ns));
-  double* tin_d = (t_q || t_qd || t_qdd) ? s->jvp_dev : nullptr;
-  double* tp_d = t_par ? s->jvp_dev + ti * ns : nullptr;
-  double* to_d = s->jvp_dev + (ti + tp) * ns;
-  double* tau_d = tau ? to_d + to * ns : nullptr;
-  if (tin_d) {
-    const double* parts[3] = {t_q, t_qd, t_qdd};
-    const size_t rows[3] = {(size_t)n_q * m, (size_t)nd * m, (size_t)nd * m};
-    double* d = tin_d;
-    for (int i = 0; i < 3; d += rows[i] * ns, ++i)
-      CUDA_TRY(parts[i] ? put_rows(d, parts[i], rows[i], n, ns, s->stream) : cudaMemsetAsync(d, 0, sizeof(double) * rows[i] * ns, s->stream));
-  }
-  if (t_par) CUDA_TRY(put_rows(tp_d, t_par, tp, n, ns, s->stream));
-  if (int rc = inv_jvp_run(s, s->q, qd_d, qdd_d, m, tin_d, tp_d, tau_d, to_d, s->stream)) return rc;
-  CUDA_TRY(get_rows(t_tau, to_d, to, n, ns, s->stream));
-  if (tau) CUDA_TRY(get_rows(tau, tau_d, nd, n, ns, s->stream));
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + tp + to + nd + 1) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + (ti + tp) * ns;
+  if (ti) CUDA_TRY(put_parts<double>(d, {{t_q, n_q * m}, {t_qd, nd * m}, {t_qdd, nd * m}}, n, ns, s->stream));
+  if (t_par) CUDA_TRY(put_rows(d + ti * ns, t_par, tp, n, ns, s->stream));
+  if (int rc = inv_jvp_run(s, s->q, qd_d, qdd_d, m, ti ? d : nullptr, t_par ? d + ti * ns : nullptr, tau ? to_d + to * ns : nullptr, to_d,
+                           s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{t_tau, to}, {tau, nd}}, to_d, n, ns, s->stream));
   return 0;
 }
 
 static int inv_vjp_check(tds_b200_sim* s, const void* q, const void* G, const void* g_q, const void* g_qd, const void* g_qdd,
                          const void* g_par) {
   if (!s || !q || !G || (!g_q && !g_qd && !g_qdd && !g_par)) return -1;
-  if (g_par && s->par.n == 0) { set_err("inverse dynamics vjp: parameter cotangents without installed physical parameters"); return -4; }
-  return 0;
+  return par_without_installed(s, g_par, "inverse dynamics vjp: parameter cotangents");
 }
 
 int tds_b200_inverse_dynamics_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const double* G, double* g_q,
                                          double* g_qd, double* g_qdd, double* g_par, void* stream) {
   if (int rc = inv_vjp_check(s, q, G, g_q, g_qd, g_qdd, g_par)) return rc;
-  const int n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
   cudaStream_t sm = (cudaStream_t)stream;
   // g_q | g_qd | g_qdd are one array for the contraction: computed in s->vjp_g, then copied out
-  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)inv_n_in(s) * ns));
-  double* g_in = s->vjp_g;
-  if (int rc = inv_vjp_run(s, q, qd, qdd, G, g_in, g_par, sm)) return rc;
-  if (int rc = rows_d2d(g_q, g_in, n_q, ns, sm)) return rc;
-  if (int rc = rows_d2d(g_qd, g_in + (size_t)n_q * ns, nd, ns, sm)) return rc;
-  return rows_d2d(g_qdd, g_in + (size_t)(n_q + nd) * ns, nd, ns, sm);
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)inv_n_in(s) * s->ns));
+  if (int rc = inv_vjp_run(s, q, qd, qdd, G, s->vjp_g, g_par, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}}, s->vjp_g, s->ns, sm));
+  return 0;
 }
 
 int tds_b200_inverse_dynamics_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, const double* G, double* g_q,
                                        double* g_qd, double* g_qdd, double* g_par) {
   if (int rc = inv_vjp_check(s, q, G, g_q, g_qd, g_qdd, g_par)) return rc;
   if (int rc = enter_derivative_host(s)) return rc;
-  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, k = s->par.n;
-  const int n_in = inv_n_in(s);
+  const int n = s->n, ns = s->ns, n_in = inv_n_in(s);
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, k = s->par.n;
   const float *qd_d, *qdd_d;
   if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
-  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)(nd + n_in + k + 1) * ns));
-  double* G_d = s->vjp_g;
-  double* gin_d = G_d + (size_t)nd * ns;
-  double* gp_d = gin_d + (size_t)n_in * ns;
-  CUDA_TRY(put_rows(G_d, G, nd, n, ns, s->stream));
-  if (int rc = inv_vjp_run(s, s->q, qd_d, qdd_d, G_d, gin_d, g_par ? gp_d : nullptr, s->stream)) return rc;
-  if (g_q) CUDA_TRY(get_rows(g_q, gin_d, n_q, n, ns, s->stream));
-  if (g_qd) CUDA_TRY(get_rows(g_qd, gin_d + (size_t)n_q * ns, nd, n, ns, s->stream));
-  if (g_qdd) CUDA_TRY(get_rows(g_qdd, gin_d + (size_t)(n_q + nd) * ns, nd, n, ns, s->stream));
-  if (g_par) CUDA_TRY(get_rows(g_par, gp_d, k, n, ns, s->stream));
+  // G | g_q | g_qd | g_qdd | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (nd + n_in + k + 1) * ns));
+  double* g_d = s->vjp_g + nd * ns;
+  CUDA_TRY(put_rows(s->vjp_g, G, nd, n, ns, s->stream));
+  if (int rc = inv_vjp_run(s, s->q, qd_d, qdd_d, s->vjp_g, g_d, g_par ? g_d + (size_t)n_in * ns : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}, {g_par, k}}, g_d, n, ns, s->stream));
   return 0;
 }
 

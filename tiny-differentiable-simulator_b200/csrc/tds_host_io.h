@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stddef.h>
 
+#include <initializer_list>
 #include <vector>
 
 // Grows the device buffer *p of *have bytes to at least `bytes`; the old contents are not kept.  A caller whose stream may still
@@ -40,5 +41,54 @@ inline cudaError_t get_rows(T* host, const T* dev, size_t rows, int n, int ns, c
   if (err != cudaSuccess) return err;
   for (int e = 0; e < n; ++e)
     for (size_t r = 0; r < rows; ++r) host[(size_t)e * rows + r] = t[r * ns + e];
+  return cudaSuccess;
+}
+
+// One part of a concatenation: `rows` rows at p, or NULL.  The parts lie in consecutive [rows][ns] blocks of one device array.
+template <typename T>
+struct RowPart { T* p; size_t rows; };
+
+// host parts [n][rows] -> their blocks of dev; a NULL part's block is zeroed
+template <typename T>
+inline cudaError_t put_parts(T* dev, std::initializer_list<RowPart<const T>> parts, int n, int ns, cudaStream_t stream) {
+  for (const RowPart<const T>& a : parts) {
+    const cudaError_t err = a.p ? put_rows(dev, a.p, a.rows, n, ns, stream) : cudaMemsetAsync(dev, 0, sizeof(T) * a.rows * ns, stream);
+    if (err != cudaSuccess) return err;
+    dev += a.rows * ns;
+  }
+  return cudaSuccess;
+}
+
+// blocks of dev -> host parts [n][rows], as get_rows; a NULL part is skipped
+template <typename T>
+inline cudaError_t get_parts(std::initializer_list<RowPart<T>> parts, const T* dev, int n, int ns, cudaStream_t stream) {
+  for (const RowPart<T>& a : parts) {
+    if (a.p)
+      if (const cudaError_t err = get_rows(a.p, dev, a.rows, n, ns, stream)) return err;
+    dev += a.rows * ns;
+  }
+  return cudaSuccess;
+}
+
+// The same concatenation of device parts [rows][ns], device to device and asynchronous on `stream`: put_parts_d2d copies every
+// part into its block (NULL: zeros), get_parts_d2d every block out to its part (NULL: skipped).
+template <typename T>
+inline cudaError_t put_parts_d2d(T* dev, std::initializer_list<RowPart<const T>> parts, int ns, cudaStream_t stream) {
+  for (const RowPart<const T>& a : parts) {
+    const size_t bytes = sizeof(T) * a.rows * ns;
+    const cudaError_t err = a.p ? cudaMemcpyAsync(dev, a.p, bytes, cudaMemcpyDeviceToDevice, stream) : cudaMemsetAsync(dev, 0, bytes, stream);
+    if (err != cudaSuccess) return err;
+    dev += a.rows * ns;
+  }
+  return cudaSuccess;
+}
+
+template <typename T>
+inline cudaError_t get_parts_d2d(std::initializer_list<RowPart<T>> parts, const T* dev, int ns, cudaStream_t stream) {
+  for (const RowPart<T>& a : parts) {
+    if (a.p)
+      if (const cudaError_t err = cudaMemcpyAsync(a.p, dev, sizeof(T) * a.rows * ns, cudaMemcpyDeviceToDevice, stream)) return err;
+    dev += a.rows * ns;
+  }
   return cudaSuccess;
 }

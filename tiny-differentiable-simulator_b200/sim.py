@@ -25,6 +25,12 @@ def _ptr(t):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
+def _stream(stream):
+    """The CUDA stream handle of a device call: `stream`, or torch's current stream when None."""
+    import torch
+    return ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+
+
 class BatchSim:
     def __init__(self, model, n_envs, device=0, dt=1e-3, gravity=(0.0, 0.0, -9.81), friction=0.5,
                  restitution=0.0, erp=0.2, cfm=1e-5, pgs_iterations=1, keep_all_points=False,
@@ -58,6 +64,25 @@ class BatchSim:
     def _check(self, rc, what):
         if rc:
             raise RuntimeError(f"{what} failed (rc={rc}): {_lib.last_error()}")
+
+    def _tangents(self, tangents, what="tangent", names="tangents"):
+        """Tangents of a host JVP, pairs (x [n_envs, dim, m] or [n_envs, dim] or None, dim), as contiguous float64 [n_envs, dim, m]
+        arrays (None stays None): (arrays, m, single), m = 0 when none is given, single when the first given one is [n_envs, dim]."""
+        arrays = []
+        for x, dim in tangents:
+            if x is not None:
+                x = np.asarray(x, dtype=np.float64)
+                if x.ndim == 2:
+                    x = x[:, :, None]
+                if x.shape[:2] != (self.n_envs, dim):
+                    raise ValueError(f"{what}: [n_envs, {dim}, m] or [n_envs, {dim}] expected, got {x.shape}")
+                x = np.ascontiguousarray(x)
+            arrays.append(x)
+        ms = {x.shape[2] for x in arrays if x is not None}
+        if len(ms) > 1:
+            raise ValueError(f"{names}: the same number of tangents m expected")
+        first = next((x for x, _ in tangents if x is not None), None)
+        return arrays, (ms.pop() if ms else 0), first is not None and np.ndim(first) == 2
 
     def set_params(self, dt=1e-3, gravity=(0.0, 0.0, -9.81), friction=0.5, restitution=0.0, erp=0.2, cfm=1e-5,
                    pgs_iterations=1, keep_all_points=False):
@@ -104,10 +129,9 @@ class BatchSim:
 
     def step_device(self, mode, q, qd, tau_or_action=None, q_out=None, qd_out=None, qdd_out=None, reward=None,
                     done=None, contact_dist=None, link_xf=None, use_pd=False, stream=None):
-        import torch
         q_out = q if q_out is None else q_out
         qd_out = qd if qd_out is None else qd_out
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         rc = self._L.tds_b200_step_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action),
                                           _ptr(q_out), _ptr(qd_out), _ptr(qdd_out), _ptr(reward), _ptr(done),
                                           _ptr(contact_dist), _ptr(link_xf), st)
@@ -183,8 +207,7 @@ class BatchSim:
         """Device version of step_vjp_host on the SoA layout: q, qd, tau_or_action float32 CUDA tensors [dim, n_stride] as for
         step_device, g_out [rows, n_stride] and g_in [cols, n_stride] float64 CUDA tensors.  Synchronises the stream once per chunk
         of environments (see include/tds_b200.h)."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_step_vjp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), _ptr(g_out),
                                                      _ptr(g_in), st), "step_vjp_device")
 
@@ -255,8 +278,7 @@ class BatchSim:
 
     def step_vjp_params_device(self, mode, q, qd, tau_or_action, g_out, g_in, g_par, use_pd=False, stream=None):
         """step_vjp_device with the installed parameters: g_par [k, n_stride] float64 CUDA tensor; g_in may be None."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_step_vjp_params_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action),
                                                             _ptr(g_out), _ptr(g_in), _ptr(g_par), st), "step_vjp_params_device")
 
@@ -269,22 +291,7 @@ class BatchSim:
         qd = np.ascontiguousarray(qd, dtype=np.float64)
         t = None if tau_or_action is None else np.ascontiguousarray(tau_or_action, dtype=np.float64)
         rows, cols = self.jacobian_dims(mode, use_pd)
-        k = len(self.param_ids)
-        single = (t_in if t_in is not None else t_par) is not None and np.ndim(t_in if t_in is not None else t_par) == 2
-
-        def prep(x, dim):
-            if x is None:
-                return None
-            x = np.asarray(x, dtype=np.float64)
-            if x.ndim == 2:
-                x = x[:, :, None]
-            if x.shape[:2] != (self.n_envs, dim):
-                raise ValueError(f"tangent: [n_envs, {dim}, m] or [n_envs, {dim}] expected, got {x.shape}")
-            return np.ascontiguousarray(x)
-        ti, tp = prep(t_in, cols), prep(t_par, k)
-        if ti is not None and tp is not None and ti.shape[2] != tp.shape[2]:
-            raise ValueError("t_in and t_par: the same number of tangents m expected")
-        m = (ti if ti is not None else tp).shape[2] if (ti is not None or tp is not None) else 0
+        (ti, tp), m, single = self._tangents([(t_in, cols), (t_par, len(self.param_ids))], names="t_in and t_par")
         out = np.zeros((self.n_envs, rows, max(m, 1)))
         self._check(self._L.tds_b200_step_jvp_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), m, _dp(ti), _dp(tp), _dp(out)),
                     "step_jvp_host")
@@ -294,8 +301,7 @@ class BatchSim:
         """Device version of step_jvp_host on the SoA layout: q, qd, tau_or_action float32 CUDA tensors [dim, n_stride] as for
         step_device; t_in [cols * m, n_stride], t_par [k * m, n_stride] (either may be None) and t_out [rows * m, n_stride] float64
         CUDA tensors, entry (c, j) at row c * m + j.  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_step_jvp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), int(m), _ptr(t_in),
                                                      _ptr(t_par), _ptr(t_out), st), "step_jvp_device")
 
@@ -313,8 +319,7 @@ class BatchSim:
     def mass_matrix_device(self, q, M, stream=None):
         """Device version of mass_matrix_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride] as for step_device, M float64
         CUDA tensor [n_qd * n_qd, n_stride], entry (r, c) at row r * n_qd + c.  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_mass_matrix_device(self._h, _ptr(q), _ptr(M), st), "mass_matrix_device")
 
     def mass_matrix_jvp_host(self, q, t_q, t_par=None):
@@ -322,24 +327,8 @@ class BatchSim:
         t_q [n, n_q, m] of q and t_par [n, k, m] of the installed parameters (either may be None); a tangent given as [n, n_q] (or
         [n, k]) is m = 1 and the result is then [n, n_qd, n_qd].  Returns (M, dM)."""
         q = np.ascontiguousarray(q, dtype=np.float64)
-        k = len(self.param_ids)
-        lead = t_q if t_q is not None else t_par
-        single = lead is not None and np.ndim(lead) == 2
-
-        def prep(x, dim):
-            if x is None:
-                return None
-            x = np.asarray(x, dtype=np.float64)
-            if x.ndim == 2:
-                x = x[:, :, None]
-            if x.shape[:2] != (self.n_envs, dim):
-                raise ValueError(f"tangent: [n_envs, {dim}, m] or [n_envs, {dim}] expected, got {x.shape}")
-            return np.ascontiguousarray(x)
-        tq, tp = prep(t_q, self.n_q), prep(t_par, k)
-        if tq is not None and tp is not None and tq.shape[2] != tp.shape[2]:
-            raise ValueError("t_q and t_par: the same number of tangents m expected")
-        m = (tq if tq is not None else tp).shape[2] if lead is not None else 0
-        M = np.zeros((self.n_envs, self.n_qd, self.n_qd))
+        (tq, tp), m, single = self._tangents([(t_q, self.n_q), (t_par, len(self.param_ids))], names="t_q and t_par")
+        M =np.zeros((self.n_envs, self.n_qd, self.n_qd))
         dM = np.zeros((self.n_envs, self.n_qd, self.n_qd, max(m, 1)))
         self._check(self._L.tds_b200_mass_matrix_jvp_host(self._h, _dp(q), m, _dp(tq), _dp(tp), _dp(M), _dp(dM)), "mass_matrix_jvp_host")
         return M, (dM[..., 0] if single else dM)
@@ -348,8 +337,7 @@ class BatchSim:
         """Device version of mass_matrix_jvp_host: q float32 [n_q, n_stride]; t_q [n_q * m, n_stride], t_par [k * m, n_stride] (either
         may be None), t_M [n_qd * n_qd * m, n_stride] and M [n_qd * n_qd, n_stride] (or None) float64 CUDA tensors, entry (c, j) at row
         c * m + j.  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_mass_matrix_jvp_device(self._h, _ptr(q), int(m), _ptr(t_q), _ptr(t_par), _ptr(M), _ptr(t_M), st),
                     "mass_matrix_jvp_device")
 
@@ -367,8 +355,7 @@ class BatchSim:
     def mass_matrix_vjp_device(self, q, G, g_q, g_par=None, stream=None):
         """Device version of mass_matrix_vjp_host: q float32 [n_q, n_stride], G float64 [n_qd * n_qd, n_stride] in M's layout, g_q
         [n_q, n_stride] and g_par [k, n_stride] float64 CUDA tensors (either may be None, not both).  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_mass_matrix_vjp_device(self._h, _ptr(q), _ptr(G), _ptr(g_q), _ptr(g_par), st), "mass_matrix_vjp_device")
 
     # ---- inverse dynamics tau = ID(q, qd, qdd) (DESIGN.md section 7.14) ----
@@ -395,8 +382,7 @@ class BatchSim:
     def inverse_dynamics_device(self, q, qd, qdd, tau, stream=None):
         """Device version of inverse_dynamics_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd and qdd [n_qd, n_stride]
         (either may be None), tau float64 [n_qd, n_stride].  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_inverse_dynamics_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(tau), st), "inverse_dynamics_device")
 
     def inverse_dynamics_jvp_host(self, q, qd, qdd, t_q=None, t_qd=None, t_qdd=None, t_par=None):
@@ -405,26 +391,9 @@ class BatchSim:
         [n, n_qd].  Returns (tau, dtau)."""
         q = self._inv_in(q, self.n_q, "q")
         qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
-        k = len(self.param_ids)
-        given = [t for t in (t_q, t_qd, t_qdd, t_par) if t is not None]
-        if not given:
+        if all(t is None for t in (t_q, t_qd, t_qdd, t_par)):
             raise ValueError("at least one tangent is expected")
-        single = np.ndim(given[0]) == 2
-
-        def prep(x, dim):
-            if x is None:
-                return None
-            x = np.asarray(x, dtype=np.float64)
-            if x.ndim == 2:
-                x = x[:, :, None]
-            if x.shape[:2] != (self.n_envs, dim):
-                raise ValueError(f"tangent: [n_envs, {dim}, m] or [n_envs, {dim}] expected, got {x.shape}")
-            return np.ascontiguousarray(x)
-        ts = [prep(t_q, self.n_q), prep(t_qd, self.n_qd), prep(t_qdd, self.n_qd), prep(t_par, k)]
-        ms = {t.shape[2] for t in ts if t is not None}
-        if len(ms) != 1:
-            raise ValueError("tangents: the same number of tangents m expected")
-        m = ms.pop()
+        ts, m, single = self._tangents([(t_q, self.n_q), (t_qd, self.n_qd), (t_qdd, self.n_qd), (t_par, len(self.param_ids))])
         tau = np.zeros((self.n_envs, self.n_qd))
         dtau = np.zeros((self.n_envs, self.n_qd, m))
         self._check(self._L.tds_b200_inverse_dynamics_jvp_host(self._h, _dp(q), _dp(qd), _dp(qdd), m, *(_dp(t) for t in ts), _dp(tau),
@@ -435,8 +404,7 @@ class BatchSim:
         """Device version of inverse_dynamics_jvp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None); t_q
         [n_q * m, n_stride], t_qd and t_qdd [n_qd * m, n_stride], t_par [k * m, n_stride] (each may be None, not all), t_tau
         [n_qd * m, n_stride] and tau [n_qd, n_stride] (or None) float64 CUDA tensors, entry (c, j) at row c * m + j.  Asynchronous."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_inverse_dynamics_jvp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), int(m), _ptr(t_q), _ptr(t_qd),
                                                                  _ptr(t_qdd), _ptr(t_par), _ptr(tau), _ptr(t_tau), st),
                     "inverse_dynamics_jvp_device")
@@ -458,8 +426,7 @@ class BatchSim:
         """Device version of inverse_dynamics_vjp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None), G float64
         [n_qd, n_stride], g_q [n_q, n_stride], g_qd and g_qdd [n_qd, n_stride], g_par [k, n_stride] float64 CUDA tensors (each may be
         None, not all).  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_inverse_dynamics_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(G), _ptr(g_q), _ptr(g_qd),
                                                                  _ptr(g_qdd), _ptr(g_par), st), "inverse_dynamics_vjp_device")
 
@@ -495,8 +462,7 @@ class BatchSim:
         """Device version of kinematics_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride]; xf [n_links * 12, n_stride], x [3K,
         n_stride] and J [3K * n_qd, n_stride] float64 CUDA tensors (any may be None, not all three), entry (point k, row r, column c) of J
         at row (3k + r) * n_qd + c.  The point table is host data.  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         keep, K, lp, cp = self._kin_args(links, local)
         self._check(self._L.tds_b200_kinematics_device(self._h, _ptr(q), K, lp, cp, _ptr(xf), _ptr(x), _ptr(J), st), "kinematics_device")
 
@@ -504,14 +470,7 @@ class BatchSim:
         """Directional derivatives along m tangents t_q [n, n_q, m] of q: (dxf [n, n_links, 12, m], dx [n, K, 3, m], dJ [n, K, 3, n_qd, m])
         (xf in the layout R row-major | p); a tangent given as [n, n_q] is m = 1 and the trailing axis is dropped."""
         q = np.ascontiguousarray(q, dtype=np.float64)
-        tq = np.asarray(t_q, dtype=np.float64)
-        single = tq.ndim == 2
-        if single:
-            tq = tq[:, :, None]
-        if tq.shape[:2] != (self.n_envs, self.n_q):
-            raise ValueError(f"t_q: [n_envs, {self.n_q}, m] or [n_envs, {self.n_q}] expected, got {tq.shape}")
-        tq = np.ascontiguousarray(tq)
-        m = tq.shape[2]
+        (tq,), m, single = self._tangents([(t_q, self.n_q)], what="t_q")
         keep, K, lp, cp = self._kin_args(links, local)
         n = self.n_envs
         dxf, dx, dJ = np.zeros((n, self.n_links, 12, m)), np.zeros((n, K, 3, m)), np.zeros((n, K, 3, self.n_qd, m))
@@ -523,8 +482,7 @@ class BatchSim:
         """Device version of kinematics_jvp_host: q float32 [n_q, n_stride]; t_q [n_q * m, n_stride] and t_xf [n_links * 12 * m, n_stride],
         t_x [3K * m, n_stride], t_J [3K * n_qd * m, n_stride] (any may be None, not all three) float64 CUDA tensors, entry (r, j) at row
         r * m + j.  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         keep, K, lp, cp = self._kin_args(links, local)
         self._check(self._L.tds_b200_kinematics_jvp_device(self._h, _ptr(q), K, lp, cp, int(m), _ptr(t_q), _ptr(t_xf), _ptr(t_x), _ptr(t_J),
                                                            st), "kinematics_jvp_device")
@@ -551,8 +509,7 @@ class BatchSim:
     def kinematics_vjp_device(self, q, links, local, G_xf, G_x, G_J, g_q, stream=None):
         """Device version of kinematics_vjp_host: q float32 [n_q, n_stride], cotangents float64 in the layouts of kinematics_device (None:
         zero, not all three), g_q float64 [n_q, n_stride] CUDA tensors.  Asynchronous on the stream."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         keep, K, lp, cp = self._kin_args(links, local)
         self._check(self._L.tds_b200_kinematics_vjp_device(self._h, _ptr(q), K, lp, cp, _ptr(G_xf), _ptr(G_x), _ptr(G_J), _ptr(g_q), st),
                     "kinematics_vjp_device")
@@ -632,8 +589,7 @@ class BatchSim:
     def env_step_visual_device(self, actions, positions, orientations, reward=None, done=None, stream=None):
         """Env step that also streams the visual transforms in the instancing renderer's layout:
         positions / orientations are float32 CUDA tensors [n_envs * n_visuals, 4] (xyz1 / quaternion xyzw)."""
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_env_step_visual_device(self._h, _ptr(actions), _ptr(reward), _ptr(done), _ptr(positions),
                                                             _ptr(orientations), st), "env_step_visual_device")
 
@@ -711,7 +667,6 @@ class BatchSim:
         return step
 
     def env_step_device(self, actions, reward=None, done=None, stream=None):
-        import torch
-        st = ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
+        st = _stream(stream)
         self._check(self._L.tds_b200_env_step_device(self._h, _ptr(actions), _ptr(reward), _ptr(done), st),
                     "env_step_device")
