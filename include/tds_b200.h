@@ -289,6 +289,42 @@ int tds_b200_inverse_dynamics_vjp_device(tds_b200_sim* sim, const float* q, cons
 int tds_b200_inverse_dynamics_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, const double* G, double* g_q,
                                        double* g_qd, double* g_qdd, double* g_par);
 
+/* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
+ * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
+ * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,
+ * in world coordinates:
+ *   rows 0-2  world_normal_on_b        rows 3-5  world_point_on_b        row 6  distance
+ *   rows 7-9  F, the impulse on body B at world_point_on_b (N s; the force is F / dt).  Body A receives -F at the point on A.
+ * Rows 0-6 are the reference's ContactPoint fields (contact_point.hpp); the point on A is point_on_b + distance * normal_on_b (plane
+ * contacts and contacts between multibodies alike) and is not output.  F = -(p_n n_b + p_1 t_1 + p_2 t_2) with p the solver's row
+ * vector of the contact (the PGS result, or the closed-form spring-damper impulse with contact_model 1) and t_1, t_2 the friction
+ * directions of the solve (the model's plane_space(-plane normal) for plane contacts, plane_space(normal) between multibodies, as the
+ * reference evaluates it: not unit vectors in general, so recover p from F with these directions, not by projection).  A
+ * candidate outside the active set (distance >= 0, beyond the solver's contact cap) has F = 0; a candidate between multibodies whose
+ * contact function emitted no point has distance +inf and zeros elsewhere.  In a world of several multibodies each contact between
+ * multibodies reports the impulse of its own pair's solve.
+ * The step always runs on the generic world-frame kernel at the simulator's precision, with the installed parameters if any: q' and qd'
+ * are bitwise those of tds_b200_step_device on that kernel (TDS_B200_KERNEL=world).  Arguments as tds_b200_step_device / _host, without
+ * qdd_out, reward, done, contact_dist and link_xf.
+ *   device: contacts [10 n_points][n_stride] fp32 (asynchronous).  host: contacts [n][n_points][10] fp64; q_out, qd_out may be NULL.
+ * _jvp (MODE_FULL): as tds_b200_step_jvp_*, with the output rows q' | qd' | records (n_q + n_qd + 10 n_points).
+ * _vjp (MODE_FULL): g_in = g_out^T d(q' | qd' | records) / d(the step's inputs) [cols] and, while a set is installed and g_par is not
+ *   NULL, the parameters' cotangents [k], by the JVP along identity tangents.  g_in or g_par may be NULL, not both.  Device g_out
+ *   [rows][n_stride], g_in [cols][n_stride], g_par [k][n_stride] fp64 (asynchronous); host g_out [n][rows], g_in [n][cols], g_par [n][k].
+ * Returns -1 (bad argument), -2 (mode), -3 (use_pd without tds_b200_set_env), -4 (t_par / g_par without installed parameters). */
+int tds_b200_step_contacts_device(tds_b200_sim* sim, int mode, int use_pd, const float* q_in, const float* qd_in, const float* tau_or_action,
+                                  float* q_out, float* qd_out, float* contacts, void* stream);
+int tds_b200_step_contacts_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                double* q_out, double* qd_out, double* contacts);
+int tds_b200_step_contacts_jvp_device(tds_b200_sim* sim, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                                      int m, const double* t_in, const double* t_par, double* t_out, void* stream);
+int tds_b200_step_contacts_jvp_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                    int m, const double* t_in, const double* t_par, double* t_out);
+int tds_b200_step_contacts_vjp_device(tds_b200_sim* sim, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                                      const double* g_out, double* g_in, double* g_par, void* stream);
+int tds_b200_step_contacts_vjp_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                    const double* g_out, double* g_in, double* g_par);
+
 /* Stand-alone integration stages of the fine-grained surface (device SoA arrays as above):
  * integrate_euler (src/dynamics/integrator.hpp:10-133): qd += qdd dt (qdd may be NULL = zero), q += qd dt, floating base
  * quaternion increment + normalisation; integrate_euler_qdd (:141-195): qd += qdd dt only. */

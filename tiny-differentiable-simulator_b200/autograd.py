@@ -31,6 +31,12 @@ inverse_dynamics(sim, q, qd, qdd=None, params=None) is tau = ID(q, qd, qdd) [n_e
 backward rule (BatchSim.inverse_dynamics_vjp_device: float32 q.grad, qd.grad, qdd.grad, float64 params.grad) and a forward-mode rule
 (BatchSim.inverse_dynamics_jvp_device).
 
+step_contacts(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False, params=None) is the step that also reports its contacts
+(DESIGN.md section 7.15): (q', qd', C) with C [n_envs, n_contact_points, 10] float32 (normal on b, point on b, distance, impulse on b),
+on the world-frame kernel at the simulator's precision.  Its backward rule (BatchSim.step_contacts_vjp_device) takes cotangents of all
+three outputs (float32 q.grad, qd.grad, tau_or_action.grad, float64 params.grad) and its forward-mode rule runs
+BatchSim.step_contacts_jvp_device; both in MODE_FULL.  step itself is unchanged.
+
 forward_kinematics(sim, q, links, local) is every link's world transform and every point's world position and linear Jacobian (float64,
 DESIGN.md section 7.13) with a backward rule (BatchSim.kinematics_vjp_device: float32 q.grad) and a forward-mode rule
 (BatchSim.kinematics_jvp_device).
@@ -501,3 +507,98 @@ def forward_kinematics(sim, q, links, local):
     if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
         raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
     return _ForwardKinematics.apply(sim, q, links, local)
+
+
+class _StepContacts(torch.autograd.Function):
+    @staticmethod
+    def forward(sim, mode, use_pd, q, qd, tau, params):
+        n, ns, npts = sim.n_envs, sim.n_stride, sim.n_contact_points
+        if params is not None:
+            sim.set_physical_params(sim.param_ids, params.detach())
+        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), _soa_opt(tau, ns, torch.float32)
+        q_out, qd_out = torch.empty_like(qs), torch.empty_like(qds)
+        C = torch.zeros((max(10 * npts, 1), ns), dtype=torch.float32, device=q.device)
+        _on_side_stream(q.device, lambda st: sim.step_contacts_device(mode, qs, qds, ts, q_out, qd_out, C, use_pd=use_pd, stream=st),
+                        (qs, qds, ts, q_out, qd_out, C))
+        return (q_out[:sim.n_q, :n].t().contiguous(), qd_out[:sim.n_qd, :n].t().contiguous(),
+                C[:10 * npts, :n].t().reshape(n, npts, 10).contiguous())
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        sim, mode, use_pd, q, qd, tau, params = inputs
+        ns = sim.n_stride
+        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), _soa_opt(tau, ns, torch.float32)
+        par = params.detach() if params is not None else None
+        ctx.sim, ctx.mode, ctx.use_pd, ctx.has_tau, ctx.has_params = sim, mode, use_pd, tau is not None, params is not None
+        ctx.save_for_backward(qs, qds, ts if ts is not None else qs, par if par is not None else qs)
+        ctx.jvp_inputs = (qs, qds, ts, par)
+
+    @staticmethod
+    def backward(ctx, gq_out, gqd_out, gC):
+        sim, mode, use_pd = ctx.sim, ctx.mode, ctx.use_pd
+        qs, qds, ts, par = ctx.saved_tensors
+        ts = ts if ctx.has_tau else None
+        n, ns, nq, nd, npts = sim.n_envs, sim.n_stride, sim.n_q, sim.n_qd, sim.n_contact_points
+        rows, cols = sim.contact_rows(mode, use_pd)
+        G = torch.zeros((rows, ns), dtype=torch.float64, device=qs.device)
+        for g, r0, d in ((gq_out, 0, nq), (gqd_out, nq, nd), (None if gC is None else gC.reshape(n, 10 * npts), nq + nd, 10 * npts)):
+            if g is not None and d:
+                G[r0:r0 + d, :n] = g.to(torch.float64).t()
+        g_in = torch.zeros((cols, ns), dtype=torch.float64, device=qs.device)
+        g_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=qs.device) if ctx.has_params else None
+        if ctx.has_params:
+            sim.set_physical_params(sim.param_ids, par)   # the values of this call
+        _on_side_stream(qs.device, lambda st: sim.step_contacts_vjp_device(mode, qs, qds, ts, G, g_in, g_par, use_pd=use_pd, stream=st),
+                        (qs, qds, ts, G, g_in, g_par))
+        gt = None
+        if ctx.has_tau:
+            k0 = nq + nd
+            gt = g_in[k0:k0 + (sim.n_act if use_pd else sim.n_tau), :n].t().to(torch.float32).contiguous()
+        gp = g_par[:, :n].t().contiguous() if ctx.has_params else None
+        return (None, None, None, g_in[:nq, :n].t().to(torch.float32).contiguous(), g_in[nq:nq + nd, :n].t().to(torch.float32).contiguous(),
+                gt, gp)
+
+    @staticmethod
+    def jvp(ctx, _sim, _mode, _use_pd, *tangents):
+        with torch._C._DisableFuncTorch():
+            return _StepContacts._jvp(ctx, *(_plain(t) for t in tangents))
+
+    @staticmethod
+    def _jvp(ctx, tq, tqd, ttau, tpar):
+        sim, mode, use_pd = ctx.sim, ctx.mode, ctx.use_pd
+        qs, qds, ts, par = (_plain(t) for t in ctx.jvp_inputs)
+        n, ns, nq, nd, npts = sim.n_envs, sim.n_stride, sim.n_q, sim.n_qd, sim.n_contact_points
+        rows, cols = sim.contact_rows(mode, use_pd)
+        t_in = t_par = None
+        if tq is not None or tqd is not None or (ttau is not None and ctx.has_tau):
+            t_in = torch.zeros((cols, ns), dtype=torch.float64, device=qs.device)
+            for t, r0 in ((tq, 0), (tqd, nq), (ttau if ctx.has_tau else None, nq + nd)):   # the PD gains: zero tangent
+                if t is not None and t.shape[1]:
+                    t_in[r0:r0 + t.shape[1], :n] = t.to(torch.float64).t()
+        if tpar is not None and ctx.has_params:
+            t_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=qs.device)
+            t_par[:, :n] = tpar.to(torch.float64).t()
+        t_out = torch.zeros((rows, ns), dtype=torch.float64, device=qs.device)
+        if t_in is not None or t_par is not None:
+            if ctx.has_params:
+                sim.set_physical_params(sim.param_ids, par)   # the values of this call
+            _on_side_stream(qs.device, lambda st: sim.step_contacts_jvp_device(mode, qs, qds, ts, 1, t_in, t_par, t_out, use_pd=use_pd,
+                                                                               stream=st), (qs, qds, ts, t_in, t_par, t_out))
+        out = lambda r0, d: t_out[r0:r0 + d, :n].t().to(torch.float32).contiguous()
+        return out(0, nq), out(nq, nd), out(nq + nd, 10 * npts).reshape(n, npts, 10)
+
+
+def step_contacts(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False, params=None):
+    """One differentiable step of every environment of `sim` (a BatchSim) that also reports its contacts: (q' [n_envs, n_q], qd'
+    [n_envs, n_qd], C [n_envs, n_contact_points, 10]) float32, a record per contact candidate - normal on b [3], point on b [3],
+    distance, impulse on body b [3] in N s - in world coordinates (DESIGN.md section 7.15).  The step runs on the world-frame kernel at
+    the simulator's precision (mode MODE_FULL or MODE_WORLD); q' and qd' are those of that kernel's step.  Inputs as for step.  The
+    derivatives (MODE_FULL) are those of the fp64 world-frame step at the fp32-rounded inputs, of the branch taken (contact set,
+    clamps of the Gauss-Seidel sweep), with cotangents or tangents of all three outputs."""
+    for name, t in (("q", q), ("qd", qd), ("tau_or_action", tau_or_action)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or t.shape[0] != sim.n_envs):
+            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, dim] is expected")
+    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
+                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
+        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    return _StepContacts.apply(sim, int(mode), bool(use_pd), q, qd, tau_or_action, params)

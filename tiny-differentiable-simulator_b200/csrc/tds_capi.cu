@@ -66,6 +66,12 @@ extern "C" int tds_launch_kin_jvp(const DevModel* M, const StepIO* io, const Tds
 extern "C" int tds_launch_inv(const DevModel* M, const SimParams* P, const StepIO* io, const ParMap* pm, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_inv_jvp(const DevModel* M, const SimParams* P, const StepIO* io, const ParMap* pm, const double* t_in,
                                   const double* t_par, int m, int n_dirs, char* gscratch, cudaStream_t stream);
+// the step that reports its contacts, and its Jacobian-vector products (tds_contacts.cu)
+extern "C" int tds_launch_contacts(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm, float* cf,
+                                   int mode, int use_pd, int precision, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_contacts_jvp(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
+                                       const double* t_in, const double* t_par, int m, int mode, int use_pd, int n_dirs, char* gscratch,
+                                       cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
@@ -884,12 +890,14 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
   return 0;
 }
 
-// what a Jacobian-vector product differentiates: the step, or one of the dynamics queries of DESIGN.md sections 7.12-7.14
-enum class Query { step, mass, kin, inv };
+// what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14, or the step
+// with its contact records (section 7.15)
+enum class Query { step, mass, kin, inv, contacts };
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
 // inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
-// (t_in = the q tangents, t_par unused); inv: t_in = the q | qd | qdd tangents (qd and qdd in the step's qd and tau_or_action)
+// (t_in = the q tangents, t_par unused); inv: t_in = the q | qd | qdd tangents (qd and qdd in the step's qd and tau_or_action);
+// contacts: as step, with the rows q' | qd' | records
 struct JvpTangents { const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr; };
 
 // the installed physical parameters as a launch argument in *pmv, or NULL without any
@@ -949,6 +957,9 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
         case Query::mass: rc = tds_launch_mass_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
         case Query::kin: rc = tds_launch_kin_jvp(&s->dm_ad, &io, jv->kin, jv->t_in, jv->m, nd, s->jac_scratch, sm); break;
         case Query::inv: rc = tds_launch_inv_jvp(&s->dm_ad, &s->P, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
+        case Query::contacts:
+          rc = tds_launch_contacts_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch, sm);
+          break;
       }
     }
     if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
@@ -1022,23 +1033,30 @@ int tds_b200_step_jvp_device(tds_b200_sim* s, int mode, int use_pd, const float*
   return jacobian_run(s, mode, use_pd, q, qd, tau_or_action, t_out, stream, false, &jv);
 }
 
-int tds_b200_step_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
-                           int m, const double* t_in, const double* t_par, double* t_out) {
-  if (int rc = jvp_check(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out)) return rc;
+// host JVP of the step (query step) or of the step with its contact records (query contacts, rows q' | qd' | records)
+static int step_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action, int m,
+                         const double* t_in, const double* t_par, double* t_out, Query query) {
   if (int rc = enter_derivative_host(s)) return rc;
   const int n = s->n, ns = s->ns, k = s->par.n;
   int dims[2];
   tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  if (query == Query::contacts) dims[0] += 10 * s->n_points;
   // tangents: host [n][dim][m] <-> device [dim * m][ns]; t_in | t_par | t_out
   const size_t ti = (size_t)(t_in ? dims[1] : 0) * m, tp = (size_t)(t_par ? k : 0) * m, to = (size_t)dims[0] * m;
   CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + tp + to) * ns));
   if (int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action)) return rc;
   double* tout_d = s->jac_dev + (ti + tp) * ns;
   CUDA_TRY(put_parts<double>(s->jac_dev, {{t_in, ti}, {t_par, tp}, {nullptr, to}}, n, ns, s->stream));
-  const JvpTangents jv{t_in ? s->jac_dev : nullptr, t_par ? s->jac_dev + ti * ns : nullptr, m};
+  const JvpTangents jv{t_in ? s->jac_dev : nullptr, t_par ? s->jac_dev + ti * ns : nullptr, m, query};
   if (int rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, tout_d, s->stream, false, &jv)) return rc;
   CUDA_TRY(get_rows(t_out, tout_d, to, n, ns, s->stream));
   return 0;
+}
+
+int tds_b200_step_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                           int m, const double* t_in, const double* t_par, double* t_out) {
+  if (int rc = jvp_check(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out)) return rc;
+  return step_jvp_host(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out, Query::step);
 }
 
 // ---- dynamics queries (DESIGN.md sections 7.12-7.14): the mass matrix, forward kinematics and inverse dynamics by the MASS, KIN and
@@ -1560,6 +1578,127 @@ int tds_b200_vjp_tape_info(const tds_b200_sim* s, int info[2]) {
   const size_t warps = tape_warps(s);
   info[0] = s->tape_cap;
   info[1] = (int)(warps * 32 < (size_t)1 << 30 ? warps * 32 : (size_t)1 << 30);
+  return 0;
+}
+
+// ---- the step with its contact records (DESIGN.md section 7.15): the CF instances of the world-frame kernel (tds_contacts.cu).  Values
+// in MODE_FULL and MODE_WORLD at the simulator's precision, on the world-frame kernel whatever kernel tds_b200_step_device would choose;
+// the JVP through the Jacobian's chunk loop and the VJP by identity tangents, in MODE_FULL.
+static size_t contact_rows(const tds_b200_sim* s) { return (size_t)10 * s->n_points; }
+
+static int contacts_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* tau_or_action,
+                          bool derivative) {
+  if (!s || !q || !qd || (use_pd && !tau_or_action)) return -1;
+  if (derivative && mode != TDS_B200_MODE_FULL) { set_err("step contacts derivatives: mode FULL"); return -2; }
+  if (mode != TDS_B200_MODE_FULL && mode != TDS_B200_MODE_WORLD) { set_err("step contacts: modes FULL, WORLD"); return -2; }
+  if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+  return 0;
+}
+
+// q', qd' [dim][ns] and the records [10 n_pts][ns] fp32 of one step
+static int contacts_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action, float* q_out,
+                        float* qd_out, float* contacts, cudaStream_t sm) {
+  const int p = s->precision;
+  if (int rc = ensure_scratch(s, p)) return rc;
+  StepIO io;
+  memset(&io, 0, sizeof(io));
+  io.q_in = q; io.qd_in = qd; io.tau_in = tau_or_action;
+  io.q_out = q_out; io.qd_out = qd_out;
+  io.n = s->n; io.n_stride = s->ns;
+  ParMap pmv;
+  const int rc = tds_launch_contacts(&s->dm[p], &s->P, &s->E, &io, installed_par(s, &pmv), contacts, mode, use_pd, p, s->scratch, sm);
+  if (rc) set_err(std::string("step contacts launch: ") + cudaGetErrorString((cudaError_t)rc));
+  return rc;
+}
+
+int tds_b200_step_contacts_device(tds_b200_sim* s, int mode, int use_pd, const float* q_in, const float* qd_in, const float* tau_or_action,
+                                  float* q_out, float* qd_out, float* contacts, void* stream) {
+  if (int rc = contacts_check(s, mode, use_pd, q_in, qd_in, tau_or_action, false)) return rc;
+  if (!q_out || !qd_out || (!contacts && s->n_points > 0)) return -1;
+  return contacts_run(s, mode, use_pd, q_in, qd_in, tau_or_action, q_out, qd_out, contacts, (cudaStream_t)stream);
+}
+
+int tds_b200_step_contacts_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                double* q_out, double* qd_out, double* contacts) {
+  if (int rc = contacts_check(s, mode, use_pd, q, qd, tau_or_action, false)) return rc;
+  if (!contacts && s->n_points > 0) return -1;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const DevModel& M = s->dm[0];
+  const size_t rows = contact_rows(s);
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(float) * (rows + 1) * s->ns));
+  float* rec = (float*)s->jac_dev;
+  int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action);
+  if (!rc) rc = contacts_run(s, mode, use_pd, s->q, s->qd, s->act, s->q, s->qd, rec, s->stream);
+  if (!rc) rc = get_state(s, s->q, M.n_q, q_out);
+  if (!rc) rc = get_state(s, s->qd, M.n_qd, qd_out);
+  if (!rc) rc = get_state(s, rec, (int)rows, contacts);
+  if (rc) return rc;
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  return 0;
+}
+
+static int contacts_jvp_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* tau_or_action, int m,
+                              const void* t_in, const void* t_par, const void* t_out) {
+  if (int rc = contacts_check(s, mode, use_pd, q, qd, tau_or_action, true)) return rc;
+  if (!t_out || m < 1 || (!t_in && !t_par)) return -1;
+  return par_without_installed(s, t_par, "step contacts jvp: parameter tangents");
+}
+
+int tds_b200_step_contacts_jvp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                                      int m, const double* t_in, const double* t_par, double* t_out, void* stream) {
+  if (int rc = contacts_jvp_check(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out)) return rc;
+  const JvpTangents jv{t_in, t_par, m, Query::contacts};
+  return jacobian_run(s, mode, use_pd, q, qd, tau_or_action, t_out, stream, false, &jv);
+}
+
+int tds_b200_step_contacts_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                    int m, const double* t_in, const double* t_par, double* t_out) {
+  if (int rc = contacts_jvp_check(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out)) return rc;
+  return step_jvp_host(s, mode, use_pd, q, qd, tau_or_action, m, t_in, t_par, t_out, Query::contacts);
+}
+
+static int contacts_vjp_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* tau_or_action,
+                              const void* g_out, const void* g_in, const void* g_par) {
+  if (int rc = contacts_check(s, mode, use_pd, q, qd, tau_or_action, true)) return rc;
+  if (!g_out || (!g_in && !g_par)) return -1;
+  return par_without_installed(s, g_par, "step contacts vjp: parameter cotangents");
+}
+
+// g_in [cols][ns] (may be NULL) and g_par [k][ns] (NULL: not wanted) = <g_out, d(q' | qd' | records)> for g_out [rows][ns]
+static int contacts_vjp_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                            const double* g_out, double* g_in, double* g_par, cudaStream_t sm) {
+  int dims[2];
+  tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  return vjp_by_eye(s, "step contacts", dims[1], (size_t)dims[0] + contact_rows(s), g_out, g_in, g_par, sm,
+                    [&](int nd, const double* t_in, const double* t_par, double* dO) {
+                      const JvpTangents jv{t_in, t_par, nd, Query::contacts};
+                      return jacobian_run(s, mode, use_pd, q, qd, tau_or_action, dO, sm, false, &jv);
+                    });
+}
+
+int tds_b200_step_contacts_vjp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                                      const double* g_out, double* g_in, double* g_par, void* stream) {
+  if (int rc = contacts_vjp_check(s, mode, use_pd, q, qd, tau_or_action, g_out, g_in, g_par)) return rc;
+  return contacts_vjp_run(s, mode, use_pd, q, qd, tau_or_action, g_out, g_in, g_par, (cudaStream_t)stream);
+}
+
+int tds_b200_step_contacts_vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                    const double* g_out, double* g_in, double* g_par) {
+  if (int rc = contacts_vjp_check(s, mode, use_pd, q, qd, tau_or_action, g_out, g_in, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, k = g_par ? s->par.n : 0;
+  int dims[2];
+  tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  const size_t rows = (size_t)dims[0] + contact_rows(s);
+  // g_out | g_in | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (rows + dims[1] + k + 1) * ns));
+  double* g_d = s->vjp_g + rows * ns;
+  if (int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action)) return rc;
+  CUDA_TRY(put_rows(s->vjp_g, g_out, rows, n, ns, s->stream));
+  if (int rc = contacts_vjp_run(s, mode, use_pd, s->q, s->qd, s->act, s->vjp_g, g_d, g_par ? g_d + (size_t)dims[1] * ns : nullptr,
+                                s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{g_in, (size_t)dims[1]}, {g_par, (size_t)k}}, g_d, n, ns, s->stream));
   return 0;
 }
 

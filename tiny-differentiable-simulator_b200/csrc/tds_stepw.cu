@@ -49,12 +49,33 @@ struct KinArg {
   double local[3 * TDS_MAX_KIN_POINTS];
 };
 struct KinArgJvp : KinArg { JvpTan jv; };
-template <bool PAR, bool JV = false, bool KIN = false> struct ParArg { typedef NoPar type; };
+// kernel argument of the contact-reporting value instances (CF, DESIGN.md section 7.15): the records [10 * n_pts][ns] fp32.  The JVP
+// instances write the records' dual parts into io.jac behind q' | qd' and take the plain JVP arguments.
+struct CfArg { float* cf; };
+struct CfArgPar : ParMap { float* cf; };
+template <bool PAR, bool JV = false, bool KIN = false, bool CF = false> struct ParArg { typedef NoPar type; };
 template <> struct ParArg<true, false> { typedef ParMap type; };
 template <> struct ParArg<false, true> { typedef NoParJvp type; };
 template <> struct ParArg<true, true> { typedef ParMapJvp type; };
 template <> struct ParArg<false, false, true> { typedef KinArg type; };
 template <> struct ParArg<false, true, true> { typedef KinArgJvp type; };
+template <> struct ParArg<false, false, false, true> { typedef CfArg type; };
+template <> struct ParArg<true, false, false, true> { typedef CfArgPar type; };
+template <> struct ParArg<false, true, false, true> { typedef NoParJvp type; };
+template <> struct ParArg<true, true, false, true> { typedef ParMapJvp type; };
+
+// CF, dual instances: the part of a record's dual number they write - the tangent (d).  The host build of the tests also compiles them
+// with the value (v), for an fp64 value path of the records that central differences can resolve.
+#ifndef TDS_CF_DUAL_PART
+#define TDS_CF_DUAL_PART d
+#endif
+
+// CF: the (c + 1)-th set bit of mask (the candidate index of active contact c; the active contacts are compacted in candidate order)
+TDS_D int cf_nth_bit(unsigned long long mask, int c) {
+  for (int i = 0; i < 64; ++i)
+    if ((mask >> i) & 1ull) { if (c-- == 0) return i; }
+  return -1;
+}
 
 // joint stiffness and damping enter the step at fp32, as DevModel stores them; the derivative is taken at the rounded value
 TDS_D double f32_round(double x) { return (double)(float)x; }
@@ -89,12 +110,18 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // for i and its moving ancestors j (all in the common frame: no transforms); a branch point's a_i is kept over its rigid-inertia words,
 // which nothing else reads.  Then the stiffness and damping terms the ABA subtracts, the floating base's wrench in the base frame, and
 // tau [n_qd] at io.jac[r * ns + e] (fp64 instance) or its dual part at io.jac[(r * m + j) * ns + e] (JV instance).  Returns before pass 2.
+// CF: the step (MODE_FULL or MODE_WORLD) that also reports its contacts (DESIGN.md section 7.15): one record of 10 rows per contact
+// candidate k (plane candidates, then the candidates between multibodies), row r at 10 k + r, world coordinates: normal on b [3],
+// point on b [3], distance, impulse on b [3] at the point on b.  The geometry rows are written where the candidate's distance is
+// computed; every impulse row is zeroed there and the active contacts' rows are written after their group's PGS sweep or spring-damper
+// loop.  Row r at pm.cf[r * ns + e] (value instances, fp32), or its dual part at io.jac[((n_q + n_qd + r) * m + j) * ns + e] behind the
+// rows q' | qd' (JV instances).  Nothing else differs from the step.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
-          bool KIN = false, bool INV = false>
+          bool KIN = false, bool INV = false, bool CF = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
-                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN>::type pm = {}) {
+                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF>::type pm = {}) {
   extern __shared__ __align__(16) char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp_in_blk = threadIdx.x >> 5;
@@ -271,10 +298,32 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   const V3<RC> pn = v3<RC>(RC(M.plane_n[0]), RC(M.plane_n[1]), RC(M.plane_n[2]));
   const RC plane_off = dot(O, pn) - RC(M.plane_c);   // n.(O + x) - c = n.x + plane_off
   int n_active = 0, pt_index = 0;
+  // CF: row r of the records; the geometry of candidate k (xb relative to O) with zero impulse rows; the active candidates as bits
+  // (plane candidate k, candidate pt between multibodies), from which the impulse rows recover each compacted contact's candidate
+  auto cf_put = [&](int r, auto x) {
+    if constexpr (CF) {
+      if (!live) return;
+      if constexpr (AD) io.jac[((size_t)(M.n_q + n + r) * io.jac_n_in + jcol) * ns + e] = x.TDS_CF_DUAL_PART;
+      else pm.cf[(size_t)r * ns + e] = (float)val_of(x);
+    }
+  };
+  auto cf_geom = [&](int k, const V3<RC>& n_b, const V3<RC>& xb, const RC& dist) {
+    if constexpr (CF) {
+      cf_put(10 * k, n_b.x); cf_put(10 * k + 1, n_b.y); cf_put(10 * k + 2, n_b.z);
+      cf_put(10 * k + 3, xb.x + O.x); cf_put(10 * k + 4, xb.y + O.y); cf_put(10 * k + 5, xb.z + O.z);
+      cf_put(10 * k + 6, dist);
+      for (int r = 7; r < 10; ++r) cf_put(10 * k + r, RC(0));
+    }
+  };
+  unsigned long long cf_plane = 0ull, cf_pair = 0ull;
   auto emit_point = [&](int li, const V3<RC>& pos, const RC rad) {
     if (!M.has_plane) return;
     const RC dist = dot(pos, pn) + plane_off - rad;       // contact_plane_sphere, contact_point.hpp:112-116
     if (io.contact_dist && live) io.contact_dist[(size_t)pt_index * ns + e] = (float)val_of(dist);
+    if constexpr (CF) {
+      cf_geom(pt_index, v3<RC>(-pn.x, -pn.y, -pn.z), pos - pn * rad, dist);
+      if (dist < RC(0) && n_active < M.max_contacts) cf_plane |= 1ull << pt_index;
+    }
     ++pt_index;
     if (dist < RC(0) && n_active < M.max_contacts) {
       RC* pc = A.ptr<RC>(M.x_con + n_active * 5 * RCW);
@@ -592,6 +641,11 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
           const RC t = dot(c + O, pnrm);                         // -(dot(position, -normal) + constant), constant = 0
           const RC dist = t - rad;
           if (io.contact_dist && live) io.contact_dist[(size_t)(pt_index + pt) * ns + e] = (float)val_of(dist);
+          if constexpr (CF) {   // point on b: on the sphere (the plane on a), else on the plane
+            if (!swapped) cf_geom(pt_index + pt, v3<RC>(-pnrm.x, -pnrm.y, -pnrm.z), c - pnrm * rad, dist);
+            else cf_geom(pt_index + pt, pnrm, c - pnrm * t, dist);
+            if (dist < RC(0)) cf_pair |= 1ull << pt;
+          }
           if (dist < RC(0)) {
             RC* pr = A.ptr<RC>(M.x_pcon + n_pair_active * 9 * RCW);
             if (!swapped) { st3<RC>(pr, ST, c - pnrm * t); st3<RC>(pr + 3 * ST, ST, v3<RC>(-pnrm.x, -pnrm.y, -pnrm.z)); }   // point on the plane, normal on b = -n
@@ -613,6 +667,19 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
         const RC dist = len - (r1 + r2);
         // candidate distances behind the plane candidates; +inf: the contact function emitted no point (centres closer than CONTACT_EPSILON)
         if (io.contact_dist && live) io.contact_dist[(size_t)(pt_index + pt) * ns + e] = len > RC(1e-5) ? (float)val_of(dist) : __int_as_float(0x7f800000);
+        if constexpr (CF) {   // the record's point on b and normal on b, as stored below; no point emitted: zeros and distance +inf
+          if (len > RC(1e-5)) {
+            const V3<RC> nrm = diff * (RC(1) / len);
+            const V3<RC> p1 = (swapped ? cb : ca) - nrm * r1;
+            if (swapped) cf_geom(pt_index + pt, v3<RC>(-nrm.x, -nrm.y, -nrm.z), p1, dist);
+            else cf_geom(pt_index + pt, nrm, p1 - nrm * dist, dist);
+          } else {
+            const V3<RC> z = v3<RC>(RC(0), RC(0), RC(0));
+            cf_geom(pt_index + pt, z, z, RC(__int_as_float(0x7f800000)));
+            for (int r = 3; r < 6; ++r) cf_put(10 * (pt_index + pt) + r, RC(0));   // (cf_geom adds O)
+          }
+          if (len > RC(1e-5) && dist < RC(0)) cf_pair |= 1ull << pt;
+        }
         if (len > RC(1e-5) && dist < RC(0)) {                  // CONTACT_EPSILON; resolve_collision keeps distance < 0 (the others are zero rows)
           const V3<RC> nrm = diff * (RC(1) / len);
           const V3<RC> p1 = (swapped ? cb : ca) - nrm * r1;    // point_a_world of the call
@@ -1031,6 +1098,22 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     // (world.hpp:351-355).  Group 0: every plane contact (the plane is multibody 0; its lists (plane, b) share no dof, so
     // their Gauss-Seidel sweeps do not see each other and one LCP over all of them is the same arithmetic).  Groups 1..: the
     // pairs of multibodies (a, b) in lexicographic order, rows J_b - J_a over the dofs of both.
+    // CF: the impulse rows of active contact c of group grp (pair records at prec): F = -(p0 n_b + p1 t1 + p2 t2) on body b
+    auto cf_impulse = [&](int grp, int c, const RC* prec, RS p0, RS p1, RS p2) {
+      if constexpr (CF) {
+        int k;
+        V3<RC> n_b, t1, t2;
+        if (grp == 0) { k = cf_nth_bit(cf_plane, c); n_b = nbv; t1 = f1; t2 = f2; }
+        else {
+          const int lo = M.pg_begin[grp - 1];
+          k = pt_index + lo + cf_nth_bit(cf_pair >> lo, c);
+          n_b = ld3<RC>(prec + (c * 9 + 3) * ST, ST);
+          plane_space_t(n_b, t1, t2);
+        }
+        const V3<RC> F = n_b * RC(p0) + t1 * RC(p1) + t2 * RC(p2);
+        cf_put(10 * k + 7, -F.x); cf_put(10 * k + 8, -F.y); cf_put(10 * k + 9, -F.z);
+      }
+    };
     int pbase = 0;   // first record of the current pair group
     for (int grp = 0; grp <= M.n_pair_groups; ++grp) {
     const int n_act = grp == 0 ? n_active : pgc[grp - 1];
@@ -1147,6 +1230,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
           const RS vt = sqrt_t(v1 * v1 + v2 * v2);
           const RS sc = vt > RS(1e-12) ? mu * fn * tanh_t(vt / RS(P.v_transition)) / vt * RS(P.dt) : RS(0);
           const RS p[3] = {fn * RS(P.dt), sc * v1, sc * v2};
+          if constexpr (CF) cf_impulse(grp, c, prec, p[0], p[1], p[2]);
           const RS* y = A.ptr<RS>(M.x_Y) + (c * n3 * 3) * ST;
           for (int k = 0; k < n3; ++k)
             wv[k * ST] += p[0] * y[(3 * k) * ST] + p[1] * y[(3 * k + 1) * ST] + p[2] * y[(3 * k + 2) * ST];
@@ -1188,6 +1272,13 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
           }
         }
       }
+    }
+    if constexpr (CF) {
+      if (P.contact_model != 1)
+        for (int c = 0; c < n_act; ++c) {
+          const RS* cs = A.ptr<RS>(M.x_conS) + c * 6 * ST;
+          cf_impulse(grp, c, prec, cs[3 * ST], cs[4 * ST], cs[5 * ST]);
+        }
     }
     if (grp == 0) TDSW_PHASE();  // 7
     // qd_b -= M^-1 Jc^T p = L^-T w   (mb_constraint_solver.hpp:476-497), blocked back substitution

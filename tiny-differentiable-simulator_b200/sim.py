@@ -430,6 +430,78 @@ class BatchSim:
         self._check(self._L.tds_b200_inverse_dynamics_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(G), _ptr(g_q), _ptr(g_qd),
                                                                  _ptr(g_qdd), _ptr(g_par), st), "inverse_dynamics_vjp_device")
 
+    # ---- the step with its contact records (DESIGN.md section 7.15) ----
+    def contact_rows(self, mode=MODE_FULL, use_pd=False):
+        """(rows, cols) of the derivatives of step_contacts: rows q' | qd' | records (n_q + n_qd + 10 n_contact_points), cols as in
+        step_jacobian_host."""
+        rows, cols = self.jacobian_dims(mode, use_pd)
+        return rows + 10 * self.n_contact_points, cols
+
+    def _step_args(self, q, qd, tau_or_action):
+        q = np.ascontiguousarray(q, dtype=np.float64)
+        qd = np.ascontiguousarray(qd, dtype=np.float64)
+        if q.shape != (self.n_envs, self.n_q) or qd.shape != (self.n_envs, self.n_qd):
+            raise ValueError(f"q [n_envs, {self.n_q}] and qd [n_envs, {self.n_qd}] expected, got {q.shape} and {qd.shape}")
+        t = None if tau_or_action is None else np.ascontiguousarray(tau_or_action, dtype=np.float64)
+        return q, qd, t
+
+    def step_contacts_host(self, mode, q, qd, tau_or_action=None, use_pd=False):
+        """One step (MODE_FULL or MODE_WORLD) on the world-frame kernel that also reports its contacts: (q' [n, n_q], qd' [n, n_qd],
+        C [n, n_contact_points, 10] float64), a record per contact candidate: normal on b [3], point on b [3], distance, impulse on
+        body b [3] (N s) at the point on b, world coordinates (include/tds_b200.h).  q' and qd' are bitwise those of step_device on
+        the world-frame kernel."""
+        q, qd, t = self._step_args(q, qd, tau_or_action)
+        qo, qdo = np.zeros_like(q), np.zeros_like(qd)
+        C = np.zeros((self.n_envs, max(self.n_contact_points, 1), 10))
+        self._check(self._L.tds_b200_step_contacts_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), _dp(qo), _dp(qdo), _dp(C)),
+                    "step_contacts_host")
+        return qo, qdo, C[:, :self.n_contact_points]
+
+    def step_contacts_device(self, mode, q, qd, tau_or_action, q_out, qd_out, contacts, use_pd=False, stream=None):
+        """Device version of step_contacts_host on the SoA layout: q, qd, tau_or_action, q_out, qd_out float32 CUDA tensors
+        [dim, n_stride] as for step_device, contacts float32 [10 * n_contact_points, n_stride] (row r of candidate k at 10 k + r).
+        Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_step_contacts_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), _ptr(q_out),
+                                                          _ptr(qd_out), _ptr(contacts), st), "step_contacts_device")
+
+    def step_contacts_jvp_host(self, mode, q, qd, tau_or_action, t_in, t_par=None, use_pd=False):
+        """step_jvp_host of step_contacts: t_out [n, rows, m] with rows q' | qd' | records (contact_rows), MODE_FULL."""
+        q, qd, t = self._step_args(q, qd, tau_or_action)
+        rows, cols = self.contact_rows(mode, use_pd)
+        (ti, tp), m, single = self._tangents([(t_in, cols), (t_par, len(self.param_ids))], names="t_in and t_par")
+        out = np.zeros((self.n_envs, rows, max(m, 1)))
+        self._check(self._L.tds_b200_step_contacts_jvp_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), m, _dp(ti), _dp(tp),
+                                                            _dp(out)), "step_contacts_jvp_host")
+        return out[:, :, 0] if single else out
+
+    def step_contacts_jvp_device(self, mode, q, qd, tau_or_action, m, t_in, t_par, t_out, use_pd=False, stream=None):
+        """Device version of step_contacts_jvp_host, layouts as step_jvp_device with t_out [rows * m, n_stride] (contact_rows)."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_step_contacts_jvp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), int(m),
+                                                              _ptr(t_in), _ptr(t_par), _ptr(t_out), st), "step_contacts_jvp_device")
+
+    def step_contacts_vjp_host(self, mode, q, qd, tau_or_action, g_out, use_pd=False):
+        """Vector-Jacobian product of step_contacts (MODE_FULL): g_out [n, rows] over q' | qd' | records (contact_rows) -> (g_in
+        [n, cols], g_par [n, k] or None without installed parameters)."""
+        q, qd, t = self._step_args(q, qd, tau_or_action)
+        rows, cols = self.contact_rows(mode, use_pd)
+        g = np.ascontiguousarray(g_out, dtype=np.float64)
+        if g.shape != (self.n_envs, rows):
+            raise ValueError(f"g_out: [n_envs, {rows}] expected, got {g.shape}")
+        g_in = np.zeros((self.n_envs, cols))
+        g_par = np.zeros((self.n_envs, len(self.param_ids))) if self.param_ids else None
+        self._check(self._L.tds_b200_step_contacts_vjp_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), _dp(g), _dp(g_in),
+                                                            _dp(g_par)), "step_contacts_vjp_host")
+        return g_in, g_par
+
+    def step_contacts_vjp_device(self, mode, q, qd, tau_or_action, g_out, g_in, g_par=None, use_pd=False, stream=None):
+        """Device version of step_contacts_vjp_host: g_out [rows, n_stride], g_in [cols, n_stride], g_par [k, n_stride] float64 CUDA
+        tensors (g_in or g_par may be None, not both).  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_step_contacts_vjp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action),
+                                                              _ptr(g_out), _ptr(g_in), _ptr(g_par), st), "step_contacts_vjp_device")
+
     # ---- forward kinematics and linear point Jacobians (DESIGN.md section 7.13) ----
     @staticmethod
     def _points(links, local):
