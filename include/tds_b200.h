@@ -289,6 +289,43 @@ int tds_b200_inverse_dynamics_vjp_device(tds_b200_sim* sim, const float* q, cons
 int tds_b200_inverse_dynamics_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, const double* G, double* g_q,
                                        double* g_qd, double* g_qdd, double* g_par);
 
+/* ---- centre of mass, centroidal momentum matrix and its bias (DESIGN.md section 7.16) -------------------------------------------------
+ * At the fp32-rounded q and qd (qd may be NULL, meaning zero), fp64 outputs, each of which may be NULL (not all three):
+ *   com [10]: the body record of the whole system in the order of the parameter ids' body record: the total mass m, the centre of mass
+ *     c [3] in world coordinates, the rotational inertia I_G about c in world axes [6] (xx, xy, xz, yy, yz, zz).  The counted bodies are
+ *     the links and a floating base; a fixed base belongs to the world and is not counted.
+ *   A [6 n_qd]: the centroidal momentum matrix A_G, entry (r, c) at r * n_qd + c.  Rows: [angular momentum about c; linear momentum] in
+ *     world axes; columns: the coordinates of tds_b200_mass_matrix (a floating base's qd[0:6] is the base-frame twist [w; v]).  So the
+ *     centroidal momentum is h_G = A qd and the Jacobian of c is A[3:6] / m.
+ *   bias [6]: A_G' qd, the rate of h_G when qdd = 0, rows and axes as A.  Velocity terms only: gravity, joint stiffness and damping do
+ *     not enter.  With every external wrench W about c, A qdd + bias = sum W + [0; m g].
+ * While a parameter set is installed, each environment's masses, centres of mass and inertias (links and floating base) are used;
+ * friction, restitution, stiffness and damping do not enter.  An environment whose installed masses do not sum to a positive value
+ * gets non-finite c and I_G.
+ * Argument checks: NULL q, no output, m < 1, every tangent NULL, no cotangent or no cotangent output -> -1; a world of several
+ * multibodies (TDSM_H_NBODIES > 1) or a model whose counted bodies have zero total mass -> -2; t_par / g_par without an installed set
+ * -> -4.
+ *   device: q [n_q][n_stride], qd [n_qd][n_stride] fp32; com [10][n_stride], A [6 n_qd][n_stride], bias [6][n_stride].  Asynchronous.
+ *   host:   q [n][n_q], qd [n][n_qd] fp64 (rounded to fp32); com [n][10], A [n][6 n_qd], bias [n][6].  Synchronous.
+ * _jvp: the outputs' derivatives along m tangents of q, qd and the installed parameters (each may be NULL: zero, not all), as
+ *   tds_b200_inverse_dynamics_jvp_*.  Device t_q [n_q * m][n_stride], t_qd [n_qd * m][n_stride], t_par [k * m][n_stride], t_com
+ *   [10 m][n_stride], t_A [6 n_qd m][n_stride], t_bias [6 m][n_stride] (entry (r, j) at (r * m + j) * n_stride + e); host t_q
+ *   [n][n_q][m], t_qd [n][n_qd][m], t_par [n][k][m], t_com [n][10][m], t_A [n][6 n_qd][m], t_bias [n][6][m].  NULL outputs are skipped.
+ * _vjp: g_x[c] = <G, d(com | A | bias)/dx_c> for x = q, qd and, while a set is installed, the parameters, for cotangents G_com, G_A,
+ *   G_bias in the outputs' layouts (NULL: zero, not all): the JVP along the n_q + n_qd (+ k) identity tangents contracted with G on the
+ *   device.  Any of g_q, g_qd, g_par may be NULL, not all.  Device g_q [n_q][n_stride], g_qd [n_qd][n_stride], g_par [k][n_stride] fp64
+ *   (asynchronous); host g_q [n][n_q], g_qd [n][n_qd], g_par [n][k] (synchronous). */
+int tds_b200_centroidal_device(tds_b200_sim* sim, const float* q, const float* qd, double* com, double* A, double* bias, void* stream);
+int tds_b200_centroidal_host(tds_b200_sim* sim, const double* q, const double* qd, double* com, double* A, double* bias);
+int tds_b200_centroidal_jvp_device(tds_b200_sim* sim, const float* q, const float* qd, int m, const double* t_q, const double* t_qd,
+                                   const double* t_par, double* t_com, double* t_A, double* t_bias, void* stream);
+int tds_b200_centroidal_jvp_host(tds_b200_sim* sim, const double* q, const double* qd, int m, const double* t_q, const double* t_qd,
+                                 const double* t_par, double* t_com, double* t_A, double* t_bias);
+int tds_b200_centroidal_vjp_device(tds_b200_sim* sim, const float* q, const float* qd, const double* G_com, const double* G_A,
+                                   const double* G_bias, double* g_q, double* g_qd, double* g_par, void* stream);
+int tds_b200_centroidal_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* G_com, const double* G_A,
+                                 const double* G_bias, double* g_q, double* g_qd, double* g_par);
+
 /* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
  * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
  * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,

@@ -37,6 +37,10 @@ on the world-frame kernel at the simulator's precision.  Its backward rule (Batc
 three outputs (float32 q.grad, qd.grad, tau_or_action.grad, float64 params.grad) and its forward-mode rule runs
 BatchSim.step_contacts_jvp_device; both in MODE_FULL.  step itself is unchanged.
 
+centroidal(sim, q, qd=None, params=None) is the body record, centroidal momentum matrix and its bias (DESIGN.md section 7.16): (m, c,
+I_G, A, bias) float64, with a backward rule (BatchSim.centroidal_vjp_device: cotangents of all five outputs; float32 q.grad, qd.grad,
+float64 params.grad) and a forward-mode rule (BatchSim.centroidal_jvp_device).
+
 forward_kinematics(sim, q, links, local) is every link's world transform and every point's world position and linear Jacobian (float64,
 DESIGN.md section 7.13) with a backward rule (BatchSim.kinematics_vjp_device: float32 q.grad) and a forward-mode rule
 (BatchSim.kinematics_jvp_device).
@@ -427,6 +431,107 @@ def inverse_dynamics(sim, q, qd, qdd=None, params=None):
                                tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
         raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
     return _InverseDynamics.apply(sim, q, qd, qdd, params)
+
+
+_SYM = [0, 1, 2, 1, 3, 4, 2, 4, 5]   # [3, 3] from the components xx, xy, xz, yy, yz, zz
+
+
+def _cen_outputs(sim, com, A, bias):
+    """Device outputs [rows, n_stride] of the centroidal entries -> (m [n], c [n, 3], I_G [n, 3, 3], A [n, 6, n_qd], bias [n, 6])."""
+    n, nd = sim.n_envs, sim.n_qd
+    com = com[:, :n].t()
+    return (com[:, 0].contiguous(), com[:, 1:4].contiguous(), com[:, 4:10][:, _SYM].reshape(n, 3, 3).contiguous(),
+            A[:6 * nd, :n].t().reshape(n, 6, nd).contiguous(), bias[:, :n].t().contiguous())
+
+
+def _cen_buffers(sim, device):
+    z = lambda rows: torch.zeros((max(rows, 1), sim.n_stride), dtype=torch.float64, device=device)
+    return z(10), z(6 * sim.n_qd), z(6)
+
+
+class _Centroidal(torch.autograd.Function):
+    @staticmethod
+    def forward(sim, q, qd, params):
+        ns = sim.n_stride
+        if params is not None:
+            sim.set_physical_params(sim.param_ids, params.detach())
+        qs, qds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32)
+        com, A, bias = _cen_buffers(sim, q.device)
+        _on_side_stream(q.device, lambda st: sim.centroidal_device(qs, qds, com, A, bias, stream=st), (qs, qds, com, A, bias))
+        return _cen_outputs(sim, com, A, bias)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        sim, q, qd, params = inputs
+        ns = sim.n_stride
+        qs, qds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32)
+        par = params.detach() if params is not None else None
+        ctx.sim, ctx.has = sim, (qd is not None, params is not None)
+        ctx.save_for_backward(qs, *(t if t is not None else qs for t in (qds, par)))
+        ctx.jvp_inputs = (qs, qds, par)
+
+    @staticmethod
+    def backward(ctx, g_m, g_c, g_I, g_A, g_bias):
+        sim = ctx.sim
+        has_qd, has_par = ctx.has
+        qs, qds, par = ctx.saved_tensors
+        qds = qds if has_qd else None
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        # I_G's symmetric entries are read from the six components: an off-diagonal component collects both of its entries
+        gI = g_I.reshape(n, 9).to(torch.float64)
+        gIc = torch.stack([gI[:, 0], gI[:, 1] + gI[:, 3], gI[:, 2] + gI[:, 6], gI[:, 4], gI[:, 5] + gI[:, 7], gI[:, 8]], dim=1)
+        G_com = _soa(torch.cat([g_m.reshape(n, 1).to(torch.float64), g_c.to(torch.float64), gIc], dim=1), ns, torch.float64)
+        G_A = _soa(g_A.reshape(n, 6 * nd), ns, torch.float64)
+        G_bias = _soa(g_bias, ns, torch.float64)
+        z = lambda rows: torch.zeros((max(rows, 1), ns), dtype=torch.float64, device=qs.device)
+        g_q, g_qd = z(sim.n_q), (z(nd) if has_qd else None)
+        g_par = z(par.shape[1]) if has_par else None
+        if has_par:
+            sim.set_physical_params(sim.param_ids, par)   # the values of this call
+        _on_side_stream(qs.device, lambda st: sim.centroidal_vjp_device(qs, qds, G_com, G_A, G_bias, g_q, g_qd, g_par, stream=st),
+                        (qs, qds, G_com, G_A, G_bias, g_q, g_qd, g_par))
+        out = lambda t, rows, dt: None if t is None else t[:rows, :n].t().to(dt).contiguous()
+        return None, out(g_q, sim.n_q, torch.float32), out(g_qd, nd, torch.float32), out(g_par, par.shape[1], torch.float64)
+
+    @staticmethod
+    def jvp(ctx, _sim, t_q, t_qd, t_params):
+        with torch._C._DisableFuncTorch():
+            return _Centroidal._jvp(ctx, _plain(t_q), _plain(t_qd), _plain(t_params))
+
+    @staticmethod
+    def _jvp(ctx, t_q, t_qd, t_params):
+        sim = ctx.sim
+        has_qd, has_par = ctx.has
+        qs, qds, par = (_plain(t) for t in ctx.jvp_inputs)
+        ns = sim.n_stride
+        tq = _soa_opt(t_q, ns, torch.float64)
+        tqd = _soa_opt(t_qd if has_qd else None, ns, torch.float64)
+        tp = _soa_opt(t_params if has_par else None, ns, torch.float64)
+        t_com, t_A, t_bias = _cen_buffers(sim, qs.device)
+        if any(t is not None for t in (tq, tqd, tp)):
+            if has_par:
+                sim.set_physical_params(sim.param_ids, par)   # the values of this call
+            _on_side_stream(qs.device, lambda st: sim.centroidal_jvp_device(qs, qds, 1, tq, tqd, tp, t_com, t_A, t_bias, stream=st),
+                            (qs, qds, tq, tqd, tp, t_com, t_A, t_bias))
+        return _cen_outputs(sim, t_com, t_A, t_bias)
+
+
+def centroidal(sim, q, qd=None, params=None):
+    """The centroidal quantities of every environment of `sim` (a BatchSim), DESIGN.md section 7.16, in fp64 at the fp32-rounded inputs:
+    (m [n_envs], c [n_envs, 3], I_G [n_envs, 3, 3], A [n_envs, 6, n_qd], bias [n_envs, 6]) float64 - the total mass of the links and a
+    floating base, their centre of mass in world coordinates, the rotational inertia about it in world axes, the centroidal momentum
+    matrix (h_G = A qd, rows [angular about c; linear] in world axes, columns in the coordinates of mass_matrix) and its bias A' qd (the
+    rate of h_G at qdd = 0, without gravity).  q [n_envs, n_q], qd [n_envs, n_qd] float32 CUDA tensors (qd None: zero).  params: None, or
+    a float64 CUDA tensor [n_envs, k] of values for the parameters installed by sim.set_physical_params (then also differentiated).
+    Differentiable in reverse and forward mode."""
+    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
+        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
+    if qd is not None and (qd.dtype != torch.float32 or not qd.is_cuda or qd.dim() != 2 or tuple(qd.shape) != (sim.n_envs, sim.n_qd)):
+        raise ValueError("qd: a float32 CUDA tensor [n_envs, n_qd] is expected")
+    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
+                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
+        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    return _Centroidal.apply(sim, q, qd, params)
 
 
 def _kin_outputs(sim, K, xf, x, J):

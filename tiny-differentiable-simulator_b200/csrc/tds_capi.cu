@@ -72,6 +72,11 @@ extern "C" int tds_launch_contacts(const DevModel* M, const SimParams* P, const 
 extern "C" int tds_launch_contacts_jvp(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
                                        const double* t_in, const double* t_par, int m, int mode, int use_pd, int n_dirs, char* gscratch,
                                        cudaStream_t stream);
+// the body record, centroidal momentum matrix and its bias, and their Jacobian-vector products (tds_centroidal.cu)
+extern "C" int tds_launch_centroidal(const DevModel* M, const StepIO* io, const ParMap* pm, const TdsCenCall* out, char* gscratch,
+                                     cudaStream_t stream);
+extern "C" int tds_launch_centroidal_jvp(const DevModel* M, const StepIO* io, const ParMap* pm, const TdsCenCall* out, const double* t_in,
+                                         const double* t_par, int m, int n_dirs, char* gscratch, cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
@@ -890,15 +895,18 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
   return 0;
 }
 
-// what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14, or the step
-// with its contact records (section 7.15)
-enum class Query { step, mass, kin, inv, contacts };
+// what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14 and 7.16, or
+// the step with its contact records (section 7.15)
+enum class Query { step, mass, kin, inv, contacts, centroidal };
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
 // inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
 // (t_in = the q tangents, t_par unused); inv: t_in = the q | qd | qdd tangents (qd and qdd in the step's qd and tau_or_action);
-// contacts: as step, with the rows q' | qd' | records
-struct JvpTangents { const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr; };
+// contacts: as step, with the rows q' | qd' | records; centroidal: t_in = the q | qd tangents (qd in the step's qd), outputs `cen`
+struct JvpTangents {
+  const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr;
+  const TdsCenCall* cen = nullptr;
+};
 
 // the installed physical parameters as a launch argument in *pmv, or NULL without any
 static const ParMap* installed_par(const tds_b200_sim* s, ParMap* pmv) {
@@ -959,6 +967,9 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
         case Query::inv: rc = tds_launch_inv_jvp(&s->dm_ad, &s->P, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
         case Query::contacts:
           rc = tds_launch_contacts_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch, sm);
+          break;
+        case Query::centroidal:
+          rc = tds_launch_centroidal_jvp(&s->dm_ad, &io, pm, jv->cen, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm);
           break;
       }
     }
@@ -1460,6 +1471,168 @@ int tds_b200_inverse_dynamics_vjp_host(tds_b200_sim* s, const double* q, const d
   CUDA_TRY(put_rows(s->vjp_g, G, nd, n, ns, s->stream));
   if (int rc = inv_vjp_run(s, s->q, qd_d, qdd_d, s->vjp_g, g_d, g_par ? g_d + (size_t)n_in * ns : nullptr, s->stream)) return rc;
   CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}, {g_par, k}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- centre of mass, centroidal momentum matrix and its bias (DESIGN.md section 7.16): the CEN instances of the world-frame kernel
+// (tds_centroidal.cu) -------------------------------------------------------------------------------------------------------------------
+// rows of the outputs com | A | bias
+struct CenRows { size_t com, A, bias; size_t all() const { return com + A + bias; } };
+static CenRows cen_rows(const tds_b200_sim* s) { return CenRows{10, (size_t)6 * s->dm[0].n_qd, 6}; }
+
+// -2 for the models the query refuses: a world of several multibodies, counted bodies (links, a floating base) without mass
+static int cen_model_check(tds_b200_sim* s) {
+  const DevModel& M = s->dm[0];
+  if (M.n_bodies > 1) { set_err("centroidal: a world of several multibodies (TDSM_H_NBODIES > 1)"); return -2; }
+  double m = M.floating ? M.base_rbic[0] : 0.0;
+  for (int i = 0; i < M.n_links; ++i) m += M.rbic[i][0];
+  if (!(m > 0.0)) { set_err("centroidal: the counted bodies have zero total mass"); return -2; }
+  return 0;
+}
+
+// fp64 outputs from q [n_q][ns] and qd [n_qd][ns] fp32 (NULL: zero)
+static int cen_run(tds_b200_sim* s, const float* q, const float* qd, const TdsCenCall* out, cudaStream_t sm) {
+  return value_run(s, "centroidal", q, qd, nullptr, nullptr, [&](const StepIO* io, const ParMap* pm) {
+    return tds_launch_centroidal(&s->dm_m, io, pm, out, s->jac_scratch, sm);
+  });
+}
+
+// inputs of the centroidal derivatives: q | qd
+static int cen_n_in(const tds_b200_sim* s) { return s->dm[0].n_q + s->dm[0].n_qd; }
+
+// the outputs' columns [rows * m][ns] along t_in [(n_q + n_qd) * m][ns] (q | qd tangents, contiguous) and t_par (either may be NULL)
+static int cen_jvp_run(tds_b200_sim* s, const float* q, const float* qd, int m, const double* t_in, const double* t_par,
+                       const TdsCenCall* out, cudaStream_t sm) {
+  JvpTangents jv{t_in, t_par, m, Query::centroidal};
+  jv.cen = out;
+  return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, nullptr, nullptr, sm, false, &jv);
+}
+
+// g_in [n_q + n_qd][ns] (q | qd, contiguous) and g_par [k][ns] (NULL: not wanted) = <G, d(com | A | bias)>, G [rows][ns] concatenated
+static int cen_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const double* G, double* g_in, double* g_par, cudaStream_t sm) {
+  const CenRows R = cen_rows(s);
+  const size_t ns = s->ns;
+  return vjp_by_eye(s, "centroidal", cen_n_in(s), R.all(), G, g_in, g_par, sm, [&](int nd, const double* t_in, const double* t_par, double* dO) {
+    const TdsCenCall out{dO, dO + R.com * nd * ns, dO + (R.com + R.A) * nd * ns};
+    return cen_jvp_run(s, q, qd, nd, t_in, t_par, &out, sm);
+  });
+}
+
+// host q [n][n_q], qd [n][n_qd] (NULL: zero) -> s->q, s->qd; the device pointer of qd (NULL for NULL)
+static int put_cen_inputs(tds_b200_sim* s, const double* q, const double* qd, const float** qd_d) {
+  int rc = put_q(s, q);
+  if (!rc && qd) rc = put_state(s, qd, s->dm[0].n_qd, s->qd);
+  *qd_d = qd ? s->qd : nullptr;
+  return rc;
+}
+
+static int cen_check(tds_b200_sim* s, const void* q, const void* com, const void* A, const void* bias) {
+  if (!s || !q || (!com && !A && !bias)) return -1;
+  return cen_model_check(s);
+}
+
+int tds_b200_centroidal_device(tds_b200_sim* s, const float* q, const float* qd, double* com, double* A, double* bias, void* stream) {
+  if (int rc = cen_check(s, q, com, A, bias)) return rc;
+  const TdsCenCall out{com, A, bias};
+  return cen_run(s, q, qd, &out, (cudaStream_t)stream);
+}
+
+int tds_b200_centroidal_host(tds_b200_sim* s, const double* q, const double* qd, double* com, double* A, double* bias) {
+  if (int rc = cen_check(s, q, com, A, bias)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const CenRows R = cen_rows(s);
+  const float* qd_d;
+  if (int rc = put_cen_inputs(s, q, qd, &qd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * R.all() * ns));
+  double* d = s->jac_dev;
+  const TdsCenCall out{com ? d : nullptr, A ? d + R.com * ns : nullptr, bias ? d + (R.com + R.A) * ns : nullptr};
+  if (int rc = cen_run(s, s->q, qd_d, &out, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{com, R.com}, {A, R.A}, {bias, R.bias}}, d, n, ns, s->stream));
+  return 0;
+}
+
+static int cen_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_qd, const void* t_par, const void* t_com,
+                         const void* t_A, const void* t_bias) {
+  if (!s || !q || m < 1 || (!t_q && !t_qd && !t_par) || (!t_com && !t_A && !t_bias)) return -1;
+  if (int rc = cen_model_check(s)) return rc;
+  return par_without_installed(s, t_par, "centroidal jvp: parameter tangents");
+}
+
+int tds_b200_centroidal_jvp_device(tds_b200_sim* s, const float* q, const float* qd, int m, const double* t_q, const double* t_qd,
+                                   const double* t_par, double* t_com, double* t_A, double* t_bias, void* stream) {
+  if (int rc = cen_jvp_check(s, q, m, t_q, t_qd, t_par, t_com, t_A, t_bias)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  cudaStream_t sm = (cudaStream_t)stream;
+  double* tin = nullptr;
+  if (t_q || t_qd) {   // the kernel reads the q | qd tangents as one array
+    CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (size_t)cen_n_in(s) * m * s->ns));
+    tin = s->jac_dev;
+    CUDA_TRY(put_parts_d2d<double>(tin, {{t_q, n_q * m}, {t_qd, nd * m}}, s->ns, sm));
+  }
+  const TdsCenCall out{t_com, t_A, t_bias};
+  return cen_jvp_run(s, q, qd, m, tin, t_par, &out, sm);
+}
+
+int tds_b200_centroidal_jvp_host(tds_b200_sim* s, const double* q, const double* qd, int m, const double* t_q, const double* t_qd,
+                                 const double* t_par, double* t_com, double* t_A, double* t_bias) {
+  if (int rc = cen_jvp_check(s, q, m, t_q, t_qd, t_par, t_com, t_A, t_bias)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  const CenRows R = cen_rows(s);
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; q | qd (contiguous, zero where NULL, none if both are), t_par, the outputs
+  const size_t ti = (t_q || t_qd) ? (size_t)cen_n_in(s) * m : 0, tp = (size_t)(t_par ? s->par.n : 0) * m;
+  const float* qd_d;
+  if (int rc = put_cen_inputs(s, q, qd, &qd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + tp + R.all() * m) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + (ti + tp) * ns;
+  if (ti) CUDA_TRY(put_parts<double>(d, {{t_q, n_q * m}, {t_qd, nd * m}}, n, ns, s->stream));
+  if (t_par) CUDA_TRY(put_rows(d + ti * ns, t_par, tp, n, ns, s->stream));
+  const TdsCenCall out{t_com ? to_d : nullptr, t_A ? to_d + R.com * m * ns : nullptr, t_bias ? to_d + (R.com + R.A) * m * ns : nullptr};
+  if (int rc = cen_jvp_run(s, s->q, qd_d, m, ti ? d : nullptr, t_par ? d + ti * ns : nullptr, &out, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{t_com, R.com * m}, {t_A, R.A * m}, {t_bias, R.bias * m}}, to_d, n, ns, s->stream));
+  return 0;
+}
+
+static int cen_vjp_check(tds_b200_sim* s, const void* q, const void* G_com, const void* G_A, const void* G_bias, const void* g_q,
+                         const void* g_qd, const void* g_par) {
+  if (!s || !q || (!G_com && !G_A && !G_bias) || (!g_q && !g_qd && !g_par)) return -1;
+  if (int rc = cen_model_check(s)) return rc;
+  return par_without_installed(s, g_par, "centroidal vjp: parameter cotangents");
+}
+
+int tds_b200_centroidal_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const double* G_com, const double* G_A,
+                                   const double* G_bias, double* g_q, double* g_qd, double* g_par, void* stream) {
+  if (int rc = cen_vjp_check(s, q, G_com, G_A, G_bias, g_q, g_qd, g_par)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  const CenRows R = cen_rows(s);
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the concatenated cotangent com | A | bias (zero where a part is NULL), then g_q | g_qd as one array for the contraction
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (R.all() + cen_n_in(s)) * s->ns));
+  double* g_d = s->vjp_g + R.all() * s->ns;
+  CUDA_TRY(put_parts_d2d<double>(s->vjp_g, {{G_com, R.com}, {G_A, R.A}, {G_bias, R.bias}}, s->ns, sm));
+  if (int rc = cen_vjp_run(s, q, qd, s->vjp_g, g_d, g_par, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, n_q}, {g_qd, nd}}, g_d, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_centroidal_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* G_com, const double* G_A,
+                                 const double* G_bias, double* g_q, double* g_qd, double* g_par) {
+  if (int rc = cen_vjp_check(s, q, G_com, G_A, G_bias, g_q, g_qd, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, n_in = cen_n_in(s);
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, k = s->par.n;
+  const CenRows R = cen_rows(s);
+  const float* qd_d;
+  if (int rc = put_cen_inputs(s, q, qd, &qd_d)) return rc;
+  // G (com | A | bias, zero where a part is NULL) | g_q | g_qd | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (R.all() + n_in + k + 1) * ns));
+  double* g_d = s->vjp_g + R.all() * ns;
+  CUDA_TRY(put_parts<double>(s->vjp_g, {{G_com, R.com}, {G_A, R.A}, {G_bias, R.bias}}, n, ns, s->stream));
+  if (int rc = cen_vjp_run(s, s->q, qd_d, s->vjp_g, g_d, g_par ? g_d + (size_t)n_in * ns : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_par, k}}, g_d, n, ns, s->stream));
   return 0;
 }
 

@@ -53,7 +53,9 @@ struct KinArgJvp : KinArg { JvpTan jv; };
 // instances write the records' dual parts into io.jac behind q' | qd' and take the plain JVP arguments.
 struct CfArg { float* cf; };
 struct CfArgPar : ParMap { float* cf; };
-template <bool PAR, bool JV = false, bool KIN = false, bool CF = false> struct ParArg { typedef NoPar type; };
+// kernel argument of the centroidal instances (CEN, DESIGN.md section 7.16): the argument of the same instance without CEN and the outputs
+template <typename B> struct CenArg : B { double* com; double* A; double* bias; };
+template <bool PAR, bool JV = false, bool KIN = false, bool CF = false, bool CEN = false> struct ParArg { typedef NoPar type; };
 template <> struct ParArg<true, false> { typedef ParMap type; };
 template <> struct ParArg<false, true> { typedef NoParJvp type; };
 template <> struct ParArg<true, true> { typedef ParMapJvp type; };
@@ -63,6 +65,7 @@ template <> struct ParArg<false, false, false, true> { typedef CfArg type; };
 template <> struct ParArg<true, false, false, true> { typedef CfArgPar type; };
 template <> struct ParArg<false, true, false, true> { typedef NoParJvp type; };
 template <> struct ParArg<true, true, false, true> { typedef ParMapJvp type; };
+template <bool PAR, bool JV> struct ParArg<PAR, JV, false, false, true> { typedef CenArg<typename ParArg<PAR, JV>::type> type; };
 
 // CF, dual instances: the part of a record's dual number they write - the tangent (d).  The host build of the tests also compiles them
 // with the value (v), for an fp64 value path of the records that central differences can resolve.
@@ -116,12 +119,19 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // computed; every impulse row is zeroed there and the active contacts' rows are written after their group's PGS sweep or spring-damper
 // loop.  Row r at pm.cf[r * ns + e] (value instances, fp32), or its dual part at io.jac[((n_q + n_qd + r) * m + j) * ns + e] behind the
 // rows q' | qd' (JV instances).  Nothing else differs from the step.
+// CEN: the centroidal quantities (DESIGN.md section 7.16), launched in MODE_NOCONTACT with qd in io.qd_in (null: zero).  Pass 1 adds
+// every link's rigid inertia r_i about O (and the floating base's) into the body record and v_i x* (r_i v_i) into the velocity-only rate of
+// momentum about O; pass 2 accumulates the composites Ic_i as MASS does, takes F = Ic_i S_i as column qd_idx of the momentum about O and
+// adds Ic_i (v_i x S_i qd_i) to the rate.  A floating base's columns are the total inertia times the base twist's unit columns.  Then
+// everything shifts to the centroid c: k_G = k_O - (c - O) x l.  Outputs pm.com [10], pm.A [6 n_qd] and pm.bias [6] (each may be null),
+// row r at out[r * ns + e] (fp64 instances) or its dual part at out[(r * m + j) * ns + e] (JV instances).  ABA and integration are not
+// compiled in.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
-          bool KIN = false, bool INV = false, bool CF = false>
+          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
-                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF>::type pm = {}) {
+                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF, CEN>::type pm = {}) {
   extern __shared__ __align__(16) char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp_in_blk = threadIdx.x >> 5;
@@ -240,7 +250,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // input directions of the differentiable instance: q | qd | tau or action | kp, kd, max_force (with PD)
   const int in0 = M.n_q + n;
   for (int k = 0; k < M.n_q; ++k) qv[k * ST] = seed(RQ(io.q_in[(size_t)k * ns + e]), k);
-  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ((INV && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
+  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(((INV || CEN) && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
   for (int k = 0; k < n; ++k) tauv[k * ST] = RQ(0.f);
   if (!MASS && use_pd) {
     const RQ kp = seed(RQ(E.kp), in0 + E.n_act), kd = seed(RQ(E.kd), in0 + E.n_act + 1), fmax_ = seed(RQ(E.max_force), in0 + E.n_act + 2);
@@ -447,6 +457,20 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   }();
   SvInv a_prev_inv = a_base_inv, f_links = SvInv{};
   if constexpr (INV) { f_links.top = v3<RC>(RC(0), RC(0), RC(0)); f_links.bot = f_links.top; }
+  // CEN: the rigid inertia of the counted bodies about O in world axes (the root composite) and the velocity-only rate of momentum about O
+  typename std::conditional<CEN, Rbi<RC>, NoPar>::type cen_I{};
+  typename std::conditional<CEN, Sv<RC>, NoPar>::type cen_f{};
+  if constexpr (CEN) {
+    static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the CEN instances run in one scalar type");
+    cen_I.m = RC(0); cen_I.h = v3<RC>(RC(0), RC(0), RC(0)); cen_I.I = {RC(0), RC(0), RC(0), RC(0), RC(0), RC(0)};
+    cen_f.top = cen_I.h; cen_f.bot = cen_I.h;
+    if (M.floating) {   // the base: its inertia about its origin O rotated to world axes, and its term v_b x* (I_b v_b) (qdd = 0)
+      Rbi<RC> Ib = model_rbi_of<RC>(M.base_rbi);
+      if constexpr (PAR) { if (pm.any_base) installed_base(Ib); }
+      cen_I.m = Ib.m; cen_I.h = mul(Rb, Ib.h); cen_I.I = rot_sym(Rb, Ib.I);
+      cen_f = cross_mf(v_base, rbi_mul(cen_I, v_base));
+    }
+  }
   for (int i = 0; i < n_links; ++i) {
     const int p = M.parent[i];
     const int fl = M.flags[i];
@@ -540,6 +564,11 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       v.bot = axpy(Sf.bot, qdi, v.bot);
     }
     st6<RA>(A.ptr<RA>(M.x_link + i * LWD + VOFF), ST, v);
+    if constexpr (CEN) {   // the link's share of the body record and its term v_i x* (r_i v_i) of the rate
+      const Rbi<RC> r = ld_rbi<RC>(A.ptr<RC>(M.x_link + i * LWD), ST);
+      rbi_add(cen_I, r);
+      cen_f = cen_f + cross_mf(v, rbi_mul(r, v));
+    }
     if (want_contacts) emit_geoms(i, Ri, pi);
     if (io.link_xf && live) {
       float* o = io.link_xf + (size_t)i * 12 * ns + e;
@@ -607,6 +636,23 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       }
     return;
   }
+  // CEN: the centre of mass relative to O; row r of an output; column col of A from the momentum F about O of qd_col = 1: [k_O - c x l; l]
+  typename std::conditional<CEN, V3<RC>, NoPar>::type cen_c{};
+  if constexpr (CEN) cen_c = cen_I.h * (RC(1) / cen_I.m);
+  auto cen_put = [&](double* o, size_t r, const RC& x) {
+    if constexpr (CEN) {
+      if (!o || !live) return;
+      if constexpr (AD) o[(r * io.jac_n_in + jcol) * ns + e] = x.d;
+      else o[r * ns + e] = x;
+    }
+  };
+  auto cen_col = [&](int col, const Sv<RC>& F) {
+    if constexpr (CEN) {
+      const V3<RC> k = F.top - cross(cen_c, F.bot);
+      cen_put(pm.A, col, k.x); cen_put(pm.A, n + col, k.y); cen_put(pm.A, 2 * n + col, k.z);
+      cen_put(pm.A, 3 * n + col, F.bot.x); cen_put(pm.A, 4 * n + col, F.bot.y); cen_put(pm.A, 5 * n + col, F.bot.z);
+    }
+  };
   // ---- contacts between the multibodies of the world (world.hpp:206-282), group = ordered pair of multibodies -----------------------
   // contact_sphere_sphere (contact_point.hpp:44-94) on sphere centres / capsule end spheres (contact_capsule_sphere, :406-438);
   // sphere A x capsule B goes through the dispatcher's swapped call (:478-492): points exchanged, normal negated.
@@ -739,9 +785,9 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     const Sv<RA> v = ld6<RA>(vrec, ST);
     Abi<RA> Ia = abi_from_rbi(rb);
     Sv<RA> pA = cross_mf(v, rbi_mul(rb, v));                 // kinematics.hpp:132
-    if (fl & TDS_LF_CHILD_ADJ) { if constexpr (!MASS) { abi_add(Ia, cA); pA = pA + cP; } rbi_add(Ic, cC); }
+    if (fl & TDS_LF_CHILD_ADJ) { if constexpr (!MASS && !CEN) { abi_add(Ia, cA); pA = pA + cP; } rbi_add(Ic, cC); }
     if (M.acc_slot[i] >= 0) {
-      if constexpr (!MASS) {
+      if constexpr (!MASS && !CEN) {
         Abi<RA> sa; Sv<RA> sp;
         acc_ld27<RA>(A.ptr<RA>(M.x_acc + M.acc_slot[i] * M.x_acc_words), ST, sa, sp);
         abi_add(Ia, sa); pA = pA + sp;
@@ -753,7 +799,16 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     // every lane must have finished reading its RC record before any lane writes the RA view.
     __syncwarp();
     RA* const urec = A.ptr<RA>(M.x_link + i * LWD);
-    if constexpr (MASS) {   // the CRBA columns of the two branches below (mass_matrix.hpp:58-111), without the ABA
+    if constexpr (CEN) {   // the columns of link i's dofs, F = Ic S; Ic (v x S qd) into the rate (Ic c summed over links = sum r a)
+      Sv<RC> vJ; vJ.top = v3<RC>(RC(0), RC(0), RC(0)); vJ.bot = vJ.top;
+      for (int a = 0; a < n_cols(i); ++a) {
+        const Sv<RC> Sc = S_col(i, a);
+        const RC qda = qdv[(M.qd_idx[i] + a) * ST];
+        vJ.top = axpy(Sc.top, qda, vJ.top); vJ.bot = axpy(Sc.bot, qda, vJ.bot);
+        cen_col(M.qd_idx[i] + a, rbi_mul(Ic, Sc));
+      }
+      cen_f = cen_f + rbi_mul(Ic, cross_mm(v, vJ));
+    } else if constexpr (MASS) {   // the CRBA columns of the two branches below (mass_matrix.hpp:58-111), without the ABA
       const int d0 = M.qd_idx[i];
       for (int a = 0; a < n_cols(i); ++a) {
         const Sv<RC> F = rbi_mul(Ic, S_col(i, a));
@@ -872,10 +927,34 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     else {
       const int slot = (p >= 0) ? M.acc_slot[p] : M.base_acc;
       if (slot >= 0) {
-        if constexpr (!MASS) acc_add27<RA>(A.ptr<RA>(M.x_acc + slot * M.x_acc_words), ST, Ia, pa);
+        if constexpr (!MASS && !CEN) acc_add27<RA>(A.ptr<RA>(M.x_acc + slot * M.x_acc_words), ST, Ia, pa);
         rbi_acc<RC>(A.ptr<RC>(M.x_acc + slot * M.x_acc_words + M.x_acc_ic_word), ST, Ic);
       }
     }
+  }
+  if constexpr (CEN) {
+    if (M.floating) {   // the base twist's unit columns [R_b e_k; 0], [0; R_b e_k] move every body: the momentum is the total inertia's
+      const Sv<RC> z = Sv<RC>{v3<RC>(RC(0), RC(0), RC(0)), v3<RC>(RC(0), RC(0), RC(0))};
+      for (int k = 0; k < 3; ++k) {
+        const V3<RC> u = k == 0 ? col_x(Rb) : (k == 1 ? col_y(Rb) : col_z(Rb));
+        Sv<RC> s = z; s.top = u; cen_col(k, rbi_mul(cen_I, s));
+        s = z; s.bot = u; cen_col(3 + k, rbi_mul(cen_I, s));
+      }
+    }
+    // m, c + O, and the inertia about c: I_O - m (|c|^2 1 - c c^T)
+    const RC m = cen_I.m;
+    const V3<RC> c = cen_c;
+    const RC cc = dot(c, c);
+    cen_put(pm.com, 0, m);
+    cen_put(pm.com, 1, c.x + O.x); cen_put(pm.com, 2, c.y + O.y); cen_put(pm.com, 3, c.z + O.z);
+    cen_put(pm.com, 4, cen_I.I.xx - m * (cc - c.x * c.x)); cen_put(pm.com, 5, cen_I.I.xy + m * c.x * c.y);
+    cen_put(pm.com, 6, cen_I.I.xz + m * c.x * c.z); cen_put(pm.com, 7, cen_I.I.yy - m * (cc - c.y * c.y));
+    cen_put(pm.com, 8, cen_I.I.yz + m * c.y * c.z); cen_put(pm.com, 9, cen_I.I.zz - m * (cc - c.z * c.z));
+    // the bias about c: d/dt k_G = d/dt k_O - (c - O) x d/dt l (the term c' x l vanishes: l = m c')
+    const V3<RC> kb = cen_f.top - cross(c, cen_f.bot);
+    cen_put(pm.bias, 0, kb.x); cen_put(pm.bias, 1, kb.y); cen_put(pm.bias, 2, kb.z);
+    cen_put(pm.bias, 3, cen_f.bot.x); cen_put(pm.bias, 4, cen_f.bot.y); cen_put(pm.bias, 5, cen_f.bot.z);
+    return;
   }
   TDSW_PHASE();  // 3
 

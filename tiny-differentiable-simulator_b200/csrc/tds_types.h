@@ -156,6 +156,10 @@ struct TdsKinCall {
   double* xf; double* x; double* J;
 };
 
+// The outputs of one call of the centroidal instances (tds_centroidal.cu, DESIGN.md section 7.16): the body record com [10][ns], the
+// centroidal momentum matrix A [6 * n_qd][ns] and its bias A' qd [6][ns] (each may be null; columns of an m-column block in the JVP)
+struct TdsCenCall { double* com; double* A; double* bias; };
+
 // Installed physical parameters (tds_b200_set_physical_params_*): the slot of each model quantity in the lane's value vector,
 // or -1 = the model's value, and the values themselves.  Passed only to the instances of the world-frame kernel that read them
 // (StepIO stays as it is: the other instances keep it on their stack).

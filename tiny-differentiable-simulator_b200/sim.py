@@ -31,6 +31,11 @@ def _stream(stream):
     return ctypes.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream().cuda_stream)
 
 
+def _sym3(c):
+    """[..., 3, 3] symmetric matrices from their components [..., 6] (xx, xy, xz, yy, yz, zz)."""
+    return c[..., [0, 1, 2, 1, 3, 4, 2, 4, 5]].reshape(c.shape[:-1] + (3, 3))
+
+
 class BatchSim:
     def __init__(self, model, n_envs, device=0, dt=1e-3, gravity=(0.0, 0.0, -9.81), friction=0.5,
                  restitution=0.0, erp=0.2, cfm=1e-5, pgs_iterations=1, keep_all_points=False,
@@ -429,6 +434,74 @@ class BatchSim:
         st = _stream(stream)
         self._check(self._L.tds_b200_inverse_dynamics_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(G), _ptr(g_q), _ptr(g_qd),
                                                                  _ptr(g_qdd), _ptr(g_par), st), "inverse_dynamics_vjp_device")
+
+    # ---- centre of mass, centroidal momentum matrix and its bias (DESIGN.md section 7.16) ----
+    def centroidal_host(self, q, qd=None):
+        """(m [n], c [n, 3], I_G [n, 3, 3], A [n, 6, n_qd], bias [n, 6]) float64 at the fp32-rounded q [n, n_q] and qd [n, n_qd] (None:
+        zero): the total mass of the links and a floating base, their centre of mass c in world coordinates and rotational inertia about c
+        in world axes, the centroidal momentum matrix A_G (rows [angular momentum about c; linear momentum] in world axes, columns in
+        the coordinates of the mass matrix: h_G = A qd) and its bias A_G' qd (the rate of h_G at qdd = 0, velocity terms only).
+        Installed masses, centres of mass and inertias apply per environment (include/tds_b200.h)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd = self._inv_in(qd, self.n_qd, "qd")
+        com, A, bias = np.zeros((self.n_envs, 10)), np.zeros((self.n_envs, 6, self.n_qd)), np.zeros((self.n_envs, 6))
+        self._check(self._L.tds_b200_centroidal_host(self._h, _dp(q), _dp(qd), _dp(com), _dp(A), _dp(bias)), "centroidal_host")
+        return com[:, 0], com[:, 1:4], _sym3(com[:, 4:10]), A, bias
+
+    def centroidal_device(self, q, qd, com, A, bias, stream=None):
+        """Device version of centroidal_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd [n_qd, n_stride] (or None); com
+        [10, n_stride] (m, c, I_G xx xy xz yy yz zz), A [6 n_qd, n_stride], bias [6, n_stride] float64 (each may be None, not all).
+        Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_centroidal_device(self._h, _ptr(q), _ptr(qd), _ptr(com), _ptr(A), _ptr(bias), st), "centroidal_device")
+
+    def centroidal_jvp_host(self, q, qd=None, t_q=None, t_qd=None, t_par=None):
+        """Directional derivatives (dcom [n, 10, m], dA [n, 6, n_qd, m], dbias [n, 6, m]) of the outputs of centroidal_host in its
+        com-record layout (m, c, I_G xx xy xz yy yz zz) along m tangents t_q [n, n_q, m], t_qd [n, n_qd, m] and t_par [n, k, m] (each may
+        be None, not all); tangents given as [n, dim] are m = 1 and drop the last axis."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd = self._inv_in(qd, self.n_qd, "qd")
+        if all(t is None for t in (t_q, t_qd, t_par)):
+            raise ValueError("at least one tangent is expected")
+        ts, m, single = self._tangents([(t_q, self.n_q), (t_qd, self.n_qd), (t_par, len(self.param_ids))])
+        n = self.n_envs
+        dcom, dA, dbias = np.zeros((n, 10, m)), np.zeros((n, 6, self.n_qd, m)), np.zeros((n, 6, m))
+        self._check(self._L.tds_b200_centroidal_jvp_host(self._h, _dp(q), _dp(qd), m, *(_dp(t) for t in ts), _dp(dcom), _dp(dA), _dp(dbias)),
+                    "centroidal_jvp_host")
+        return (dcom[..., 0], dA[..., 0], dbias[..., 0]) if single else (dcom, dA, dbias)
+
+    def centroidal_jvp_device(self, q, qd, m, t_q, t_qd, t_par, t_com, t_A, t_bias, stream=None):
+        """Device version of centroidal_jvp_host: q float32 [n_q, n_stride], qd [n_qd, n_stride] (or None); t_q [n_q * m, n_stride], t_qd
+        [n_qd * m, n_stride], t_par [k * m, n_stride] (each may be None, not all), t_com [10 m, n_stride], t_A [6 n_qd m, n_stride], t_bias
+        [6 m, n_stride] (each may be None, not all) float64 CUDA tensors, entry (r, j) at row r * m + j.  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_centroidal_jvp_device(self._h, _ptr(q), _ptr(qd), int(m), _ptr(t_q), _ptr(t_qd), _ptr(t_par), _ptr(t_com),
+                                                           _ptr(t_A), _ptr(t_bias), st), "centroidal_jvp_device")
+
+    def centroidal_vjp_host(self, q, qd=None, G_com=None, G_A=None, G_bias=None):
+        """Cotangents G_com [n, 10] (com-record layout), G_A [n, 6, n_qd], G_bias [n, 6] (None: zero, not all) -> (g_q [n, n_q], g_qd
+        [n, n_qd], g_par [n, k] or None without installed parameters)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd = self._inv_in(qd, self.n_qd, "qd")
+        if G_com is None and G_A is None and G_bias is None:
+            raise ValueError("at least one cotangent is expected")
+        G_com = self._inv_in(G_com, 10, "G_com")
+        G_A = None if G_A is None else self._inv_in(np.reshape(G_A, (self.n_envs, -1)), 6 * self.n_qd, "G_A")
+        G_bias = self._inv_in(G_bias, 6, "G_bias")
+        k = len(self.param_ids)
+        g_q, g_qd = np.zeros((self.n_envs, self.n_q)), np.zeros((self.n_envs, self.n_qd))
+        g_par = np.zeros((self.n_envs, k)) if k else None
+        self._check(self._L.tds_b200_centroidal_vjp_host(self._h, _dp(q), _dp(qd), _dp(G_com), _dp(G_A), _dp(G_bias), _dp(g_q), _dp(g_qd),
+                                                         _dp(g_par)), "centroidal_vjp_host")
+        return g_q, g_qd, g_par
+
+    def centroidal_vjp_device(self, q, qd, G_com, G_A, G_bias, g_q, g_qd, g_par=None, stream=None):
+        """Device version of centroidal_vjp_host: q float32 [n_q, n_stride], qd [n_qd, n_stride] (or None), G_com [10, n_stride], G_A
+        [6 n_qd, n_stride], G_bias [6, n_stride] (each may be None, not all), g_q [n_q, n_stride], g_qd [n_qd, n_stride], g_par [k, n_stride]
+        float64 CUDA tensors (each may be None, not all).  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_centroidal_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(G_com), _ptr(G_A), _ptr(G_bias), _ptr(g_q),
+                                                           _ptr(g_qd), _ptr(g_par), st), "centroidal_vjp_device")
 
     # ---- the step with its contact records (DESIGN.md section 7.15) ----
     def contact_rows(self, mode=MODE_FULL, use_pd=False):
