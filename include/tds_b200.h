@@ -326,6 +326,52 @@ int tds_b200_centroidal_vjp_device(tds_b200_sim* sim, const float* q, const floa
 int tds_b200_centroidal_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* G_com, const double* G_A,
                                  const double* G_bias, double* g_q, double* g_qd, double* g_par);
 
+/* ---- spatial point Jacobians, point velocities and accelerations J qdd + J' qd (DESIGN.md section 7.17; kinematics.hpp:18-148) ------
+ * At the fp32-rounded q, qd and qdd (qd or qdd may be NULL, meaning zero), for the point table of tds_b200_kinematics_* (K points,
+ * 0 <= K <= TDS_B200_MAX_KIN_POINTS, point k on links[k] (-1: the base) at local[3k .. 3k+2] in that link's frame, host memory), fp64
+ * outputs in world axes, each may be NULL but not all three:
+ *   J [6 n_qd] per point: the spatial point Jacobian, rows [w; x'] with [w; x'] = J qd, entry (point k, row r, column c) at row
+ *     (6k + r) * n_qd + c.  A joint column is [S.top; S.bot + S.top x (x - O)] for the joint's world motion subspace S at the world
+ *     origin O, so the linear rows equal tds_b200_kinematics' J on the joint columns.  Fixed links have no columns, a spherical joint has
+ *     3; in a world of several multibodies a point has entries in its own multibody's dofs only.
+ *     FLOATING BASE - unlike tds_b200_kinematics: the columns are the coordinates of tds_b200_mass_matrix, inverse_dynamics and
+ *     centroidal, where qd[0:6] is the base-frame twist [w_b; v_b] and qdd[0:6] its time derivative.  The base columns are [R_b | 0] in
+ *     the angular rows and [-[x - p_b]x R_b | R_b] in the linear rows (p_b the base position), i.e. tds_b200_kinematics' base columns
+ *     times diag(R_b, R_b), whose reference convention ignores the base rotation.  With these columns J composes with M, h and A.
+ *   vel [6] per point: [w; x'], the angular velocity of the point's link and the velocity of the point's world position x.
+ *   acc [6] per point: [w'; x''], the time derivatives of w and of x (classical, not spatial, acceleration): acc = J qdd + J' qd, and
+ *     with qdd = NULL the drift J' qd.
+ * Gravity does not enter; installed physical parameters do not enter (outputs are bit-identical with or without a set).  Argument
+ * checks -> -1: NULL q; K out of range, a link index out of [-1, n_links), or NULL links / local with K > 0; no output or no cotangent;
+ * m < 1 or every tangent NULL; no cotangent output.
+ *   device: q [n_q][n_stride], qd and qdd [n_qd][n_stride] fp32 as tds_b200_step_device; J [6K * n_qd][n_stride], vel [6K][n_stride],
+ *           acc [6K][n_stride] fp64.  Asynchronous on `stream`.
+ *   host:   q [n][n_q], qd and qdd [n][n_qd] fp64 (rounded to fp32); J [n][K][6][n_qd], vel [n][K][6], acc [n][K][6].  Synchronous.
+ * _jvp: the outputs' derivatives along m tangents of q, qd and qdd (each may be NULL: zero, not all), one lane per (environment,
+ *   tangent) of the dual-number instance, in chunks as tds_b200_step_jvp_*; NULL outputs are skipped.  Device t_q [n_q * m][n_stride],
+ *   t_qd and t_qdd [n_qd * m][n_stride], t_J [6K * n_qd * m][n_stride], t_vel and t_acc [6K * m][n_stride] (entry (r, j) at
+ *   (r * m + j) * n_stride + e); host t_q [n][n_q][m], t_qd and t_qdd [n][n_qd][m], t_J [n][6K * n_qd][m], t_vel and t_acc [n][6K][m].
+ * _vjp: g_x[c] = <G, d(J | vel | acc)/dx_c> for x = q, qd, qdd, for cotangents G_J, G_vel, G_acc in the outputs' layouts (NULL: zero,
+ *   not all): the JVP along the n_q + 2 n_qd identity tangents contracted with G on the device.  Any of g_q, g_qd, g_qdd may be NULL,
+ *   not all.  Device g_q [n_q][n_stride], g_qd and g_qdd [n_qd][n_stride] fp64 (asynchronous); host g_q [n][n_q], g_qd and g_qdd
+ *   [n][n_qd] (synchronous). */
+int tds_b200_point_motion_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, int K, const int* links,
+                                 const double* local, double* J, double* vel, double* acc, void* stream);
+int tds_b200_point_motion_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, int K, const int* links,
+                               const double* local, double* J, double* vel, double* acc);
+int tds_b200_point_motion_jvp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, int K, const int* links,
+                                     const double* local, int m, const double* t_q, const double* t_qd, const double* t_qdd, double* t_J,
+                                     double* t_vel, double* t_acc, void* stream);
+int tds_b200_point_motion_jvp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, int K, const int* links,
+                                   const double* local, int m, const double* t_q, const double* t_qd, const double* t_qdd, double* t_J,
+                                   double* t_vel, double* t_acc);
+int tds_b200_point_motion_vjp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, int K, const int* links,
+                                     const double* local, const double* G_J, const double* G_vel, const double* G_acc, double* g_q,
+                                     double* g_qd, double* g_qdd, void* stream);
+int tds_b200_point_motion_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, int K, const int* links,
+                                   const double* local, const double* G_J, const double* G_vel, const double* G_acc, double* g_q,
+                                   double* g_qd, double* g_qdd);
+
 /* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
  * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
  * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,

@@ -158,6 +158,18 @@ def lib():
     L.tds_b200_centroidal_vjp_device.argtypes = [vp, fp, fp, vp, vp, vp, vp, vp, vp, vp]
     L.tds_b200_centroidal_vjp_host.restype = ci
     L.tds_b200_centroidal_vjp_host.argtypes = [vp, dp, dp, dp, dp, dp, dp, dp, dp]
+    L.tds_b200_point_motion_device.restype = ci
+    L.tds_b200_point_motion_device.argtypes = [vp, fp, fp, fp, ci, vp, dp, vp, vp, vp, vp]
+    L.tds_b200_point_motion_host.restype = ci
+    L.tds_b200_point_motion_host.argtypes = [vp, dp, dp, dp, ci, vp, dp, dp, dp, dp]
+    L.tds_b200_point_motion_jvp_device.restype = ci
+    L.tds_b200_point_motion_jvp_device.argtypes = [vp, fp, fp, fp, ci, vp, dp, ci, vp, vp, vp, vp, vp, vp, vp]
+    L.tds_b200_point_motion_jvp_host.restype = ci
+    L.tds_b200_point_motion_jvp_host.argtypes = [vp, dp, dp, dp, ci, vp, dp, ci, dp, dp, dp, dp, dp, dp]
+    L.tds_b200_point_motion_vjp_device.restype = ci
+    L.tds_b200_point_motion_vjp_device.argtypes = [vp, fp, fp, fp, ci, vp, dp, vp, vp, vp, vp, vp, vp, vp]
+    L.tds_b200_point_motion_vjp_host.restype = ci
+    L.tds_b200_point_motion_vjp_host.argtypes = [vp, dp, dp, dp, ci, vp, dp, dp, dp, dp, dp, dp, dp]
     L.tds_b200_step_contacts_device.restype = ci
     L.tds_b200_step_contacts_device.argtypes = [vp, ci, ci, fp, fp, fp, fp, fp, fp, vp]
     L.tds_b200_step_contacts_host.restype = ci
@@ -274,6 +286,8 @@ DECLARED_SYMBOLS = [
     "tds_b200_inverse_dynamics_jvp_host", "tds_b200_inverse_dynamics_vjp_device", "tds_b200_inverse_dynamics_vjp_host",
     "tds_b200_centroidal_device", "tds_b200_centroidal_host", "tds_b200_centroidal_jvp_device", "tds_b200_centroidal_jvp_host",
     "tds_b200_centroidal_vjp_device", "tds_b200_centroidal_vjp_host",
+    "tds_b200_point_motion_device", "tds_b200_point_motion_host", "tds_b200_point_motion_jvp_device", "tds_b200_point_motion_jvp_host",
+    "tds_b200_point_motion_vjp_device", "tds_b200_point_motion_vjp_host",
     "tds_b200_step_contacts_device", "tds_b200_step_contacts_host", "tds_b200_step_contacts_jvp_device", "tds_b200_step_contacts_jvp_host",
     "tds_b200_step_contacts_vjp_device", "tds_b200_step_contacts_vjp_host",
     "tds_b200_integrate_euler_device", "tds_b200_integrate_euler_qdd_device", "tds_b200_contact_pairs", "tds_b200_model_contact_pairs", "tds_b200_contact_tuples", "tds_b200_model_contact_tuples", "tds_b200_contact_list_device", "tds_b200_contact_list_host", "tds_b200_contact_list_candidates_host",

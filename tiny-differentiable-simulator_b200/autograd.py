@@ -44,6 +44,10 @@ float64 params.grad) and a forward-mode rule (BatchSim.centroidal_jvp_device).
 forward_kinematics(sim, q, links, local) is every link's world transform and every point's world position and linear Jacobian (float64,
 DESIGN.md section 7.13) with a backward rule (BatchSim.kinematics_vjp_device: float32 q.grad) and a forward-mode rule
 (BatchSim.kinematics_jvp_device).
+
+point_motion(sim, q, qd, links, local, qdd=None) is every point's spatial Jacobian, velocity and acceleration J qdd + J' qd (float64,
+DESIGN.md section 7.17) with a backward rule (BatchSim.point_motion_vjp_device: float32 q.grad, qd.grad, qdd.grad) and a forward-mode
+rule (BatchSim.point_motion_jvp_device).
 """
 import torch
 
@@ -612,6 +616,97 @@ def forward_kinematics(sim, q, links, local):
     if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
         raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
     return _ForwardKinematics.apply(sim, q, links, local)
+
+
+def _mot_outputs(sim, K, J, vel, acc):
+    """Device outputs [rows, n_stride] of the point-motion entries -> (J [n, K, 6, n_qd], vel [n, K, 6], acc [n, K, 6])."""
+    n, nd = sim.n_envs, sim.n_qd
+    return (J[:6 * K * nd, :n].t().reshape(n, K, 6, nd).contiguous(), vel[:6 * K, :n].t().reshape(n, K, 6).contiguous(),
+            acc[:6 * K, :n].t().reshape(n, K, 6).contiguous())
+
+
+def _mot_buffers(sim, K, device):
+    z = lambda rows: torch.zeros((max(rows, 1), sim.n_stride), dtype=torch.float64, device=device)
+    return z(6 * K * sim.n_qd), z(6 * K), z(6 * K)
+
+
+class _PointMotion(torch.autograd.Function):
+    @staticmethod
+    def forward(sim, q, qd, qdd, links, local):
+        lk, lc, K = sim._points(links, local)
+        ns = sim.n_stride
+        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
+        J, vel, acc = _mot_buffers(sim, K, q.device)
+        _on_side_stream(q.device, lambda st: sim.point_motion_device(qs, qds, qdds, lk, lc, J, vel, acc, stream=st), (qs, qds, qdds, J, vel, acc))
+        return _mot_outputs(sim, K, J, vel, acc)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        sim, q, qd, qdd, links, local = inputs
+        ns = sim.n_stride
+        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
+        ctx.sim, ctx.points, ctx.has = sim, sim._points(links, local), (qd is not None, qdd is not None)
+        ctx.save_for_backward(qs, *(t if t is not None else qs for t in (qds, qdds)))
+        ctx.jvp_inputs = (qs, qds, qdds)
+
+    @staticmethod
+    def backward(ctx, gJ, gvel, gacc):
+        sim = ctx.sim
+        has_qd, has_qdd = ctx.has
+        qs, qds, qdds = ctx.saved_tensors
+        qds, qdds = (qds if has_qd else None), (qdds if has_qdd else None)
+        lk, lc, K = ctx.points
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        dev = qs.device
+
+        def cot(g, rows):
+            return _soa(torch.zeros((n, rows), dtype=torch.float64, device=dev) if g is None else g.reshape(n, rows), ns, torch.float64)
+        G_J, G_vel, G_acc = cot(gJ, 6 * K * nd), cot(gvel, 6 * K), cot(gacc, 6 * K)
+        z = lambda rows: torch.zeros((max(rows, 1), ns), dtype=torch.float64, device=dev)
+        g_q, g_qd, g_qdd = z(sim.n_q), (z(nd) if has_qd else None), (z(nd) if has_qdd else None)
+        _on_side_stream(dev, lambda st: sim.point_motion_vjp_device(qs, qds, qdds, lk, lc, G_J, G_vel, G_acc, g_q, g_qd, g_qdd, stream=st),
+                        (qs, qds, qdds, G_J, G_vel, G_acc, g_q, g_qd, g_qdd))
+        out = lambda t, rows: None if t is None else t[:rows, :n].t().to(torch.float32).contiguous()
+        return None, out(g_q, sim.n_q), out(g_qd, nd), out(g_qdd, nd), None, None
+
+    @staticmethod
+    def jvp(ctx, _sim, t_q, t_qd, t_qdd, _links, _local):
+        with torch._C._DisableFuncTorch():
+            return _PointMotion._jvp(ctx, _plain(t_q), _plain(t_qd), _plain(t_qdd))
+
+    @staticmethod
+    def _jvp(ctx, t_q, t_qd, t_qdd):
+        sim = ctx.sim
+        has_qd, has_qdd = ctx.has
+        qs, qds, qdds = (_plain(t) for t in ctx.jvp_inputs)
+        lk, lc, K = ctx.points
+        ns = sim.n_stride
+        tq = _soa_opt(t_q, ns, torch.float64)
+        tqd = _soa_opt(t_qd if has_qd else None, ns, torch.float64)
+        tqdd = _soa_opt(t_qdd if has_qdd else None, ns, torch.float64)
+        t_J, t_vel, t_acc = _mot_buffers(sim, K, qs.device)
+        if any(t is not None for t in (tq, tqd, tqdd)):
+            _on_side_stream(qs.device, lambda st: sim.point_motion_jvp_device(qs, qds, qdds, lk, lc, 1, tq, tqd, tqdd, t_J, t_vel, t_acc,
+                                                                              stream=st), (qs, qds, qdds, tq, tqd, tqdd, t_J, t_vel, t_acc))
+        return _mot_outputs(sim, K, t_J, t_vel, t_acc)
+
+
+def point_motion(sim, q, qd, links, local, qdd=None):
+    """Spatial point Jacobians, point velocities and accelerations of every environment of `sim` (a BatchSim), DESIGN.md section 7.17,
+    in fp64 at the fp32-rounded inputs, for the point table links [K] (-1: the base) / local [K, 3] (coordinates in the link's frame; both
+    constants of the call): (J [n_envs, K, 6, n_qd], vel [n_envs, K, 6], acc [n_envs, K, 6]) float64, world axes, rows [w; x'] (the
+    angular velocity of the point's link and the velocity of the point's world position), vel = J qd and acc = [w'; x''] = J qdd + J' qd
+    (the drift J' qd when qdd is None).  Columns in the coordinates of mass_matrix and inverse_dynamics: a floating base's qd[0:6] is the
+    base-frame twist, so J composes with M, h and A (its base columns differ from forward_kinematics' J, which ignores the base
+    rotation).  q [n_envs, n_q], qd and qdd [n_envs, n_qd] float32 CUDA tensors (qd or qdd None: zero).  Gravity and installed physical
+    parameters do not enter.  Differentiable along q, qd and qdd in reverse mode (float32 gradients from the cotangents of all three
+    outputs) and forward mode."""
+    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
+        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
+    for name, t in (("qd", qd), ("qdd", qdd)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or tuple(t.shape) != (sim.n_envs, sim.n_qd)):
+            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, n_qd] is expected")
+    return _PointMotion.apply(sim, q, qd, qdd, links, local)
 
 
 class _StepContacts(torch.autograd.Function):

@@ -77,6 +77,10 @@ extern "C" int tds_launch_centroidal(const DevModel* M, const StepIO* io, const 
                                      cudaStream_t stream);
 extern "C" int tds_launch_centroidal_jvp(const DevModel* M, const StepIO* io, const ParMap* pm, const TdsCenCall* out, const double* t_in,
                                          const double* t_par, int m, int n_dirs, char* gscratch, cudaStream_t stream);
+// spatial point Jacobians, point velocities and accelerations, and their Jacobian-vector products (tds_point_motion.cu)
+extern "C" int tds_launch_point_motion(const DevModel* M, const StepIO* io, const TdsMotCall* mc, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_point_motion_jvp(const DevModel* M, const StepIO* io, const TdsMotCall* mc, const double* t_in, int m, int n_dirs,
+                                           char* gscratch, cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
@@ -895,17 +899,18 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
   return 0;
 }
 
-// what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14 and 7.16, or
-// the step with its contact records (section 7.15)
-enum class Query { step, mass, kin, inv, contacts, centroidal };
+// what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14, 7.16 and 7.17,
+// or the step with its contact records (section 7.15)
+enum class Query { step, mass, kin, inv, contacts, centroidal, motion };
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
 // inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
 // (t_in = the q tangents, t_par unused); inv: t_in = the q | qd | qdd tangents (qd and qdd in the step's qd and tau_or_action);
-// contacts: as step, with the rows q' | qd' | records; centroidal: t_in = the q | qd tangents (qd in the step's qd), outputs `cen`
+// contacts: as step, with the rows q' | qd' | records; centroidal: t_in = the q | qd tangents (qd in the step's qd), outputs `cen`;
+// motion: t_in = the q | qd | qdd tangents (qd and qdd as for inv), the point table and outputs `mot`
 struct JvpTangents {
   const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr;
-  const TdsCenCall* cen = nullptr;
+  const TdsCenCall* cen = nullptr; const TdsMotCall* mot = nullptr;
 };
 
 // the installed physical parameters as a launch argument in *pmv, or NULL without any
@@ -971,6 +976,7 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
         case Query::centroidal:
           rc = tds_launch_centroidal_jvp(&s->dm_ad, &io, pm, jv->cen, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm);
           break;
+        case Query::motion: rc = tds_launch_point_motion_jvp(&s->dm_ad, &io, jv->mot, jv->t_in, jv->m, nd, s->jac_scratch, sm); break;
       }
     }
     if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
@@ -1633,6 +1639,156 @@ int tds_b200_centroidal_vjp_host(tds_b200_sim* s, const double* q, const double*
   CUDA_TRY(put_parts<double>(s->vjp_g, {{G_com, R.com}, {G_A, R.A}, {G_bias, R.bias}}, n, ns, s->stream));
   if (int rc = cen_vjp_run(s, s->q, qd_d, s->vjp_g, g_d, g_par ? g_d + (size_t)n_in * ns : nullptr, s->stream)) return rc;
   CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_par, k}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- spatial point Jacobians, point velocities and accelerations (DESIGN.md section 7.17): the MOT instances of the world-frame kernel
+// (tds_point_motion.cu).  The point table is checked as for the kinematics (kin_check); the inputs q | qd | qdd are those of inverse
+// dynamics (inv_n_in, put_inv_inputs). -----------------------------------------------------------------------------------------------------
+// rows of the outputs J | vel | acc
+struct MotRows { size_t J, vel, acc; size_t all() const { return J + vel + acc; } };
+static MotRows mot_rows(const tds_b200_sim* s, int K) { return MotRows{(size_t)6 * K * s->dm[0].n_qd, (size_t)6 * K, (size_t)6 * K}; }
+
+// fp64 outputs from q [n_q][ns], qd and qdd [n_qd][ns] fp32 (either NULL: zero; installed parameters do not enter)
+static int mot_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const TdsMotCall* mc, cudaStream_t sm) {
+  return value_run(s, "point motion", q, qd, qdd, nullptr, [&](const StepIO* io, const ParMap*) {
+    return tds_launch_point_motion(&s->dm_m, io, mc, s->jac_scratch, sm);
+  });
+}
+
+// m tangents t_in [(n_q + 2 n_qd) * m][ns] (q | qd | qdd, contiguous) -> the outputs' columns [rows * m][ns], through the Jacobian's chunk
+// loop
+static int mot_jvp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const TdsMotCall* mc, int m, const double* t_in,
+                       cudaStream_t sm) {
+  JvpTangents jv{t_in, nullptr, m, Query::motion};
+  jv.mot = mc;
+  return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, qdd, nullptr, sm, false, &jv);
+}
+
+// g_in [n_q + 2 n_qd][ns] (q | qd | qdd, contiguous) = <G, d(J | vel | acc)>, G [rows][ns] concatenated
+static int mot_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int K, const int* links, const double* local,
+                       const double* G, double* g_in, cudaStream_t sm) {
+  const MotRows R = mot_rows(s, K);
+  const size_t ns = s->ns;
+  return vjp_by_eye(s, "point motion", inv_n_in(s), R.all(), G, g_in, nullptr, sm, [&](int nd, const double* t_in, const double*, double* dO) {
+    const TdsMotCall mc{K, links, local, dO, dO + R.J * nd * ns, dO + (R.J + R.vel) * nd * ns};
+    return mot_jvp_run(s, q, qd, qdd, &mc, nd, t_in, sm);
+  });
+}
+
+static int mot_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local, const void* J, const void* vel,
+                     const void* acc) {
+  if (int rc = kin_check(s, q, K, links, local)) return rc;
+  if (!J && !vel && !acc) return -1;
+  return 0;
+}
+
+int tds_b200_point_motion_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int K, const int* links,
+                                 const double* local, double* J, double* vel, double* acc, void* stream) {
+  if (int rc = mot_check(s, q, K, links, local, J, vel, acc)) return rc;
+  const TdsMotCall mc{K, links, local, J, vel, acc};
+  return mot_run(s, q, qd, qdd, &mc, (cudaStream_t)stream);
+}
+
+int tds_b200_point_motion_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, int K, const int* links,
+                               const double* local, double* J, double* vel, double* acc) {
+  if (int rc = mot_check(s, q, K, links, local, J, vel, acc)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const MotRows R = mot_rows(s, K);
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (R.all() + 1) * ns));
+  double* d = s->jac_dev;
+  const TdsMotCall mc{K, links, local, J ? d : nullptr, vel ? d + R.J * ns : nullptr, acc ? d + (R.J + R.vel) * ns : nullptr};
+  if (int rc = mot_run(s, s->q, qd_d, qdd_d, &mc, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{J, R.J}, {vel, R.vel}, {acc, R.acc}}, d, n, ns, s->stream));
+  return 0;
+}
+
+static int mot_jvp_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local, int m, const void* t_q,
+                         const void* t_qd, const void* t_qdd, const void* t_J, const void* t_vel, const void* t_acc) {
+  if (int rc = mot_check(s, q, K, links, local, t_J, t_vel, t_acc)) return rc;
+  if (m < 1 || (!t_q && !t_qd && !t_qdd)) return -1;
+  return 0;
+}
+
+int tds_b200_point_motion_jvp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int K, const int* links,
+                                     const double* local, int m, const double* t_q, const double* t_qd, const double* t_qdd, double* t_J,
+                                     double* t_vel, double* t_acc, void* stream) {
+  if (int rc = mot_jvp_check(s, q, K, links, local, m, t_q, t_qd, t_qdd, t_J, t_vel, t_acc)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the kernel reads the q | qd | qdd tangents as one array
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (size_t)inv_n_in(s) * m * s->ns));
+  double* tin = s->jac_dev;
+  CUDA_TRY(put_parts_d2d<double>(tin, {{t_q, n_q * m}, {t_qd, nd * m}, {t_qdd, nd * m}}, s->ns, sm));
+  const TdsMotCall mc{K, links, local, t_J, t_vel, t_acc};
+  return mot_jvp_run(s, q, qd, qdd, &mc, m, tin, sm);
+}
+
+int tds_b200_point_motion_jvp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, int K, const int* links,
+                                   const double* local, int m, const double* t_q, const double* t_qd, const double* t_qdd, double* t_J,
+                                   double* t_vel, double* t_acc) {
+  if (int rc = mot_jvp_check(s, q, K, links, local, m, t_q, t_qd, t_qdd, t_J, t_vel, t_acc)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  const MotRows R = mot_rows(s, K);
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; q | qd | qdd (contiguous, zero where NULL), then the outputs
+  const size_t ti = (size_t)inv_n_in(s) * m;
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + R.all() * m + 1) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + ti * ns;
+  CUDA_TRY(put_parts<double>(d, {{t_q, n_q * m}, {t_qd, nd * m}, {t_qdd, nd * m}}, n, ns, s->stream));
+  const TdsMotCall mc{K, links, local, t_J ? to_d : nullptr, t_vel ? to_d + R.J * m * ns : nullptr,
+                      t_acc ? to_d + (R.J + R.vel) * m * ns : nullptr};
+  if (int rc = mot_jvp_run(s, s->q, qd_d, qdd_d, &mc, m, d, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{t_J, R.J * m}, {t_vel, R.vel * m}, {t_acc, R.acc * m}}, to_d, n, ns, s->stream));
+  return 0;
+}
+
+static int mot_vjp_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local, const void* G_J, const void* G_vel,
+                         const void* G_acc, const void* g_q, const void* g_qd, const void* g_qdd) {
+  if (int rc = mot_check(s, q, K, links, local, G_J, G_vel, G_acc)) return rc;
+  if (!g_q && !g_qd && !g_qdd) return -1;
+  return 0;
+}
+
+int tds_b200_point_motion_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int K, const int* links,
+                                     const double* local, const double* G_J, const double* G_vel, const double* G_acc, double* g_q,
+                                     double* g_qd, double* g_qdd, void* stream) {
+  if (int rc = mot_vjp_check(s, q, K, links, local, G_J, G_vel, G_acc, g_q, g_qd, g_qdd)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  const MotRows R = mot_rows(s, K);
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the concatenated cotangent J | vel | acc (zero where a part is NULL), then g_q | g_qd | g_qdd as one array for the contraction
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (R.all() + inv_n_in(s)) * s->ns));
+  double* g_d = s->vjp_g + R.all() * s->ns;
+  CUDA_TRY(put_parts_d2d<double>(s->vjp_g, {{G_J, R.J}, {G_vel, R.vel}, {G_acc, R.acc}}, s->ns, sm));
+  if (int rc = mot_vjp_run(s, q, qd, qdd, K, links, local, s->vjp_g, g_d, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}}, g_d, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_point_motion_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, int K, const int* links,
+                                   const double* local, const double* G_J, const double* G_vel, const double* G_acc, double* g_q,
+                                   double* g_qd, double* g_qdd) {
+  if (int rc = mot_vjp_check(s, q, K, links, local, G_J, G_vel, G_acc, g_q, g_qd, g_qdd)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  const MotRows R = mot_rows(s, K);
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  // G (J | vel | acc, zero where a part is NULL) | g_q | g_qd | g_qdd
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (R.all() + inv_n_in(s)) * ns));
+  double* g_d = s->vjp_g + R.all() * ns;
+  CUDA_TRY(put_parts<double>(s->vjp_g, {{G_J, R.J}, {G_vel, R.vel}, {G_acc, R.acc}}, n, ns, s->stream));
+  if (int rc = mot_vjp_run(s, s->q, qd_d, qdd_d, K, links, local, s->vjp_g, g_d, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}}, g_d, n, ns, s->stream));
   return 0;
 }
 

@@ -55,7 +55,10 @@ struct CfArg { float* cf; };
 struct CfArgPar : ParMap { float* cf; };
 // kernel argument of the centroidal instances (CEN, DESIGN.md section 7.16): the argument of the same instance without CEN and the outputs
 template <typename B> struct CenArg : B { double* com; double* A; double* bias; };
-template <bool PAR, bool JV = false, bool KIN = false, bool CF = false, bool CEN = false> struct ParArg { typedef NoPar type; };
+// kernel argument of the point-motion instances (MOT, DESIGN.md section 7.17): the point table of KinArg (B = KinArg or KinArgJvp), whose
+// J is the 6-row spatial point Jacobian here (xf and x are not read), and the outputs vel and acc
+template <typename B> struct MotArg : B { double* vel; double* acc; };
+template <bool PAR, bool JV = false, bool KIN = false, bool CF = false, bool CEN = false, bool MOT = false> struct ParArg { typedef NoPar type; };
 template <> struct ParArg<true, false> { typedef ParMap type; };
 template <> struct ParArg<false, true> { typedef NoParJvp type; };
 template <> struct ParArg<true, true> { typedef ParMapJvp type; };
@@ -66,6 +69,8 @@ template <> struct ParArg<true, false, false, true> { typedef CfArgPar type; };
 template <> struct ParArg<false, true, false, true> { typedef NoParJvp type; };
 template <> struct ParArg<true, true, false, true> { typedef ParMapJvp type; };
 template <bool PAR, bool JV> struct ParArg<PAR, JV, false, false, true> { typedef CenArg<typename ParArg<PAR, JV>::type> type; };
+template <> struct ParArg<false, false, false, false, false, true> { typedef MotArg<KinArg> type; };
+template <> struct ParArg<false, true, false, false, false, true> { typedef MotArg<KinArgJvp> type; };
 
 // CF, dual instances: the part of a record's dual number they write - the tangent (d).  The host build of the tests also compiles them
 // with the value (v), for an fp64 value path of the records that central differences can resolve.
@@ -126,12 +131,19 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // everything shifts to the centroid c: k_G = k_O - (c - O) x l.  Outputs pm.com [10], pm.A [6 n_qd] and pm.bias [6] (each may be null),
 // row r at out[r * ns + e] (fp64 instances) or its dual part at out[(r * m + j) * ns + e] (JV instances).  ABA and integration are not
 // compiled in.
+// MOT: point velocities, accelerations and spatial point Jacobians (DESIGN.md section 7.17), launched in MODE_NOCONTACT with the point
+// table as pm, qd in io.qd_in and qdd in io.tau_in (either null: zero; tangent input indices n_q + k and n_q + n_qd + k).  Pass 1 carries
+// a_i = a_parent + S_i qdd_i + v_i x (S_i qd_i) as INV does but without gravity (a_base = 0, or the floating base's R_b qdd[0:6]); as it
+// reaches link l it writes, for every point on l at x (relative to O), [w; x'] = [v.top; v.bot + w x x], [w'; x''] = [a.top; a.bot +
+// a.top x x + w x x'] and the 6 x n_qd Jacobian (rows [w; x'], joint column [S.top; S.bot + S.top x x], floating-base columns [R_b | 0;
+// -[x]x R_b | R_b] in the base-twist coordinates of qd[0:6]).  Outputs pm.J [6K n_qd], pm.vel [6K], pm.acc [6K] (each may be null), row r
+// at out[r * ns + e] (fp64 instance) or its dual part at out[(r * m + j) * ns + e] (JV instance).  Returns before pass 2.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
-          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false>
+          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
-                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF, CEN>::type pm = {}) {
+                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF, CEN, MOT>::type pm = {}) {
   extern __shared__ __align__(16) char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp_in_blk = threadIdx.x >> 5;
@@ -250,7 +262,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // input directions of the differentiable instance: q | qd | tau or action | kp, kd, max_force (with PD)
   const int in0 = M.n_q + n;
   for (int k = 0; k < M.n_q; ++k) qv[k * ST] = seed(RQ(io.q_in[(size_t)k * ns + e]), k);
-  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(((INV || CEN) && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
+  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(((INV || CEN || MOT) && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
   for (int k = 0; k < n; ++k) tauv[k * ST] = RQ(0.f);
   if (!MASS && use_pd) {
     const RQ kp = seed(RQ(E.kp), in0 + E.n_act), kd = seed(RQ(E.kd), in0 + E.n_act + 1), fmax_ = seed(RQ(E.max_force), in0 + E.n_act + 2);
@@ -263,11 +275,11 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       f = min_t(max_t(f, -fmax_), fmax_);
       tauv[M.qd_idx[li] * ST] = f;
     }
-  } else if (!MASS && !INV && io.tau_in) {
+  } else if (!MASS && !INV && !MOT && io.tau_in) {
     const int off = M.floating ? 6 : 0;
     for (int k = off; k < n; ++k) tauv[k * ST] = seed(RQ(io.tau_in[(size_t)(k - off) * ns + e]), in0 + k - off);
   }
-  if constexpr (!KIN && !INV) {   // (the KIN and INV lanes return before pass 2 reads the accumulators)
+  if constexpr (!KIN && !INV && !MOT) {   // (the KIN, INV and MOT lanes return before pass 2 reads the accumulators)
     for (int s = 0; s < M.n_acc; ++s) {
       RA* pa = A.ptr<RA>(M.x_acc + s * M.x_acc_words);
       for (int k = 0; k < 27; ++k) pa[k * ST] = RA(0);
@@ -419,6 +431,46 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       }
     }
   };
+  // MOT: the outputs of the points on link l (-1: the base) at its world rotation R, position p (relative to O), spatial velocity v and
+  // acceleration a (common frame).  The Jacobian reads the stored S of l and its ancestors, as kin_link does.
+  auto mot_link = [&](int l, const M3<RC>& R, const V3<RC>& p, const Sv<RC>& v, const Sv<RC>& a) {
+    if constexpr (MOT) {
+      if (!live) return;
+      auto put = [&](double* o, size_t r, const RC& x) {
+        if constexpr (AD) o[(r * io.jac_n_in + jcol) * ns + e] = x.d;
+        else o[r * ns + e] = x;
+      };
+      auto put6 = [&](double* o, size_t r0, size_t stride, const V3<RC>& top, const V3<RC>& bot) {
+        put(o, r0, top.x); put(o, r0 + stride, top.y); put(o, r0 + 2 * stride, top.z);
+        put(o, r0 + 3 * stride, bot.x); put(o, r0 + 4 * stride, bot.y); put(o, r0 + 5 * stride, bot.z);
+      };
+      for (int k = 0; k < pm.K; ++k) {
+        if (pm.link[k] != l) continue;
+        const V3<RC> xr = p + mul(R, v3<RC>(RC(pm.local[3 * k]), RC(pm.local[3 * k + 1]), RC(pm.local[3 * k + 2])));
+        const V3<RC> xd = v.bot + cross(v.top, xr);
+        if (pm.vel) put6(pm.vel, 6 * k, 1, v.top, xd);
+        if (pm.acc) put6(pm.acc, 6 * k, 1, a.top, a.bot + cross(a.top, xr) + cross(v.top, xd));
+        if (!pm.J) continue;
+        // rows 6k .. 6k + 5 of n_qd columns: zero outside the point's chain (and outside its multibody)
+        const size_t r0 = (size_t)6 * k * n;
+        const V3<RC> z = v3<RC>(RC(0), RC(0), RC(0));
+        for (int c = 0; c < n; ++c) put6(pm.J, r0 + c, n, z, z);
+        if (M.floating) {   // the base twist's unit columns [R_b e_c; 0] and [0; R_b e_c], moved to the point
+          for (int c = 0; c < 3; ++c) {
+            const V3<RC> u = c == 0 ? col_x(Rb) : (c == 1 ? col_y(Rb) : col_z(Rb));
+            put6(pm.J, r0 + c, n, u, cross(u, xr));
+            put6(pm.J, r0 + 3 + c, n, z, u);
+          }
+        }
+        for (int j = l; j >= 0; j = M.parent[j]) {   // column = S_j at the point (fixed links: none)
+          for (int cj = 0; cj < n_cols(j); ++cj) {
+            const Sv<RC> S = S_col(j, cj);
+            put6(pm.J, r0 + M.qd_idx[j] + cj, n, S.top, S.bot + cross(S.top, xr));
+          }
+        }
+      }
+    }
+  };
   M3<RC> R_prev = Rb;
   V3<RC> p_prev = M.floating ? v3<RC>(RC(0), RC(0), RC(0)) : v3<RC>(-O.x, -O.y, -O.z);
   Sv<RA> v_prev;
@@ -438,9 +490,19 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // INV: qdd of dof k (seeded at input n_q + n_qd + k); the acceleration of the previous link, of the base; the sum of the link forces
   auto qdd_in = [&](int k) -> RQ { return seed(RQ(io.tau_in ? io.tau_in[(size_t)k * ns + e] : 0.f), M.n_q + n + k); };
   // (empty placeholders in the other instances, whose code must not change)
-  typedef typename std::conditional<INV, Sv<RC>, NoPar>::type SvInv;
+  typedef typename std::conditional<INV || MOT, Sv<RC>, NoPar>::type SvInv;
   const SvInv a_base_inv = [&]() -> SvInv {
-    if constexpr (INV) {
+    if constexpr (MOT) {   // the base's acceleration without gravity: zero, or the base-frame qdd[0:6] in the common frame
+      static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the MOT instances run in one scalar type");
+      Sv<RC> a;
+      a.top = v3<RC>(RC(0), RC(0), RC(0));
+      a.bot = a.top;
+      if (M.floating) {
+        a.top = mul(Rb, v3<RC>(qdd_in(0), qdd_in(1), qdd_in(2)));
+        a.bot = mul(Rb, v3<RC>(qdd_in(3), qdd_in(4), qdd_in(5)));
+      }
+      return a;
+    } else if constexpr (INV) {
       static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the INV instances run in one scalar type");
       const V3<RC> g = v3<RC>(RC(P.gravity[0]), RC(P.gravity[1]), RC(P.gravity[2]));
       Sv<RC> a;
@@ -457,6 +519,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   }();
   SvInv a_prev_inv = a_base_inv, f_links = SvInv{};
   if constexpr (INV) { f_links.top = v3<RC>(RC(0), RC(0), RC(0)); f_links.bot = f_links.top; }
+  if constexpr (MOT) mot_link(-1, R_base, p_base, v_base, a_base_inv);
   // CEN: the rigid inertia of the counted bodies about O in world axes (the root composite) and the velocity-only rate of momentum about O
   typename std::conditional<CEN, Rbi<RC>, NoPar>::type cen_I{};
   typename std::conditional<CEN, Sv<RC>, NoPar>::type cen_f{};
@@ -531,7 +594,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     if (M.xw_slot[i] >= 0) { RC* px = A.ptr<RC>(M.x_xw + (M.xw_slot[i] + 1) * 12 * RCW); st9<RC>(px, ST, Ri); st3<RC>(px + 9 * ST, ST, pi); }
     // rigid-body inertia about O in world axes: com c = p_i + R_i com_l, I = R Icom R^T + m (|c|^2 1 - c c^T)
     typename std::conditional<INV, Rbi<RC>, NoPar>::type r_inv;   // (INV: kept for f_i below)
-    if constexpr (!KIN) {
+    if constexpr (!KIN && !MOT) {
       const double* rb = M.rbic[i];
       auto rbc = [&](int c) -> RP { return par_of(body_slot(i + 1, c), rb[c]); };
       Rbi<RC> r;
@@ -598,9 +661,26 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       st6<RC>(A.ptr<RC>(M.x_link + i * LWD), ST, a);
       a_prev_inv = a;
     }
+    if constexpr (MOT) {   // a_i as INV carries it (a branch point's over its rigid-inertia words), then the outputs of the points on i
+      Sv<RC> a;
+      if (fl & TDS_LF_PARENT_ADJ) a = a_prev_inv;
+      else if (p >= 0) a = ld6<RC>(A.ptr<RC>(M.x_link + p * LWD), ST);
+      else a = a_base_inv;
+      Sv<RC> vJ; vJ.top = v3<RC>(RC(0), RC(0), RC(0)); vJ.bot = vJ.top;
+      for (int c = 0; c < n_cols(i); ++c) {
+        const Sv<RC> Sc = (fl & TDS_LF_SPHERICAL) ? S_col(i, c) : S;
+        const RC qdc = qdv[(M.qd_idx[i] + c) * ST], qddc = qdd_in(M.qd_idx[i] + c);
+        vJ.top = axpy(Sc.top, qdc, vJ.top); vJ.bot = axpy(Sc.bot, qdc, vJ.bot);
+        a.top = axpy(Sc.top, qddc, a.top); a.bot = axpy(Sc.bot, qddc, a.bot);
+      }
+      a = a + cross_mm(v, vJ);
+      st6<RC>(A.ptr<RC>(M.x_link + i * LWD), ST, a);
+      a_prev_inv = a;
+      mot_link(i, Ri, pi, v, a);
+    }
     R_prev = Ri; p_prev = pi; v_prev = v;
   }
-  if constexpr (KIN) return;
+  if constexpr (KIN || MOT) return;
   if constexpr (INV) {
     for (int i = 0; i < n_links; ++i) {   // the stiffness and damping terms the ABA subtracts from tau
       const int fl = M.flags[i];

@@ -160,6 +160,15 @@ struct TdsKinCall {
 // centroidal momentum matrix A [6 * n_qd][ns] and its bias A' qd [6][ns] (each may be null; columns of an m-column block in the JVP)
 struct TdsCenCall { double* com; double* A; double* bias; };
 
+// One call of the point-motion instances (tds_point_motion.cu, DESIGN.md section 7.17): the point table as in TdsKinCall and the outputs
+// J [6K * n_qd][ns], vel [6K][ns], acc [6K][ns] (each may be null; columns of an m-column block in the JVP)
+struct TdsMotCall {
+  int K;
+  const int* link;       // [K], -1 = the base
+  const double* local;   // [3K]
+  double* J; double* vel; double* acc;
+};
+
 // Installed physical parameters (tds_b200_set_physical_params_*): the slot of each model quantity in the lane's value vector,
 // or -1 = the model's value, and the values themselves.  Passed only to the instances of the world-frame kernel that read them
 // (StepIO stays as it is: the other instances keep it on their stack).

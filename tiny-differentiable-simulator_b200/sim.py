@@ -659,6 +659,82 @@ class BatchSim:
         self._check(self._L.tds_b200_kinematics_vjp_device(self._h, _ptr(q), K, lp, cp, _ptr(G_xf), _ptr(G_x), _ptr(G_J), _ptr(g_q), st),
                     "kinematics_vjp_device")
 
+    # ---- spatial point Jacobians, point velocities and accelerations (DESIGN.md section 7.17) ----
+    def point_motion_host(self, q, qd, links, local, qdd=None):
+        """Spatial point Jacobians, velocities and accelerations at the fp32-rounded q [n, n_q], qd and qdd [n, n_qd] (None: zero) for the
+        point table of kinematics_host: (J [n, K, 6, n_qd], vel [n, K, 6], acc [n, K, 6]) float64, world axes, rows [w; x'] of the
+        point's link angular velocity and the velocity of its world position: vel = J qd, acc = [w'; x''] = J qdd + J' qd.  Columns in
+        the coordinates of mass_matrix_host: a floating base's are the base twist's, [R_b | 0; -[x - p_b]x R_b | R_b] - unlike
+        kinematics_host, whose base columns ignore the base rotation.  Gravity and installed physical parameters do not enter."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        keep, K, lp, cp = self._kin_args(links, local)
+        n = self.n_envs
+        J, vel, acc = np.zeros((n, K, 6, self.n_qd)), np.zeros((n, K, 6)), np.zeros((n, K, 6))
+        self._check(self._L.tds_b200_point_motion_host(self._h, _dp(q), _dp(qd), _dp(qdd), K, lp, cp, _dp(J), _dp(vel), _dp(acc)),
+                    "point_motion_host")
+        return J, vel, acc
+
+    def point_motion_device(self, q, qd, qdd, links, local, J=None, vel=None, acc=None, stream=None):
+        """Device version of point_motion_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd and qdd [n_qd, n_stride] (or
+        None); J [6K * n_qd, n_stride], vel and acc [6K, n_stride] float64 CUDA tensors (any may be None, not all three), entry (point k,
+        row r, column c) of J at row (6k + r) * n_qd + c.  The point table is host data.  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_point_motion_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), K, lp, cp, _ptr(J), _ptr(vel), _ptr(acc), st),
+                    "point_motion_device")
+
+    def point_motion_jvp_host(self, q, qd, links, local, qdd=None, t_q=None, t_qd=None, t_qdd=None):
+        """Directional derivatives (dJ [n, K, 6, n_qd, m], dvel [n, K, 6, m], dacc [n, K, 6, m]) of the outputs of point_motion_host along
+        m tangents t_q [n, n_q, m], t_qd and t_qdd [n, n_qd, m] (each may be None, not all); tangents given as [n, dim] are m = 1 and
+        drop the last axis."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        if all(t is None for t in (t_q, t_qd, t_qdd)):
+            raise ValueError("at least one tangent is expected")
+        ts, m, single = self._tangents([(t_q, self.n_q), (t_qd, self.n_qd), (t_qdd, self.n_qd)])
+        keep, K, lp, cp = self._kin_args(links, local)
+        n = self.n_envs
+        dJ, dvel, dacc = np.zeros((n, K, 6, self.n_qd, m)), np.zeros((n, K, 6, m)), np.zeros((n, K, 6, m))
+        self._check(self._L.tds_b200_point_motion_jvp_host(self._h, _dp(q), _dp(qd), _dp(qdd), K, lp, cp, m, *(_dp(t) for t in ts), _dp(dJ),
+                                                           _dp(dvel), _dp(dacc)), "point_motion_jvp_host")
+        return (dJ[..., 0], dvel[..., 0], dacc[..., 0]) if single else (dJ, dvel, dacc)
+
+    def point_motion_jvp_device(self, q, qd, qdd, links, local, m, t_q, t_qd, t_qdd, t_J=None, t_vel=None, t_acc=None, stream=None):
+        """Device version of point_motion_jvp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None); t_q [n_q * m,
+        n_stride], t_qd and t_qdd [n_qd * m, n_stride] (each may be None, not all), t_J [6K * n_qd * m, n_stride], t_vel and t_acc [6K * m,
+        n_stride] (any may be None, not all three) float64 CUDA tensors, entry (r, j) at row r * m + j.  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_point_motion_jvp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), K, lp, cp, int(m), _ptr(t_q), _ptr(t_qd),
+                                                             _ptr(t_qdd), _ptr(t_J), _ptr(t_vel), _ptr(t_acc), st), "point_motion_jvp_device")
+
+    def point_motion_vjp_host(self, q, qd, links, local, qdd=None, G_J=None, G_vel=None, G_acc=None):
+        """Cotangents G_J [n, K, 6, n_qd], G_vel and G_acc [n, K, 6] (None: zero, not all three) -> (g_q [n, n_q], g_qd [n, n_qd], g_qdd
+        [n, n_qd]) = sum G * d(outputs)/dx."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        keep, K, lp, cp = self._kin_args(links, local)
+        if G_J is None and G_vel is None and G_acc is None:
+            raise ValueError("at least one cotangent is expected")
+        n = self.n_envs
+        G_J = None if G_J is None else self._inv_in(np.reshape(G_J, (n, -1)), 6 * K * self.n_qd, "G_J")
+        G_vel = None if G_vel is None else self._inv_in(np.reshape(G_vel, (n, -1)), 6 * K, "G_vel")
+        G_acc = None if G_acc is None else self._inv_in(np.reshape(G_acc, (n, -1)), 6 * K, "G_acc")
+        g_q, g_qd, g_qdd = np.zeros((n, self.n_q)), np.zeros((n, self.n_qd)), np.zeros((n, self.n_qd))
+        self._check(self._L.tds_b200_point_motion_vjp_host(self._h, _dp(q), _dp(qd), _dp(qdd), K, lp, cp, _dp(G_J), _dp(G_vel), _dp(G_acc),
+                                                           _dp(g_q), _dp(g_qd), _dp(g_qdd)), "point_motion_vjp_host")
+        return g_q, g_qd, g_qdd
+
+    def point_motion_vjp_device(self, q, qd, qdd, links, local, G_J, G_vel, G_acc, g_q, g_qd, g_qdd, stream=None):
+        """Device version of point_motion_vjp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None), cotangents float64
+        in the layouts of point_motion_device (None: zero, not all three), g_q [n_q, n_stride], g_qd and g_qdd [n_qd, n_stride] float64
+        CUDA tensors (each may be None, not all).  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_point_motion_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), K, lp, cp, _ptr(G_J), _ptr(G_vel),
+                                                             _ptr(G_acc), _ptr(g_q), _ptr(g_qd), _ptr(g_qdd), st), "point_motion_vjp_device")
+
     def jacobian_chunk(self):
         """Directions (Jacobian columns or JVP tangents) one launch of the dual-number step takes; more run in several launches."""
         return self._L.tds_b200_jacobian_chunk(self._h)
