@@ -408,6 +408,48 @@ int tds_b200_step_contacts_vjp_device(tds_b200_sim* sim, int mode, int use_pd, c
 int tds_b200_step_contacts_vjp_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
                                     const double* g_out, double* g_in, double* g_par);
 
+/* ---- the step with external wrenches (DESIGN.md section 7.18) ----------------------------------------------------------------------
+ * One step (MODE_FD, MODE_NOCONTACT or MODE_FULL) with a wrench W_k = [n_k; f_k] in world axes at every point of a point table: the
+ * force f_k acts along a line through the point's world position x_k(q), n_k is a pure moment.  The table is that of the kinematics
+ * (0 <= K <= TDS_B200_MAX_KIN_POINTS, point k on links[k] (-1: the base) at local[3k .. 3k+2] in that link's frame, host memory); every
+ * environment has its own wrenches.  The generalised force of W_k is J_k^T W_k with J_k the 6-row point Jacobian of
+ * tds_b200_point_motion_* at the same q and point (w . n + x' . f is the power).  In the step the wrenches act as the reference's f_ext:
+ * each enters the articulated-body bias force of the body it acts on (pA = v x* I v - f_ext, kinematics.hpp:132; a point on a floating
+ * base enters the base's bias force), so it reaches qdd through the forward dynamics and q', qd' through the integration and, in
+ * MODE_FULL, the contact solve.  A wrench on a fixed base does nothing; in a world of several multibodies a wrench moves only its own
+ * multibody.  Gravity, stiffness, damping, PD and installed parameters act as in the step without wrenches, and K = 0 is that step.
+ * Inverse dynamics with wrenches is tds_b200_inverse_dynamics_* minus sum_k J_k^T W_k.
+ * The step always runs on the generic world-frame kernel at the simulator's precision, with the installed parameters if any.  In the
+ * mixed precision the wrenches enter the fp32 forward dynamics as tau does.
+ *   device: W [6K][n_stride] fp32 (row 6k + r: component r of [n; f] of point k), q_out, qd_out [dim][n_stride] (MODE_NOCONTACT,
+ *   MODE_FULL) or qdd_out [n_qd][n_stride] (MODE_FD), the others may be NULL; asynchronous.
+ *   host: W [n][K][6] fp64 (rounded to fp32), outputs [n][dim] fp64.
+ * _jvp: as tds_b200_step_jvp_*, rows q' | qd' (qdd in MODE_FD) and columns the step's (tds_b200_jacobian_dims), with the wrenches' tangents
+ *   t_W as a block of their own: device t_W [6K * m][n_stride] (row (6k + r) * m + j), host t_W [n][K][6][m].  t_in, t_W and t_par may be
+ *   NULL (zero), not all three.
+ * _vjp: g_in [cols], g_W (device [6K][n_stride], host [n][K][6]) and, while a set is installed and g_par is not NULL, the parameters'
+ *   cotangents g_par [k] = g_out^T d(outputs) / d(inputs), by the JVP along identity tangents (the wrench directions follow the step's
+ *   columns and precede the parameters).  g_in, g_W, g_par may be NULL, not all three.  Layouts as tds_b200_step_contacts_vjp_*.
+ * Returns -1 (bad argument: a NULL required pointer, K or a link index out of range, m < 1, every tangent or cotangent NULL), -2 (MODE_WORLD),
+ * -3 (use_pd without tds_b200_set_env), -4 (t_par / g_par without installed parameters). */
+int tds_b200_step_wrench_device(tds_b200_sim* sim, int mode, int use_pd, const float* q_in, const float* qd_in, const float* tau_or_action,
+                                int K, const int* links, const double* local, const float* W, float* q_out, float* qd_out, float* qdd_out,
+                                void* stream);
+int tds_b200_step_wrench_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action, int K,
+                              const int* links, const double* local, const double* W, double* q_out, double* qd_out, double* qdd_out);
+int tds_b200_step_wrench_jvp_device(tds_b200_sim* sim, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                                    int K, const int* links, const double* local, const float* W, int m, const double* t_in,
+                                    const double* t_W, const double* t_par, double* t_out, void* stream);
+int tds_b200_step_wrench_jvp_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                  int K, const int* links, const double* local, const double* W, int m, const double* t_in, const double* t_W,
+                                  const double* t_par, double* t_out);
+int tds_b200_step_wrench_vjp_device(tds_b200_sim* sim, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action,
+                                    int K, const int* links, const double* local, const float* W, const double* g_out, double* g_in,
+                                    double* g_W, double* g_par, void* stream);
+int tds_b200_step_wrench_vjp_host(tds_b200_sim* sim, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                  int K, const int* links, const double* local, const double* W, const double* g_out, double* g_in,
+                                  double* g_W, double* g_par);
+
 /* Stand-alone integration stages of the fine-grained surface (device SoA arrays as above):
  * integrate_euler (src/dynamics/integrator.hpp:10-133): qd += qdd dt (qdd may be NULL = zero), q += qd dt, floating base
  * quaternion increment + normalisation; integrate_euler_qdd (:141-195): qd += qdd dt only. */

@@ -182,6 +182,18 @@ def lib():
     L.tds_b200_step_contacts_vjp_device.argtypes = [vp, ci, ci, fp, fp, fp, vp, vp, vp, vp]
     L.tds_b200_step_contacts_vjp_host.restype = ci
     L.tds_b200_step_contacts_vjp_host.argtypes = [vp, ci, ci, dp, dp, dp, dp, dp, dp]
+    L.tds_b200_step_wrench_device.restype = ci
+    L.tds_b200_step_wrench_device.argtypes = [vp, ci, ci, fp, fp, fp, ci, vp, dp, fp, fp, fp, fp, vp]
+    L.tds_b200_step_wrench_host.restype = ci
+    L.tds_b200_step_wrench_host.argtypes = [vp, ci, ci, dp, dp, dp, ci, vp, dp, dp, dp, dp, dp]
+    L.tds_b200_step_wrench_jvp_device.restype = ci
+    L.tds_b200_step_wrench_jvp_device.argtypes = [vp, ci, ci, fp, fp, fp, ci, vp, dp, fp, ci, vp, vp, vp, vp, vp]
+    L.tds_b200_step_wrench_jvp_host.restype = ci
+    L.tds_b200_step_wrench_jvp_host.argtypes = [vp, ci, ci, dp, dp, dp, ci, vp, dp, dp, ci, dp, dp, dp, dp]
+    L.tds_b200_step_wrench_vjp_device.restype = ci
+    L.tds_b200_step_wrench_vjp_device.argtypes = [vp, ci, ci, fp, fp, fp, ci, vp, dp, fp, vp, vp, vp, vp, vp]
+    L.tds_b200_step_wrench_vjp_host.restype = ci
+    L.tds_b200_step_wrench_vjp_host.argtypes = [vp, ci, ci, dp, dp, dp, ci, vp, dp, dp, dp, dp, dp, dp]
     L.tds_b200_rigid_jvp_device.restype = ci
     L.tds_b200_rigid_jvp_device.argtypes = [vp, vp, vp, ci, ci, vp, vp, vp, vp, vp]
     L.tds_b200_rigid_jvp_host.restype = ci
@@ -290,6 +302,8 @@ DECLARED_SYMBOLS = [
     "tds_b200_point_motion_vjp_device", "tds_b200_point_motion_vjp_host",
     "tds_b200_step_contacts_device", "tds_b200_step_contacts_host", "tds_b200_step_contacts_jvp_device", "tds_b200_step_contacts_jvp_host",
     "tds_b200_step_contacts_vjp_device", "tds_b200_step_contacts_vjp_host",
+    "tds_b200_step_wrench_device", "tds_b200_step_wrench_host", "tds_b200_step_wrench_jvp_device", "tds_b200_step_wrench_jvp_host",
+    "tds_b200_step_wrench_vjp_device", "tds_b200_step_wrench_vjp_host",
     "tds_b200_integrate_euler_device", "tds_b200_integrate_euler_qdd_device", "tds_b200_contact_pairs", "tds_b200_model_contact_pairs", "tds_b200_contact_tuples", "tds_b200_model_contact_tuples", "tds_b200_contact_list_device", "tds_b200_contact_list_host", "tds_b200_contact_list_candidates_host",
     "tds_b200_rigid_create", "tds_b200_rigid_destroy", "tds_b200_rigid_set_params", "tds_b200_rigid_step_device", "tds_b200_rigid_step_host", "tds_b200_rigid_jacobian_host",
     "tds_b200_rigid_vjp_device", "tds_b200_rigid_vjp_host", "tds_b200_rigid_jvp_device", "tds_b200_rigid_jvp_host",

@@ -48,6 +48,11 @@ DESIGN.md section 7.13) with a backward rule (BatchSim.kinematics_vjp_device: fl
 point_motion(sim, q, qd, links, local, qdd=None) is every point's spatial Jacobian, velocity and acceleration J qdd + J' qd (float64,
 DESIGN.md section 7.17) with a backward rule (BatchSim.point_motion_vjp_device: float32 q.grad, qd.grad, qdd.grad) and a forward-mode
 rule (BatchSim.point_motion_jvp_device).
+
+step_wrench(sim, q, qd, tau_or_action, links, local, W, mode=MODE_FULL, use_pd=False, params=None) is the step with a wrench [n; f] per
+environment at every point of a point table (DESIGN.md section 7.18), on the world-frame kernel at the simulator's precision, with a
+backward rule (BatchSim.step_wrench_vjp_device: float32 q.grad, qd.grad, tau_or_action.grad, W.grad, float64 params.grad) and a
+forward-mode rule (BatchSim.step_wrench_jvp_device).
 """
 import torch
 
@@ -802,3 +807,118 @@ def step_contacts(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False, 
                                tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
         raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
     return _StepContacts.apply(sim, int(mode), bool(use_pd), q, qd, tau_or_action, params)
+
+
+class _StepWrench(torch.autograd.Function):
+    @staticmethod
+    def forward(sim, mode, use_pd, links, local, q, qd, tau, W, params):
+        n, ns = sim.n_envs, sim.n_stride
+        if params is not None:
+            sim.set_physical_params(sim.param_ids, params.detach())
+        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), _soa_opt(tau, ns, torch.float32)
+        Ws = _soa(W.reshape(n, -1), ns, torch.float32)
+        fd = mode == MODE_FD
+        q_out = None if fd else torch.empty_like(qs)
+        qd_out = None if fd else torch.empty_like(qds)
+        qdd_out = torch.empty_like(qds) if fd else None
+        _on_side_stream(q.device, lambda st: sim.step_wrench_device(mode, qs, qds, ts, links, local, Ws, q_out, qd_out, qdd_out, use_pd=use_pd,
+                                                                    stream=st), (qs, qds, ts, Ws, q_out, qd_out, qdd_out))
+        if fd:
+            return qdd_out[:sim.n_qd, :n].t().contiguous()
+        return q_out[:sim.n_q, :n].t().contiguous(), qd_out[:sim.n_qd, :n].t().contiguous()
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        sim, mode, use_pd, links, local, q, qd, tau, W, params = inputs
+        ns = sim.n_stride
+        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), _soa_opt(tau, ns, torch.float32)
+        Ws = _soa(W.reshape(sim.n_envs, -1), ns, torch.float32)
+        par = params.detach() if params is not None else None
+        ctx.sim, ctx.mode, ctx.use_pd, ctx.links, ctx.local = sim, mode, use_pd, links, local
+        ctx.has_tau, ctx.has_params, ctx.K = tau is not None, params is not None, len(links)
+        ctx.save_for_backward(qs, qds, ts if ts is not None else qs, Ws, par if par is not None else qs)
+        ctx.jvp_inputs = (qs, qds, ts, Ws, par)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        sim, mode, use_pd, K = ctx.sim, ctx.mode, ctx.use_pd, ctx.K
+        qs, qds, ts, Ws, par = ctx.saved_tensors
+        ts = ts if ctx.has_tau else None
+        n, ns, nq, nd = sim.n_envs, sim.n_stride, sim.n_q, sim.n_qd
+        rows, cols = sim.jacobian_dims(mode, use_pd)
+        dims = [(0, nd)] if mode == MODE_FD else [(0, nq), (nq, nd)]
+        G = torch.zeros((rows, ns), dtype=torch.float64, device=qs.device)
+        for g, (r0, d) in zip(grads, dims):
+            if g is not None and d:
+                G[r0:r0 + d, :n] = g.to(torch.float64).t()
+        g_in = torch.zeros((cols, ns), dtype=torch.float64, device=qs.device)
+        g_W = torch.zeros((max(6 * K, 1), ns), dtype=torch.float64, device=qs.device)
+        g_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=qs.device) if ctx.has_params else None
+        if ctx.has_params:
+            sim.set_physical_params(sim.param_ids, par)   # the values of this call
+        _on_side_stream(qs.device, lambda st: sim.step_wrench_vjp_device(mode, qs, qds, ts, ctx.links, ctx.local, Ws, G, g_in, g_W, g_par,
+                                                                         use_pd=use_pd, stream=st), (qs, qds, ts, Ws, G, g_in, g_W, g_par))
+        gt = None
+        if ctx.has_tau:
+            k0 = nq + nd
+            gt = g_in[k0:k0 + (sim.n_act if use_pd else sim.n_tau), :n].t().to(torch.float32).contiguous()
+        gW = g_W[:6 * K, :n].t().to(torch.float32).reshape(n, K, 6).contiguous()
+        gp = g_par[:, :n].t().contiguous() if ctx.has_params else None
+        return (None, None, None, None, None, g_in[:nq, :n].t().to(torch.float32).contiguous(),
+                g_in[nq:nq + nd, :n].t().to(torch.float32).contiguous(), gt, gW, gp)
+
+    @staticmethod
+    def jvp(ctx, _sim, _mode, _use_pd, _links, _local, *tangents):
+        with torch._C._DisableFuncTorch():
+            return _StepWrench._jvp(ctx, *(_plain(t) for t in tangents))
+
+    @staticmethod
+    def _jvp(ctx, tq, tqd, ttau, tW, tpar):
+        sim, mode, use_pd, K = ctx.sim, ctx.mode, ctx.use_pd, ctx.K
+        qs, qds, ts, Ws, par = (_plain(t) for t in ctx.jvp_inputs)
+        n, ns, nq, nd = sim.n_envs, sim.n_stride, sim.n_q, sim.n_qd
+        rows, cols = sim.jacobian_dims(mode, use_pd)
+        t_in = t_W = t_par = None
+        if tq is not None or tqd is not None or (ttau is not None and ctx.has_tau):
+            t_in = torch.zeros((cols, ns), dtype=torch.float64, device=qs.device)
+            for t, r0 in ((tq, 0), (tqd, nq), (ttau if ctx.has_tau else None, nq + nd)):   # the PD gains: zero tangent
+                if t is not None and t.shape[1]:
+                    t_in[r0:r0 + t.shape[1], :n] = t.to(torch.float64).t()
+        if tW is not None and K:
+            t_W = _soa(tW.reshape(n, 6 * K), ns, torch.float64)
+        if tpar is not None and ctx.has_params:
+            t_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=qs.device)
+            t_par[:, :n] = tpar.to(torch.float64).t()
+        t_out = torch.zeros((rows, ns), dtype=torch.float64, device=qs.device)
+        if t_in is not None or t_W is not None or t_par is not None:
+            if ctx.has_params:
+                sim.set_physical_params(sim.param_ids, par)   # the values of this call
+            _on_side_stream(qs.device, lambda st: sim.step_wrench_jvp_device(mode, qs, qds, ts, ctx.links, ctx.local, Ws, 1, t_in, t_W, t_par,
+                                                                             t_out, use_pd=use_pd, stream=st),
+                            (qs, qds, ts, Ws, t_in, t_W, t_par, t_out))
+        out = lambda r0, d: t_out[r0:r0 + d, :n].t().to(torch.float32).contiguous()
+        if mode == MODE_FD:
+            return out(0, nd)
+        return out(0, nq), out(nq, nd)
+
+
+def step_wrench(sim, q, qd, tau_or_action, links, local, W, mode=MODE_FULL, use_pd=False, params=None):
+    """One differentiable step of every environment of `sim` (a BatchSim) with external wrenches (DESIGN.md section 7.18): W float32 CUDA
+    tensor [n_envs, K, 6], W[e, k] = [n; f] in world axes at point k of the table links [K] (-1: the base) / local [K, 3] (the force acts
+    along a line through the point, n is a pure moment).  Returns (q', qd'), or qdd in MODE_FD, float32.  The step runs on the world-frame
+    kernel at the simulator's precision; other inputs as for step.  The derivatives are those of the fp64 world-frame step at the
+    fp32-rounded inputs, of the branch taken, along q, qd, tau_or_action, W and params (backward rule BatchSim.step_wrench_vjp_device,
+    forward-mode rule BatchSim.step_wrench_jvp_device)."""
+    for name, t in (("q", q), ("qd", qd), ("tau_or_action", tau_or_action)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or t.shape[0] != sim.n_envs):
+            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, dim] is expected")
+    lk = tuple(int(x) for x in torch.as_tensor(links).reshape(-1).tolist())
+    lc = tuple(tuple(float(v) for v in row) for row in torch.as_tensor(local, dtype=torch.float64).reshape(-1, 3).tolist())
+    if len(lc) != len(lk):
+        raise ValueError("links [K] and local [K, 3] expected")
+    if W.dtype != torch.float32 or not W.is_cuda or tuple(W.shape) != (sim.n_envs, len(lk), 6):
+        raise ValueError("W: a float32 CUDA tensor [n_envs, K, 6] is expected")
+    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
+                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
+        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    return _StepWrench.apply(sim, int(mode), bool(use_pd), lk, lc, q, qd, tau_or_action, W, params)

@@ -77,6 +77,12 @@ extern "C" int tds_launch_centroidal(const DevModel* M, const StepIO* io, const 
                                      cudaStream_t stream);
 extern "C" int tds_launch_centroidal_jvp(const DevModel* M, const StepIO* io, const ParMap* pm, const TdsCenCall* out, const double* t_in,
                                          const double* t_par, int m, int n_dirs, char* gscratch, cudaStream_t stream);
+// the step with external wrenches, and its Jacobian-vector products (tds_wrench.cu)
+extern "C" int tds_launch_wrench(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
+                                 const TdsExtCall* xc, int mode, int use_pd, int precision, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_wrench_jvp(const DevModel* M, const SimParams* P, const EnvParams* E, const StepIO* io, const ParMap* pm,
+                                     const TdsExtCall* xc, const double* t_in, const double* t_par, int m, int mode, int use_pd, int n_dirs,
+                                     char* gscratch, cudaStream_t stream);
 // spatial point Jacobians, point velocities and accelerations, and their Jacobian-vector products (tds_point_motion.cu)
 extern "C" int tds_launch_point_motion(const DevModel* M, const StepIO* io, const TdsMotCall* mc, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_point_motion_jvp(const DevModel* M, const StepIO* io, const TdsMotCall* mc, const double* t_in, int m, int n_dirs,
@@ -430,6 +436,7 @@ struct tds_b200_sim {
   int* vjp_flag = nullptr;
   double* vjp_g = nullptr; size_t vjp_g_bytes = 0;   // (also the cotangents G | g of the dynamics queries' VJPs)
   DevModel dm_m;          // layout of the fp64 mass-matrix instance (8-byte scalars)
+  float* wrench_dev = nullptr; size_t wrench_dev_bytes = 0;   // host paths of the step with wrenches: W [6K][ns] fp32
   double* mass_dev = nullptr; size_t mass_dev_bytes = 0; // dynamics queries' VJPs: identity tangents | output columns of a chunk
   // installed physical parameters (tds_b200_set_physical_params_*): slot map (par.n == 0: none) and values [k][ns] fp64
   ParMap par;
@@ -709,7 +716,7 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->rq); cudaFree(s->rqd); cudaFree(s->zero_act); cudaFree(s->pol_act); cudaFree(s->sticky); cudaFree(s->r_total);
   cudaFree(s->pol_params); cudaFree(s->act_qidx); cudaFree(s->r_steps);
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
-  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->mass_dev);
+  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->mass_dev); cudaFree(s->wrench_dev);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
@@ -901,16 +908,17 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
 
 // what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14, 7.16 and 7.17,
 // or the step with its contact records (section 7.15)
-enum class Query { step, mass, kin, inv, contacts, centroidal, motion };
+enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench };
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
 // inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
 // (t_in = the q tangents, t_par unused); inv: t_in = the q | qd | qdd tangents (qd and qdd in the step's qd and tau_or_action);
 // contacts: as step, with the rows q' | qd' | records; centroidal: t_in = the q | qd tangents (qd in the step's qd), outputs `cen`;
-// motion: t_in = the q | qd | qdd tangents (qd and qdd as for inv), the point table and outputs `mot`
+// motion: t_in = the q | qd | qdd tangents (qd and qdd as for inv), the point table and outputs `mot`; wrench: as step, with the point
+// table, wrenches and wrench tangents `ext`
 struct JvpTangents {
   const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr;
-  const TdsCenCall* cen = nullptr; const TdsMotCall* mot = nullptr;
+  const TdsCenCall* cen = nullptr; const TdsMotCall* mot = nullptr; const TdsExtCall* ext = nullptr;
 };
 
 // the installed physical parameters as a launch argument in *pmv, or NULL without any
@@ -932,11 +940,20 @@ static size_t lane_arena_bytes(const tds_b200_sim* s, const DevModel& M) {
   return (size_t)(s->n + 31) / 32 * (size_t)M.x_total * 32 * 4;
 }
 
-// directions (Jacobian columns or tangents) one launch of the dual instance takes: the scratch stays within 2 GB
-static int dir_chunk(const tds_b200_sim* s) {
-  const size_t chunk = ((size_t)2 << 30) / lane_arena_bytes(s, s->dm_ad);
+// scratch of one launch of the external-wrench instances (tds_wrench.cu) on layout M with RA of size_ra bytes: the grown layout's words
+static size_t wrench_arena_bytes(const tds_b200_sim* s, const DevModel& M, int size_ra) {
+  int words;
+  tds_ext_layout_w(&M, size_ra, &words);
+  return (size_t)(s->n + 31) / 32 * (size_t)words * 32 * 4;
+}
+
+// directions (Jacobian columns or tangents) one launch of the dual instance takes: the scratch (arena bytes per direction) stays within
+// 2 GB
+static int dir_chunk_of(const tds_b200_sim* s, size_t arena) {
+  const size_t chunk = ((size_t)2 << 30) / arena;
   return (int)(chunk < 1 ? 1 : (chunk > 65535 ? 65535 : chunk));   // (gridDim.y)
 }
+static int dir_chunk(const tds_b200_sim* s) { return dir_chunk_of(s, lane_arena_bytes(s, s->dm_ad)); }
 
 // Jacobian columns: the step's inputs (params == false) or the installed physical parameters, which are the dual instance's
 // directions dims[1] + s (params == true); or, with jv, the m columns J V of the tangent-seeded instance
@@ -952,8 +969,9 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   io.n = s->n; io.n_stride = s->ns;
   ParMap pmv;
   const ParMap* pm = installed_par(s, &pmv);
-  const int chunk = std::min(dir_chunk(s), n_dirs);
-  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, lane_arena_bytes(s, s->dm_ad) * chunk));
+  const size_t arena = (jv && jv->query == Query::wrench) ? wrench_arena_bytes(s, s->dm_ad, 16) : lane_arena_bytes(s, s->dm_ad);
+  const int chunk = std::min(dir_chunk_of(s, arena), n_dirs);
+  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, arena * chunk));
   const cudaStream_t sm = (cudaStream_t)stream;
   for (int d0 = 0; d0 < n_dirs; d0 += chunk) {
     io.jac_dir0 = dir_base + d0;
@@ -977,6 +995,10 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
           rc = tds_launch_centroidal_jvp(&s->dm_ad, &io, pm, jv->cen, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm);
           break;
         case Query::motion: rc = tds_launch_point_motion_jvp(&s->dm_ad, &io, jv->mot, jv->t_in, jv->m, nd, s->jac_scratch, sm); break;
+        case Query::wrench:
+          rc = tds_launch_wrench_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->ext, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch,
+                                     sm);
+          break;
       }
     }
     if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
@@ -2028,6 +2050,177 @@ int tds_b200_step_contacts_vjp_host(tds_b200_sim* s, int mode, int use_pd, const
                                 s->stream))
     return rc;
   CUDA_TRY(get_parts<double>({{g_in, (size_t)dims[1]}, {g_par, (size_t)k}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- the step with external wrenches (DESIGN.md section 7.18): the EXT instances of the world-frame kernel (tds_wrench.cu).  Values in
+// MODE_FD, MODE_NOCONTACT and MODE_FULL at the simulator's precision, on the world-frame kernel whatever kernel tds_b200_step_device would
+// choose; the JVP through the Jacobian's chunk loop and the VJP by identity tangents.  The point table is checked as for the kinematics
+// (kin_check); the wrench columns follow the step's columns (tds_b200_jacobian_dims) and precede the installed parameters.
+static int wrench_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* tau_or_action, int K,
+                        const int* links, const double* local, const void* W) {
+  if (int rc = kin_check(s, q, K, links, local)) return rc;
+  if (!qd || (use_pd && !tau_or_action) || (K > 0 && !W)) return -1;
+  if (mode == TDS_B200_MODE_WORLD) { set_err("step wrench: modes FD, NOCONTACT, FULL"); return -2; }
+  if (use_pd && s->E.n_act == 0) { set_err("use_pd without tds_b200_set_env"); return -3; }
+  return 0;
+}
+
+// q', qd' [dim][ns] (MODE_NOCONTACT, MODE_FULL) or qdd [n_qd][ns] (MODE_FD) fp32 of one step with the wrenches W [6K][ns] fp32
+static int wrench_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action, const TdsExtCall* xc,
+                      float* q_out, float* qd_out, float* qdd_out, cudaStream_t sm) {
+  const int p = s->precision;
+  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, wrench_arena_bytes(s, s->dm[p], p == TDS_B200_PREC_F64 ? 8 : 4)));
+  StepIO io;
+  memset(&io, 0, sizeof(io));
+  io.q_in = q; io.qd_in = qd; io.tau_in = tau_or_action;
+  io.q_out = q_out; io.qd_out = qd_out; io.qdd_out = qdd_out;
+  io.n = s->n; io.n_stride = s->ns;
+  ParMap pmv;
+  const int rc = tds_launch_wrench(&s->dm[p], &s->P, &s->E, &io, installed_par(s, &pmv), xc, mode, use_pd, p, s->jac_scratch, sm);
+  if (rc) set_err(std::string("step wrench launch: ") + cudaGetErrorString((cudaError_t)rc));
+  return rc;
+}
+
+// the outputs a mode needs: qdd in MODE_FD, q' and qd' otherwise
+static int wrench_out_check(int mode, const void* q_out, const void* qd_out, const void* qdd_out) {
+  if (mode == TDS_B200_MODE_FD ? !qdd_out : (!q_out || !qd_out)) return -1;
+  return 0;
+}
+
+int tds_b200_step_wrench_device(tds_b200_sim* s, int mode, int use_pd, const float* q_in, const float* qd_in, const float* tau_or_action,
+                                int K, const int* links, const double* local, const float* W, float* q_out, float* qd_out, float* qdd_out,
+                                void* stream) {
+  if (int rc = wrench_check(s, mode, use_pd, q_in, qd_in, tau_or_action, K, links, local, W)) return rc;
+  if (int rc = wrench_out_check(mode, q_out, qd_out, qdd_out)) return rc;
+  const TdsExtCall xc{K, links, local, W, nullptr};
+  return wrench_run(s, mode, use_pd, q_in, qd_in, tau_or_action, &xc, q_out, qd_out, qdd_out, (cudaStream_t)stream);
+}
+
+// W [n][K][6] fp64 -> s->wrench_dev [6K][ns] fp32, with the step's inputs
+static int put_wrench_inputs(tds_b200_sim* s, int use_pd, const double* q, const double* qd, const double* tau_or_action, int K,
+                             const double* W) {
+  if (int rc = put_step_inputs(s, use_pd, q, qd, tau_or_action)) return rc;
+  CUDA_TRY(grow_dev(&s->wrench_dev, &s->wrench_dev_bytes, sizeof(float) * (size_t)(6 * K + 1) * s->ns));
+  if (K == 0) return 0;
+  if (int rc = ensure_stage(s, sizeof(double) * s->n * 6 * K)) return rc;
+  return put_state(s, W, 6 * K, s->wrench_dev);
+}
+
+int tds_b200_step_wrench_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action, int K,
+                              const int* links, const double* local, const double* W, double* q_out, double* qd_out, double* qdd_out) {
+  if (int rc = wrench_check(s, mode, use_pd, q, qd, tau_or_action, K, links, local, W)) return rc;
+  if (int rc = wrench_out_check(mode, q_out, qd_out, qdd_out)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const DevModel& M = s->dm[0];
+  int rc = put_wrench_inputs(s, use_pd, q, qd, tau_or_action, K, W);
+  const TdsExtCall xc{K, links, local, s->wrench_dev, nullptr};
+  if (!rc) rc = wrench_run(s, mode, use_pd, s->q, s->qd, s->act, &xc, s->q, s->qd, s->qdd, s->stream);
+  if (!rc && mode == TDS_B200_MODE_FD) rc = get_state(s, s->qdd, M.n_qd, qdd_out);
+  if (!rc && mode != TDS_B200_MODE_FD) rc = get_state(s, s->q, M.n_q, q_out);
+  if (!rc && mode != TDS_B200_MODE_FD) rc = get_state(s, s->qd, M.n_qd, qd_out);
+  if (rc) return rc;
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  return 0;
+}
+
+static int wrench_jvp_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* tau_or_action, int K,
+                            const int* links, const double* local, const void* W, int m, const void* t_in, const void* t_W, const void* t_par,
+                            const void* t_out) {
+  if (int rc = wrench_check(s, mode, use_pd, q, qd, tau_or_action, K, links, local, W)) return rc;
+  if (!t_out || m < 1 || (!t_in && !t_W && !t_par)) return -1;
+  return par_without_installed(s, t_par, "step wrench jvp: parameter tangents");
+}
+
+int tds_b200_step_wrench_jvp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action, int K,
+                                    const int* links, const double* local, const float* W, int m, const double* t_in, const double* t_W,
+                                    const double* t_par, double* t_out, void* stream) {
+  if (int rc = wrench_jvp_check(s, mode, use_pd, q, qd, tau_or_action, K, links, local, W, m, t_in, t_W, t_par, t_out)) return rc;
+  const TdsExtCall xc{K, links, local, W, t_W};
+  JvpTangents jv{t_in, t_par, m, Query::wrench};
+  jv.ext = &xc;
+  return jacobian_run(s, mode, use_pd, q, qd, tau_or_action, t_out, stream, false, &jv);
+}
+
+int tds_b200_step_wrench_jvp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                  int K, const int* links, const double* local, const double* W, int m, const double* t_in, const double* t_W,
+                                  const double* t_par, double* t_out) {
+  if (int rc = wrench_jvp_check(s, mode, use_pd, q, qd, tau_or_action, K, links, local, W, m, t_in, t_W, t_par, t_out)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, k = s->par.n;
+  int dims[2];
+  tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; t_in | t_W | t_par | t_out
+  const size_t ti = (size_t)(t_in ? dims[1] : 0) * m, tw = (size_t)(t_W ? 6 * K : 0) * m, tp = (size_t)(t_par ? k : 0) * m,
+               to = (size_t)dims[0] * m;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + tw + tp + to) * ns));
+  if (int rc = put_wrench_inputs(s, use_pd, q, qd, tau_or_action, K, W)) return rc;
+  double* tout_d = s->jac_dev + (ti + tw + tp) * ns;
+  CUDA_TRY(put_parts<double>(s->jac_dev, {{t_in, ti}, {t_W, tw}, {t_par, tp}, {nullptr, to}}, n, ns, s->stream));
+  const TdsExtCall xc{K, links, local, s->wrench_dev, t_W ? s->jac_dev + ti * ns : nullptr};
+  JvpTangents jv{t_in ? s->jac_dev : nullptr, t_par ? s->jac_dev + (ti + tw) * ns : nullptr, m, Query::wrench};
+  jv.ext = &xc;
+  if (int rc = jacobian_run(s, mode, use_pd, s->q, s->qd, s->act, tout_d, s->stream, false, &jv)) return rc;
+  CUDA_TRY(get_rows(t_out, tout_d, to, n, ns, s->stream));
+  return 0;
+}
+
+static int wrench_vjp_check(tds_b200_sim* s, int mode, int use_pd, const void* q, const void* qd, const void* tau_or_action, int K,
+                            const int* links, const double* local, const void* W, const void* g_out, const void* g_in, const void* g_W,
+                            const void* g_par) {
+  if (int rc = wrench_check(s, mode, use_pd, q, qd, tau_or_action, K, links, local, W)) return rc;
+  if (!g_out || (!g_in && !g_W && !g_par)) return -1;
+  return par_without_installed(s, g_par, "step wrench vjp: parameter cotangents");
+}
+
+// g_inw [cols + 6K][ns] (the step's inputs, then the wrenches) and g_par [k][ns] (NULL: not wanted) = <g_out, d(q' | qd', or qdd)> for
+// g_out [rows][ns]; the wrench tangents are the identity tangents' rows behind the step's columns
+static int wrench_vjp_run(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action, int K,
+                          const int* links, const double* local, const float* W, const double* g_out, double* g_inw, double* g_par,
+                          cudaStream_t sm) {
+  int dims[2];
+  tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  const size_t ns = s->ns;
+  return vjp_by_eye(s, "step wrench", dims[1] + 6 * K, dims[0], g_out, g_inw, g_par, sm,
+                    [&](int nd, const double* t_in, const double* t_par, double* dO) {
+                      const TdsExtCall xc{K, links, local, W, t_in + (size_t)dims[1] * nd * ns};
+                      JvpTangents jv{t_in, t_par, nd, Query::wrench};
+                      jv.ext = &xc;
+                      return jacobian_run(s, mode, use_pd, q, qd, tau_or_action, dO, sm, false, &jv);
+                    });
+}
+
+int tds_b200_step_wrench_vjp_device(tds_b200_sim* s, int mode, int use_pd, const float* q, const float* qd, const float* tau_or_action, int K,
+                                    const int* links, const double* local, const float* W, const double* g_out, double* g_in, double* g_W,
+                                    double* g_par, void* stream) {
+  if (int rc = wrench_vjp_check(s, mode, use_pd, q, qd, tau_or_action, K, links, local, W, g_out, g_in, g_W, g_par)) return rc;
+  int dims[2];
+  tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  cudaStream_t sm = (cudaStream_t)stream;
+  // g_in | g_W as one array for the contraction
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)(dims[1] + 6 * K) * s->ns));
+  if (int rc = wrench_vjp_run(s, mode, use_pd, q, qd, tau_or_action, K, links, local, W, g_out, s->vjp_g, g_par, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_in, (size_t)dims[1]}, {g_W, (size_t)6 * K}}, s->vjp_g, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_step_wrench_vjp_host(tds_b200_sim* s, int mode, int use_pd, const double* q, const double* qd, const double* tau_or_action,
+                                  int K, const int* links, const double* local, const double* W, const double* g_out, double* g_in,
+                                  double* g_W, double* g_par) {
+  if (int rc = wrench_vjp_check(s, mode, use_pd, q, qd, tau_or_action, K, links, local, W, g_out, g_in, g_W, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, k = g_par ? s->par.n : 0;
+  int dims[2];
+  tds_b200_jacobian_dims(s, mode, use_pd, dims);
+  // g_out | g_in | g_W | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * ((size_t)dims[0] + dims[1] + 6 * K + k + 1) * ns));
+  double* g_d = s->vjp_g + (size_t)dims[0] * ns;
+  if (int rc = put_wrench_inputs(s, use_pd, q, qd, tau_or_action, K, W)) return rc;
+  CUDA_TRY(put_rows(s->vjp_g, g_out, dims[0], n, ns, s->stream));
+  if (int rc = wrench_vjp_run(s, mode, use_pd, s->q, s->qd, s->act, K, links, local, s->wrench_dev, s->vjp_g, g_d,
+                              g_par ? g_d + (size_t)(dims[1] + 6 * K) * ns : nullptr, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{g_in, (size_t)dims[1]}, {g_W, (size_t)6 * K}, {g_par, (size_t)k}}, g_d, n, ns, s->stream));
   return 0;
 }
 

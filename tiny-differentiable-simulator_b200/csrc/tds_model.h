@@ -334,6 +334,15 @@ TDS_HOST_INLINE void tds_build_layout_w(DevModel* D, int size_ra, int size_rc, i
   D->x_total = w;
 }
 
+// Layout of the world-frame kernel's external-wrench instances (tds_stepw.cu, template flag EXT; DESIGN.md section 7.18): the layout D
+// (built by tds_build_layout_w) followed by the links' wrench sums, 6 RA words per link, 16-byte aligned so that every scalar type
+// addresses them.  Returns the region's first word and sets *x_total to the words per lane of the grown layout; D itself is unchanged.
+TDS_HOST_INLINE int tds_ext_layout_w(const DevModel* D, int size_ra, int* x_total) {
+  const int x_ext = (D->x_total + 3) & ~3;
+  *x_total = x_ext + ((D->n_links * 6 * (size_ra / 4) + 3) & ~3);
+  return x_ext;
+}
+
 // ---- physical parameter ids (include/tds_b200.h, tds_b200_set_physical_params_*) ----------------------------------------------------
 // 0 friction, 1 restitution, 2 + 10 b + c body b (0 = base, i + 1 = link i; c: mass, com x y z, I_com xx xy xz yy yz zz),
 // 2 + 10 (n_links + 1) + 2 i + c link i (c: joint stiffness, joint damping)

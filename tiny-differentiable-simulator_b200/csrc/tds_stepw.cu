@@ -58,7 +58,19 @@ template <typename B> struct CenArg : B { double* com; double* A; double* bias; 
 // kernel argument of the point-motion instances (MOT, DESIGN.md section 7.17): the point table of KinArg (B = KinArg or KinArgJvp), whose
 // J is the 6-row spatial point Jacobian here (xf and x are not read), and the outputs vel and acc
 template <typename B> struct MotArg : B { double* vel; double* acc; };
-template <bool PAR, bool JV = false, bool KIN = false, bool CF = false, bool CEN = false, bool MOT = false> struct ParArg { typedef NoPar type; };
+// kernel argument of the external-wrench instances (EXT, DESIGN.md section 7.18): the argument of the same instance without EXT (B = NoPar,
+// ParMap, NoParJvp or ParMapJvp) and the point table of KinArg with the wrenches W [6K][ns] fp32 (row 6k + r: component r of [n; f] of
+// point k), their tangents t_W [6K * m][ns] (JV instances; null: zero tangent), the arena word x_ext of the per-link wrench sums and the
+// links that have points (bit i: link i), the only ones whose sums are stored and read
+struct ExtPts {
+  const float* W; const double* t_W;
+  unsigned long long links_with_points;
+  int K, x_ext;
+  int link[TDS_MAX_KIN_POINTS];
+  double local[3 * TDS_MAX_KIN_POINTS];
+};
+template <typename B> struct ExtArg : B { ExtPts ext; };
+template <bool PAR, bool JV = false, bool KIN = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false> struct ParArg { typedef NoPar type; };
 template <> struct ParArg<true, false> { typedef ParMap type; };
 template <> struct ParArg<false, true> { typedef NoParJvp type; };
 template <> struct ParArg<true, true> { typedef ParMapJvp type; };
@@ -71,6 +83,7 @@ template <> struct ParArg<true, true, false, true> { typedef ParMapJvp type; };
 template <bool PAR, bool JV> struct ParArg<PAR, JV, false, false, true> { typedef CenArg<typename ParArg<PAR, JV>::type> type; };
 template <> struct ParArg<false, false, false, false, false, true> { typedef MotArg<KinArg> type; };
 template <> struct ParArg<false, true, false, false, false, true> { typedef MotArg<KinArgJvp> type; };
+template <bool PAR, bool JV> struct ParArg<PAR, JV, false, false, false, false, true> { typedef ExtArg<typename ParArg<PAR, JV>::type> type; };
 
 // CF, dual instances: the part of a record's dual number they write - the tangent (d).  The host build of the tests also compiles them
 // with the value (v), for an fp64 value path of the records that central differences can resolve.
@@ -138,12 +151,19 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // a.top x x + w x x'] and the 6 x n_qd Jacobian (rows [w; x'], joint column [S.top; S.bot + S.top x x], floating-base columns [R_b | 0;
 // -[x]x R_b | R_b] in the base-twist coordinates of qd[0:6]).  Outputs pm.J [6K n_qd], pm.vel [6K], pm.acc [6K] (each may be null), row r
 // at out[r * ns + e] (fp64 instance) or its dual part at out[(r * m + j) * ns + e] (JV instance).  Returns before pass 2.
+// EXT: the step with external wrenches (DESIGN.md section 7.18), point table and wrenches in pm.ext.  As pass 1 reaches link l it sums the
+// wrenches about O of l's points at x (relative to O), [n + x x f; f] in RC, and stores the sum at RA precision in l's 6 RA words at arena
+// word pm.ext.x_ext (a region behind the layout's x_total, present only in the EXT launches; links without points skip both the store
+// and the load); pass 2 subtracts it from l's bias force pA
+// (kinematics.hpp:132, pA = v x* I v - f_ext), and the floating base's points go into the base's bias force in the base frame.  Component r
+// of point k's wrench is input direction n_in_ad + 6k + r (JV instances: entry 6k + r of the tangent pm.ext.t_W).  Nothing else differs
+// from the step.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
-          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false>
+          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
-                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF, CEN, MOT>::type pm = {}) {
+                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF, CEN, MOT, EXT>::type pm = {}) {
   extern __shared__ __align__(16) char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp_in_blk = threadIdx.x >> 5;
@@ -471,6 +491,32 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       }
     }
   };
+  // EXT: the wrench about O of point k on a body at world rotation R and position p (relative to O), [n + x x f; f] at x = p + R local
+  // (JV: seeded with the tangent's entries 6k + r), and their sum over the points on body l (-1: the base)
+  auto ext_wrench = [&](int k, const M3<RC>& R, const V3<RC>& p) -> Sv<RC> {
+    Sv<RC> w;
+    if constexpr (EXT) {
+      RC c[6];
+      for (int r = 0; r < 6; ++r) {
+        const RQ x = RQ(pm.ext.W[(size_t)(6 * k + r) * ns + e]);
+        if constexpr (JV) c[r] = RC(jv_seed(x, pm.ext.t_W, 6 * k + r, pm.jv.m, dir, ns, e));
+        else c[r] = RC(x);
+      }
+      const V3<RC> x = p + mul(R, v3<RC>(RC(pm.ext.local[3 * k]), RC(pm.ext.local[3 * k + 1]), RC(pm.ext.local[3 * k + 2])));
+      const V3<RC> f = v3<RC>(c[3], c[4], c[5]);
+      w.top = v3<RC>(c[0], c[1], c[2]) + cross(x, f);
+      w.bot = f;
+    }
+    return w;
+  };
+  auto ext_sum = [&](int l, const M3<RC>& R, const V3<RC>& p) -> Sv<RC> {
+    Sv<RC> w;
+    w.top = v3<RC>(RC(0), RC(0), RC(0)); w.bot = w.top;
+    if constexpr (EXT)
+      for (int k = 0; k < pm.ext.K; ++k)
+        if (pm.ext.link[k] == l) w = w + ext_wrench(k, R, p);
+    return w;
+  };
   M3<RC> R_prev = Rb;
   V3<RC> p_prev = M.floating ? v3<RC>(RC(0), RC(0), RC(0)) : v3<RC>(-O.x, -O.y, -O.z);
   Sv<RA> v_prev;
@@ -627,6 +673,9 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       v.bot = axpy(Sf.bot, qdi, v.bot);
     }
     st6<RA>(A.ptr<RA>(M.x_link + i * LWD + VOFF), ST, v);
+    if constexpr (EXT) {
+      if ((pm.ext.links_with_points >> i) & 1ull) st6<RA>(A.ptr<RA>(pm.ext.x_ext + i * 6 * RAW), ST, cvt_sv<RA>(ext_sum(i, Ri, pi)));
+    }
     if constexpr (CEN) {   // the link's share of the body record and its term v_i x* (r_i v_i) of the rate
       const Rbi<RC> r = ld_rbi<RC>(A.ptr<RC>(M.x_link + i * LWD), ST);
       rbi_add(cen_I, r);
@@ -865,6 +914,12 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     const Sv<RA> v = ld6<RA>(vrec, ST);
     Abi<RA> Ia = abi_from_rbi(rb);
     Sv<RA> pA = cross_mf(v, rbi_mul(rb, v));                 // kinematics.hpp:132
+    if constexpr (EXT) {                                     // - f_ext, the sum pass 1 stored
+      if ((pm.ext.links_with_points >> i) & 1ull) {
+        const Sv<RA> w = ld6<RA>(A.ptr<RA>(pm.ext.x_ext + i * 6 * RAW), ST);
+        pA.top = pA.top - w.top; pA.bot = pA.bot - w.bot;
+      }
+    }
     if (fl & TDS_LF_CHILD_ADJ) { if constexpr (!MASS && !CEN) { abi_add(Ia, cA); pA = pA + cP; } rbi_add(Ic, cC); }
     if (M.acc_slot[i] >= 0) {
       if constexpr (!MASS && !CEN) {
@@ -1103,6 +1158,11 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       const V3<RA> wb = v3<RA>(RA(qdv[0]), RA(qdv[ST]), RA(qdv[2 * ST]));
       pb.top = cross(wb, mul(Iw, wb)) + mul(Rt, pch.top);
       pb.bot = mul(Rt, pch.bot);
+      if constexpr (EXT) {   // - f_ext of the base's points in the base frame (O is the base origin)
+        const Sv<RC> w = ext_sum(-1, Rb, v3<RC>(RC(0), RC(0), RC(0)));
+        pb.top = pb.top - cvt<RA>(mulT(Rb, w.top));
+        pb.bot = pb.bot - cvt<RA>(mulT(Rb, w.bot));
+      }
     }
     if (any_contact) {  // mass_matrix.hpp:114-120: base block = composite inertia in the base frame
       Rbi<RC> Ib = base_par ? cvt_rbi<RC>(bp) : model_rbi_of<RC>(M.base_rbi);

@@ -169,6 +169,16 @@ struct TdsMotCall {
   double* J; double* vel; double* acc;
 };
 
+// One call of the external-wrench instances (tds_wrench.cu, DESIGN.md section 7.18), as the C-ABI hands it to the launchers: the point
+// table as in TdsKinCall and the wrenches W [6K][ns] fp32 ([n; f] in world axes, row 6k + r) with, for the JVP, their tangents
+// t_W [6K * m][ns] fp64 (null: zero tangent)
+struct TdsExtCall {
+  int K;
+  const int* link;       // [K], -1 = the base
+  const double* local;   // [3K]
+  const float* W; const double* t_W;
+};
+
 // Installed physical parameters (tds_b200_set_physical_params_*): the slot of each model quantity in the lane's value vector,
 // or -1 = the model's value, and the values themselves.  Passed only to the instances of the world-frame kernel that read them
 // (StepIO stays as it is: the other instances keep it on their stack).

@@ -575,6 +575,88 @@ class BatchSim:
         self._check(self._L.tds_b200_step_contacts_vjp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action),
                                                               _ptr(g_out), _ptr(g_in), _ptr(g_par), st), "step_contacts_vjp_device")
 
+    # ---- the step with external wrenches (DESIGN.md section 7.18) ----
+    def _wrench_args(self, links, local, W):
+        """The point table and the wrenches W [n_envs, K, 6] (or [K, 6] for every environment) as the host entry points take them."""
+        keep, K, lp, cp = self._kin_args(links, local)
+        w = np.ascontiguousarray(np.broadcast_to(np.asarray(W, dtype=np.float64), (self.n_envs, K, 6))) if K else None
+        return keep, K, lp, cp, w
+
+    def step_wrench_host(self, mode, q, qd, tau_or_action, links, local, W, use_pd=False):
+        """One step (MODE_FD, MODE_NOCONTACT or MODE_FULL) on the world-frame kernel with a wrench W[e, k] = [n; f] (world axes, rounded to
+        fp32) at every point of the table links [K] (-1: the base) / local [K, 3]: (q' [n, n_q], qd' [n, n_qd]), or qdd [n, n_qd] in
+        MODE_FD.  The force f acts along a line through the point, n is a pure moment; the generalised force is J^T W with J the 6-row
+        point Jacobian of point_motion_host (include/tds_b200.h).  K = 0 is the world-frame step."""
+        q, qd, t = self._step_args(q, qd, tau_or_action)
+        keep, K, lp, cp, w = self._wrench_args(links, local, W)
+        qo, qdo, qddo = np.zeros_like(q), np.zeros_like(qd), np.zeros_like(qd)
+        self._check(self._L.tds_b200_step_wrench_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), K, lp, cp, _dp(w), _dp(qo),
+                                                      _dp(qdo), _dp(qddo)), "step_wrench_host")
+        return qddo if mode == MODE_FD else (qo, qdo)
+
+    def step_wrench_device(self, mode, q, qd, tau_or_action, links, local, W, q_out=None, qd_out=None, qdd_out=None, use_pd=False,
+                           stream=None):
+        """Device version of step_wrench_host on the SoA layout: q, qd, tau_or_action float32 CUDA tensors [dim, n_stride] as for
+        step_device, W float32 [6K, n_stride] (row 6k + r: component r of [n; f] of point k); q_out, qd_out (MODE_NOCONTACT, MODE_FULL)
+        or qdd_out (MODE_FD) float32 [dim, n_stride].  The point table is host data.  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_step_wrench_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), K, lp, cp,
+                                                        _ptr(W), _ptr(q_out), _ptr(qd_out), _ptr(qdd_out), st), "step_wrench_device")
+
+    def step_wrench_jvp_host(self, mode, q, qd, tau_or_action, links, local, W, t_in=None, t_W=None, t_par=None, use_pd=False):
+        """Directional derivatives t_out [n, rows, m] of step_wrench_host (rows q' | qd', or qdd in MODE_FD, as step_jacobian_host)
+        along m tangents t_in [n, cols, m] of the step's inputs, t_W [n, K, 6, m] of the wrenches and t_par [n, k, m] of the installed
+        parameters (each may be None, not all three); tangents given without the last axis are m = 1 and drop it."""
+        q, qd, t = self._step_args(q, qd, tau_or_action)
+        keep, K, lp, cp, w = self._wrench_args(links, local, W)
+        rows, cols = self.jacobian_dims(mode, use_pd)
+        tw = None if t_W is None else np.asarray(t_W, dtype=np.float64)
+        single_w = tw is not None and tw.ndim == 3
+        if tw is not None:
+            tw = tw.reshape(self.n_envs, 6 * K, -1) if not single_w else tw.reshape(self.n_envs, 6 * K)
+        (ti, tww, tp), m, single = self._tangents([(t_in, cols), (tw, 6 * K), (t_par, len(self.param_ids))], names="t_in, t_W and t_par")
+        if m == 0:
+            raise ValueError("at least one tangent is expected")
+        out = np.zeros((self.n_envs, rows, m))
+        self._check(self._L.tds_b200_step_wrench_jvp_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), K, lp, cp, _dp(w), m, _dp(ti),
+                                                          _dp(tww), _dp(tp), _dp(out)), "step_wrench_jvp_host")
+        return out[:, :, 0] if single else out
+
+    def step_wrench_jvp_device(self, mode, q, qd, tau_or_action, links, local, W, m, t_in, t_W, t_par, t_out, use_pd=False, stream=None):
+        """Device version of step_wrench_jvp_host, layouts as step_jvp_device with t_W [6K * m, n_stride] float64 (entry (6k + r, j) at
+        row (6k + r) * m + j); t_in, t_W and t_par may be None, not all three.  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_step_wrench_jvp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), K, lp, cp,
+                                                            _ptr(W), int(m), _ptr(t_in), _ptr(t_W), _ptr(t_par), _ptr(t_out), st),
+                    "step_wrench_jvp_device")
+
+    def step_wrench_vjp_host(self, mode, q, qd, tau_or_action, links, local, W, g_out, use_pd=False):
+        """Vector-Jacobian product of step_wrench_host: g_out [n, rows] -> (g_in [n, cols], g_W [n, K, 6], g_par [n, k] or None without
+        installed parameters)."""
+        q, qd, t = self._step_args(q, qd, tau_or_action)
+        keep, K, lp, cp, w = self._wrench_args(links, local, W)
+        rows, cols = self.jacobian_dims(mode, use_pd)
+        g = np.ascontiguousarray(g_out, dtype=np.float64)
+        if g.shape != (self.n_envs, rows):
+            raise ValueError(f"g_out: [n_envs, {rows}] expected, got {g.shape}")
+        g_in, g_W = np.zeros((self.n_envs, cols)), np.zeros((self.n_envs, K, 6))
+        g_par = np.zeros((self.n_envs, len(self.param_ids))) if self.param_ids else None
+        self._check(self._L.tds_b200_step_wrench_vjp_host(self._h, mode, int(use_pd), _dp(q), _dp(qd), _dp(t), K, lp, cp, _dp(w), _dp(g),
+                                                          _dp(g_in), _dp(g_W) if K else None, _dp(g_par)), "step_wrench_vjp_host")
+        return g_in, g_W, g_par
+
+    def step_wrench_vjp_device(self, mode, q, qd, tau_or_action, links, local, W, g_out, g_in=None, g_W=None, g_par=None, use_pd=False,
+                               stream=None):
+        """Device version of step_wrench_vjp_host: g_out [rows, n_stride], g_in [cols, n_stride], g_W [6K, n_stride], g_par [k, n_stride]
+        float64 CUDA tensors (g_in, g_W or g_par may be None, not all three).  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._kin_args(links, local)
+        self._check(self._L.tds_b200_step_wrench_vjp_device(self._h, mode, int(use_pd), _ptr(q), _ptr(qd), _ptr(tau_or_action), K, lp, cp,
+                                                            _ptr(W), _ptr(g_out), _ptr(g_in), _ptr(g_W), _ptr(g_par), st),
+                    "step_wrench_vjp_device")
+
     # ---- forward kinematics and linear point Jacobians (DESIGN.md section 7.13) ----
     @staticmethod
     def _points(links, local):
