@@ -372,6 +372,44 @@ int tds_b200_point_motion_vjp_host(tds_b200_sim* sim, const double* q, const dou
                                    const double* local, const double* G_J, const double* G_vel, const double* G_acc, double* g_q,
                                    double* g_qd, double* g_qdd);
 
+/* ---- joint-torque and energy regressors of the inertial parameters (DESIGN.md section 7.19) -----------------------------------------
+ * tau = Y(q, qd, qdd) pi exactly, with pi [n_pi], n_pi = tds_b200_param_count(sim) - 2: column j is physical-parameter id j + 2 (friction and
+ * restitution do not enter inverse dynamics).  Body b (0 = the floating base, i + 1 = link i): columns 10 b + [m, m c_x, m c_y, m c_z,
+ * I_xx, I_xy, I_xz, I_yy, I_yz, I_zz], the barycentric parameters of the body: c the centre of mass in the body frame (the frame of the
+ * model's com and inertia), I the inertia about the BODY-FRAME ORIGIN in body axes, I = I_com + m (|c|^2 1 - c c^T).  A fixed base's ten
+ * columns are zero.  Link i: column 10 (n_links + 1) + 2 i its joint stiffness, the next its damping, as in the parameter ids.
+ *   Y [n_qd x n_pi]: at the fp32-rounded q, qd and qdd (qd or qdd may be NULL, meaning zero: Y(q, qd, 0) is the bias regressor, Y(q, 0, 0)
+ *     the gravity regressor), Y pi = tds_b200_inverse_dynamics_* at the same inputs (floating base: rows 0..5 the base wrench in the base
+ *     frame); the stiffness columns hold q (the axis-angle vector of a spherical joint), the damping columns qd.
+ *   yT [n_pi]: the kinetic energy T = yT . pi = sum_b 1/2 v_b^T I_b v_b = 1/2 qd^T M qd with M of tds_b200_mass_matrix_*.
+ *   yV [n_pi]: the potential energy V = yV . pi = -sum_b g . (m_b x_com,b) (world coordinates) + 1/2 k q^2 (1/2 k |axis-angle|^2 for a
+ *     spherical joint); the damping columns are zero.
+ * All fp64; installed physical parameters do not enter (the outputs are bit-identical with or without a set); every entry of a live
+ * environment is written, zeros included.  tds_b200.model.inertial_parameters gives pi of the model or of a parameter set.  Argument
+ * checks -> -1: NULL q; no output or no cotangent; m < 1 or every tangent NULL; no cotangent output.
+ *   device: q [n_q][n_stride], qd and qdd [n_qd][n_stride] fp32 as tds_b200_step_device; Y [n_qd * n_pi][n_stride] (entry (r, c) at row
+ *           r * n_pi + c), yT and yV [n_pi][n_stride] fp64.  Asynchronous on `stream`.
+ *   host:   q [n][n_q], qd and qdd [n][n_qd] fp64 (rounded to fp32); Y [n][n_qd][n_pi], yT and yV [n][n_pi].  Synchronous.
+ * _jvp: the outputs' derivatives along m tangents of q, qd and qdd (each may be NULL: zero, not all), one lane per (environment, tangent)
+ *   of the dual-number instance, in chunks as tds_b200_step_jvp_*; NULL outputs are skipped.  Device t_q [n_q * m][n_stride], t_qd and
+ *   t_qdd [n_qd * m][n_stride], t_Y [n_qd * n_pi * m][n_stride], t_yT and t_yV [n_pi * m][n_stride] (entry (r, j) at (r * m + j) *
+ *   n_stride + e); host t_q [n][n_q][m], t_qd and t_qdd [n][n_qd][m], t_Y [n][n_qd * n_pi][m], t_yT and t_yV [n][n_pi][m].
+ * _vjp: g_x[c] = <G, d(Y | yT | yV)/dx_c> for x = q, qd, qdd, for cotangents G_Y, G_yT, G_yV in the outputs' layouts (NULL: zero, not
+ *   all): the JVP along the n_q + 2 n_qd identity tangents contracted with G on the device, in chunks of directions within 1 GB.  Any of
+ *   g_q, g_qd, g_qdd may be NULL, not all.  Device g_q [n_q][n_stride], g_qd and g_qdd [n_qd][n_stride] fp64 (asynchronous); host g_q
+ *   [n][n_q], g_qd and g_qdd [n][n_qd] (synchronous). */
+int tds_b200_regressor_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, double* Y, double* yT, double* yV,
+                              void* stream);
+int tds_b200_regressor_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, double* Y, double* yT, double* yV);
+int tds_b200_regressor_jvp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, int m, const double* t_q,
+                                  const double* t_qd, const double* t_qdd, double* t_Y, double* t_yT, double* t_yV, void* stream);
+int tds_b200_regressor_jvp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, int m, const double* t_q,
+                                const double* t_qd, const double* t_qdd, double* t_Y, double* t_yT, double* t_yV);
+int tds_b200_regressor_vjp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, const double* G_Y,
+                                  const double* G_yT, const double* G_yV, double* g_q, double* g_qd, double* g_qdd, void* stream);
+int tds_b200_regressor_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, const double* G_Y,
+                                const double* G_yT, const double* G_yV, double* g_q, double* g_qd, double* g_qdd);
+
 /* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
  * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
  * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,

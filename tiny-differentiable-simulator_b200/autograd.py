@@ -53,6 +53,10 @@ step_wrench(sim, q, qd, tau_or_action, links, local, W, mode=MODE_FULL, use_pd=F
 environment at every point of a point table (DESIGN.md section 7.18), on the world-frame kernel at the simulator's precision, with a
 backward rule (BatchSim.step_wrench_vjp_device: float32 q.grad, qd.grad, tau_or_action.grad, W.grad, float64 params.grad) and a
 forward-mode rule (BatchSim.step_wrench_jvp_device).
+
+regressor(sim, q, qd=None, qdd=None) is the joint-torque regressor Y and the energy regressors yT, yV of the inertial parameters (float64,
+DESIGN.md section 7.19) with a backward rule (BatchSim.regressor_vjp_device: float32 q.grad, qd.grad, qdd.grad) and a forward-mode rule
+(BatchSim.regressor_jvp_device).
 """
 import torch
 
@@ -922,3 +926,88 @@ def step_wrench(sim, q, qd, tau_or_action, links, local, W, mode=MODE_FULL, use_
                                tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
         raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
     return _StepWrench.apply(sim, int(mode), bool(use_pd), lk, lc, q, qd, tau_or_action, W, params)
+
+
+def _reg_outputs(sim, Y, yT, yV):
+    """Device outputs [rows, n_stride] of the regressors -> (Y [n, n_qd, n_pi], yT [n, n_pi], yV [n, n_pi])."""
+    n, nd, npi = sim.n_envs, sim.n_qd, sim.n_pi
+    return (Y[:nd * npi, :n].t().reshape(n, nd, npi).contiguous(), yT[:npi, :n].t().contiguous(), yV[:npi, :n].t().contiguous())
+
+
+def _reg_buffers(sim, device):
+    z = lambda rows: torch.zeros((max(rows, 1), sim.n_stride), dtype=torch.float64, device=device)
+    return z(sim.n_qd * sim.n_pi), z(sim.n_pi), z(sim.n_pi)
+
+
+class _Regressor(torch.autograd.Function):
+    @staticmethod
+    def forward(sim, q, qd, qdd):
+        ns = sim.n_stride
+        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
+        Y, yT, yV = _reg_buffers(sim, q.device)
+        _on_side_stream(q.device, lambda st: sim.regressor_device(qs, qds, qdds, Y, yT, yV, stream=st), (qs, qds, qdds, Y, yT, yV))
+        return _reg_outputs(sim, Y, yT, yV)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        sim, q, qd, qdd = inputs
+        ns = sim.n_stride
+        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
+        ctx.sim, ctx.has = sim, (qd is not None, qdd is not None)
+        ctx.save_for_backward(qs, *(t if t is not None else qs for t in (qds, qdds)))
+        ctx.jvp_inputs = (qs, qds, qdds)
+
+    @staticmethod
+    def backward(ctx, gY, gT, gV):
+        sim = ctx.sim
+        has_qd, has_qdd = ctx.has
+        qs, qds, qdds = ctx.saved_tensors
+        qds, qdds = (qds if has_qd else None), (qdds if has_qdd else None)
+        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+        dev = qs.device
+
+        def cot(g, rows):
+            return _soa(torch.zeros((n, rows), dtype=torch.float64, device=dev) if g is None else g.reshape(n, rows), ns, torch.float64)
+        G_Y, G_yT, G_yV = cot(gY, nd * sim.n_pi), cot(gT, sim.n_pi), cot(gV, sim.n_pi)
+        z = lambda rows: torch.zeros((max(rows, 1), ns), dtype=torch.float64, device=dev)
+        g_q, g_qd, g_qdd = z(sim.n_q), (z(nd) if has_qd else None), (z(nd) if has_qdd else None)
+        _on_side_stream(dev, lambda st: sim.regressor_vjp_device(qs, qds, qdds, G_Y, G_yT, G_yV, g_q, g_qd, g_qdd, stream=st),
+                        (qs, qds, qdds, G_Y, G_yT, G_yV, g_q, g_qd, g_qdd))
+        out = lambda t, rows: None if t is None else t[:rows, :n].t().to(torch.float32).contiguous()
+        return None, out(g_q, sim.n_q), out(g_qd, nd), out(g_qdd, nd)
+
+    @staticmethod
+    def jvp(ctx, _sim, t_q, t_qd, t_qdd):
+        with torch._C._DisableFuncTorch():
+            return _Regressor._jvp(ctx, _plain(t_q), _plain(t_qd), _plain(t_qdd))
+
+    @staticmethod
+    def _jvp(ctx, t_q, t_qd, t_qdd):
+        sim = ctx.sim
+        has_qd, has_qdd = ctx.has
+        qs, qds, qdds = (_plain(t) for t in ctx.jvp_inputs)
+        ns = sim.n_stride
+        tq = _soa_opt(t_q, ns, torch.float64)
+        tqd = _soa_opt(t_qd if has_qd else None, ns, torch.float64)
+        tqdd = _soa_opt(t_qdd if has_qdd else None, ns, torch.float64)
+        t_Y, t_yT, t_yV = _reg_buffers(sim, qs.device)
+        if any(t is not None for t in (tq, tqd, tqdd)):
+            _on_side_stream(qs.device, lambda st: sim.regressor_jvp_device(qs, qds, qdds, 1, tq, tqd, tqdd, t_Y, t_yT, t_yV, stream=st),
+                            (qs, qds, qdds, tq, tqd, tqdd, t_Y, t_yT, t_yV))
+        return _reg_outputs(sim, t_Y, t_yT, t_yV)
+
+
+def regressor(sim, q, qd=None, qdd=None):
+    """The regressors of the inertial parameters of every environment of `sim` (a BatchSim), DESIGN.md section 7.19, in fp64 at the
+    fp32-rounded inputs: (Y [n_envs, n_qd, n_pi], yT [n_envs, n_pi], yV [n_envs, n_pi]) float64 with inverse_dynamics(sim, q, qd, qdd) =
+    Y @ pi, the kinetic energy 1/2 qd^T M qd = yT . pi and the potential energy yV . pi, for pi of tds_b200.model.inertial_parameters
+    (per body: mass, first moment m c and inertia about the body-frame origin; per joint: stiffness and damping; column names from
+    tds_b200.model.regressor_names).  q [n_envs, n_q], qd and qdd [n_envs, n_qd] float32 CUDA tensors (qd or qdd None: zero).  Installed
+    physical parameters do not enter.  Differentiable along q, qd and qdd in reverse mode (float32 gradients from the cotangents of all
+    three outputs) and forward mode."""
+    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
+        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
+    for name, t in (("qd", qd), ("qdd", qdd)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or tuple(t.shape) != (sim.n_envs, sim.n_qd)):
+            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, n_qd] is expected")
+    return _Regressor.apply(sim, q, qd, qdd)

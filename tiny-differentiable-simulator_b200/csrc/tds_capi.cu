@@ -87,6 +87,11 @@ extern "C" int tds_launch_wrench_jvp(const DevModel* M, const SimParams* P, cons
 extern "C" int tds_launch_point_motion(const DevModel* M, const StepIO* io, const TdsMotCall* mc, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_point_motion_jvp(const DevModel* M, const StepIO* io, const TdsMotCall* mc, const double* t_in, int m, int n_dirs,
                                            char* gscratch, cudaStream_t stream);
+// joint-torque and energy regressors of the inertial parameters, and their Jacobian-vector products (tds_regressor.cu)
+extern "C" int tds_launch_regressor(const DevModel* M, const SimParams* P, const StepIO* io, const TdsRegCall* out, char* gscratch,
+                                    cudaStream_t stream);
+extern "C" int tds_launch_regressor_jvp(const DevModel* M, const SimParams* P, const StepIO* io, const TdsRegCall* out, const double* t_in,
+                                        int m, int n_dirs, char* gscratch, cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
@@ -908,17 +913,19 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
 
 // what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14, 7.16 and 7.17,
 // or the step with its contact records (section 7.15)
-enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench };
+enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, regressor };
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
 // inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
 // (t_in = the q tangents, t_par unused); inv: t_in = the q | qd | qdd tangents (qd and qdd in the step's qd and tau_or_action);
 // contacts: as step, with the rows q' | qd' | records; centroidal: t_in = the q | qd tangents (qd in the step's qd), outputs `cen`;
 // motion: t_in = the q | qd | qdd tangents (qd and qdd as for inv), the point table and outputs `mot`; wrench: as step, with the point
-// table, wrenches and wrench tangents `ext`
+// table, wrenches and wrench tangents `ext`; regressor: t_in = the q | qd | qdd tangents (as for inv), Y in jac and the
+// energy outputs `reg`
 struct JvpTangents {
   const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr;
   const TdsCenCall* cen = nullptr; const TdsMotCall* mot = nullptr; const TdsExtCall* ext = nullptr;
+  const TdsRegCall* reg = nullptr;
 };
 
 // the installed physical parameters as a launch argument in *pmv, or NULL without any
@@ -999,6 +1006,7 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
           rc = tds_launch_wrench_jvp(&s->dm_ad, &s->P, &s->E, &io, pm, jv->ext, jv->t_in, jv->t_par, jv->m, mode, use_pd, nd, s->jac_scratch,
                                      sm);
           break;
+        case Query::regressor: rc = tds_launch_regressor_jvp(&s->dm_ad, &s->P, &io, jv->reg, jv->t_in, jv->m, nd, s->jac_scratch, sm); break;
       }
     }
     if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
@@ -1810,6 +1818,150 @@ int tds_b200_point_motion_vjp_host(tds_b200_sim* s, const double* q, const doubl
   double* g_d = s->vjp_g + R.all() * ns;
   CUDA_TRY(put_parts<double>(s->vjp_g, {{G_J, R.J}, {G_vel, R.vel}, {G_acc, R.acc}}, n, ns, s->stream));
   if (int rc = mot_vjp_run(s, s->q, qd_d, qdd_d, K, links, local, s->vjp_g, g_d, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- joint-torque and energy regressors of the inertial parameters (DESIGN.md section 7.19): the REG instances of the world-frame kernel
+// (tds_regressor.cu).  The inputs q | qd | qdd are those of inverse dynamics (inv_n_in, put_inv_inputs). ----------------------------------
+// rows of the outputs Y | yT | yV, with n_pi = 12 n_links + 10 parameter columns (the physical-parameter ids from 2 on)
+struct RegRows { size_t Y, yT, yV; size_t all() const { return Y + yT + yV; } };
+static RegRows reg_rows(const tds_b200_sim* s) {
+  const size_t n_pi = (size_t)12 * s->dm[0].n_links + 10;
+  return RegRows{(size_t)s->dm[0].n_qd * n_pi, n_pi, n_pi};
+}
+
+// fp64 Y [n_qd * n_pi][ns] and out->yT, out->yV [n_pi][ns] (each may be NULL) from q [n_q][ns], qd and qdd [n_qd][ns] fp32 (either NULL:
+// zero; installed parameters do not enter)
+static int reg_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* Y, const TdsRegCall* out, cudaStream_t sm) {
+  return value_run(s, "regressor", q, qd, qdd, Y, [&](const StepIO* io, const ParMap*) {
+    return tds_launch_regressor(&s->dm_m, &s->P, io, out, s->jac_scratch, sm);
+  });
+}
+
+// m tangents t_in [(n_q + 2 n_qd) * m][ns] (q | qd | qdd, contiguous) -> the outputs' columns t_Y [R.Y * m][ns], out->yT and out->yV
+// [n_pi * m][ns], through the Jacobian's chunk loop
+static int reg_jvp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const TdsRegCall* out, int m, const double* t_in,
+                       double* t_Y, cudaStream_t sm) {
+  JvpTangents jv{t_in, nullptr, m, Query::regressor};
+  jv.reg = out;
+  return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, qdd, t_Y, sm, false, &jv);
+}
+
+// g_in [n_q + 2 n_qd][ns] (q | qd | qdd, contiguous) = <G, d(Y | yT | yV)>, G [rows][ns] concatenated
+static int reg_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const double* G, double* g_in, cudaStream_t sm) {
+  const RegRows R = reg_rows(s);
+  const size_t ns = s->ns;
+  return vjp_by_eye(s, "regressor", inv_n_in(s), R.all(), G, g_in, nullptr, sm, [&](int nd, const double* t_in, const double*, double* dO) {
+    const TdsRegCall out{dO + R.Y * nd * ns, dO + (R.Y + R.yT) * nd * ns};
+    return reg_jvp_run(s, q, qd, qdd, &out, nd, t_in, dO, sm);
+  });
+}
+
+static int reg_check(tds_b200_sim* s, const void* q, const void* Y, const void* yT, const void* yV) {
+  if (!s || !q || (!Y && !yT && !yV)) return -1;
+  return 0;
+}
+
+int tds_b200_regressor_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* Y, double* yT, double* yV,
+                              void* stream) {
+  if (int rc = reg_check(s, q, Y, yT, yV)) return rc;
+  const TdsRegCall out{yT, yV};
+  return reg_run(s, q, qd, qdd, Y, &out, (cudaStream_t)stream);
+}
+
+int tds_b200_regressor_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, double* Y, double* yT, double* yV) {
+  if (int rc = reg_check(s, q, Y, yT, yV)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const RegRows R = reg_rows(s);
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (R.all() + 1) * ns));
+  double* d = s->jac_dev;
+  const TdsRegCall out{yT ? d + R.Y * ns : nullptr, yV ? d + (R.Y + R.yT) * ns : nullptr};
+  if (int rc = reg_run(s, s->q, qd_d, qdd_d, Y ? d : nullptr, &out, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{Y, R.Y}, {yT, R.yT}, {yV, R.yV}}, d, n, ns, s->stream));
+  return 0;
+}
+
+static int reg_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_qd, const void* t_qdd, const void* t_Y,
+                         const void* t_yT, const void* t_yV) {
+  if (int rc = reg_check(s, q, t_Y, t_yT, t_yV)) return rc;
+  if (m < 1 || (!t_q && !t_qd && !t_qdd)) return -1;
+  return 0;
+}
+
+int tds_b200_regressor_jvp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int m, const double* t_q,
+                                  const double* t_qd, const double* t_qdd, double* t_Y, double* t_yT, double* t_yV, void* stream) {
+  if (int rc = reg_jvp_check(s, q, m, t_q, t_qd, t_qdd, t_Y, t_yT, t_yV)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the kernel reads the q | qd | qdd tangents as one array
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (size_t)inv_n_in(s) * m * s->ns));
+  double* tin = s->jac_dev;
+  CUDA_TRY(put_parts_d2d<double>(tin, {{t_q, n_q * m}, {t_qd, nd * m}, {t_qdd, nd * m}}, s->ns, sm));
+  const TdsRegCall out{t_yT, t_yV};
+  return reg_jvp_run(s, q, qd, qdd, &out, m, tin, t_Y, sm);
+}
+
+int tds_b200_regressor_jvp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, int m, const double* t_q,
+                                const double* t_qd, const double* t_qdd, double* t_Y, double* t_yT, double* t_yV) {
+  if (int rc = reg_jvp_check(s, q, m, t_q, t_qd, t_qdd, t_Y, t_yT, t_yV)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  const RegRows R = reg_rows(s);
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; q | qd | qdd (contiguous, zero where NULL), then the outputs
+  const size_t ti = (size_t)inv_n_in(s) * m;
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + R.all() * m + 1) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + ti * ns;
+  CUDA_TRY(put_parts<double>(d, {{t_q, n_q * m}, {t_qd, nd * m}, {t_qdd, nd * m}}, n, ns, s->stream));
+  const TdsRegCall out{t_yT ? to_d + R.Y * m * ns : nullptr, t_yV ? to_d + (R.Y + R.yT) * m * ns : nullptr};
+  if (int rc = reg_jvp_run(s, s->q, qd_d, qdd_d, &out, m, d, t_Y ? to_d : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{t_Y, R.Y * m}, {t_yT, R.yT * m}, {t_yV, R.yV * m}}, to_d, n, ns, s->stream));
+  return 0;
+}
+
+static int reg_vjp_check(tds_b200_sim* s, const void* q, const void* G_Y, const void* G_yT, const void* G_yV, const void* g_q,
+                         const void* g_qd, const void* g_qdd) {
+  if (int rc = reg_check(s, q, G_Y, G_yT, G_yV)) return rc;
+  if (!g_q && !g_qd && !g_qdd) return -1;
+  return 0;
+}
+
+int tds_b200_regressor_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const double* G_Y, const double* G_yT,
+                                  const double* G_yV, double* g_q, double* g_qd, double* g_qdd, void* stream) {
+  if (int rc = reg_vjp_check(s, q, G_Y, G_yT, G_yV, g_q, g_qd, g_qdd)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  const RegRows R = reg_rows(s);
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the concatenated cotangent Y | yT | yV (zero where a part is NULL), then g_q | g_qd | g_qdd as one array for the contraction
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (R.all() + inv_n_in(s)) * s->ns));
+  double* g_d = s->vjp_g + R.all() * s->ns;
+  CUDA_TRY(put_parts_d2d<double>(s->vjp_g, {{G_Y, R.Y}, {G_yT, R.yT}, {G_yV, R.yV}}, s->ns, sm));
+  if (int rc = reg_vjp_run(s, q, qd, qdd, s->vjp_g, g_d, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}}, g_d, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_regressor_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, const double* G_Y, const double* G_yT,
+                                const double* G_yV, double* g_q, double* g_qd, double* g_qdd) {
+  if (int rc = reg_vjp_check(s, q, G_Y, G_yT, G_yV, g_q, g_qd, g_qdd)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  const RegRows R = reg_rows(s);
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  // G (Y | yT | yV, zero where a part is NULL) | g_q | g_qd | g_qdd
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (R.all() + inv_n_in(s)) * ns));
+  double* g_d = s->vjp_g + R.all() * ns;
+  CUDA_TRY(put_parts<double>(s->vjp_g, {{G_Y, R.Y}, {G_yT, R.yT}, {G_yV, R.yV}}, n, ns, s->stream));
+  if (int rc = reg_vjp_run(s, s->q, qd_d, qdd_d, s->vjp_g, g_d, s->stream)) return rc;
   CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}}, g_d, n, ns, s->stream));
   return 0;
 }

@@ -70,7 +70,11 @@ struct ExtPts {
   double local[3 * TDS_MAX_KIN_POINTS];
 };
 template <typename B> struct ExtArg : B { ExtPts ext; };
-template <bool PAR, bool JV = false, bool KIN = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false> struct ParArg { typedef NoPar type; };
+// kernel argument of the regressor instances (REG, DESIGN.md section 7.19): the argument of the same instance without REG (B = NoPar or
+// NoParJvp) and the energy regressors' outputs yT and yV (each may be null)
+template <typename B> struct RegArg : B { double* yT; double* yV; };
+template <bool PAR, bool JV = false, bool KIN = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false,
+          bool REG = false> struct ParArg { typedef NoPar type; };
 template <> struct ParArg<true, false> { typedef ParMap type; };
 template <> struct ParArg<false, true> { typedef NoParJvp type; };
 template <> struct ParArg<true, true> { typedef ParMapJvp type; };
@@ -84,6 +88,7 @@ template <bool PAR, bool JV> struct ParArg<PAR, JV, false, false, true> { typede
 template <> struct ParArg<false, false, false, false, false, true> { typedef MotArg<KinArg> type; };
 template <> struct ParArg<false, true, false, false, false, true> { typedef MotArg<KinArgJvp> type; };
 template <bool PAR, bool JV> struct ParArg<PAR, JV, false, false, false, false, true> { typedef ExtArg<typename ParArg<PAR, JV>::type> type; };
+template <bool JV> struct ParArg<false, JV, false, false, false, false, false, true> { typedef RegArg<typename ParArg<false, JV>::type> type; };
 
 // CF, dual instances: the part of a record's dual number they write - the tangent (d).  The host build of the tests also compiles them
 // with the value (v), for an fp64 value path of the records that central differences can resolve.
@@ -158,12 +163,20 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // (kinematics.hpp:132, pA = v x* I v - f_ext), and the floating base's points go into the base's bias force in the base frame.  Component r
 // of point k's wrench is input direction n_in_ad + 6k + r (JV instances: entry 6k + r of the tangent pm.ext.t_W).  Nothing else differs
 // from the step.
+// REG (with INV): the joint-torque regressor Y(q, qd, qdd) and the energy regressors yT(q, qd), yV(q) of the inertial parameters
+// (DESIGN.md section 7.19), launched as INV.  Column 10 b + c of body b (0: the floating base, i + 1: link i) is the unit barycentric
+// parameter c of [m, m c, I about the body origin] in body axes, column 10 (n_links + 1) + 2 i (+ 1) link i's stiffness (damping).  Pass 1
+// carries v_i and a_i as INV does; for each unit parameter it forms the rigid inertia r about O in world axes, f = r a_i + v_i x* (r v_i),
+// and writes S_j . f for every row j (zero off the chain of i), R_b^T f in a floating base's rows, 1/2 v_i . (r v_i) and -g . (h + m O).
+// Then the base's own columns (base frame) and the stiffness and damping columns.  Y [n_qd * n_pi] at io.jac, entry (r, c) at row
+// r * n_pi + c, yT and yV [n_pi] at pm.yT and pm.yV (each may be null); row k at out[k * ns + e] (fp64 instance) or its dual part at
+// out[(k * m + j) * ns + e] (JV instance).  Returns before pass 2.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
-          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false>
+          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false, bool REG = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
-                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF, CEN, MOT, EXT>::type pm = {}) {
+                 char* __restrict__ gscratch, const __grid_constant__ typename ParArg<PAR, JV, KIN, CF, CEN, MOT, EXT, REG>::type pm = {}) {
   extern __shared__ __align__(16) char smem_raw[];
   const int lane = threadIdx.x & 31;
   const int warp_in_blk = threadIdx.x >> 5;
@@ -517,6 +530,66 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
         if (pm.ext.link[k] == l) w = w + ext_wrench(k, R, p);
     return w;
   };
+  // REG: the number of parameter columns; row k of an output; the rigid inertia about O in world axes of unit parameter c of a body at
+  // world rotation R and position p (relative to O): the linear map of the rigid-inertia statements of pass 1 applied to a unit
+  // [m, m c, I about the body origin]
+  const int n_pi = 12 * n_links + 10;
+  auto reg_put = [&](double* o, size_t k, const RC& x) {
+    if constexpr (REG) {
+      if (!o || !live) return;
+      if constexpr (AD) o[(k * io.jac_n_in + jcol) * ns + e] = x.d;
+      else o[k * ns + e] = x;
+    }
+  };
+  auto reg_unit = [&](int c, const M3<RC>& R, const V3<RC>& p) -> Rbi<RC> {
+    Rbi<RC> r;
+    const V3<RC> z = v3<RC>(RC(0), RC(0), RC(0));
+    // I = s (u w^T + w u^T) + d 1
+    V3<RC> u = z, w = z;
+    RC s = RC(0), d = RC(0);
+    r.m = RC(0); r.h = z;
+    if (c == 0) { r.m = RC(1); r.h = p; u = p; w = p; s = RC(-0.5); d = dot(p, p); }   // m (|p|^2 1 - p p^T)
+    else if (c < 4) {                                                                    // 2 (p . h) 1 - p h^T - h p^T
+      r.h = c == 1 ? col_x(R) : (c == 2 ? col_y(R) : col_z(R));
+      u = p; w = r.h; s = RC(-1); d = RC(2) * dot(p, r.h);
+    } else {                                                                             // R E R^T, E the unit symmetric entry
+      const int a = c < 7 ? 0 : (c < 9 ? 1 : 2), b = c < 7 ? c - 4 : (c < 9 ? c - 6 : 2);
+      u = a == 0 ? col_x(R) : (a == 1 ? col_y(R) : col_z(R));
+      w = b == 0 ? col_x(R) : (b == 1 ? col_y(R) : col_z(R));
+      s = a == b ? RC(0.5) : RC(1);
+    }
+    r.I.xx = s * (u.x * w.x + w.x * u.x) + d; r.I.yy = s * (u.y * w.y + w.y * u.y) + d; r.I.zz = s * (u.z * w.z + w.z * u.z) + d;
+    r.I.xy = s * (u.x * w.y + w.x * u.y); r.I.xz = s * (u.x * w.z + w.x * u.z); r.I.yz = s * (u.y * w.z + w.y * u.z);
+    return r;
+  };
+  // REG: the ten columns of body b (0: the base, i + 1: link i) with velocity v and acceleration a, at rotation R and position p: the
+  // joint rows of link i's chain (l = i; l = -1: none) and of a floating base (S_j . f, R_b^T f), zeros elsewhere, and the energy rows
+  auto reg_body = [&](int b, int l, const M3<RC>& R, const V3<RC>& p, const Sv<RC>& v, const Sv<RC>& a, bool base_frame) {
+    if constexpr (REG) {
+      const V3<RC> g = v3<RC>(RC(P.gravity[0]), RC(P.gravity[1]), RC(P.gravity[2]));
+      for (int c = 0; c < 10; ++c) {
+        const int col = 10 * b + c;
+        const Rbi<RC> r = reg_unit(c, R, p);
+        const Sv<RC> rv = rbi_mul(r, v);
+        const Sv<RC> f = rbi_mul(r, a) + cross_mf(v, rv);
+        if (M.floating) {
+          const V3<RC> ft = base_frame ? f.top : mulT(Rb, f.top), fb = base_frame ? f.bot : mulT(Rb, f.bot);
+          const RC fr[6] = {ft.x, ft.y, ft.z, fb.x, fb.y, fb.z};
+          for (int k = 0; k < 6; ++k) reg_put(io.jac, (size_t)k * n_pi + col, fr[k]);
+        }
+        int anc = l;
+        for (int j = n_links - 1; j >= 0; --j) {   // links are ordered parent first: the chain of l, walked downwards
+          const bool on = j == anc;
+          if (on) anc = M.parent[j];
+          for (int cj = 0; cj < n_cols(j); ++cj)
+            reg_put(io.jac, (size_t)(M.qd_idx[j] + cj) * n_pi + col, on ? dot(S_col(j, cj), f) : RC(0));
+        }
+        reg_put(pm.yT, col, RC(0.5) * dot(v, rv));
+        const V3<RC> hw = base_frame ? mul(Rb, r.h) : r.h;
+        reg_put(pm.yV, col, -dot(g, hw + O * r.m));
+      }
+    }
+  };
   M3<RC> R_prev = Rb;
   V3<RC> p_prev = M.floating ? v3<RC>(RC(0), RC(0), RC(0)) : v3<RC>(-O.x, -O.y, -O.z);
   Sv<RA> v_prev;
@@ -710,6 +783,9 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       st6<RC>(A.ptr<RC>(M.x_link + i * LWD), ST, a);
       a_prev_inv = a;
     }
+    // (REG also runs INV's statements above, the model's tau included, and never writes that tau: putting them under !REG reorders
+    // four instructions of an existing INV instance)
+    if constexpr (REG) reg_body(i + 1, i, Ri, pi, v, a_prev_inv, false);
     if constexpr (MOT) {   // a_i as INV carries it (a branch point's over its rigid-inertia words), then the outputs of the points on i
       Sv<RC> a;
       if (fl & TDS_LF_PARENT_ADJ) a = a_prev_inv;
@@ -730,6 +806,37 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     R_prev = Ri; p_prev = pi; v_prev = v;
   }
   if constexpr (KIN || MOT) return;
+  if constexpr (REG) {
+    // the base's columns: its own f in the base frame (rows 0..5) on a floating base, zero on a fixed one
+    if (M.floating) {
+      Sv<RC> vb, ab;
+      vb.top = v3<RC>(qdv[0], qdv[ST], qdv[2 * ST]); vb.bot = v3<RC>(qdv[3 * ST], qdv[4 * ST], qdv[5 * ST]);
+      ab.top = mulT(Rb, a_base_inv.top); ab.bot = mulT(Rb, a_base_inv.bot);
+      reg_body(0, -1, m3_identity<RC>(), v3<RC>(RC(0), RC(0), RC(0)), vb, ab, true);
+    } else {
+      for (int c = 0; c < 10; ++c) {
+        for (int k = 0; k < n; ++k) reg_put(io.jac, (size_t)k * n_pi + c, RC(0));
+        reg_put(pm.yT, c, RC(0)); reg_put(pm.yV, c, RC(0));
+      }
+    }
+    // stiffness (q, or a spherical joint's axis-angle vector) and damping (qd) columns of link i: nonzero in its own rows only
+    for (int i = 0; i < n_links; ++i) {
+      const int col = 10 * (n_links + 1) + 2 * i, nc = n_cols(i), d0 = M.qd_idx[i];
+      RC sv[3] = {RC(0), RC(0), RC(0)};
+      if (M.flags[i] & TDS_LF_SPHERICAL) { const V3<RC> aa = axis_angle(i); sv[0] = aa.x; sv[1] = aa.y; sv[2] = aa.z; }
+      else if (nc > 0) sv[0] = qv[M.q_idx[i] * ST];
+      RC vk = RC(0);
+      for (int k = 0; k < n; ++k) {
+        const bool own = nc > 0 && k >= d0 && k < d0 + nc;
+        reg_put(io.jac, (size_t)k * n_pi + col, own ? sv[k - d0] : RC(0));
+        reg_put(io.jac, (size_t)k * n_pi + col + 1, own ? RC(qdv[k * ST]) : RC(0));
+      }
+      for (int c = 0; c < nc; ++c) vk += sv[c] * sv[c];
+      reg_put(pm.yT, col, RC(0)); reg_put(pm.yT, col + 1, RC(0));
+      reg_put(pm.yV, col, RC(0.5) * vk); reg_put(pm.yV, col + 1, RC(0));
+    }
+    return;
+  }
   if constexpr (INV) {
     for (int i = 0; i < n_links; ++i) {   // the stiffness and damping terms the ABA subtracts from tau
       const int fl = M.flags[i];

@@ -169,6 +169,10 @@ struct TdsMotCall {
   double* J; double* vel; double* acc;
 };
 
+// The energy outputs of one call of the regressor instances (tds_regressor.cu, DESIGN.md section 7.19): yT [n_pi][ns] and yV [n_pi][ns]
+// (each may be null; columns of an m-column block in the JVP).  Y itself goes to StepIO::jac.
+struct TdsRegCall { double* yT; double* yV; };
+
 // One call of the external-wrench instances (tds_wrench.cu, DESIGN.md section 7.18), as the C-ABI hands it to the launchers: the point
 // table as in TdsKinCall and the wrenches W [6K][ns] fp32 ([n; f] in world axes, row 6k + r) with, for the JVP, their tangents
 // t_W [6K * m][ns] fp64 (null: zero tangent)

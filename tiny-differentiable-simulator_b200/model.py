@@ -160,6 +160,53 @@ def set_param_values(model, ids, values):
     return m
 
 
+_REGRESSOR_COMPONENTS = ("m", "mcx", "mcy", "mcz", "Ixx", "Ixy", "Ixz", "Iyy", "Iyz", "Izz")
+
+
+def regressor_names(model):
+    """One name per column of the regressors (BatchSim.regressor_host, DESIGN.md section 7.19): "base.m", "base.mcx", ...,
+    "link<i>.Izz" (mass, first moment m c and inertia about the body-frame origin of each body), then "link<i>.stiffness",
+    "link<i>.damping".  Column j is physical-parameter id j + 2.  Host only."""
+    n_links = model_dims(model)["n_links"]
+    names = []
+    for b in range(n_links + 1):
+        body = "base" if b == 0 else f"link{b - 1}"
+        names += [f"{body}.{c}" for c in _REGRESSOR_COMPONENTS]
+    for i in range(n_links):
+        names += [f"link{i}.stiffness", f"link{i}.damping"]
+    return names
+
+
+def inertial_parameters(model, ids=None, values=None):
+    """The regressors' parameter vector pi (float64, DESIGN.md section 7.19): [n_pi] from the model's own values, or [n, n_pi] from a
+    per-environment set (ids, values [n, k]) laid out as BatchSim.set_physical_params takes it (the other parameters keep the model's
+    values).  Body b: [m, m c, I_com + m (|c|^2 1 - c c^T)] (xx, xy, xz, yy, yz, zz), c the centre of mass in the body frame; link i:
+    stiffness and damping rounded to fp32, as the step and inverse dynamics read them.  Host only."""
+    base = param_values(model)[2:]
+    if ids is None:
+        theta = base[None, :]
+    else:
+        vals = np.atleast_2d(np.asarray(values, dtype=np.float64))
+        theta = np.repeat(base[None, :], vals.shape[0], axis=0)
+        for k, i in enumerate(ids):
+            if int(i) < 2:
+                raise ValueError("friction / restitution do not enter the regressors")
+            theta[:, int(i) - 2] = vals[:, k]
+    n_links = model_dims(model)["n_links"]
+    pi = theta.copy()
+    for b in range(n_links + 1):
+        t = theta[:, 10 * b:10 * b + 10]
+        m, c = t[:, 0], t[:, 1:4]
+        cc = np.sum(c * c, axis=1)
+        out = pi[:, 10 * b:10 * b + 10]
+        out[:, 1:4] = m[:, None] * c
+        for k, (r, s) in enumerate(_INERTIA_SYM):
+            out[:, 4 + k] = t[:, 4 + k] + m * ((cc if r == s else 0.0) - c[:, r] * c[:, s])
+    j0 = 10 * (n_links + 1)
+    pi[:, j0:] = pi[:, j0:].astype(np.float32).astype(np.float64)
+    return pi[0] if ids is None else pi
+
+
 def save_model(path, model, meta=None):
     with open(path, "w") as f:
         json.dump({"layout": "tds_b200_model.h", "meta": meta or {}, "model": [float(v) for v in model]}, f)

@@ -817,6 +817,79 @@ class BatchSim:
         self._check(self._L.tds_b200_point_motion_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), K, lp, cp, _ptr(G_J), _ptr(G_vel),
                                                              _ptr(G_acc), _ptr(g_q), _ptr(g_qd), _ptr(g_qdd), st), "point_motion_vjp_device")
 
+    # ---- joint-torque and energy regressors of the inertial parameters (DESIGN.md section 7.19) ----
+    @property
+    def n_pi(self):
+        """Columns of the regressors: the physical-parameter ids from 2 on (tds_b200.model.regressor_names)."""
+        return 12 * self.n_links + 10
+
+    def regressor_host(self, q, qd=None, qdd=None):
+        """(Y [n, n_qd, n_pi], yT [n, n_pi], yV [n, n_pi]) float64 at the fp32-rounded q [n, n_q], qd and qdd [n, n_qd] (None: zero):
+        inverse_dynamics_host(q, qd, qdd) = Y @ pi, the kinetic energy 1/2 qd^T M qd = yT . pi and the potential energy yV . pi, for the
+        barycentric inertial parameters, stiffness and damping pi of tds_b200.model.inertial_parameters.  Installed physical parameters
+        do not enter."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        n = self.n_envs
+        Y, yT, yV = np.zeros((n, self.n_qd, self.n_pi)), np.zeros((n, self.n_pi)), np.zeros((n, self.n_pi))
+        self._check(self._L.tds_b200_regressor_host(self._h, _dp(q), _dp(qd), _dp(qdd), _dp(Y), _dp(yT), _dp(yV)), "regressor_host")
+        return Y, yT, yV
+
+    def regressor_device(self, q, qd, qdd, Y=None, yT=None, yV=None, stream=None):
+        """Device version of regressor_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd and qdd [n_qd, n_stride] (or
+        None); Y [n_qd * n_pi, n_stride] (entry (r, c) at row r * n_pi + c), yT and yV [n_pi, n_stride] float64 CUDA tensors (any may be
+        None, not all three).  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_regressor_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(Y), _ptr(yT), _ptr(yV), st),
+                    "regressor_device")
+
+    def regressor_jvp_host(self, q, qd=None, qdd=None, t_q=None, t_qd=None, t_qdd=None):
+        """Directional derivatives (dY [n, n_qd, n_pi, m], dyT [n, n_pi, m], dyV [n, n_pi, m]) of the outputs of regressor_host along m
+        tangents t_q [n, n_q, m], t_qd and t_qdd [n, n_qd, m] (each may be None, not all); tangents given as [n, dim] are m = 1 and drop
+        the last axis."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        if all(t is None for t in (t_q, t_qd, t_qdd)):
+            raise ValueError("at least one tangent is expected")
+        ts, m, single = self._tangents([(t_q, self.n_q), (t_qd, self.n_qd), (t_qdd, self.n_qd)])
+        n = self.n_envs
+        dY, dyT, dyV = np.zeros((n, self.n_qd, self.n_pi, m)), np.zeros((n, self.n_pi, m)), np.zeros((n, self.n_pi, m))
+        self._check(self._L.tds_b200_regressor_jvp_host(self._h, _dp(q), _dp(qd), _dp(qdd), m, *(_dp(t) for t in ts), _dp(dY), _dp(dyT),
+                                                        _dp(dyV)), "regressor_jvp_host")
+        return (dY[..., 0], dyT[..., 0], dyV[..., 0]) if single else (dY, dyT, dyV)
+
+    def regressor_jvp_device(self, q, qd, qdd, m, t_q, t_qd, t_qdd, t_Y=None, t_yT=None, t_yV=None, stream=None):
+        """Device version of regressor_jvp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None); t_q [n_q * m,
+        n_stride], t_qd and t_qdd [n_qd * m, n_stride] (each may be None, not all), t_Y [n_qd * n_pi * m, n_stride], t_yT and t_yV
+        [n_pi * m, n_stride] (any may be None, not all three) float64 CUDA tensors, entry (r, j) at row r * m + j.  Asynchronous."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_regressor_jvp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), int(m), _ptr(t_q), _ptr(t_qd), _ptr(t_qdd),
+                                                          _ptr(t_Y), _ptr(t_yT), _ptr(t_yV), st), "regressor_jvp_device")
+
+    def regressor_vjp_host(self, q, qd=None, qdd=None, G_Y=None, G_yT=None, G_yV=None):
+        """Cotangents G_Y [n, n_qd, n_pi], G_yT and G_yV [n, n_pi] (None: zero, not all three) -> (g_q [n, n_q], g_qd [n, n_qd], g_qdd
+        [n, n_qd]) = sum G * d(outputs)/dx."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        if G_Y is None and G_yT is None and G_yV is None:
+            raise ValueError("at least one cotangent is expected")
+        n = self.n_envs
+        G_Y = None if G_Y is None else self._inv_in(np.reshape(G_Y, (n, -1)), self.n_qd * self.n_pi, "G_Y")
+        G_yT = None if G_yT is None else self._inv_in(G_yT, self.n_pi, "G_yT")
+        G_yV = None if G_yV is None else self._inv_in(G_yV, self.n_pi, "G_yV")
+        g_q, g_qd, g_qdd = np.zeros((n, self.n_q)), np.zeros((n, self.n_qd)), np.zeros((n, self.n_qd))
+        self._check(self._L.tds_b200_regressor_vjp_host(self._h, _dp(q), _dp(qd), _dp(qdd), _dp(G_Y), _dp(G_yT), _dp(G_yV), _dp(g_q),
+                                                        _dp(g_qd), _dp(g_qdd)), "regressor_vjp_host")
+        return g_q, g_qd, g_qdd
+
+    def regressor_vjp_device(self, q, qd, qdd, G_Y, G_yT, G_yV, g_q, g_qd, g_qdd, stream=None):
+        """Device version of regressor_vjp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None), cotangents float64 in
+        the layouts of regressor_device (None: zero, not all three), g_q [n_q, n_stride], g_qd and g_qdd [n_qd, n_stride] float64 CUDA
+        tensors (each may be None, not all).  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_regressor_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(G_Y), _ptr(G_yT), _ptr(G_yV),
+                                                          _ptr(g_q), _ptr(g_qd), _ptr(g_qdd), st), "regressor_vjp_device")
+
     def jacobian_chunk(self):
         """Directions (Jacobian columns or JVP tangents) one launch of the dual-number step takes; more run in several launches."""
         return self._L.tds_b200_jacobian_chunk(self._h)
