@@ -58,6 +58,8 @@ regressor(sim, q, qd=None, qdd=None) is the joint-torque regressor Y and the ene
 DESIGN.md section 7.19) with a backward rule (BatchSim.regressor_vjp_device: float32 q.grad, qd.grad, qdd.grad) and a forward-mode rule
 (BatchSim.regressor_jvp_device).
 """
+from collections import namedtuple
+
 import torch
 
 from .sim import MODE_FD, MODE_FULL
@@ -80,6 +82,12 @@ def _plain(t):
     while t is not None and is_functorch_wrapped_tensor(t):
         t = get_unwrapped(t)
     return t
+
+
+def _check_params(sim, params):
+    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
+                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
+        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
 
 
 class _Step(torch.autograd.Function):
@@ -182,9 +190,7 @@ def step(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False, params=No
     for name, t in (("q", q), ("qd", qd), ("tau_or_action", tau_or_action)):
         if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or t.shape[0] != sim.n_envs):
             raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, dim] is expected")
-    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
-                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
-        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    _check_params(sim, params)
     return _Step.apply(sim, int(mode), bool(use_pd), q, qd, tau_or_action, params)
 
 
@@ -291,139 +297,127 @@ def rigid_step(world, state, force=None, steps=1, params=None):
     return _RigidStep.apply(world, int(steps), state, force, params)
 
 
-class _MassMatrix(torch.autograd.Function):
+_In = namedtuple("_In", "q qd qdd params")   # a query's inputs, and their tangents or gradients, in _Query.apply's order
+
+# What one dynamics query adds to _Query; p is the call's point table _Points, or None for a query without one:
+#   rows(sim, p)                  row counts of the output buffers [rows, n_stride] (float64)
+#   unpack(sim, p, *views)        views [n_envs, rows] of those buffers -> the outputs the user gets
+#   pack(sim, p, *grads)          the outputs' cotangents -> the device's cotangent buffers, the inverse of unpack
+#   value(sim, p, x, out, st)     the BatchSim value entry on the SoA inputs x (an _In; absent inputs None) and output buffers
+#   jvp(sim, p, x, t, out, st)    the m = 1 JVP entry along the SoA tangents t (an _In; None: zero)
+#   vjp(sim, p, x, G, g, st)      the VJP entry from the cotangent buffers G into the gradient buffers g (an _In; None: not computed)
+# The three entries keep their own argument orders; st is the side stream they run on.
+_QuerySpec = namedtuple("_QuerySpec", "rows unpack pack value jvp vjp")
+_Points = namedtuple("_Points", "links local K")   # sim._points(links, local): int32 [K], float64 [K, 3], K
+
+
+def _zeros(sim, rows, device):
+    return torch.zeros((max(rows, 1), sim.n_stride), dtype=torch.float64, device=device)
+
+
+def _cot(g, sim):
+    """Cotangent [n_envs, ...] -> [rows, n_stride] float64."""
+    return _soa(g.flatten(1), sim.n_stride, torch.float64)
+
+
+def _check_state(sim, q, qd=None, qdd=None):
+    for name, t, dim in (("q", q, "n_q"), ("qd", qd, "n_qd"), ("qdd", qdd, "n_qd")):
+        if t is None and name != "q":
+            continue
+        if t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or tuple(t.shape) != (sim.n_envs, getattr(sim, dim)):
+            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, {dim}] is expected")
+
+
+def _state_soa(sim, q, qd, qdd):
+    return [None if x is None else _soa(x, sim.n_stride, torch.float32) for x in (q, qd, qdd)]
+
+
+class _Query(torch.autograd.Function):
+    """The dynamics queries (mass_matrix, inverse_dynamics, centroidal, forward_kinematics, point_motion, regressor) as one Function over
+    a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
+    float64 output buffers, every C-ABI call ordered on a side stream, and the gradients as float32 (q, qd, qdd) and float64 (params).
+    An input the query does not take, or the call leaves out, is None and gets no gradient; a tangent on it is ignored.  With params
+    the forward installs their values, and the backward and forward-mode rule reinstall the values of this call (a later call of the
+    graph may have installed others)."""
+
     @staticmethod
-    def forward(sim, q, params):
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
+    def forward(spec, sim, points, q, qd, qdd, params):
         if params is not None:
             sim.set_physical_params(sim.param_ids, params.detach())
-        qs = _soa(q, ns, torch.float32)
-        M = torch.zeros((max(nd * nd, 1), ns), dtype=torch.float64, device=q.device)
-        _on_side_stream(q.device, lambda st: sim.mass_matrix_device(qs, M, stream=st), (qs, M))
-        return M[:nd * nd, :n].t().reshape(n, nd, nd).contiguous()
+        x = _state_soa(sim, q, qd, qdd)
+        rows = spec.rows(sim, points)
+        out = [_zeros(sim, r, q.device) for r in rows]
+        _on_side_stream(q.device, lambda st: spec.value(sim, points, _In(*x, None), out, st), (*x, *out))
+        return spec.unpack(sim, points, *(b[:r, :sim.n_envs].t() for b, r in zip(out, rows)))
 
     @staticmethod
     def setup_context(ctx, inputs, output):
-        sim, q, params = inputs
-        qs = _soa(q, sim.n_stride, torch.float32)
-        par = params.detach() if params is not None else None
-        ctx.sim, ctx.has_params = sim, params is not None
-        ctx.save_for_backward(qs, par if par is not None else qs)
-        ctx.jvp_inputs = (qs, par)
+        # (separate from forward so that torch.func transforms accept the Function; the SoA inputs are rebuilt here, the values
+        # forward used)
+        spec, sim, points, q, qd, qdd, params = inputs
+        x = _In(*_state_soa(sim, q, qd, qdd), None if params is None else params.detach())
+        ctx.spec, ctx.sim, ctx.points, ctx.has = spec, sim, points, [t is not None for t in x]
+        ctx.save_for_backward(*(x.q if t is None else t for t in x))
+        ctx.jvp_inputs = x
 
     @staticmethod
-    def backward(ctx, g):
-        sim = ctx.sim
-        qs, par = ctx.saved_tensors
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
-        G = _soa(g.reshape(n, nd * nd), ns, torch.float64)
-        g_q = torch.zeros((max(sim.n_q, 1), ns), dtype=torch.float64, device=g.device)
-        g_par = torch.zeros((par.shape[1], ns), dtype=torch.float64, device=g.device) if ctx.has_params else None
-        if ctx.has_params:
-            sim.set_physical_params(sim.param_ids, par)   # the values of this call
-        _on_side_stream(g.device, lambda st: sim.mass_matrix_vjp_device(qs, G, g_q, g_par, stream=st), (qs, G, g_q, g_par))
-        gq = g_q[:sim.n_q, :n].t().to(torch.float32)
-        gp = g_par[:, :n].t().contiguous() if ctx.has_params else None
-        return None, gq, gp
+    def backward(ctx, *grads):
+        spec, sim, p = ctx.spec, ctx.sim, ctx.points
+        x = _In(*(t if has else None for t, has in zip(ctx.saved_tensors, ctx.has)))
+        n, dev = sim.n_envs, x.q.device
+        G = spec.pack(sim, p, *grads)
+        dims = (sim.n_q, sim.n_qd, sim.n_qd, 0 if x.params is None else x.params.shape[1])
+        g = _In(*(None if t is None else _zeros(sim, d, dev) for t, d in zip(x, dims)))
+        if x.params is not None:
+            sim.set_physical_params(sim.param_ids, x.params)
+        _on_side_stream(dev, lambda st: spec.vjp(sim, p, x, G, g, st), (x.q, x.qd, x.qdd, *G, *g))
+        dtypes = (torch.float32, torch.float32, torch.float32, torch.float64)
+        return (None, None, None) + tuple(None if t is None else t[:d, :n].t().to(dt).contiguous() for t, d, dt in zip(g, dims, dtypes))
 
     @staticmethod
-    def jvp(ctx, _sim, t_q, t_params):
+    def jvp(ctx, _spec, _sim, _points, *tangents):
         with torch._C._DisableFuncTorch():
-            return _MassMatrix._jvp(ctx, _plain(t_q), _plain(t_params))
+            return _Query._jvp(ctx, *(_plain(t) for t in tangents))
 
     @staticmethod
-    def _jvp(ctx, t_q, t_params):
-        sim = ctx.sim
-        qs, par = (_plain(t) for t in ctx.jvp_inputs)
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
-        tq = None if t_q is None else _soa(t_q, ns, torch.float64)
-        tp = None if t_params is None or not ctx.has_params else _soa(t_params, ns, torch.float64)
-        t_M = torch.zeros((max(nd * nd, 1), ns), dtype=torch.float64, device=qs.device)
-        if tq is not None or tp is not None:
-            if ctx.has_params:
-                sim.set_physical_params(sim.param_ids, par)   # the values of this call
-            _on_side_stream(qs.device, lambda st: sim.mass_matrix_jvp_device(qs, 1, tq, tp, t_M, stream=st), (qs, tq, tp, t_M))
-        return t_M[:nd * nd, :n].t().reshape(n, nd, nd).contiguous()
+    def _jvp(ctx, *tangents):
+        spec, sim, p = ctx.spec, ctx.sim, ctx.points
+        x = _In(*(_plain(t) for t in ctx.jvp_inputs))
+        t = _In(*(None if v is None or xi is None else _soa(v, sim.n_stride, torch.float64) for v, xi in zip(tangents, x)))
+        rows = spec.rows(sim, p)
+        out = [_zeros(sim, r, x.q.device) for r in rows]
+        if any(v is not None for v in t):
+            if x.params is not None:
+                sim.set_physical_params(sim.param_ids, x.params)
+            _on_side_stream(x.q.device, lambda st: spec.jvp(sim, p, x, t, out, st), (x.q, x.qd, x.qdd, *t, *out))
+        return spec.unpack(sim, p, *(b[:r, :sim.n_envs].t() for b, r in zip(out, rows)))
+
+
+_MASS_MATRIX = _QuerySpec(
+    rows=lambda sim, p: [sim.n_qd * sim.n_qd],
+    unpack=lambda sim, p, M: M.reshape(sim.n_envs, sim.n_qd, sim.n_qd).contiguous(),
+    pack=lambda sim, p, gM: [_cot(gM, sim)],
+    value=lambda sim, p, x, out, st: sim.mass_matrix_device(x.q, *out, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.mass_matrix_jvp_device(x.q, 1, t.q, t.params, *out, stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.mass_matrix_vjp_device(x.q, *G, g.q, g.params, stream=st))
 
 
 def mass_matrix(sim, q, params=None):
     """The joint-space mass matrix M(q) of every environment of `sim` (a BatchSim): [n_envs, n_qd, n_qd] float64, from q [n_envs, n_q]
     float32 CUDA tensor (fp64 CRBA at the fp32-rounded q).  params: None, or a float64 CUDA tensor [n_envs, k] of values for the
     parameters installed by sim.set_physical_params (then also differentiated).  Differentiable in reverse and forward mode."""
-    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
-        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
-    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
-                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
-        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
-    return _MassMatrix.apply(sim, q, params)
+    _check_state(sim, q)
+    _check_params(sim, params)
+    return _Query.apply(_MASS_MATRIX, sim, None, q, None, None, params)
 
 
-class _InverseDynamics(torch.autograd.Function):
-    @staticmethod
-    def forward(sim, q, qd, qdd, params):
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
-        if params is not None:
-            sim.set_physical_params(sim.param_ids, params.detach())
-        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
-        tau = torch.zeros((max(nd, 1), ns), dtype=torch.float64, device=q.device)
-        _on_side_stream(q.device, lambda st: sim.inverse_dynamics_device(qs, qds, qdds, tau, stream=st), (qs, qds, qdds, tau))
-        return tau[:nd, :n].t().contiguous()
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        sim, q, qd, qdd, params = inputs
-        ns = sim.n_stride
-        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
-        par = params.detach() if params is not None else None
-        ctx.sim, ctx.has = sim, (qd is not None, qdd is not None, params is not None)
-        ctx.save_for_backward(qs, *(t if t is not None else qs for t in (qds, qdds, par)))
-        ctx.jvp_inputs = (qs, qds, qdds, par)
-
-    @staticmethod
-    def backward(ctx, g):
-        sim = ctx.sim
-        has_qd, has_qdd, has_par = ctx.has
-        qs, qds, qdds, par = ctx.saved_tensors
-        qds, qdds = (qds if has_qd else None), (qdds if has_qdd else None)
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
-        G = _soa(g, ns, torch.float64)
-        z = lambda rows: torch.zeros((max(rows, 1), ns), dtype=torch.float64, device=g.device)
-        g_q, g_qd, g_qdd = z(sim.n_q), (z(nd) if has_qd else None), (z(nd) if has_qdd else None)
-        g_par = z(par.shape[1]) if has_par else None
-        if has_par:
-            sim.set_physical_params(sim.param_ids, par)   # the values of this call
-        _on_side_stream(g.device, lambda st: sim.inverse_dynamics_vjp_device(qs, qds, qdds, G, g_q, g_qd, g_qdd, g_par, stream=st),
-                        (qs, qds, qdds, G, g_q, g_qd, g_qdd, g_par))
-        out = lambda t, rows, dt: None if t is None else t[:rows, :n].t().to(dt).contiguous()
-        return None, out(g_q, sim.n_q, torch.float32), out(g_qd, nd, torch.float32), out(g_qdd, nd, torch.float32), \
-            out(g_par, par.shape[1], torch.float64)
-
-    @staticmethod
-    def jvp(ctx, _sim, t_q, t_qd, t_qdd, t_params):
-        with torch._C._DisableFuncTorch():
-            return _InverseDynamics._jvp(ctx, _plain(t_q), _plain(t_qd), _plain(t_qdd), _plain(t_params))
-
-    @staticmethod
-    def _jvp(ctx, t_q, t_qd, t_qdd, t_params):
-        sim = ctx.sim
-        has_qd, has_qdd, has_par = ctx.has
-        qs, qds, qdds, par = (_plain(t) for t in ctx.jvp_inputs)
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
-        tq = _soa_opt(t_q, ns, torch.float64)
-        tqd = _soa_opt(t_qd if has_qd else None, ns, torch.float64)
-        tqdd = _soa_opt(t_qdd if has_qdd else None, ns, torch.float64)
-        tp = _soa_opt(t_params if has_par else None, ns, torch.float64)
-        t_tau = torch.zeros((max(nd, 1), ns), dtype=torch.float64, device=qs.device)
-        if any(t is not None for t in (tq, tqd, tqdd, tp)):
-            if has_par:
-                sim.set_physical_params(sim.param_ids, par)   # the values of this call
-            _on_side_stream(qs.device, lambda st: sim.inverse_dynamics_jvp_device(qs, qds, qdds, 1, tq, tqd, tqdd, tp, t_tau, stream=st),
-                            (qs, qds, qdds, tq, tqd, tqdd, tp, t_tau))
-        return t_tau[:nd, :n].t().contiguous()
-
-
-def _soa_opt(x, n_stride, dtype):
-    return None if x is None else _soa(x, n_stride, dtype)
+_INVERSE_DYNAMICS = _QuerySpec(
+    rows=lambda sim, p: [sim.n_qd],
+    unpack=lambda sim, p, tau: tau.contiguous(),
+    pack=lambda sim, p, gtau: [_cot(gtau, sim)],
+    value=lambda sim, p, x, out, st: sim.inverse_dynamics_device(x.q, x.qd, x.qdd, *out, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.inverse_dynamics_jvp_device(x.q, x.qd, x.qdd, 1, *t, *out, stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.inverse_dynamics_vjp_device(x.q, x.qd, x.qdd, *G, *g, stream=st))
 
 
 def inverse_dynamics(sim, q, qd, qdd=None, params=None):
@@ -435,98 +429,31 @@ def inverse_dynamics(sim, q, qd, qdd=None, params=None):
     acceleration qdd[0:6], with gravity rotated into the base frame - the textbook RNEA in the coordinates of mass_matrix, not the
     inverse of the reference's floating-base forward dynamics.  params: None, or a float64 CUDA tensor [n_envs, k] of values for the
     parameters installed by sim.set_physical_params (then also differentiated).  Differentiable in reverse and forward mode."""
-    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
-        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
-    for name, t in (("qd", qd), ("qdd", qdd)):
-        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or tuple(t.shape) != (sim.n_envs, sim.n_qd)):
-            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, n_qd] is expected")
-    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
-                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
-        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
-    return _InverseDynamics.apply(sim, q, qd, qdd, params)
+    _check_state(sim, q, qd, qdd)
+    _check_params(sim, params)
+    return _Query.apply(_INVERSE_DYNAMICS, sim, None, q, qd, qdd, params)
 
 
 _SYM = [0, 1, 2, 1, 3, 4, 2, 4, 5]   # [3, 3] from the components xx, xy, xz, yy, yz, zz
 
 
-def _cen_outputs(sim, com, A, bias):
-    """Device outputs [rows, n_stride] of the centroidal entries -> (m [n], c [n, 3], I_G [n, 3, 3], A [n, 6, n_qd], bias [n, 6])."""
-    n, nd = sim.n_envs, sim.n_qd
-    com = com[:, :n].t()
-    return (com[:, 0].contiguous(), com[:, 1:4].contiguous(), com[:, 4:10][:, _SYM].reshape(n, 3, 3).contiguous(),
-            A[:6 * nd, :n].t().reshape(n, 6, nd).contiguous(), bias[:, :n].t().contiguous())
+def _fold_sym(g):
+    """Cotangent [n, 3, 3] of a symmetric matrix read by _SYM -> [n, 6]: an off-diagonal component collects both of its entries."""
+    g = g.flatten(1)
+    return torch.stack([g[:, 0], g[:, 1] + g[:, 3], g[:, 2] + g[:, 6], g[:, 4], g[:, 5] + g[:, 7], g[:, 8]], dim=1)
 
 
-def _cen_buffers(sim, device):
-    z = lambda rows: torch.zeros((max(rows, 1), sim.n_stride), dtype=torch.float64, device=device)
-    return z(10), z(6 * sim.n_qd), z(6)
-
-
-class _Centroidal(torch.autograd.Function):
-    @staticmethod
-    def forward(sim, q, qd, params):
-        ns = sim.n_stride
-        if params is not None:
-            sim.set_physical_params(sim.param_ids, params.detach())
-        qs, qds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32)
-        com, A, bias = _cen_buffers(sim, q.device)
-        _on_side_stream(q.device, lambda st: sim.centroidal_device(qs, qds, com, A, bias, stream=st), (qs, qds, com, A, bias))
-        return _cen_outputs(sim, com, A, bias)
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        sim, q, qd, params = inputs
-        ns = sim.n_stride
-        qs, qds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32)
-        par = params.detach() if params is not None else None
-        ctx.sim, ctx.has = sim, (qd is not None, params is not None)
-        ctx.save_for_backward(qs, *(t if t is not None else qs for t in (qds, par)))
-        ctx.jvp_inputs = (qs, qds, par)
-
-    @staticmethod
-    def backward(ctx, g_m, g_c, g_I, g_A, g_bias):
-        sim = ctx.sim
-        has_qd, has_par = ctx.has
-        qs, qds, par = ctx.saved_tensors
-        qds = qds if has_qd else None
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
-        # I_G's symmetric entries are read from the six components: an off-diagonal component collects both of its entries
-        gI = g_I.reshape(n, 9).to(torch.float64)
-        gIc = torch.stack([gI[:, 0], gI[:, 1] + gI[:, 3], gI[:, 2] + gI[:, 6], gI[:, 4], gI[:, 5] + gI[:, 7], gI[:, 8]], dim=1)
-        G_com = _soa(torch.cat([g_m.reshape(n, 1).to(torch.float64), g_c.to(torch.float64), gIc], dim=1), ns, torch.float64)
-        G_A = _soa(g_A.reshape(n, 6 * nd), ns, torch.float64)
-        G_bias = _soa(g_bias, ns, torch.float64)
-        z = lambda rows: torch.zeros((max(rows, 1), ns), dtype=torch.float64, device=qs.device)
-        g_q, g_qd = z(sim.n_q), (z(nd) if has_qd else None)
-        g_par = z(par.shape[1]) if has_par else None
-        if has_par:
-            sim.set_physical_params(sim.param_ids, par)   # the values of this call
-        _on_side_stream(qs.device, lambda st: sim.centroidal_vjp_device(qs, qds, G_com, G_A, G_bias, g_q, g_qd, g_par, stream=st),
-                        (qs, qds, G_com, G_A, G_bias, g_q, g_qd, g_par))
-        out = lambda t, rows, dt: None if t is None else t[:rows, :n].t().to(dt).contiguous()
-        return None, out(g_q, sim.n_q, torch.float32), out(g_qd, nd, torch.float32), out(g_par, par.shape[1], torch.float64)
-
-    @staticmethod
-    def jvp(ctx, _sim, t_q, t_qd, t_params):
-        with torch._C._DisableFuncTorch():
-            return _Centroidal._jvp(ctx, _plain(t_q), _plain(t_qd), _plain(t_params))
-
-    @staticmethod
-    def _jvp(ctx, t_q, t_qd, t_params):
-        sim = ctx.sim
-        has_qd, has_par = ctx.has
-        qs, qds, par = (_plain(t) for t in ctx.jvp_inputs)
-        ns = sim.n_stride
-        tq = _soa_opt(t_q, ns, torch.float64)
-        tqd = _soa_opt(t_qd if has_qd else None, ns, torch.float64)
-        tp = _soa_opt(t_params if has_par else None, ns, torch.float64)
-        t_com, t_A, t_bias = _cen_buffers(sim, qs.device)
-        if any(t is not None for t in (tq, tqd, tp)):
-            if has_par:
-                sim.set_physical_params(sim.param_ids, par)   # the values of this call
-            _on_side_stream(qs.device, lambda st: sim.centroidal_jvp_device(qs, qds, 1, tq, tqd, tp, t_com, t_A, t_bias, stream=st),
-                            (qs, qds, tq, tqd, tp, t_com, t_A, t_bias))
-        return _cen_outputs(sim, t_com, t_A, t_bias)
+# the com record [10, n_stride]: m, c, I_G xx xy xz yy yz zz
+_CENTROIDAL = _QuerySpec(
+    rows=lambda sim, p: [10, 6 * sim.n_qd, 6],
+    unpack=lambda sim, p, com, A, bias: (com[:, 0].contiguous(), com[:, 1:4].contiguous(),
+                                         com[:, 4:10][:, _SYM].reshape(sim.n_envs, 3, 3).contiguous(),
+                                         A.reshape(sim.n_envs, 6, sim.n_qd).contiguous(), bias.contiguous()),
+    pack=lambda sim, p, gm, gc, gI, gA, gbias: [_cot(torch.cat([gm[:, None], gc, _fold_sym(gI)], dim=1), sim), _cot(gA, sim),
+                                                _cot(gbias, sim)],
+    value=lambda sim, p, x, out, st: sim.centroidal_device(x.q, x.qd, *out, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.centroidal_jvp_device(x.q, x.qd, 1, t.q, t.qd, t.params, *out, stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.centroidal_vjp_device(x.q, x.qd, *G, g.q, g.qd, g.params, stream=st))
 
 
 def centroidal(sim, q, qd=None, params=None):
@@ -537,84 +464,23 @@ def centroidal(sim, q, qd=None, params=None):
     rate of h_G at qdd = 0, without gravity).  q [n_envs, n_q], qd [n_envs, n_qd] float32 CUDA tensors (qd None: zero).  params: None, or
     a float64 CUDA tensor [n_envs, k] of values for the parameters installed by sim.set_physical_params (then also differentiated).
     Differentiable in reverse and forward mode."""
-    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
-        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
-    if qd is not None and (qd.dtype != torch.float32 or not qd.is_cuda or qd.dim() != 2 or tuple(qd.shape) != (sim.n_envs, sim.n_qd)):
-        raise ValueError("qd: a float32 CUDA tensor [n_envs, n_qd] is expected")
-    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
-                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
-        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
-    return _Centroidal.apply(sim, q, qd, params)
+    _check_state(sim, q, qd)
+    _check_params(sim, params)
+    return _Query.apply(_CENTROIDAL, sim, None, q, qd, None, params)
 
 
-def _kin_outputs(sim, K, xf, x, J):
-    """Device outputs [rows, n_stride] of the kinematics entries -> (R [n, n_links, 3, 3], p [n, n_links, 3], x [n, K, 3],
-    J [n, K, 3, n_qd])."""
-    n, nl, nd = sim.n_envs, sim.n_links, sim.n_qd
-    xf = xf[:nl * 12, :n].t().reshape(n, nl, 12)
-    return (xf[..., :9].reshape(n, nl, 3, 3).contiguous(), xf[..., 9:].contiguous(), x[:3 * K, :n].t().reshape(n, K, 3).contiguous(),
-            J[:3 * K * nd, :n].t().reshape(n, K, 3, nd).contiguous())
-
-
-def _kin_buffers(sim, K, device):
-    ns, nl, nd = sim.n_stride, sim.n_links, sim.n_qd
-    z = dict(dtype=torch.float64, device=device)
-    return torch.zeros((max(nl * 12, 1), ns), **z), torch.zeros((max(3 * K, 1), ns), **z), torch.zeros((max(3 * K * nd, 1), ns), **z)
-
-
-class _ForwardKinematics(torch.autograd.Function):
-    @staticmethod
-    def forward(sim, q, links, local):
-        lk, lc, K = sim._points(links, local)
-        qs = _soa(q, sim.n_stride, torch.float32)
-        xf, x, J = _kin_buffers(sim, K, q.device)
-        xo, Jo = (x, J) if K else (None, None)
-        _on_side_stream(q.device, lambda st: sim.kinematics_device(qs, lk, lc, xf, xo, Jo, stream=st), (qs, xf, x, J))
-        return _kin_outputs(sim, K, xf, x, J)
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        sim, q, links, local = inputs
-        lk, lc, K = sim._points(links, local)
-        qs = _soa(q, sim.n_stride, torch.float32)
-        ctx.sim, ctx.points = sim, (lk, lc, K)
-        ctx.save_for_backward(qs)
-        ctx.jvp_q = qs
-
-    @staticmethod
-    def backward(ctx, gR, gp, gx, gJ):
-        sim = ctx.sim
-        (qs,) = ctx.saved_tensors
-        lk, lc, K = ctx.points
-        n, ns, nl, nd = sim.n_envs, sim.n_stride, sim.n_links, sim.n_qd
-        dev = qs.device
-
-        def zero_if_none(g, shape):
-            return torch.zeros(shape, dtype=torch.float64, device=dev) if g is None else g.to(torch.float64)
-        gxf = torch.cat([zero_if_none(gR, (n, nl, 3, 3)).reshape(n, nl, 9), zero_if_none(gp, (n, nl, 3))], dim=2).reshape(n, nl * 12)
-        G_xf = _soa(gxf, ns, torch.float64)
-        G_x = _soa(zero_if_none(gx, (n, K, 3)).reshape(n, 3 * K), ns, torch.float64) if K else None
-        G_J = _soa(zero_if_none(gJ, (n, K, 3, nd)).reshape(n, 3 * K * nd), ns, torch.float64) if K and nd else None
-        g_q = torch.zeros((max(sim.n_q, 1), ns), dtype=torch.float64, device=dev)
-        _on_side_stream(dev, lambda st: sim.kinematics_vjp_device(qs, lk, lc, G_xf, G_x, G_J, g_q, stream=st), (qs, G_xf, G_x, G_J, g_q))
-        return None, g_q[:sim.n_q, :n].t().to(torch.float32), None, None
-
-    @staticmethod
-    def jvp(ctx, _sim, t_q, _links, _local):
-        with torch._C._DisableFuncTorch():
-            return _ForwardKinematics._jvp(ctx, _plain(t_q))
-
-    @staticmethod
-    def _jvp(ctx, t_q):
-        sim = ctx.sim
-        qs = _plain(ctx.jvp_q)
-        lk, lc, K = ctx.points
-        t_xf, t_x, t_J = _kin_buffers(sim, K, qs.device)
-        if t_q is not None:
-            tq = _soa(t_q, sim.n_stride, torch.float64)
-            xo, Jo = (t_x, t_J) if K else (None, None)
-            _on_side_stream(qs.device, lambda st: sim.kinematics_jvp_device(qs, lk, lc, 1, tq, t_xf, xo, Jo, stream=st), (qs, tq, t_xf, t_x, t_J))
-        return _kin_outputs(sim, K, t_xf, t_x, t_J)
+# xf [12 n_links, n_stride]: per link R row-major | p.  Without points (K = 0) the entries get None for x and J and their cotangents.
+_KINEMATICS = _QuerySpec(
+    rows=lambda sim, p: [12 * sim.n_links, 3 * p.K, 3 * p.K * sim.n_qd],
+    unpack=lambda sim, p, xf, x, J: (xf.reshape(sim.n_envs, sim.n_links, 4, 3)[:, :, :3].contiguous(),
+                                     xf.reshape(sim.n_envs, sim.n_links, 4, 3)[:, :, 3].contiguous(),
+                                     x.reshape(sim.n_envs, p.K, 3).contiguous(), J.reshape(sim.n_envs, p.K, 3, sim.n_qd).contiguous()),
+    pack=lambda sim, p, gR, gp, gx, gJ: [_cot(torch.cat([gR, gp[:, :, None]], dim=2), sim), _cot(gx, sim) if p.K else None,
+                                         _cot(gJ, sim) if p.K and sim.n_qd else None],
+    value=lambda sim, p, x, out, st: sim.kinematics_device(x.q, p.links, p.local, out[0], *(out[1:] if p.K else (None, None)), stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.kinematics_jvp_device(x.q, p.links, p.local, 1, t.q, out[0], *(out[1:] if p.K else (None, None)),
+                                                                stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.kinematics_vjp_device(x.q, p.links, p.local, *G, g.q, stream=st))
 
 
 def forward_kinematics(sim, q, links, local):
@@ -622,82 +488,18 @@ def forward_kinematics(sim, q, links, local):
     (fp64 at the fp32-rounded q), for the point table links [K] (-1: the base) / local [K, 3] (coordinates in the link's frame; both
     constants of the call): (R [n_envs, n_links, 3, 3], p [n_envs, n_links, 3], x [n_envs, K, 3], J [n_envs, K, 3, n_qd]), float64 world
     coordinates.  Differentiable along q in reverse mode (float32 q.grad from the cotangents of all four outputs) and forward mode."""
-    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
-        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
-    return _ForwardKinematics.apply(sim, q, links, local)
+    _check_state(sim, q)
+    return _Query.apply(_KINEMATICS, sim, _Points(*sim._points(links, local)), q, None, None, None)
 
 
-def _mot_outputs(sim, K, J, vel, acc):
-    """Device outputs [rows, n_stride] of the point-motion entries -> (J [n, K, 6, n_qd], vel [n, K, 6], acc [n, K, 6])."""
-    n, nd = sim.n_envs, sim.n_qd
-    return (J[:6 * K * nd, :n].t().reshape(n, K, 6, nd).contiguous(), vel[:6 * K, :n].t().reshape(n, K, 6).contiguous(),
-            acc[:6 * K, :n].t().reshape(n, K, 6).contiguous())
-
-
-def _mot_buffers(sim, K, device):
-    z = lambda rows: torch.zeros((max(rows, 1), sim.n_stride), dtype=torch.float64, device=device)
-    return z(6 * K * sim.n_qd), z(6 * K), z(6 * K)
-
-
-class _PointMotion(torch.autograd.Function):
-    @staticmethod
-    def forward(sim, q, qd, qdd, links, local):
-        lk, lc, K = sim._points(links, local)
-        ns = sim.n_stride
-        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
-        J, vel, acc = _mot_buffers(sim, K, q.device)
-        _on_side_stream(q.device, lambda st: sim.point_motion_device(qs, qds, qdds, lk, lc, J, vel, acc, stream=st), (qs, qds, qdds, J, vel, acc))
-        return _mot_outputs(sim, K, J, vel, acc)
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        sim, q, qd, qdd, links, local = inputs
-        ns = sim.n_stride
-        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
-        ctx.sim, ctx.points, ctx.has = sim, sim._points(links, local), (qd is not None, qdd is not None)
-        ctx.save_for_backward(qs, *(t if t is not None else qs for t in (qds, qdds)))
-        ctx.jvp_inputs = (qs, qds, qdds)
-
-    @staticmethod
-    def backward(ctx, gJ, gvel, gacc):
-        sim = ctx.sim
-        has_qd, has_qdd = ctx.has
-        qs, qds, qdds = ctx.saved_tensors
-        qds, qdds = (qds if has_qd else None), (qdds if has_qdd else None)
-        lk, lc, K = ctx.points
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
-        dev = qs.device
-
-        def cot(g, rows):
-            return _soa(torch.zeros((n, rows), dtype=torch.float64, device=dev) if g is None else g.reshape(n, rows), ns, torch.float64)
-        G_J, G_vel, G_acc = cot(gJ, 6 * K * nd), cot(gvel, 6 * K), cot(gacc, 6 * K)
-        z = lambda rows: torch.zeros((max(rows, 1), ns), dtype=torch.float64, device=dev)
-        g_q, g_qd, g_qdd = z(sim.n_q), (z(nd) if has_qd else None), (z(nd) if has_qdd else None)
-        _on_side_stream(dev, lambda st: sim.point_motion_vjp_device(qs, qds, qdds, lk, lc, G_J, G_vel, G_acc, g_q, g_qd, g_qdd, stream=st),
-                        (qs, qds, qdds, G_J, G_vel, G_acc, g_q, g_qd, g_qdd))
-        out = lambda t, rows: None if t is None else t[:rows, :n].t().to(torch.float32).contiguous()
-        return None, out(g_q, sim.n_q), out(g_qd, nd), out(g_qdd, nd), None, None
-
-    @staticmethod
-    def jvp(ctx, _sim, t_q, t_qd, t_qdd, _links, _local):
-        with torch._C._DisableFuncTorch():
-            return _PointMotion._jvp(ctx, _plain(t_q), _plain(t_qd), _plain(t_qdd))
-
-    @staticmethod
-    def _jvp(ctx, t_q, t_qd, t_qdd):
-        sim = ctx.sim
-        has_qd, has_qdd = ctx.has
-        qs, qds, qdds = (_plain(t) for t in ctx.jvp_inputs)
-        lk, lc, K = ctx.points
-        ns = sim.n_stride
-        tq = _soa_opt(t_q, ns, torch.float64)
-        tqd = _soa_opt(t_qd if has_qd else None, ns, torch.float64)
-        tqdd = _soa_opt(t_qdd if has_qdd else None, ns, torch.float64)
-        t_J, t_vel, t_acc = _mot_buffers(sim, K, qs.device)
-        if any(t is not None for t in (tq, tqd, tqdd)):
-            _on_side_stream(qs.device, lambda st: sim.point_motion_jvp_device(qs, qds, qdds, lk, lc, 1, tq, tqd, tqdd, t_J, t_vel, t_acc,
-                                                                              stream=st), (qs, qds, qdds, tq, tqd, tqdd, t_J, t_vel, t_acc))
-        return _mot_outputs(sim, K, t_J, t_vel, t_acc)
+_POINT_MOTION = _QuerySpec(
+    rows=lambda sim, p: [6 * p.K * sim.n_qd, 6 * p.K, 6 * p.K],
+    unpack=lambda sim, p, J, vel, acc: (J.reshape(sim.n_envs, p.K, 6, sim.n_qd).contiguous(), vel.reshape(sim.n_envs, p.K, 6).contiguous(),
+                                        acc.reshape(sim.n_envs, p.K, 6).contiguous()),
+    pack=lambda sim, p, gJ, gvel, gacc: [_cot(gJ, sim), _cot(gvel, sim), _cot(gacc, sim)],
+    value=lambda sim, p, x, out, st: sim.point_motion_device(x.q, x.qd, x.qdd, p.links, p.local, *out, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.point_motion_jvp_device(x.q, x.qd, x.qdd, p.links, p.local, 1, t.q, t.qd, t.qdd, *out, stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.point_motion_vjp_device(x.q, x.qd, x.qdd, p.links, p.local, *G, g.q, g.qd, g.qdd, stream=st))
 
 
 def point_motion(sim, q, qd, links, local, qdd=None):
@@ -710,12 +512,8 @@ def point_motion(sim, q, qd, links, local, qdd=None):
     rotation).  q [n_envs, n_q], qd and qdd [n_envs, n_qd] float32 CUDA tensors (qd or qdd None: zero).  Gravity and installed physical
     parameters do not enter.  Differentiable along q, qd and qdd in reverse mode (float32 gradients from the cotangents of all three
     outputs) and forward mode."""
-    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
-        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
-    for name, t in (("qd", qd), ("qdd", qdd)):
-        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or tuple(t.shape) != (sim.n_envs, sim.n_qd)):
-            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, n_qd] is expected")
-    return _PointMotion.apply(sim, q, qd, qdd, links, local)
+    _check_state(sim, q, qd, qdd)
+    return _Query.apply(_POINT_MOTION, sim, _Points(*sim._points(links, local)), q, qd, qdd, None)
 
 
 class _StepContacts(torch.autograd.Function):
@@ -724,7 +522,7 @@ class _StepContacts(torch.autograd.Function):
         n, ns, npts = sim.n_envs, sim.n_stride, sim.n_contact_points
         if params is not None:
             sim.set_physical_params(sim.param_ids, params.detach())
-        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), _soa_opt(tau, ns, torch.float32)
+        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), None if tau is None else _soa(tau, ns, torch.float32)
         q_out, qd_out = torch.empty_like(qs), torch.empty_like(qds)
         C = torch.zeros((max(10 * npts, 1), ns), dtype=torch.float32, device=q.device)
         _on_side_stream(q.device, lambda st: sim.step_contacts_device(mode, qs, qds, ts, q_out, qd_out, C, use_pd=use_pd, stream=st),
@@ -736,7 +534,7 @@ class _StepContacts(torch.autograd.Function):
     def setup_context(ctx, inputs, output):
         sim, mode, use_pd, q, qd, tau, params = inputs
         ns = sim.n_stride
-        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), _soa_opt(tau, ns, torch.float32)
+        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), None if tau is None else _soa(tau, ns, torch.float32)
         par = params.detach() if params is not None else None
         ctx.sim, ctx.mode, ctx.use_pd, ctx.has_tau, ctx.has_params = sim, mode, use_pd, tau is not None, params is not None
         ctx.save_for_backward(qs, qds, ts if ts is not None else qs, par if par is not None else qs)
@@ -807,9 +605,7 @@ def step_contacts(sim, q, qd, tau_or_action=None, mode=MODE_FULL, use_pd=False, 
     for name, t in (("q", q), ("qd", qd), ("tau_or_action", tau_or_action)):
         if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or t.shape[0] != sim.n_envs):
             raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, dim] is expected")
-    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
-                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
-        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    _check_params(sim, params)
     return _StepContacts.apply(sim, int(mode), bool(use_pd), q, qd, tau_or_action, params)
 
 
@@ -819,7 +615,7 @@ class _StepWrench(torch.autograd.Function):
         n, ns = sim.n_envs, sim.n_stride
         if params is not None:
             sim.set_physical_params(sim.param_ids, params.detach())
-        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), _soa_opt(tau, ns, torch.float32)
+        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), None if tau is None else _soa(tau, ns, torch.float32)
         Ws = _soa(W.reshape(n, -1), ns, torch.float32)
         fd = mode == MODE_FD
         q_out = None if fd else torch.empty_like(qs)
@@ -835,7 +631,7 @@ class _StepWrench(torch.autograd.Function):
     def setup_context(ctx, inputs, output):
         sim, mode, use_pd, links, local, q, qd, tau, W, params = inputs
         ns = sim.n_stride
-        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), _soa_opt(tau, ns, torch.float32)
+        qs, qds, ts = _soa(q, ns, torch.float32), _soa(qd, ns, torch.float32), None if tau is None else _soa(tau, ns, torch.float32)
         Ws = _soa(W.reshape(sim.n_envs, -1), ns, torch.float32)
         par = params.detach() if params is not None else None
         ctx.sim, ctx.mode, ctx.use_pd, ctx.links, ctx.local = sim, mode, use_pd, links, local
@@ -922,79 +718,17 @@ def step_wrench(sim, q, qd, tau_or_action, links, local, W, mode=MODE_FULL, use_
         raise ValueError("links [K] and local [K, 3] expected")
     if W.dtype != torch.float32 or not W.is_cuda or tuple(W.shape) != (sim.n_envs, len(lk), 6):
         raise ValueError("W: a float32 CUDA tensor [n_envs, K, 6] is expected")
-    if params is not None and (params.dtype != torch.float64 or not params.is_cuda or
-                               tuple(params.shape) != (sim.n_envs, len(sim.param_ids)) or not sim.param_ids):
-        raise ValueError("params: a float64 CUDA tensor [n_envs, k] for the k parameters installed by set_physical_params is expected")
+    _check_params(sim, params)
     return _StepWrench.apply(sim, int(mode), bool(use_pd), lk, lc, q, qd, tau_or_action, W, params)
 
 
-def _reg_outputs(sim, Y, yT, yV):
-    """Device outputs [rows, n_stride] of the regressors -> (Y [n, n_qd, n_pi], yT [n, n_pi], yV [n, n_pi])."""
-    n, nd, npi = sim.n_envs, sim.n_qd, sim.n_pi
-    return (Y[:nd * npi, :n].t().reshape(n, nd, npi).contiguous(), yT[:npi, :n].t().contiguous(), yV[:npi, :n].t().contiguous())
-
-
-def _reg_buffers(sim, device):
-    z = lambda rows: torch.zeros((max(rows, 1), sim.n_stride), dtype=torch.float64, device=device)
-    return z(sim.n_qd * sim.n_pi), z(sim.n_pi), z(sim.n_pi)
-
-
-class _Regressor(torch.autograd.Function):
-    @staticmethod
-    def forward(sim, q, qd, qdd):
-        ns = sim.n_stride
-        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
-        Y, yT, yV = _reg_buffers(sim, q.device)
-        _on_side_stream(q.device, lambda st: sim.regressor_device(qs, qds, qdds, Y, yT, yV, stream=st), (qs, qds, qdds, Y, yT, yV))
-        return _reg_outputs(sim, Y, yT, yV)
-
-    @staticmethod
-    def setup_context(ctx, inputs, output):
-        sim, q, qd, qdd = inputs
-        ns = sim.n_stride
-        qs, qds, qdds = _soa(q, ns, torch.float32), _soa_opt(qd, ns, torch.float32), _soa_opt(qdd, ns, torch.float32)
-        ctx.sim, ctx.has = sim, (qd is not None, qdd is not None)
-        ctx.save_for_backward(qs, *(t if t is not None else qs for t in (qds, qdds)))
-        ctx.jvp_inputs = (qs, qds, qdds)
-
-    @staticmethod
-    def backward(ctx, gY, gT, gV):
-        sim = ctx.sim
-        has_qd, has_qdd = ctx.has
-        qs, qds, qdds = ctx.saved_tensors
-        qds, qdds = (qds if has_qd else None), (qdds if has_qdd else None)
-        n, ns, nd = sim.n_envs, sim.n_stride, sim.n_qd
-        dev = qs.device
-
-        def cot(g, rows):
-            return _soa(torch.zeros((n, rows), dtype=torch.float64, device=dev) if g is None else g.reshape(n, rows), ns, torch.float64)
-        G_Y, G_yT, G_yV = cot(gY, nd * sim.n_pi), cot(gT, sim.n_pi), cot(gV, sim.n_pi)
-        z = lambda rows: torch.zeros((max(rows, 1), ns), dtype=torch.float64, device=dev)
-        g_q, g_qd, g_qdd = z(sim.n_q), (z(nd) if has_qd else None), (z(nd) if has_qdd else None)
-        _on_side_stream(dev, lambda st: sim.regressor_vjp_device(qs, qds, qdds, G_Y, G_yT, G_yV, g_q, g_qd, g_qdd, stream=st),
-                        (qs, qds, qdds, G_Y, G_yT, G_yV, g_q, g_qd, g_qdd))
-        out = lambda t, rows: None if t is None else t[:rows, :n].t().to(torch.float32).contiguous()
-        return None, out(g_q, sim.n_q), out(g_qd, nd), out(g_qdd, nd)
-
-    @staticmethod
-    def jvp(ctx, _sim, t_q, t_qd, t_qdd):
-        with torch._C._DisableFuncTorch():
-            return _Regressor._jvp(ctx, _plain(t_q), _plain(t_qd), _plain(t_qdd))
-
-    @staticmethod
-    def _jvp(ctx, t_q, t_qd, t_qdd):
-        sim = ctx.sim
-        has_qd, has_qdd = ctx.has
-        qs, qds, qdds = (_plain(t) for t in ctx.jvp_inputs)
-        ns = sim.n_stride
-        tq = _soa_opt(t_q, ns, torch.float64)
-        tqd = _soa_opt(t_qd if has_qd else None, ns, torch.float64)
-        tqdd = _soa_opt(t_qdd if has_qdd else None, ns, torch.float64)
-        t_Y, t_yT, t_yV = _reg_buffers(sim, qs.device)
-        if any(t is not None for t in (tq, tqd, tqdd)):
-            _on_side_stream(qs.device, lambda st: sim.regressor_jvp_device(qs, qds, qdds, 1, tq, tqd, tqdd, t_Y, t_yT, t_yV, stream=st),
-                            (qs, qds, qdds, tq, tqd, tqdd, t_Y, t_yT, t_yV))
-        return _reg_outputs(sim, t_Y, t_yT, t_yV)
+_REGRESSOR = _QuerySpec(
+    rows=lambda sim, p: [sim.n_qd * sim.n_pi, sim.n_pi, sim.n_pi],
+    unpack=lambda sim, p, Y, yT, yV: (Y.reshape(sim.n_envs, sim.n_qd, sim.n_pi).contiguous(), yT.contiguous(), yV.contiguous()),
+    pack=lambda sim, p, gY, gT, gV: [_cot(gY, sim), _cot(gT, sim), _cot(gV, sim)],
+    value=lambda sim, p, x, out, st: sim.regressor_device(x.q, x.qd, x.qdd, *out, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.regressor_jvp_device(x.q, x.qd, x.qdd, 1, t.q, t.qd, t.qdd, *out, stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.regressor_vjp_device(x.q, x.qd, x.qdd, *G, g.q, g.qd, g.qdd, stream=st))
 
 
 def regressor(sim, q, qd=None, qdd=None):
@@ -1005,9 +739,5 @@ def regressor(sim, q, qd=None, qdd=None):
     tds_b200.model.regressor_names).  q [n_envs, n_q], qd and qdd [n_envs, n_qd] float32 CUDA tensors (qd or qdd None: zero).  Installed
     physical parameters do not enter.  Differentiable along q, qd and qdd in reverse mode (float32 gradients from the cotangents of all
     three outputs) and forward mode."""
-    if q.dtype != torch.float32 or not q.is_cuda or q.dim() != 2 or tuple(q.shape) != (sim.n_envs, sim.n_q):
-        raise ValueError("q: a float32 CUDA tensor [n_envs, n_q] is expected")
-    for name, t in (("qd", qd), ("qdd", qdd)):
-        if t is not None and (t.dtype != torch.float32 or not t.is_cuda or t.dim() != 2 or tuple(t.shape) != (sim.n_envs, sim.n_qd)):
-            raise ValueError(f"{name}: a float32 CUDA tensor [n_envs, n_qd] is expected")
-    return _Regressor.apply(sim, q, qd, qdd)
+    _check_state(sim, q, qd, qdd)
+    return _Query.apply(_REGRESSOR, sim, None, q, qd, qdd, None)
