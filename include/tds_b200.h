@@ -410,6 +410,43 @@ int tds_b200_regressor_vjp_device(tds_b200_sim* sim, const float* q, const float
 int tds_b200_regressor_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, const double* G_Y,
                                 const double* G_yT, const double* G_yV, double* g_q, double* g_qd, double* g_qdd);
 
+/* ---- inverse mass matrix M^-1(q) and operational-space inverse inertia J M^-1 J^T (DESIGN.md section 7.20) ------------------------
+ * Minv [n_qd x n_qd]: the inverse of exactly the matrix tds_b200_mass_matrix_* returns (the CRBA M at the fp32-rounded q, fp64, with the
+ *   installed masses, centres of mass and inertias; stiffness, damping, friction and restitution do not enter), by the blocked Cholesky
+ *   factor the contact solve uses.  Both triangles, bitwise symmetric (each off-diagonal entry is computed once and written twice).  A
+ *   world of several multibodies gives the block-diagonal inverse, with exact zeros between multibodies.  For a floating base this is
+ *   NOT the derivative dqdd/dtau of the forward-dynamics step: the reference's floating-base forward dynamics does not invert its own M.
+ * Linv [6K x 6K]: the operational-space inverse inertia J M^-1 J^T of a point table of 1 <= K <= TDS_B200_MAX_OSIM_POINTS points (links /
+ *   local as in tds_b200_point_motion_*, host memory, passed with each call), with J the 6-row spatial point Jacobian of
+ *   tds_b200_point_motion_* (rows [w; x'], floating-base columns in the coordinates of M): entry (6k + r, 6l + s) at row (6k + r) 6K + 6l + s.
+ *   Symmetric (one sum per pair, written twice) and positive semi-definite; rank-deficient where a point's chain has fewer than 6 dofs,
+ *   so Lambda itself is left to the caller.
+ * Either output may be NULL, not both; K is ignored (0 allowed) when Linv and its tangents and cotangents are NULL.  Argument checks ->
+ * -1: NULL q; no output (tangent, cotangent); K out of range, a link index out of range, NULL links / local with K > 0, Linv with K = 0;
+ * m < 1 or both tangents NULL; no gradient output.  -> -4: t_par / g_par without an installed set.
+ *   device: q [n_q][n_stride] fp32 as tds_b200_step_device; Minv [n_qd * n_qd][n_stride], Linv [36 K^2][n_stride] fp64.  Asynchronous.
+ *   host:   q [n][n_q] fp64 (rounded to fp32); Minv [n][n_qd][n_qd], Linv [n][6K][6K].  Synchronous.
+ * _jvp: the derivatives along m tangents t_q of q and t_par of the installed parameters (either may be NULL: zero), one lane per
+ *   (environment, tangent) of the dual-number instance, in chunks as tds_b200_step_jvp_* (dMinv = -Minv dM Minv); Minv and Linv (may be
+ *   NULL) receive the values.  Device t_q [n_q * m][n_stride], t_par [k * m][n_stride], t_Minv [n_qd^2 * m][n_stride], t_Linv
+ *   [36 K^2 * m][n_stride] (entry (r, j) at (r * m + j) * n_stride + e); host t_q [n][n_q][m], t_par [n][k][m], t_Minv [n][n_qd^2][m],
+ *   t_Linv [n][36 K^2][m].
+ * _vjp: g_q[c] = <G_Minv, dMinv/dq_c> + <G_Linv, dLinv/dq_c> and, while a set is installed, g_par likewise, for cotangents in the
+ *   outputs' layouts (NULL: zero, not both): the JVP along the n_q (+ k) identity tangents contracted with G on the device.  g_q or g_par
+ *   may be NULL, not both.  Device g_q [n_q][n_stride], g_par [k][n_stride] fp64 (asynchronous); host g_q [n][n_q], g_par [n][k]. */
+#define TDS_B200_MAX_OSIM_POINTS 16
+int tds_b200_mass_inverse_device(tds_b200_sim* sim, const float* q, int K, const int* links, const double* local, double* Minv, double* Linv,
+                                 void* stream);
+int tds_b200_mass_inverse_host(tds_b200_sim* sim, const double* q, int K, const int* links, const double* local, double* Minv, double* Linv);
+int tds_b200_mass_inverse_jvp_device(tds_b200_sim* sim, const float* q, int K, const int* links, const double* local, int m, const double* t_q,
+                                     const double* t_par, double* Minv, double* Linv, double* t_Minv, double* t_Linv, void* stream);
+int tds_b200_mass_inverse_jvp_host(tds_b200_sim* sim, const double* q, int K, const int* links, const double* local, int m, const double* t_q,
+                                   const double* t_par, double* Minv, double* Linv, double* t_Minv, double* t_Linv);
+int tds_b200_mass_inverse_vjp_device(tds_b200_sim* sim, const float* q, int K, const int* links, const double* local, const double* G_Minv,
+                                     const double* G_Linv, double* g_q, double* g_par, void* stream);
+int tds_b200_mass_inverse_vjp_host(tds_b200_sim* sim, const double* q, int K, const int* links, const double* local, const double* G_Minv,
+                                   const double* G_Linv, double* g_q, double* g_par);
+
 /* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
  * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
  * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,

@@ -60,6 +60,7 @@ DESIGN.md section 7.19) with a backward rule (BatchSim.regressor_vjp_device: flo
 """
 from collections import namedtuple
 
+import numpy as np
 import torch
 
 from .sim import MODE_FD, MODE_FULL
@@ -333,7 +334,8 @@ def _state_soa(sim, q, qd, qdd):
 
 
 class _Query(torch.autograd.Function):
-    """The dynamics queries (mass_matrix, inverse_dynamics, centroidal, forward_kinematics, point_motion, regressor) as one Function over
+    """The dynamics queries (mass_matrix, inverse_dynamics, centroidal, forward_kinematics, point_motion, regressor, mass_inverse) as one
+    Function over
     a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
     float64 output buffers, every C-ABI call ordered on a side stream, and the gradients as float32 (q, qd, qdd) and float64 (params).
     An input the query does not take, or the call leaves out, is None and gets no gradient; a tangent on it is ignored.  With params
@@ -741,3 +743,31 @@ def regressor(sim, q, qd=None, qdd=None):
     three outputs) and forward mode."""
     _check_state(sim, q, qd, qdd)
     return _Query.apply(_REGRESSOR, sim, None, q, qd, qdd, None)
+
+
+# Without points (K = 0) the entries get None for Linv and its cotangent, and the Function's Linv is [n_envs, 0, 0].
+_MASS_INVERSE = _QuerySpec(
+    rows=lambda sim, p: [sim.n_qd * sim.n_qd, 36 * p.K * p.K],
+    unpack=lambda sim, p, Minv, Linv: (Minv.reshape(sim.n_envs, sim.n_qd, sim.n_qd).contiguous(),
+                                       Linv.reshape(sim.n_envs, 6 * p.K, 6 * p.K).contiguous()),
+    pack=lambda sim, p, gMinv, gLinv: [_cot(gMinv, sim), _cot(gLinv, sim) if p.K else None],
+    value=lambda sim, p, x, out, st: sim.mass_inverse_device(x.q, p.links, p.local, out[0], out[1] if p.K else None, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.mass_inverse_jvp_device(x.q, p.links, p.local, 1, t.q, t.params, out[0], out[1] if p.K else None,
+                                                                  stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.mass_inverse_vjp_device(x.q, p.links, p.local, *G, g.q, g.params, stream=st))
+
+
+def mass_inverse(sim, q, links=None, local=None, params=None):
+    """The inverse mass matrix and the operational-space inverse inertia of every environment of `sim` (a BatchSim), DESIGN.md section
+    7.20, in fp64 at the fp32-rounded q [n_envs, n_q] float32 CUDA tensor: (Minv [n_envs, n_qd, n_qd], Linv [n_envs, 6K, 6K] or None
+    without points) float64.  Minv is the inverse of mass_matrix(sim, q, params), bitwise symmetric (for a floating base it is not the
+    forward dynamics' dqdd/dtau); Linv = J Minv J^T for the point table links [K] (-1: the base) / local [K, 3] (K <= 16; constants of
+    the call), J the spatial point Jacobian of point_motion ([n_envs, K, 6, n_qd] as 6K rows), so that Lambda = Linv^-1 (rank-deficient
+    where a point's chain has fewer than 6 dofs: the caller chooses how to invert it).  A solve with M is Minv @ b.  params: None, or a
+    float64 CUDA tensor [n_envs, k] of values for the parameters installed by sim.set_physical_params (then also differentiated).
+    Differentiable in reverse mode (float32 q.grad, float64 params.grad) and forward mode."""
+    _check_state(sim, q)
+    _check_params(sim, params)
+    p = _Points(*sim._points([] if links is None else links, np.zeros((0, 3)) if local is None else local))
+    Minv, Linv = _Query.apply(_MASS_INVERSE, sim, p, q, None, None, params)
+    return Minv, (Linv if p.K else None)

@@ -92,6 +92,12 @@ extern "C" int tds_launch_regressor(const DevModel* M, const SimParams* P, const
                                     cudaStream_t stream);
 extern "C" int tds_launch_regressor_jvp(const DevModel* M, const SimParams* P, const StepIO* io, const TdsRegCall* out, const double* t_in,
                                         int m, int n_dirs, char* gscratch, cudaStream_t stream);
+// inverse mass matrix M^-1(q), its Jacobian-vector products, and the contraction J M^-1 J^T (tds_mass_inverse.cu)
+extern "C" int tds_launch_mass_inverse(const DevModel* M, const StepIO* io, const ParMap* pm, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_mass_inverse_jvp(const DevModel* M, const StepIO* io, const ParMap* pm, const double* t_q, const double* t_par,
+                                           int m, int n_dirs, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_osim(const double* J, const double* dJ, const double* Mi, const double* dMi, double* L, int K, int n_qd, int m,
+                               int n, int ns, cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
@@ -443,6 +449,7 @@ struct tds_b200_sim {
   DevModel dm_m;          // layout of the fp64 mass-matrix instance (8-byte scalars)
   float* wrench_dev = nullptr; size_t wrench_dev_bytes = 0;   // host paths of the step with wrenches: W [6K][ns] fp32
   double* mass_dev = nullptr; size_t mass_dev_bytes = 0; // dynamics queries' VJPs: identity tangents | output columns of a chunk
+  double* minv_dev = nullptr; size_t minv_dev_bytes = 0; // the inverse mass matrix's intermediates: M^-1, J and their tangents
   // installed physical parameters (tds_b200_set_physical_params_*): slot map (par.n == 0: none) and values [k][ns] fp64
   ParMap par;
   double* par_dev = nullptr; size_t par_dev_bytes = 0;
@@ -721,7 +728,7 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->rq); cudaFree(s->rqd); cudaFree(s->zero_act); cudaFree(s->pol_act); cudaFree(s->sticky); cudaFree(s->r_total);
   cudaFree(s->pol_params); cudaFree(s->act_qidx); cudaFree(s->r_steps);
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
-  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->mass_dev); cudaFree(s->wrench_dev);
+  cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->mass_dev); cudaFree(s->minv_dev); cudaFree(s->wrench_dev);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
@@ -913,7 +920,7 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
 
 // what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14, 7.16 and 7.17,
 // or the step with its contact records (section 7.15)
-enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, regressor };
+enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, regressor, minv };
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
 // inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
@@ -921,7 +928,7 @@ enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, r
 // contacts: as step, with the rows q' | qd' | records; centroidal: t_in = the q | qd tangents (qd in the step's qd), outputs `cen`;
 // motion: t_in = the q | qd | qdd tangents (qd and qdd as for inv), the point table and outputs `mot`; wrench: as step, with the point
 // table, wrenches and wrench tangents `ext`; regressor: t_in = the q | qd | qdd tangents (as for inv), Y in jac and the
-// energy outputs `reg`
+// energy outputs `reg`; minv: as mass, M^-1 in jac
 struct JvpTangents {
   const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr;
   const TdsCenCall* cen = nullptr; const TdsMotCall* mot = nullptr; const TdsExtCall* ext = nullptr;
@@ -1007,6 +1014,7 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
                                      sm);
           break;
         case Query::regressor: rc = tds_launch_regressor_jvp(&s->dm_ad, &s->P, &io, jv->reg, jv->t_in, jv->m, nd, s->jac_scratch, sm); break;
+        case Query::minv: rc = tds_launch_mass_inverse_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
       }
     }
     if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
@@ -1963,6 +1971,175 @@ int tds_b200_regressor_vjp_host(tds_b200_sim* s, const double* q, const double* 
   CUDA_TRY(put_parts<double>(s->vjp_g, {{G_Y, R.Y}, {G_yT, R.yT}, {G_yV, R.yV}}, n, ns, s->stream));
   if (int rc = reg_vjp_run(s, s->q, qd_d, qdd_d, s->vjp_g, g_d, s->stream)) return rc;
   CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- inverse mass matrix M^-1(q) and operational-space inverse inertia J M^-1 J^T (DESIGN.md section 7.20): the MINV instances of the
+// world-frame kernel and the contraction kernel (tds_mass_inverse.cu), with J from the point-motion value and JVP (mot_run, mot_jvp_run) --
+// rows of the outputs M^-1 | Lambda^-1
+struct MinvRows { size_t Mi, L; size_t all() const { return Mi + L; } };
+static MinvRows minv_rows(const tds_b200_sim* s, int K) {
+  return MinvRows{(size_t)s->dm[0].n_qd * s->dm[0].n_qd, (size_t)36 * K * K};
+}
+
+// M^-1 [nn][ns] and Lambda^-1 [36 K^2][ns] (either may be null) from q [n_q][ns] fp32 and, with m tangents t_q [n_q * m][ns] and t_par
+// [k * m][ns] (either may be null: zero), their tangents t_Minv [nn * m][ns] and t_Linv [36 K^2 * m][ns] (either may be null).  What the
+// outputs need and the caller does not ask for (M^-1 and its tangents, J and dJ, the q | qd | qdd tangents of the point-motion JVP) goes
+// to s->minv_dev.
+static int minv_run(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, double* Minv, double* Linv, int m,
+                    const double* t_q, const double* t_par, double* t_Minv, double* t_Linv, cudaStream_t sm) {
+  const DevModel& D = s->dm[0];
+  const size_t ns = s->ns, nn = (size_t)D.n_qd * D.n_qd, nJ = (size_t)6 * K * D.n_qd;
+  const bool lam = Linv || t_Linv, dlam_q = t_Linv && t_q;
+  const size_t sMi = (lam && !Minv) ? nn : 0, sJ = lam ? nJ : 0, sdMi = (t_Linv && !t_Minv) ? nn * m : 0, sdJ = dlam_q ? nJ * m : 0,
+               sT = dlam_q ? (size_t)inv_n_in(s) * m : 0;
+  CUDA_TRY(grow_dev(&s->minv_dev, &s->minv_dev_bytes, sizeof(double) * (sMi + sJ + sdMi + sdJ + sT + 1) * ns));
+  double* const Mi = Minv ? Minv : s->minv_dev;
+  double* const J = s->minv_dev + sMi * ns;
+  double* const dMi = t_Minv ? t_Minv : J + sJ * ns;
+  double* const dJ = J + (sJ + sdMi) * ns;
+  double* const T = dJ + sdJ * ns;
+  if (Minv || lam) {
+    int rc = value_run(s, "mass inverse", q, nullptr, nullptr, Mi, [&](const StepIO* io, const ParMap* pm) {
+      return tds_launch_mass_inverse(&s->dm_m, io, pm, s->jac_scratch, sm);
+    });
+    if (rc) return rc;
+  }
+  const TdsMotCall mc{K, links, local, J, nullptr, nullptr}, dmc{K, links, local, dJ, nullptr, nullptr};
+  if (lam) { if (int rc = mot_run(s, q, nullptr, nullptr, &mc, sm)) return rc; }
+  if (t_Minv || t_Linv) {
+    const JvpTangents jv{t_q, t_par, m, Query::minv};
+    if (int rc = jacobian_run(s, TDS_B200_MODE_FULL, 0, q, nullptr, nullptr, dMi, sm, false, &jv)) return rc;
+    if (dlam_q) {   // J depends on q alone: its tangents along the q tangents (qd and qdd tangents zero)
+      CUDA_TRY(put_parts_d2d<double>(T, {{t_q, (size_t)D.n_q * m}, {nullptr, (size_t)2 * D.n_qd * m}}, s->ns, sm));
+      if (int rc = mot_jvp_run(s, q, nullptr, nullptr, &dmc, m, T, sm)) return rc;
+    }
+  }
+  int rc = 0;
+  if (Linv) rc = tds_launch_osim(J, nullptr, Mi, nullptr, Linv, K, D.n_qd, 1, s->n, s->ns, sm);
+  if (!rc && t_Linv) rc = tds_launch_osim(J, dlam_q ? dJ : nullptr, Mi, dMi, t_Linv, K, D.n_qd, m, s->n, s->ns, sm);
+  if (rc) set_err(std::string("mass inverse: J M^-1 J^T launch: ") + cudaGetErrorString((cudaError_t)rc));
+  return rc;
+}
+
+// g_q [n_q][ns] and g_par [k][ns] (either may be null) = <G, d(M^-1 | Lambda^-1)>, G [nn + 36 K^2][ns] concatenated, or G [nn][ns] alone
+// when with_L is false
+static int minv_vjp_run(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, bool with_L, const double* G,
+                        double* g_q, double* g_par, cudaStream_t sm) {
+  const MinvRows R = minv_rows(s, K);
+  const size_t ns = s->ns;
+  return vjp_by_eye(s, "mass inverse", s->dm[0].n_q, R.Mi + (with_L ? R.L : 0), G, g_q, g_par, sm,
+                    [&](int nd, const double* t_q, const double* t_par, double* dO) {
+                      return minv_run(s, q, K, links, local, nullptr, nullptr, nd, t_q, t_par, dO, with_L ? dO + R.Mi * nd * ns : nullptr,
+                                      sm);
+                    });
+}
+
+// -1: no q, no output (Minv, Linv), K out of [0, TDS_B200_MAX_OSIM_POINTS], Linv with K = 0, a missing or bad point table
+static int minv_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local, const void* Minv, const void* Linv) {
+  if (!s || !q || (!Minv && !Linv)) return -1;
+  if (K < 0 || K > TDS_B200_MAX_OSIM_POINTS) { set_err("mass inverse: K out of [0, TDS_B200_MAX_OSIM_POINTS]"); return -1; }
+  if (Linv && K < 1) { set_err("mass inverse: J M^-1 J^T needs K >= 1 points"); return -1; }
+  return kin_check(s, q, K, links, local);
+}
+
+int tds_b200_mass_inverse_device(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, double* Minv, double* Linv,
+                                 void* stream) {
+  if (int rc = minv_check(s, q, K, links, local, Minv, Linv)) return rc;
+  return minv_run(s, q, K, links, local, Minv, Linv, 0, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+int tds_b200_mass_inverse_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, double* Minv, double* Linv) {
+  if (int rc = minv_check(s, q, K, links, local, Minv, Linv)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const MinvRows R = minv_rows(s, K);
+  if (int rc = put_q(s, q)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (R.all() + 1) * ns));
+  double* d = s->jac_dev;
+  if (int rc = minv_run(s, s->q, K, links, local, Minv ? d : nullptr, Linv ? d + R.Mi * ns : nullptr, 0, nullptr, nullptr, nullptr, nullptr,
+                        s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{Minv, R.Mi}, {Linv, R.L}}, d, n, ns, s->stream));
+  return 0;
+}
+
+static int minv_jvp_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local, int m, const void* t_q,
+                          const void* t_par, const void* Linv, const void* t_Minv, const void* t_Linv) {
+  if (int rc = minv_check(s, q, K, links, local, t_Minv, t_Linv)) return rc;
+  if (Linv && K < 1) { set_err("mass inverse: J M^-1 J^T needs K >= 1 points"); return -1; }
+  if (m < 1 || (!t_q && !t_par)) return -1;
+  return par_without_installed(s, t_par, "mass inverse jvp: parameter tangents");
+}
+
+int tds_b200_mass_inverse_jvp_device(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, int m, const double* t_q,
+                                     const double* t_par, double* Minv, double* Linv, double* t_Minv, double* t_Linv, void* stream) {
+  if (int rc = minv_jvp_check(s, q, K, links, local, m, t_q, t_par, Linv, t_Minv, t_Linv)) return rc;
+  return minv_run(s, q, K, links, local, Minv, Linv, m, t_q, t_par, t_Minv, t_Linv, (cudaStream_t)stream);
+}
+
+int tds_b200_mass_inverse_jvp_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, int m, const double* t_q,
+                                   const double* t_par, double* Minv, double* Linv, double* t_Minv, double* t_Linv) {
+  if (int rc = minv_jvp_check(s, q, K, links, local, m, t_q, t_par, Linv, t_Minv, t_Linv)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const MinvRows R = minv_rows(s, K);
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; t_q | t_par | t_Minv | t_Linv | Minv | Linv
+  const size_t tq = (size_t)(t_q ? s->dm[0].n_q : 0) * m, tp = (size_t)(t_par ? s->par.n : 0) * m, to = R.all() * m;
+  if (int rc = put_q(s, q)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (tq + tp + to + R.all() + 1) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + (tq + tp) * ns;
+  double* v_d = to_d + to * ns;
+  CUDA_TRY(put_parts<double>(d, {{t_q, tq}, {t_par, tp}}, n, ns, s->stream));
+  if (int rc = minv_run(s, s->q, K, links, local, Minv ? v_d : nullptr, Linv ? v_d + R.Mi * ns : nullptr, m, t_q ? d : nullptr,
+                        t_par ? d + tq * ns : nullptr, t_Minv ? to_d : nullptr, t_Linv ? to_d + R.Mi * m * ns : nullptr, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{t_Minv, R.Mi * m}, {t_Linv, R.L * m}, {Minv, R.Mi}, {Linv, R.L}}, to_d, n, ns, s->stream));
+  return 0;
+}
+
+static int minv_vjp_check(tds_b200_sim* s, const void* q, int K, const int* links, const double* local, const void* G_Minv,
+                          const void* G_Linv, const void* g_q, const void* g_par) {
+  if (int rc = minv_check(s, q, K, links, local, G_Minv, G_Linv)) return rc;
+  if (!g_q && !g_par) return -1;
+  return par_without_installed(s, g_par, "mass inverse vjp: parameter cotangents");
+}
+
+int tds_b200_mass_inverse_vjp_device(tds_b200_sim* s, const float* q, int K, const int* links, const double* local, const double* G_Minv,
+                                     const double* G_Linv, double* g_q, double* g_par, void* stream) {
+  if (int rc = minv_vjp_check(s, q, K, links, local, G_Minv, G_Linv, g_q, g_par)) return rc;
+  const int n_q = s->dm[0].n_q, k = s->par.n;
+  const MinvRows R = minv_rows(s, K);
+  const size_t rows = R.Mi + (G_Linv ? R.L : 0);
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the concatenated cotangent M^-1 (| Lambda^-1) (zero where a part is NULL), then g_q | g_par as one array for the contraction
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (rows + n_q + k) * s->ns));
+  double* g_d = s->vjp_g + rows * s->ns;
+  CUDA_TRY(put_parts_d2d<double>(s->vjp_g, {{G_Minv, R.Mi}, {G_Linv, rows - R.Mi}}, s->ns, sm));
+  if (int rc = minv_vjp_run(s, q, K, links, local, G_Linv != nullptr, s->vjp_g, g_q ? g_d : nullptr,
+                            g_par ? g_d + (size_t)n_q * s->ns : nullptr, sm))
+    return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, (size_t)n_q}, {g_par, (size_t)k}}, g_d, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_mass_inverse_vjp_host(tds_b200_sim* s, const double* q, int K, const int* links, const double* local, const double* G_Minv,
+                                   const double* G_Linv, double* g_q, double* g_par) {
+  if (int rc = minv_vjp_check(s, q, K, links, local, G_Minv, G_Linv, g_q, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, n_q = s->dm[0].n_q, k = s->par.n;
+  const MinvRows R = minv_rows(s, K);
+  const size_t rows = R.Mi + (G_Linv ? R.L : 0);
+  if (int rc = put_q(s, q)) return rc;
+  // G (M^-1 (| Lambda^-1), zero where a part is NULL) | g_q | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (rows + n_q + k + 1) * ns));
+  double* g_d = s->vjp_g + rows * ns;
+  CUDA_TRY(put_parts<double>(s->vjp_g, {{G_Minv, R.Mi}, {G_Linv, rows - R.Mi}}, n, ns, s->stream));
+  if (int rc = minv_vjp_run(s, s->q, K, links, local, G_Linv != nullptr, s->vjp_g, g_q ? g_d : nullptr,
+                            g_par ? g_d + (size_t)n_q * ns : nullptr, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{g_q, (size_t)n_q}, {g_par, (size_t)k}}, g_d, n, ns, s->stream));
   return 0;
 }
 

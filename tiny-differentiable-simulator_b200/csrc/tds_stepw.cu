@@ -171,8 +171,14 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // Then the base's own columns (base frame) and the stiffness and damping columns.  Y [n_qd * n_pi] at io.jac, entry (r, c) at row
 // r * n_pi + c, yT and yV [n_pi] at pm.yT and pm.yV (each may be null); row k at out[k * ns + e] (fp64 instance) or its dual part at
 // out[(k * m + j) * ns + e] (JV instance).  Returns before pass 2.
+// MINV (with MASS): the inverse mass matrix M^-1(q) (DESIGN.md section 7.20), launched as MASS.  After the floating-base block the lane
+// factors the blocked lower triangle as the contact solve does (M = L L^T: off-diagonal blocks of L over M, inverted diagonal blocks in
+// dinv), overwrites L's off-diagonal blocks with those of W = L^-1 column by column, and writes M^-1 = W^T W in place of the dense M: one
+// sum per pair (r >= c) written to (r, c) and (c, r).  The padding dofs hold an identity, so the first n_qd rows and columns of the
+// padded inverse are M^-1; they are not written.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
-          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false, bool REG = false>
+          bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false, bool REG = false,
+          bool MINV = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
@@ -1320,6 +1326,53 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   } else {
     a_prev.top = v3<RA>(RA(0), RA(0), RA(0));
     a_prev.bot = v3<RA>(RA(-P.gravity[0]), RA(-P.gravity[1]), RA(-P.gravity[2]));
+  }
+  if constexpr (MINV) {
+    auto put = [&](int k, RS x) {
+      if constexpr (AD) io.jac[((size_t)k * io.jac_n_in + jcol) * ns + e] = x.d;
+      else io.jac[(size_t)k * ns + e] = x;
+    };
+    // blocked Cholesky M = L L^T, the contact solve's loop
+    for (int bi = 0; bi < nb; ++bi) {
+      for (int bj = 0; bj <= bi; ++bj) {
+        B9<RS> Ab = ldb<RS>(Mb + btri(bi, bj) * ST, ST);
+        for (int bk = 0; bk < bj; ++bk)
+          gemm_nt_sub(Ab, ldb<RS>(Mb + btri(bi, bk) * ST, ST), ldb<RS>(Mb + btri(bj, bk) * ST, ST));
+        if (bj < bi) stb<RS>(Mb + btri(bi, bj) * ST, ST, mul_linvT(Ab, ldl6<RS>(dinv + bj * 6 * ST, ST)));
+        else stl6<RS>(dinv + bi * 6 * ST, ST, chol3_inv(Ab));
+      }
+    }
+    // W = L^-1: W_ij = -W_ii sum_{j <= k < i} L_ik W_kj.  Column j top down reads L in the columns right of j and W above row i.
+    for (int bj = 0; bj < nb; ++bj) {
+      const B9<RS> Wjj = l6_full(ldl6<RS>(dinv + bj * 6 * ST, ST));
+      for (int bi = bj + 1; bi < nb; ++bi) {
+        B9<RS> X = b9_zero<RS>();
+        gemm_nn_sub(X, ldb<RS>(Mb + btri(bi, bj) * ST, ST), Wjj);
+        for (int bk = bj + 1; bk < bi; ++bk)
+          gemm_nn_sub(X, ldb<RS>(Mb + btri(bi, bk) * ST, ST), ldb<RS>(Mb + btri(bk, bj) * ST, ST));
+        stb<RS>(Mb + btri(bi, bj) * ST, ST, linv_mul(ldl6<RS>(dinv + bi * 6 * ST, ST), X));
+      }
+    }
+    // M^-1 block (i, j), i >= j: sum_{k >= i} W_ki^T W_kj
+    if (live && io.jac) {
+      for (int bi = 0; bi < nb; ++bi) {
+        const B9<RS> Wii = l6_full(ldl6<RS>(dinv + bi * 6 * ST, ST));
+        for (int bj = 0; bj <= bi; ++bj) {
+          B9<RS> X = b9_zero<RS>();
+          gemm_tn_add(X, Wii, bj == bi ? Wii : ldb<RS>(Mb + btri(bi, bj) * ST, ST));
+          for (int bk = bi + 1; bk < nb; ++bk)
+            gemm_tn_add(X, ldb<RS>(Mb + btri(bk, bi) * ST, ST), ldb<RS>(Mb + btri(bk, bj) * ST, ST));
+          for (int a = 0; a < 3; ++a)
+            for (int b = 0; b < 3; ++b) {
+              const int r = 3 * bi + a, c = 3 * bj + b;
+              if (r >= n || c > r) continue;
+              put(r * n + c, X.a[a * 3 + b]);
+              if (c < r) put(c * n + r, X.a[a * 3 + b]);
+            }
+        }
+      }
+    }
+    return;
   }
   if constexpr (MASS) {   // dense symmetric M from the blocked lower triangle (the padding dofs are not written)
     if (live && io.jac) {

@@ -128,6 +128,20 @@ template <typename T> TDS_D void gemm_nn_sub(B9<T>& C, const B9<T>& A, const B9<
     for (int c = 0; c < 3; ++c)
       C.a[r * 3 + c] -= A.a[r * 3] * B.a[c] + A.a[r * 3 + 1] * B.a[3 + c] + A.a[r * 3 + 2] * B.a[6 + c];
 }
+// C += A^T * B
+template <typename T> TDS_D void gemm_tn_add(B9<T>& C, const B9<T>& A, const B9<T>& B) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      C.a[r * 3 + c] += A.a[r] * B.a[c] + A.a[3 + r] * B.a[3 + c] + A.a[6 + r] * B.a[6 + c];
+}
+template <typename T> TDS_D B9<T> b9_zero() {
+  B9<T> b;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) b.a[k] = T(0);
+  return b;
+}
 // inverse of the lower Cholesky factor of a diagonal block: i00, i10, i11, i20, i21, i22
 template <typename T> struct L6 { T i00, i10, i11, i20, i21, i22; };
 template <typename T> TDS_D L6<T> chol3_inv(const B9<T>& A) {
@@ -148,6 +162,12 @@ template <typename T> TDS_D L6<T> chol3_inv(const B9<T>& A) {
 }
 template <typename T> TDS_D L6<T> ldl6(const T* p, int s) { L6<T> r; r.i00 = p[0]; r.i10 = p[s]; r.i11 = p[2 * s]; r.i20 = p[3 * s]; r.i21 = p[4 * s]; r.i22 = p[5 * s]; return r; }
 template <typename T> TDS_D void stl6(T* p, int s, const L6<T>& r) { p[0] = r.i00; p[s] = r.i10; p[2 * s] = r.i11; p[3 * s] = r.i20; p[4 * s] = r.i21; p[5 * s] = r.i22; }
+// the lower-triangular block of an L6
+template <typename T> TDS_D B9<T> l6_full(const L6<T>& li) {
+  B9<T> b = b9_zero<T>();
+  b.a[0] = li.i00; b.a[3] = li.i10; b.a[4] = li.i11; b.a[6] = li.i20; b.a[7] = li.i21; b.a[8] = li.i22;
+  return b;
+}
 // X = A * Li^T   (off-diagonal block of L = A * L_jj^-T)
 template <typename T> TDS_D B9<T> mul_linvT(const B9<T>& A, const L6<T>& li) {
   B9<T> X;

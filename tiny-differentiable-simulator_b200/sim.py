@@ -890,6 +890,82 @@ class BatchSim:
         self._check(self._L.tds_b200_regressor_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(G_Y), _ptr(G_yT), _ptr(G_yV),
                                                           _ptr(g_q), _ptr(g_qd), _ptr(g_qdd), st), "regressor_vjp_device")
 
+    # ---- inverse mass matrix and operational-space inverse inertia (DESIGN.md section 7.20) ----
+    def _minv_points(self, links, local):
+        """The point table of the mass_inverse methods (None: no points, K = 0)."""
+        return self._kin_args([] if links is None else links, np.zeros((0, 3)) if local is None else local)
+
+    def mass_inverse_host(self, q, links=None, local=None):
+        """(Minv [n, n_qd, n_qd], Linv [n, 6K, 6K] or None without points) float64 at the fp32-rounded q [n, n_q]: the inverse of
+        mass_matrix_host(q) (bitwise symmetric; for a floating base not the forward dynamics' dqdd/dtau), and the operational-space
+        inverse inertia J Minv J^T of the point table links [K] / local [K, 3] (K <= 16), J the spatial point Jacobian of
+        point_motion_host ([n, K, 6, n_qd] flattened to 6K rows).  Installed masses, centres of mass and inertias enter."""
+        q = self._inv_in(q, self.n_q, "q")
+        keep, K, lp, cp = self._minv_points(links, local)
+        n = self.n_envs
+        Minv, Linv = np.zeros((n, self.n_qd, self.n_qd)), (np.zeros((n, 6 * K, 6 * K)) if K else None)
+        self._check(self._L.tds_b200_mass_inverse_host(self._h, _dp(q), K, lp, cp, _dp(Minv), _dp(Linv)), "mass_inverse_host")
+        return Minv, Linv
+
+    def mass_inverse_device(self, q, links, local, Minv=None, Linv=None, stream=None):
+        """Device version of mass_inverse_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride]; Minv [n_qd * n_qd, n_stride] and
+        Linv [36 K^2, n_stride] float64 CUDA tensors (either may be None, not both), entry (r, c) at row r * n_qd + c (r * 6K + c).  The
+        point table (None: none) is host data.  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._minv_points(links, local)
+        self._check(self._L.tds_b200_mass_inverse_device(self._h, _ptr(q), K, lp, cp, _ptr(Minv), _ptr(Linv), st), "mass_inverse_device")
+
+    def mass_inverse_jvp_host(self, q, links=None, local=None, t_q=None, t_par=None):
+        """Directional derivatives of the outputs of mass_inverse_host along m tangents t_q [n, n_q, m] of q and t_par [n, k, m] of the
+        installed parameters (either may be None, not both): (Minv, Linv, dMinv [n, n_qd, n_qd, m], dLinv [n, 6K, 6K, m] or None);
+        tangents given as [n, dim] are m = 1 and drop the last axis."""
+        q = self._inv_in(q, self.n_q, "q")
+        keep, K, lp, cp = self._minv_points(links, local)
+        (tq, tp), m, single = self._tangents([(t_q, self.n_q), (t_par, len(self.param_ids))], names="t_q and t_par")
+        n, nd = self.n_envs, self.n_qd
+        Minv, dMinv = np.zeros((n, nd, nd)), np.zeros((n, nd, nd, max(m, 1)))
+        Linv, dLinv = (np.zeros((n, 6 * K, 6 * K)), np.zeros((n, 6 * K, 6 * K, max(m, 1)))) if K else (None, None)
+        self._check(self._L.tds_b200_mass_inverse_jvp_host(self._h, _dp(q), K, lp, cp, m, _dp(tq), _dp(tp), _dp(Minv), _dp(Linv), _dp(dMinv),
+                                                           _dp(dLinv)), "mass_inverse_jvp_host")
+        if single:
+            dMinv, dLinv = dMinv[..., 0], (None if dLinv is None else dLinv[..., 0])
+        return Minv, Linv, dMinv, dLinv
+
+    def mass_inverse_jvp_device(self, q, links, local, m, t_q, t_par, t_Minv=None, t_Linv=None, Minv=None, Linv=None, stream=None):
+        """Device version of mass_inverse_jvp_host: q float32 [n_q, n_stride]; t_q [n_q * m, n_stride], t_par [k * m, n_stride] (either may
+        be None, not both); t_Minv [n_qd^2 * m, n_stride], t_Linv [36 K^2 * m, n_stride] (either may be None, not both), Minv and Linv
+        (values, or None) float64 CUDA tensors, entry (r, j) at row r * m + j.  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._minv_points(links, local)
+        self._check(self._L.tds_b200_mass_inverse_jvp_device(self._h, _ptr(q), K, lp, cp, int(m), _ptr(t_q), _ptr(t_par), _ptr(Minv),
+                                                             _ptr(Linv), _ptr(t_Minv), _ptr(t_Linv), st), "mass_inverse_jvp_device")
+
+    def mass_inverse_vjp_host(self, q, links=None, local=None, G_Minv=None, G_Linv=None):
+        """Cotangents G_Minv [n, n_qd, n_qd] and G_Linv [n, 6K, 6K] (None: zero, not both) -> (g_q [n, n_q], g_par [n, k] or None without
+        installed parameters) = sum G * d(outputs)/dx."""
+        q = self._inv_in(q, self.n_q, "q")
+        keep, K, lp, cp = self._minv_points(links, local)
+        if G_Minv is None and G_Linv is None:
+            raise ValueError("at least one cotangent is expected")
+        n = self.n_envs
+        G_Minv = None if G_Minv is None else self._inv_in(np.reshape(G_Minv, (n, -1)), self.n_qd * self.n_qd, "G_Minv")
+        G_Linv = None if G_Linv is None else self._inv_in(np.reshape(G_Linv, (n, -1)), 36 * K * K, "G_Linv")
+        k = len(self.param_ids)
+        g_q = np.zeros((n, self.n_q))
+        g_par = np.zeros((n, k)) if k else None
+        self._check(self._L.tds_b200_mass_inverse_vjp_host(self._h, _dp(q), K, lp, cp, _dp(G_Minv), _dp(G_Linv), _dp(g_q), _dp(g_par)),
+                    "mass_inverse_vjp_host")
+        return g_q, g_par
+
+    def mass_inverse_vjp_device(self, q, links, local, G_Minv, G_Linv, g_q, g_par=None, stream=None):
+        """Device version of mass_inverse_vjp_host: q float32 [n_q, n_stride], cotangents float64 in the layouts of mass_inverse_device
+        (None: zero, not both), g_q [n_q, n_stride] and g_par [k, n_stride] float64 CUDA tensors (either may be None, not both).
+        Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp = self._minv_points(links, local)
+        self._check(self._L.tds_b200_mass_inverse_vjp_device(self._h, _ptr(q), K, lp, cp, _ptr(G_Minv), _ptr(G_Linv), _ptr(g_q), _ptr(g_par),
+                                                             st), "mass_inverse_vjp_device")
+
     def jacobian_chunk(self):
         """Directions (Jacobian columns or JVP tangents) one launch of the dual-number step takes; more run in several launches."""
         return self._L.tds_b200_jacobian_chunk(self._h)
