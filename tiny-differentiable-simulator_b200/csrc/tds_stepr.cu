@@ -45,6 +45,7 @@ struct RoleWarps {
 
 }  // namespace tdsteam
 
+#ifndef TDS_TEAM_KERNEL_ONLY   // launcher: not part of the host-compiled kernel source (tests/cpp/team_host.cpp)
 // The link table lives in constant memory: one table resident per device.  `token` identifies the table of the
 // calling simulator; a different token re-uploads (after draining the device, since kernels of the previous owner
 // may still be reading the symbol).  Not allowed while the stream is being captured into a CUDA graph.
@@ -77,3 +78,4 @@ extern "C" int tds_launch_stepr(const TeamModel* TM, const TeamLink* tl_host, un
 
 // bytes of shared memory (or global scratch) one tile of 32 environments needs
 extern "C" size_t tds_stepr_tile_bytes(const TeamModel* TM) { return tdsteam::RoleWarps::tile_bytes(*TM); }
+#endif  // TDS_TEAM_KERNEL_ONLY

@@ -30,6 +30,7 @@ struct LaneTeam {
 
 }  // namespace tdsteam
 
+#ifndef TDS_TEAM_KERNEL_ONLY   // launcher: not part of the host-compiled kernel source (tests/cpp/team_host.cpp)
 extern "C" int tds_launch_stept(const TeamModel* TM, const TeamLink* tl_dev, const DevModel* M, const SimParams* P,
                                 const EnvParams* E, const StepIO* io, int mode, int use_pd, int precision,
                                 char* gscratch, int use_smem, cudaStream_t stream) {
@@ -39,3 +40,4 @@ extern "C" int tds_launch_stept(const TeamModel* TM, const TeamLink* tl_dev, con
 
 // bytes of shared memory (or global scratch) one warp of 8 environments needs
 extern "C" size_t tds_stept_tile_bytes(const TeamModel* TM) { return tdsteam::LaneTeam::tile_bytes(*TM); }
+#endif  // TDS_TEAM_KERNEL_ONLY

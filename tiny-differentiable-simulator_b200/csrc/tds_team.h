@@ -192,9 +192,6 @@ static inline int tds_build_team(const DevModel* D, const EnvParams* E, TeamMode
         L.par_slot = att_slot[p + 1];          // -1 for a fixed base: dropped
       } else if (L.lpar == k - 1 && !(k == n_trunk && !trunk[i])) {
         L.flags |= TDS_TF_PARENT_ADJ;          // carry (for k == 0 the parent is the base)
-      } else if (p < 0) {
-        // non-adjacent trunk root hanging off the base
-        if (D->floating) { if (trunk_acc[0] < 0) trunk_acc[0] = -2; }
       }
       if (k == 0 && p < 0 && trunk[i]) L.flags |= TDS_TF_PARENT_ADJ;
     }
@@ -204,7 +201,12 @@ static inline int tds_build_team(const DevModel* D, const EnvParams* E, TeamMode
       TeamLink& L = (*table)[(size_t)r * TDS_TEAM_MAXK + k];
       if (L.flags & (TDS_TF_PARENT_ADJ | TDS_TF_PARENT_TRUNK)) continue;
       const int p = D->parent[i];
-      if (p < 0) continue;  // handled through base slot below
+      if (p < 0) {           // a trunk root after the first (the trunk grew into several children of the base)
+        if (!D->floating) continue;          // fixed base: dropped, as for subtrees
+        if (trunk_acc[0] < 0) trunk_acc[0] = (att_slot[0] >= 0) ? att_slot[0] : (TM->n_att + 64 + trunk_internal++);
+        L.par_slot = trunk_acc[0];           // the base reads it through base_slot
+        continue;
+      }
       // parent p is in this list, non adjacent
       if (trunk[i]) {        // trunk-internal branch (role independent numbering)
         if (trunk_acc[p + 1] < 0) trunk_acc[p + 1] = (att_slot[p + 1] >= 0) ? att_slot[p + 1] : (TM->n_att + 64 + trunk_internal++);
@@ -222,6 +224,7 @@ static inline int tds_build_team(const DevModel* D, const EnvParams* E, TeamMode
   for (auto& L : *table) if (L.par_slot >= TM->n_att + 64) L.par_slot = L.par_slot - 64 + own_int_max;
   TM->n_acc = TM->n_att + own_int_max + trunk_internal;
   TM->base_slot = D->floating ? att_slot[0] : -1;
+  if (D->floating && TM->base_slot < 0 && trunk_acc[0] >= 0) TM->base_slot = trunk_acc[0] - 64 + own_int_max;
   // receiving side: acc_slot of a link = the par_slot its non-carried children use
   for (int r = 0; r < T; ++r)
     for (int k = 0; k < TM->n_loc[r]; ++k) {

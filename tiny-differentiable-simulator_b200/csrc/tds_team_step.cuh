@@ -87,6 +87,7 @@ tds_team_step_kernel(const __grid_constant__ TeamModel TM, const TeamLink* __res
 #define TDST_PHASE() do { if (io.phase_clk && lane == 0) io.phase_clk[Map::clock_row(tile, role) * 16 + phase_id] = clock64(); ++phase_id; } while (0)
   TDST_PHASE();
 
+#ifndef TDS_TEAM_KERNEL_ONLY   // (the host-compiled copy of the kernel source in tests/cpp has no PTX)
   if constexpr (!Map::ROLE_WARPS) {
     // warm L1 with the per-role link tables (read many times below through the non-coherent path) and issue the
     // loads of this team's coordinates early; a lone warp otherwise pays one L2 round trip per first touch
@@ -94,6 +95,7 @@ tds_team_step_kernel(const __grid_constant__ TeamModel TM, const TeamLink* __res
     const int lines = (TDS_TEAM_T * TDS_TEAM_MAXK * (int)sizeof(TeamLink) + 127) / 128;
     for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L1 [%0];" ::"l"(tbl + (size_t)l * 128));
   }
+#endif
 
   float* const tq = tp(TM.t_q, 0.f);
   float* const tqd = tp(TM.t_qd, 0.f);
@@ -922,6 +924,9 @@ tds_team_step_kernel(const __grid_constant__ TeamModel TM, const TeamLink* __res
     float& qr = q_ref(k, qi, ld);
     qr = (float)(RC(qr) + RC(qd_ref(k, qdi, ld)) * RC(P.dt));
   }
+  // reward / done read coordinates that another role may have just corrected and integrated (on a fixed base every
+  // subtree hangs off the base, so q[0..6] need not be role 0's)
+  if (E.reward_kind) Map::sync();
   int done_i = 0;
   if (role == 0) {
     bool done = false;
@@ -959,6 +964,7 @@ tds_team_step_kernel(const __grid_constant__ TeamModel TM, const TeamLink* __res
 }
 #undef TDST_PHASE
 
+#ifndef TDS_TEAM_KERNEL_ONLY   // launchers: not part of the host-compiled kernel source (tests/cpp/team_host.cpp)
 // Host side: one launch of tds_team_step_kernel<Map, RA, RC, RS, SM>.  The dynamic shared-memory limit is raised
 // once per instance and device.
 template <class Map, typename RA, typename RC, typename RS, bool SM>
@@ -995,5 +1001,6 @@ int launch_team_step(const TeamModel* TM, const TeamLink* tl, const DevModel* M,
 #undef TDST_LAUNCH
   return (int)err;
 }
+#endif  // TDS_TEAM_KERNEL_ONLY
 
 }  // namespace tdsteam
