@@ -447,6 +447,57 @@ int tds_b200_mass_inverse_vjp_device(tds_b200_sim* sim, const float* q, int K, c
 int tds_b200_mass_inverse_vjp_host(tds_b200_sim* sim, const double* q, int K, const int* links, const double* local, const double* G_Minv,
                                    const double* G_Linv, double* g_q, double* g_par);
 
+/* ---- point-constrained forward dynamics qdd, f = FD_c(q, qd, tau) (DESIGN.md section 7.21) ----------------------------------------------
+ * At the fp32-rounded q, qd and tau (qd or tau may be NULL, meaning zero; tau has one row per dof, a floating base's rows 0..5 being an
+ * applied wrench on the base in the base frame as in tds_b200_inverse_dynamics_*, zero for an unactuated base), for a point table of
+ * 0 <= K <= TDS_B200_MAX_OSIM_POINTS points (links / local as in tds_b200_point_motion_*, host memory) each held in dims = 3 rows (its
+ * linear rows: a point contact that neither slips nor lifts off) or dims = 6 rows (all: a welded frame), with a damping eps >= 0 (finite):
+ * with M, h and J, J' qd exactly what tds_b200_mass_matrix_*, tds_b200_inverse_dynamics_*(q, qd, NULL) and tds_b200_point_motion_*(q, qd,
+ * NULL) (its J and acc) return at the same inputs and installed parameters, and J_c, d_c their constrained rows (rows 6k + 3 .. 6k + 5
+ * of point k for dims 3, all six for dims 6), the KKT system
+ *     M qdd - J_c^T f = tau - h,      J_c qdd = -d_c - eps f
+ * solved as f = -(J_c M^-1 J_c^T + eps I)^-1 (J_c M^-1 (tau - h) + d_c), qdd = M^-1 (tau - h + J_c^T f), in fp64:
+ *   qdd [n_qd]; f [dims K]: per point the force (dims 3) or the wrench [n; f] (dims 6) the constraint applies to the robot at the point, in
+ *   world axes (the convention of tds_b200_step_wrench_*'s W: its generalised force is J_c^T f), component r of point k at row dims k + r.
+ * K = 0 is the unconstrained forward dynamics qdd = M^-1 (tau - h) in the coordinates of M, so tds_b200_inverse_dynamics_*(q, qd, qdd) =
+ * tau on every base; on fixed bases (worlds of several multibodies included) it is the MODE_FD step's qdd, h carrying the stiffness and
+ * damping terms.  For a floating base it is not the MODE_FD step's qdd (the reference's floating-base forward dynamics does not invert its
+ * own M).  A world of several multibodies is supported: a point constrains only its own multibody's dofs.  If a pivot of the Cholesky
+ * factor of J_c M^-1 J_c^T + eps I is <= 0 (a structurally rank-deficient table at eps = 0, e.g. a 3-row point on a planar chain), that
+ * environment's outputs are NaN and the others are unaffected; near-singular tables are the caller's to regularise with eps.
+ * Either output may be NULL, not both.  Argument checks -> -1: NULL q; no output (tangent output, cotangent); K out of range, a link
+ * index out of range, NULL links / local with K > 0; dims not 3 or 6; damping negative or not finite; f (t_f, G_f) with K = 0; m < 1 or
+ * every tangent NULL; no gradient output.  -> -4: t_par / g_par without an installed set.
+ *   device: q [n_q][n_stride], qd and tau [n_qd][n_stride] fp32 as tds_b200_step_device; qdd [n_qd][n_stride], f [dims K][n_stride] fp64.
+ *           Asynchronous on `stream`.
+ *   host:   q [n][n_q], qd and tau [n][n_qd] fp64 (rounded to fp32); qdd [n][n_qd], f [n][K][dims].  Synchronous.
+ * _jvp: the derivatives along m tangents of q, qd, tau and the installed parameters (each may be NULL: zero, not all), by the dual-number
+ *   instances of the inverse dynamics, mass inverse and point motion and of the solve (which differentiates the factorisation), one lane per
+ *   (environment, tangent), in chunks of tangents; qdd and f (may be NULL) receive the values.  Device t_q [n_q * m][n_stride], t_qd and
+ *   t_tau [n_qd * m][n_stride], t_par [k * m][n_stride], t_qdd [n_qd * m][n_stride], t_f [dims K m][n_stride] (entry (r, j) at
+ *   (r * m + j) * n_stride + e); host t_q [n][n_q][m], t_qd and t_tau [n][n_qd][m], t_par [n][k][m], t_qdd [n][n_qd][m], t_f [n][dims K][m].
+ * _vjp: g_x[c] = <G_qdd, dqdd/dx_c> + <G_f, df/dx_c> for x = q, qd, tau and, while a set is installed, the parameters, for cotangents in the
+ *   outputs' layouts (NULL: zero, not both): the JVP along the n_q + 2 n_qd (+ k) identity tangents contracted with G on the device.  Any of
+ *   g_q, g_qd, g_tau, g_par may be NULL, not all.  Device g_q [n_q][n_stride], g_qd and g_tau [n_qd][n_stride], g_par [k][n_stride] fp64
+ *   (asynchronous); host g_q [n][n_q], g_qd and g_tau [n][n_qd], g_par [n][k] (synchronous). */
+int tds_b200_constrained_dynamics_device(tds_b200_sim* sim, const float* q, const float* qd, const float* tau, int K, const int* links,
+                                         const double* local, int dims, double damping, double* qdd, double* f, void* stream);
+int tds_b200_constrained_dynamics_host(tds_b200_sim* sim, const double* q, const double* qd, const double* tau, int K, const int* links,
+                                       const double* local, int dims, double damping, double* qdd, double* f);
+int tds_b200_constrained_dynamics_jvp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* tau, int K, const int* links,
+                                             const double* local, int dims, double damping, int m, const double* t_q, const double* t_qd,
+                                             const double* t_tau, const double* t_par, double* qdd, double* f, double* t_qdd, double* t_f,
+                                             void* stream);
+int tds_b200_constrained_dynamics_jvp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* tau, int K, const int* links,
+                                           const double* local, int dims, double damping, int m, const double* t_q, const double* t_qd,
+                                           const double* t_tau, const double* t_par, double* qdd, double* f, double* t_qdd, double* t_f);
+int tds_b200_constrained_dynamics_vjp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* tau, int K, const int* links,
+                                             const double* local, int dims, double damping, const double* G_qdd, const double* G_f,
+                                             double* g_q, double* g_qd, double* g_tau, double* g_par, void* stream);
+int tds_b200_constrained_dynamics_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* tau, int K, const int* links,
+                                           const double* local, int dims, double damping, const double* G_qdd, const double* G_f,
+                                           double* g_q, double* g_qd, double* g_tau, double* g_par);
+
 /* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
  * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
  * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,

@@ -57,6 +57,11 @@ forward-mode rule (BatchSim.step_wrench_jvp_device).
 regressor(sim, q, qd=None, qdd=None) is the joint-torque regressor Y and the energy regressors yT, yV of the inertial parameters (float64,
 DESIGN.md section 7.19) with a backward rule (BatchSim.regressor_vjp_device: float32 q.grad, qd.grad, qdd.grad) and a forward-mode rule
 (BatchSim.regressor_jvp_device).
+
+constrained_dynamics(sim, q, qd=None, tau=None, links=None, local=None, dims=3, damping=0.0, params=None) is the forward dynamics qdd with
+the points of a table held in place and the constraint forces f (float64, DESIGN.md section 7.21), with a backward rule
+(BatchSim.constrained_dynamics_vjp_device: float32 q.grad, qd.grad, tau.grad, float64 params.grad) and a forward-mode rule
+(BatchSim.constrained_dynamics_jvp_device).
 """
 from collections import namedtuple
 
@@ -334,9 +339,8 @@ def _state_soa(sim, q, qd, qdd):
 
 
 class _Query(torch.autograd.Function):
-    """The dynamics queries (mass_matrix, inverse_dynamics, centroidal, forward_kinematics, point_motion, regressor, mass_inverse) as one
-    Function over
-    a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
+    """The dynamics queries (mass_matrix, inverse_dynamics, centroidal, forward_kinematics, point_motion, regressor, mass_inverse,
+    constrained_dynamics) as one Function over a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
     float64 output buffers, every C-ABI call ordered on a side stream, and the gradients as float32 (q, qd, qdd) and float64 (params).
     An input the query does not take, or the call leaves out, is None and gets no gradient; a tangent on it is ignored.  With params
     the forward installs their values, and the backward and forward-mode rule reinstall the values of this call (a later call of the
@@ -771,3 +775,43 @@ def mass_inverse(sim, q, links=None, local=None, params=None):
     p = _Points(*sim._points([] if links is None else links, np.zeros((0, 3)) if local is None else local))
     Minv, Linv = _Query.apply(_MASS_INVERSE, sim, p, q, None, None, params)
     return Minv, (Linv if p.K else None)
+
+
+_CdPoints = namedtuple("_CdPoints", "links local K dims damping")   # the point table of _Points with the constraint's dims and damping
+
+# tau rides in the qdd slot (n_qd float32, as qdd).  Without points (K = 0) the entries get None for f and its cotangent, and the
+# Function's f is [n_envs, 0, dims].
+_CONSTRAINED_DYNAMICS = _QuerySpec(
+    rows=lambda sim, p: [sim.n_qd, p.dims * p.K],
+    unpack=lambda sim, p, qdd, f: (qdd.contiguous(), f.reshape(sim.n_envs, p.K, p.dims).contiguous()),
+    pack=lambda sim, p, gqdd, gf: [_cot(gqdd, sim), _cot(gf, sim) if p.K else None],
+    value=lambda sim, p, x, out, st: sim.constrained_dynamics_device(x.q, x.qd, x.qdd, p.links, p.local, p.dims, p.damping, out[0],
+                                                                     out[1] if p.K else None, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.constrained_dynamics_jvp_device(x.q, x.qd, x.qdd, p.links, p.local, p.dims, p.damping, 1, t.q,
+                                                                         t.qd, t.qdd, t.params, out[0], out[1] if p.K else None,
+                                                                         stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.constrained_dynamics_vjp_device(x.q, x.qd, x.qdd, p.links, p.local, p.dims, p.damping, *G, g.q,
+                                                                       g.qd, g.qdd, g.params, stream=st))
+
+
+def constrained_dynamics(sim, q, qd=None, tau=None, links=None, local=None, dims=3, damping=0.0, params=None):
+    """The point-constrained forward dynamics of every environment of `sim` (a BatchSim), DESIGN.md section 7.21, in fp64 at the
+    fp32-rounded q [n_envs, n_q], qd and tau [n_envs, n_qd] float32 CUDA tensors (qd or tau None: zero; a floating base's tau[0:6] is a
+    wrench on the base in the base frame, as for inverse_dynamics): (qdd [n_envs, n_qd], f [n_envs, K, dims] or None without points)
+    float64 with M qdd - J_c^T f = tau - h and J_c qdd = -d_c - damping f, for M = mass_matrix(sim, q, params), h = inverse_dynamics(sim,
+    q, qd, params=params) and J, d = point_motion(sim, q, qd, links, local)'s J and acc, J_c and d_c their rows held by the constraint:
+    the 3 linear rows of each point (dims 3, a point contact that neither slips nor lifts off) or all 6 (dims 6, a welded frame).  f is the
+    force (or wrench [n; f]) the constraint applies to the robot at each point, in world axes, as step_wrench's W.  The point table links
+    [K] (-1: the base) / local [K, 3] (K <= 16), dims and damping >= 0 are constants of the call; K = 0 is the unconstrained forward
+    dynamics M^-1 (tau - h).  An environment whose J_c M^-1 J_c^T + damping I has a pivot <= 0 gets NaN outputs.  params: None, or a
+    float64 CUDA tensor [n_envs, k] of values for the parameters installed by sim.set_physical_params (then also differentiated).
+    Differentiable in reverse mode (float32 q.grad, qd.grad, tau.grad, float64 params.grad) and forward mode."""
+    _check_state(sim, q, qd)
+    if tau is not None and (tau.dtype != torch.float32 or not tau.is_cuda or tuple(tau.shape) != (sim.n_envs, sim.n_qd)):
+        raise ValueError("tau: a float32 CUDA tensor [n_envs, n_qd] is expected")
+    _check_params(sim, params)
+    if dims not in (3, 6):
+        raise ValueError("dims: 3 (the points' linear rows) or 6 (all six rows) is expected")
+    p = _CdPoints(*sim._points([] if links is None else links, np.zeros((0, 3)) if local is None else local), int(dims), float(damping))
+    qdd, f = _Query.apply(_CONSTRAINED_DYNAMICS, sim, p, q, qd, tau, params)
+    return qdd, (f if p.K else None)

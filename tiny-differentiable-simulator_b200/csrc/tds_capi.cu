@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -98,6 +99,8 @@ extern "C" int tds_launch_mass_inverse_jvp(const DevModel* M, const StepIO* io, 
                                            int m, int n_dirs, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_osim(const double* J, const double* dJ, const double* Mi, const double* dMi, double* L, int K, int n_qd, int m,
                                int n, int ns, cudaStream_t stream);
+// the rows and the solve of the point-constrained forward dynamics (tds_constrained.cu)
+extern "C" int tds_launch_cdyn(const TdsCdynCall* c, int dual, int n, int ns, cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
@@ -450,6 +453,7 @@ struct tds_b200_sim {
   float* wrench_dev = nullptr; size_t wrench_dev_bytes = 0;   // host paths of the step with wrenches: W [6K][ns] fp32
   double* mass_dev = nullptr; size_t mass_dev_bytes = 0; // dynamics queries' VJPs: identity tangents | output columns of a chunk
   double* minv_dev = nullptr; size_t minv_dev_bytes = 0; // the inverse mass matrix's intermediates: M^-1, J and their tangents
+  double* cdyn_dev = nullptr; size_t cdyn_dev_bytes = 0; // the constrained dynamics' intermediates: h, M^-1, J, drift, solve, tangents
   // installed physical parameters (tds_b200_set_physical_params_*): slot map (par.n == 0: none) and values [k][ns] fp64
   ParMap par;
   double* par_dev = nullptr; size_t par_dev_bytes = 0;
@@ -729,6 +733,7 @@ void tds_b200_destroy(tds_b200_sim* s) {
   cudaFree(s->pol_params); cudaFree(s->act_qidx); cudaFree(s->r_steps);
   cudaFree(s->c_count); cudaFree(s->c_links); cudaFree(s->c_cand); cudaFree(s->jac_scratch); cudaFree(s->jac_dev);
   cudaFree(s->vjp_buf); cudaFree(s->vjp_flag); cudaFree(s->vjp_g); cudaFree(s->par_dev); cudaFree(s->mass_dev); cudaFree(s->minv_dev); cudaFree(s->wrench_dev);
+  cudaFree(s->cdyn_dev);
   cudaFree(s->cdist); cudaFree(s->link_xf); cudaFree(s->scratch); cudaFree(s->stage_dev); cudaFree(s->phase_clk); cudaFree(s->team_dev);
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
@@ -2140,6 +2145,240 @@ int tds_b200_mass_inverse_vjp_host(tds_b200_sim* s, const double* q, int K, cons
                             g_par ? g_d + (size_t)n_q * ns : nullptr, s->stream))
     return rc;
   CUDA_TRY(get_parts<double>({{g_q, (size_t)n_q}, {g_par, (size_t)k}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- point-constrained forward dynamics (DESIGN.md section 7.21): h = ID(q, qd, 0), M^-1, the point Jacobian and its drift from the INV,
+// MINV and MOT instances of the world-frame kernel (inv_run, the mass inverse's value launch, mot_run, and their JVPs through
+// jacobian_run), then the rows and the solve of tds_constrained.cu.  The inputs q | qd | tau are those of inverse dynamics with tau in the
+// qdd slot (inv_n_in, put_inv_inputs).
+struct CdynCall { int K; const int* links; const double* local; int dims; double eps; };
+
+// tangents [j0, j0 + mc) of src [rows * m][ns] -> dst [rows * mc][ns] (src NULL: zeros)
+static cudaError_t tangent_slice(double* dst, const double* src, size_t rows, int m, int j0, int mc, size_t ns, cudaStream_t sm) {
+  if (!rows) return cudaSuccess;
+  if (!src) return cudaMemsetAsync(dst, 0, sizeof(double) * rows * mc * ns, sm);
+  return cudaMemcpy2DAsync(dst, sizeof(double) * mc * ns, src + (size_t)j0 * ns, sizeof(double) * m * ns, sizeof(double) * mc * ns, rows,
+                           cudaMemcpyDeviceToDevice, sm);
+}
+
+static int cdyn_launch(tds_b200_sim* s, const TdsCdynCall& c, bool dual, cudaStream_t sm) {
+  const int rc = tds_launch_cdyn(&c, dual ? 1 : 0, s->n, s->ns, sm);
+  if (rc) set_err(std::string("constrained dynamics launch: ") + cudaGetErrorString((cudaError_t)rc));
+  return rc;
+}
+
+// qdd [n_qd][ns] and f [R][ns] (R = dims K; either may be NULL) from q [n_q][ns], qd and tau [n_qd][ns] fp32 (either NULL: zero) and,
+// with m >= 1 tangents t_q [n_q * m][ns], t_qd and t_tau [n_qd * m][ns], t_par [k * m][ns] (each may be NULL: zero), their tangents
+// t_qdd [n_qd * m][ns] and t_f [R * m][ns] (either may be NULL).  Everything else goes to s->cdyn_dev: the values of h, M^-1, J, the
+// drift and the value solve's scratch, then the tangents of one chunk of directions (within 1 GB) after another.
+static int cdyn_run(tds_b200_sim* s, const float* q, const float* qd, const float* tau, const CdynCall& cc, double* qdd, double* f, int m,
+                    const double* t_q, const double* t_qd, const double* t_tau, const double* t_par, double* t_qdd, double* t_f,
+                    cudaStream_t sm) {
+  const DevModel& D = s->dm[0];
+  const int K = cc.K, nd = D.n_qd, n_q = D.n_q, k = s->par.n;
+  const size_t ns = s->ns, nn = (size_t)nd * nd, nJ = (size_t)6 * K * nd, nA = (size_t)6 * K, R = (size_t)cc.dims * K;
+  const size_t n_in = (size_t)inv_n_in(s), scr = R * nd + R * R + R;
+  const bool tan = m > 0 && (t_qdd || t_f);
+  // per tangent of a chunk: q | qd | 0 tangents, t_par, t_tau, dh, dM^-1, dJ, d drift, and the (value, tangent) pairs of the scratch
+  const size_t per = n_in + k + 2 * (size_t)nd + nn + nJ + nA + 2 * scr;
+  const size_t fit = std::max<size_t>(1, ((size_t)1 << 30) / (sizeof(double) * per * ns));
+  const int chunk = tan ? (int)std::min<size_t>(std::min<size_t>((size_t)m, 65535), fit) : 0;   // (gridDim.y, gridDim.z)
+  CUDA_TRY(grow_dev(&s->cdyn_dev, &s->cdyn_dev_bytes, sizeof(double) * (nd + nn + nJ + nA + scr + per * chunk + 1) * ns));
+  double* const h = s->cdyn_dev;
+  double* const Mi = h + nd * ns;
+  double* const J = Mi + nn * ns;
+  double* const acc = J + nJ * ns;
+  double* const Y = acc + nA * ns;
+  double* const w = Y + scr * ns;
+  if (int rc = inv_run(s, q, qd, nullptr, h, sm)) return rc;
+  int rc = value_run(s, "constrained dynamics", q, nullptr, nullptr, Mi, [&](const StepIO* io, const ParMap* pm) {
+    return tds_launch_mass_inverse(&s->dm_m, io, pm, s->jac_scratch, sm);
+  });
+  if (rc) return rc;
+  if (K > 0) {
+    const TdsMotCall mc{K, cc.links, cc.local, J, nullptr, acc};
+    if (int rc = mot_run(s, q, qd, nullptr, &mc, sm)) return rc;
+  }
+  TdsCdynCall c;
+  memset(&c, 0, sizeof(c));
+  c.K = K; c.dims = cc.dims; c.n_qd = nd; c.m = 1; c.m_out = 1; c.eps = cc.eps;
+  c.tau = tau; c.h = h; c.Mi = Mi; c.J = J; c.acc = acc;
+  c.Y = Y; c.A = Y + R * nd * ns; c.b = c.A + R * R * ns;
+  if (qdd || f) {
+    c.qdd = qdd; c.f = f;
+    if (int rc = cdyn_launch(s, c, false, sm)) return rc;
+  }
+  if (!tan) return 0;
+  const bool d_h = t_q || t_qd || t_par, d_Mi = t_q || t_par, d_J = K > 0 && (t_q || t_qd);
+  for (int j0 = 0; j0 < m; j0 += chunk) {
+    const int mc = std::min(chunk, m - j0);
+    double* const T = w;   // q | qd | qdd tangents of the INV and MOT JVPs, the qdd ones zero
+    double* const Tp = T + n_in * mc * ns;
+    double* const Tt = Tp + (size_t)k * mc * ns;
+    double* const dh = Tt + (size_t)nd * mc * ns;
+    double* const dMi = dh + (size_t)nd * mc * ns;
+    double* const dJ = dMi + nn * mc * ns;
+    double* const dacc = dJ + nJ * mc * ns;
+    double* const P = dacc + nA * mc * ns;   // Y | dY | A | dA | b | db
+    CUDA_TRY(tangent_slice(T, t_q, n_q, m, j0, mc, ns, sm));
+    CUDA_TRY(tangent_slice(T + (size_t)n_q * mc * ns, t_qd, nd, m, j0, mc, ns, sm));
+    CUDA_TRY(tangent_slice(T + (size_t)(n_q + nd) * mc * ns, nullptr, nd, m, j0, mc, ns, sm));
+    if (t_par) CUDA_TRY(tangent_slice(Tp, t_par, k, m, j0, mc, ns, sm));
+    if (t_tau) CUDA_TRY(tangent_slice(Tt, t_tau, nd, m, j0, mc, ns, sm));
+    if (d_h) {
+      const JvpTangents jv{T, t_par ? Tp : nullptr, mc, Query::inv};
+      if (int rc = jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, nullptr, dh, sm, false, &jv)) return rc;
+    }
+    if (d_Mi) {   // (the qd tangents do not enter M^-1)
+      const JvpTangents jv{t_q ? T : nullptr, t_par ? Tp : nullptr, mc, Query::minv};
+      if (int rc = jacobian_run(s, TDS_B200_MODE_FULL, 0, q, nullptr, nullptr, dMi, sm, false, &jv)) return rc;
+    }
+    if (d_J) {
+      const TdsMotCall dmc{K, cc.links, cc.local, dJ, nullptr, dacc};
+      if (int rc = mot_jvp_run(s, q, qd, nullptr, &dmc, mc, T, sm)) return rc;
+    }
+    TdsCdynCall dc = c;
+    dc.m = mc; dc.j0 = j0; dc.m_out = m;
+    dc.dtau = t_tau ? Tt : nullptr; dc.dh = d_h ? dh : nullptr; dc.dMi = d_Mi ? dMi : nullptr;
+    dc.dJ = d_J ? dJ : nullptr; dc.dacc = d_J ? dacc : nullptr;
+    dc.Y = P; dc.dY = dc.Y + R * nd * mc * ns; dc.A = dc.dY + R * nd * mc * ns; dc.dA = dc.A + R * R * mc * ns;
+    dc.b = dc.dA + R * R * mc * ns; dc.db = dc.b + R * mc * ns;
+    dc.qdd = t_qdd; dc.f = t_f;
+    if (int rc = cdyn_launch(s, dc, true, sm)) return rc;
+  }
+  return 0;
+}
+
+// g_in [n_q + 2 n_qd][ns] (q | qd | tau, contiguous) and g_par [k][ns] (NULL: not wanted) = <G, d(qdd | f)>, G [n_qd + R][ns]
+static int cdyn_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const float* tau, const CdynCall& cc, const double* G,
+                        double* g_in, double* g_par, cudaStream_t sm) {
+  const size_t ns = s->ns, n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, R = (size_t)cc.dims * cc.K;
+  return vjp_by_eye(s, "constrained dynamics", inv_n_in(s), nd + R, G, g_in, g_par, sm,
+                    [&](int m, const double* t_in, const double* t_par, double* dO) {
+                      return cdyn_run(s, q, qd, tau, cc, nullptr, nullptr, m, t_in, t_in + n_q * m * ns, t_in + (n_q + nd) * m * ns, t_par,
+                                      dO, R ? dO + nd * m * ns : nullptr, sm);
+                    });
+}
+
+// -1: no q, no output (tangent output, cotangent), K out of [0, TDS_B200_MAX_OSIM_POINTS], dims not 3 or 6, damping negative or not
+// finite, f (t_f, G_f) with K = 0, a missing or bad point table
+static int cdyn_check(tds_b200_sim* s, const void* q, const CdynCall& cc, const void* qdd, const void* f) {
+  if (!s || !q || (!qdd && !f)) return -1;
+  if (cc.K < 0 || cc.K > TDS_B200_MAX_OSIM_POINTS) { set_err("constrained dynamics: K out of [0, TDS_B200_MAX_OSIM_POINTS]"); return -1; }
+  if (cc.dims != 3 && cc.dims != 6) { set_err("constrained dynamics: dims is 3 or 6"); return -1; }
+  if (!(cc.eps >= 0.0) || !std::isfinite(cc.eps)) { set_err("constrained dynamics: damping must be finite and >= 0"); return -1; }
+  if (f && cc.K < 1) { set_err("constrained dynamics: f needs K >= 1 points"); return -1; }
+  return kin_check(s, q, cc.K, cc.links, cc.local);
+}
+
+int tds_b200_constrained_dynamics_device(tds_b200_sim* s, const float* q, const float* qd, const float* tau, int K, const int* links,
+                                         const double* local, int dims, double damping, double* qdd, double* f, void* stream) {
+  const CdynCall cc{K, links, local, dims, damping};
+  if (int rc = cdyn_check(s, q, cc, qdd, f)) return rc;
+  return cdyn_run(s, q, qd, tau, cc, qdd, f, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+int tds_b200_constrained_dynamics_host(tds_b200_sim* s, const double* q, const double* qd, const double* tau, int K, const int* links,
+                                       const double* local, int dims, double damping, double* qdd, double* f) {
+  const CdynCall cc{K, links, local, dims, damping};
+  if (int rc = cdyn_check(s, q, cc, qdd, f)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t nd = s->dm[0].n_qd, R = (size_t)dims * K;
+  const float *qd_d, *tau_d;
+  if (int rc = put_inv_inputs(s, q, qd, tau, &qd_d, &tau_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (nd + R + 1) * ns));
+  double* d = s->jac_dev;
+  if (int rc = cdyn_run(s, s->q, qd_d, tau_d, cc, qdd ? d : nullptr, f ? d + nd * ns : nullptr, 0, nullptr, nullptr, nullptr, nullptr, nullptr,
+                        nullptr, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{qdd, nd}, {f, R}}, d, n, ns, s->stream));
+  return 0;
+}
+
+static int cdyn_jvp_check(tds_b200_sim* s, const void* q, const CdynCall& cc, int m, const void* t_q, const void* t_qd, const void* t_tau,
+                          const void* t_par, const void* f, const void* t_qdd, const void* t_f) {
+  if (int rc = cdyn_check(s, q, cc, t_qdd, t_f)) return rc;
+  if (f && cc.K < 1) { set_err("constrained dynamics: f needs K >= 1 points"); return -1; }
+  if (m < 1 || (!t_q && !t_qd && !t_tau && !t_par)) return -1;
+  return par_without_installed(s, t_par, "constrained dynamics jvp: parameter tangents");
+}
+
+int tds_b200_constrained_dynamics_jvp_device(tds_b200_sim* s, const float* q, const float* qd, const float* tau, int K, const int* links,
+                                             const double* local, int dims, double damping, int m, const double* t_q, const double* t_qd,
+                                             const double* t_tau, const double* t_par, double* qdd, double* f, double* t_qdd, double* t_f,
+                                             void* stream) {
+  const CdynCall cc{K, links, local, dims, damping};
+  if (int rc = cdyn_jvp_check(s, q, cc, m, t_q, t_qd, t_tau, t_par, f, t_qdd, t_f)) return rc;
+  return cdyn_run(s, q, qd, tau, cc, qdd, f, m, t_q, t_qd, t_tau, t_par, t_qdd, t_f, (cudaStream_t)stream);
+}
+
+int tds_b200_constrained_dynamics_jvp_host(tds_b200_sim* s, const double* q, const double* qd, const double* tau, int K, const int* links,
+                                           const double* local, int dims, double damping, int m, const double* t_q, const double* t_qd,
+                                           const double* t_tau, const double* t_par, double* qdd, double* f, double* t_qdd, double* t_f) {
+  const CdynCall cc{K, links, local, dims, damping};
+  if (int rc = cdyn_jvp_check(s, q, cc, m, t_q, t_qd, t_tau, t_par, f, t_qdd, t_f)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, R = (size_t)dims * K;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; t_q | t_qd | t_tau | t_par | t_qdd | t_f | qdd | f
+  const size_t tq = (t_q ? n_q : 0) * m, tqd = (t_qd ? nd : 0) * m, tt = (t_tau ? nd : 0) * m, tp = (size_t)(t_par ? s->par.n : 0) * m;
+  const size_t ti = tq + tqd + tt + tp, to = (nd + R) * m;
+  const float *qd_d, *tau_d;
+  if (int rc = put_inv_inputs(s, q, qd, tau, &qd_d, &tau_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + to + nd + R + 1) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + ti * ns;
+  double* v_d = to_d + to * ns;
+  CUDA_TRY(put_parts<double>(d, {{t_q, tq}, {t_qd, tqd}, {t_tau, tt}, {t_par, tp}}, n, ns, s->stream));
+  if (int rc = cdyn_run(s, s->q, qd_d, tau_d, cc, qdd ? v_d : nullptr, f ? v_d + nd * ns : nullptr, m, t_q ? d : nullptr,
+                        t_qd ? d + tq * ns : nullptr, t_tau ? d + (tq + tqd) * ns : nullptr, t_par ? d + (tq + tqd + tt) * ns : nullptr,
+                        t_qdd ? to_d : nullptr, t_f ? to_d + nd * m * ns : nullptr, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{t_qdd, nd * m}, {t_f, R * m}, {qdd, nd}, {f, R}}, to_d, n, ns, s->stream));
+  return 0;
+}
+
+static int cdyn_vjp_check(tds_b200_sim* s, const void* q, const CdynCall& cc, const void* G_qdd, const void* G_f, const void* g_q,
+                          const void* g_qd, const void* g_tau, const void* g_par) {
+  if (int rc = cdyn_check(s, q, cc, G_qdd, G_f)) return rc;
+  if (!g_q && !g_qd && !g_tau && !g_par) return -1;
+  return par_without_installed(s, g_par, "constrained dynamics vjp: parameter cotangents");
+}
+
+int tds_b200_constrained_dynamics_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const float* tau, int K, const int* links,
+                                             const double* local, int dims, double damping, const double* G_qdd, const double* G_f,
+                                             double* g_q, double* g_qd, double* g_tau, double* g_par, void* stream) {
+  const CdynCall cc{K, links, local, dims, damping};
+  if (int rc = cdyn_vjp_check(s, q, cc, G_qdd, G_f, g_q, g_qd, g_tau, g_par)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, R = (size_t)dims * K, k = s->par.n, n_in = inv_n_in(s);
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the concatenated cotangent qdd | f (zero where a part is NULL), then g_q | g_qd | g_tau | g_par as one array for the contraction
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (nd + R + n_in + k) * s->ns));
+  double* g_d = s->vjp_g + (nd + R) * s->ns;
+  CUDA_TRY(put_parts_d2d<double>(s->vjp_g, {{G_qdd, nd}, {G_f, R}}, s->ns, sm));
+  if (int rc = cdyn_vjp_run(s, q, qd, tau, cc, s->vjp_g, g_d, g_par ? g_d + n_in * s->ns : nullptr, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, n_q}, {g_qd, nd}, {g_tau, nd}, {g_par, g_par ? k : 0}}, g_d, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_constrained_dynamics_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* tau, int K, const int* links,
+                                           const double* local, int dims, double damping, const double* G_qdd, const double* G_f,
+                                           double* g_q, double* g_qd, double* g_tau, double* g_par) {
+  const CdynCall cc{K, links, local, dims, damping};
+  if (int rc = cdyn_vjp_check(s, q, cc, G_qdd, G_f, g_q, g_qd, g_tau, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, R = (size_t)dims * K, k = s->par.n, n_in = inv_n_in(s);
+  const float *qd_d, *tau_d;
+  if (int rc = put_inv_inputs(s, q, qd, tau, &qd_d, &tau_d)) return rc;
+  // G (qdd | f, zero where a part is NULL) | g_q | g_qd | g_tau | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (nd + R + n_in + k + 1) * ns));
+  double* g_d = s->vjp_g + (nd + R) * ns;
+  CUDA_TRY(put_parts<double>(s->vjp_g, {{G_qdd, nd}, {G_f, R}}, n, ns, s->stream));
+  if (int rc = cdyn_vjp_run(s, s->q, qd_d, tau_d, cc, s->vjp_g, g_d, g_par ? g_d + n_in * ns : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_tau, nd}, {g_par, g_par ? k : 0}}, g_d, n, ns, s->stream));
   return 0;
 }
 

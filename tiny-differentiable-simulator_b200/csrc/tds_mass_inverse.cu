@@ -9,23 +9,10 @@
 #define TDS_STEPW_KERNEL_ONLY 1
 #endif
 #include "tds_stepw.cu"
+#include "tds_soa.cuh"
 
 namespace {
 constexpr int kMaxQd = 3 * TDS_MAX_LINKS + 6;
-
-// entry r of a [rows][ns] fp64 output: the value (T = double), or the value with the dual part of tangent j from [rows * m][ns]
-template <typename T> __device__ __forceinline__ T osim_ld(const double* v, const double* d, size_t r, int m, int j, int ns, int e);
-template <> __device__ __forceinline__ double osim_ld<double>(const double* v, const double*, size_t r, int, int, int ns, int e) {
-  return v[r * ns + e];
-}
-template <> __device__ __forceinline__ tds::Dual<double> osim_ld<tds::Dual<double>>(const double* v, const double* d, size_t r, int m, int j,
-                                                                                      int ns, int e) {
-  return tds::Dual<double>(v[r * ns + e], d ? d[(r * m + j) * ns + e] : 0.0);
-}
-__device__ __forceinline__ void osim_st(double* o, double x, size_t r, int, int, int ns, int e) { o[r * ns + e] = x; }
-__device__ __forceinline__ void osim_st(double* o, const tds::Dual<double>& x, size_t r, int m, int j, int ns, int e) {
-  o[(r * m + j) * ns + e] = x.d;
-}
 
 // Row a = blockIdx.y of L = J M^-1 J^T [R x R] (R = 6K) of environment e, tangent j = j0 + blockIdx.z: t = J_a M^-1, then L_ab = t . J_b for
 // b >= a, written to (a, b) and (b, a).  J [R * nq][ns], Mi [nq * nq][ns] (values) with their tangents dJ [R * nq * m][ns] and

@@ -169,6 +169,21 @@ struct TdsMotCall {
   double* J; double* vel; double* acc;
 };
 
+// One launch of the constrained-dynamics kernels (tds_constrained.cu, DESIGN.md section 7.21), R = dims * K constrained rows.
+// Inputs, values [rows][ns] and, for the dual-number instances, their tangents [rows * m][ns] (null: zero): tau fp32 [n_qd] (null: zero),
+// h = ID(q, qd, 0) [n_qd], M^-1 [n_qd^2], the point-motion J [6K * n_qd] and drift acc [6K].  Scratch: Y = J_c M^-1 [R * n_qd], A =
+// J_c M^-1 J_c^T [R * R] (factored in place), b [R] (then f); the value instances use Y, A, b [rows][ns], the dual instances (value,
+// tangent) pairs Y | dY, A | dA, b | db of every tangent at [rows * m][ns] each.  Outputs qdd [n_qd] and f [R] (either may be null):
+// values, or tangent j at row r * m_out + j0 + j.
+struct TdsCdynCall {
+  int K, dims, n_qd, m, j0, m_out;
+  double eps;
+  const float* tau; const double* dtau;
+  const double *h, *dh, *Mi, *dMi, *J, *dJ, *acc, *dacc;
+  double *Y, *dY, *A, *dA, *b, *db;
+  double *qdd, *f;
+};
+
 // The energy outputs of one call of the regressor instances (tds_regressor.cu, DESIGN.md section 7.19): yT [n_pi][ns] and yV [n_pi][ns]
 // (each may be null; columns of an m-column block in the JVP).  Y itself goes to StepIO::jac.
 struct TdsRegCall { double* yT; double* yV; };

@@ -966,6 +966,97 @@ class BatchSim:
         self._check(self._L.tds_b200_mass_inverse_vjp_device(self._h, _ptr(q), K, lp, cp, _ptr(G_Minv), _ptr(G_Linv), _ptr(g_q), _ptr(g_par),
                                                              st), "mass_inverse_vjp_device")
 
+    # ---- point-constrained forward dynamics (DESIGN.md section 7.21) ----
+    def _cd_points(self, links, local, dims, damping):
+        """The point table (None: no points, K = 0), dims and damping of the constrained_dynamics methods."""
+        keep, K, lp, cp = self._minv_points(links, local)
+        return keep, K, lp, cp, int(dims), float(damping)
+
+    def constrained_dynamics_host(self, q, qd=None, tau=None, links=None, local=None, dims=3, damping=0.0):
+        """(qdd [n, n_qd], f [n, K, dims] or None without points) float64 at the fp32-rounded q [n, n_q], qd and tau [n, n_qd] (None: zero):
+        the forward dynamics with the points of links [K] / local [K, 3] (K <= 16) held in their 3 linear rows (dims 3) or all 6 rows
+        (dims 6), M qdd - J_c^T f = tau - h and J_c qdd = -d_c - damping f, with M, h and J, d of mass_matrix_host,
+        inverse_dynamics_host(q, qd) and point_motion_host(q, qd).  f: the force (dims 3) or wrench [n; f] (dims 6) the constraint applies
+        at each point, world axes.  K = 0: qdd = M^-1 (tau - h).  Installed masses, centres of mass, inertias, stiffness and damping
+        enter.  An environment whose constraint system is not positive definite gets NaN outputs."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, tau = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(tau, self.n_qd, "tau")
+        keep, K, lp, cp, dims, eps = self._cd_points(links, local, dims, damping)
+        n = self.n_envs
+        qdd, f = np.zeros((n, self.n_qd)), (np.zeros((n, K, dims)) if K else None)
+        self._check(self._L.tds_b200_constrained_dynamics_host(self._h, _dp(q), _dp(qd), _dp(tau), K, lp, cp, dims, eps, _dp(qdd), _dp(f)),
+                    "constrained_dynamics_host")
+        return qdd, f
+
+    def constrained_dynamics_device(self, q, qd, tau, links, local, dims, damping, qdd=None, f=None, stream=None):
+        """Device version of constrained_dynamics_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd and tau [n_qd, n_stride]
+        (or None); qdd [n_qd, n_stride] and f [dims K, n_stride] float64 CUDA tensors (either may be None, not both), component r of point
+        k at row dims k + r.  The point table (None: none) is host data.  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp, dims, eps = self._cd_points(links, local, dims, damping)
+        self._check(self._L.tds_b200_constrained_dynamics_device(self._h, _ptr(q), _ptr(qd), _ptr(tau), K, lp, cp, dims, eps, _ptr(qdd),
+                                                                 _ptr(f), st), "constrained_dynamics_device")
+
+    def constrained_dynamics_jvp_host(self, q, qd=None, tau=None, links=None, local=None, dims=3, damping=0.0, t_q=None, t_qd=None,
+                                      t_tau=None, t_par=None):
+        """Directional derivatives of the outputs of constrained_dynamics_host along m tangents t_q [n, n_q, m], t_qd and t_tau [n, n_qd, m]
+        and t_par [n, k, m] of the installed parameters (each may be None, not all): (qdd, f, dqdd [n, n_qd, m], df [n, K, dims, m] or
+        None); tangents given as [n, dim] are m = 1 and drop the last axis."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, tau = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(tau, self.n_qd, "tau")
+        keep, K, lp, cp, dims, eps = self._cd_points(links, local, dims, damping)
+        ts, m, single = self._tangents([(t_q, self.n_q), (t_qd, self.n_qd), (t_tau, self.n_qd), (t_par, len(self.param_ids))])
+        n, nd = self.n_envs, self.n_qd
+        qdd, dqdd = np.zeros((n, nd)), np.zeros((n, nd, max(m, 1)))
+        f, df = (np.zeros((n, K, dims)), np.zeros((n, K, dims, max(m, 1)))) if K else (None, None)
+        self._check(self._L.tds_b200_constrained_dynamics_jvp_host(self._h, _dp(q), _dp(qd), _dp(tau), K, lp, cp, dims, eps, m,
+                                                                   *(_dp(t) for t in ts), _dp(qdd), _dp(f), _dp(dqdd), _dp(df)),
+                    "constrained_dynamics_jvp_host")
+        if single:
+            dqdd, df = dqdd[..., 0], (None if df is None else df[..., 0])
+        return qdd, f, dqdd, df
+
+    def constrained_dynamics_jvp_device(self, q, qd, tau, links, local, dims, damping, m, t_q, t_qd, t_tau, t_par, t_qdd=None, t_f=None,
+                                        qdd=None, f=None, stream=None):
+        """Device version of constrained_dynamics_jvp_host: q float32 [n_q, n_stride], qd and tau [n_qd, n_stride] (or None); t_q [n_q * m,
+        n_stride], t_qd and t_tau [n_qd * m, n_stride], t_par [k * m, n_stride] (each may be None, not all); t_qdd [n_qd * m, n_stride],
+        t_f [dims K m, n_stride] (either may be None, not both), qdd and f (values, or None) float64 CUDA tensors, entry (r, j) at row
+        r * m + j.  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp, dims, eps = self._cd_points(links, local, dims, damping)
+        self._check(self._L.tds_b200_constrained_dynamics_jvp_device(self._h, _ptr(q), _ptr(qd), _ptr(tau), K, lp, cp, dims, eps, int(m),
+                                                                     _ptr(t_q), _ptr(t_qd), _ptr(t_tau), _ptr(t_par), _ptr(qdd), _ptr(f),
+                                                                     _ptr(t_qdd), _ptr(t_f), st), "constrained_dynamics_jvp_device")
+
+    def constrained_dynamics_vjp_host(self, q, qd=None, tau=None, links=None, local=None, dims=3, damping=0.0, G_qdd=None, G_f=None):
+        """Cotangents G_qdd [n, n_qd] and G_f [n, K, dims] (None: zero, not both) -> (g_q [n, n_q], g_qd [n, n_qd], g_tau [n, n_qd], g_par
+        [n, k] or None without installed parameters) = sum G * d(outputs)/dx."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, tau = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(tau, self.n_qd, "tau")
+        keep, K, lp, cp, dims, eps = self._cd_points(links, local, dims, damping)
+        if G_qdd is None and G_f is None:
+            raise ValueError("at least one cotangent is expected")
+        n, nd, k = self.n_envs, self.n_qd, len(self.param_ids)
+        G_qdd = None if G_qdd is None else self._inv_in(G_qdd, nd, "G_qdd")
+        G_f = None if G_f is None else self._inv_in(np.reshape(G_f, (n, -1)), dims * K, "G_f")
+        g_q, g_qd, g_tau = np.zeros((n, self.n_q)), np.zeros((n, nd)), np.zeros((n, nd))
+        g_par = np.zeros((n, k)) if k else None
+        self._check(self._L.tds_b200_constrained_dynamics_vjp_host(self._h, _dp(q), _dp(qd), _dp(tau), K, lp, cp, dims, eps, _dp(G_qdd),
+                                                                   _dp(G_f), _dp(g_q), _dp(g_qd), _dp(g_tau), _dp(g_par)),
+                    "constrained_dynamics_vjp_host")
+        return g_q, g_qd, g_tau, g_par
+
+    def constrained_dynamics_vjp_device(self, q, qd, tau, links, local, dims, damping, G_qdd, G_f, g_q, g_qd, g_tau, g_par=None,
+                                        stream=None):
+        """Device version of constrained_dynamics_vjp_host: q float32 [n_q, n_stride], qd and tau [n_qd, n_stride] (or None), cotangents
+        float64 in the layouts of constrained_dynamics_device (None: zero, not both), g_q [n_q, n_stride], g_qd and g_tau [n_qd, n_stride],
+        g_par [k, n_stride] float64 CUDA tensors (each may be None, not all).  Asynchronous on the stream."""
+        st = _stream(stream)
+        keep, K, lp, cp, dims, eps = self._cd_points(links, local, dims, damping)
+        self._check(self._L.tds_b200_constrained_dynamics_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(tau), K, lp, cp, dims, eps, _ptr(G_qdd),
+                                                                     _ptr(G_f), _ptr(g_q), _ptr(g_qd), _ptr(g_tau), _ptr(g_par), st),
+                    "constrained_dynamics_vjp_device")
+
     def jacobian_chunk(self):
         """Directions (Jacobian columns or JVP tangents) one launch of the dual-number step takes; more run in several launches."""
         return self._L.tds_b200_jacobian_chunk(self._h)
