@@ -498,6 +498,39 @@ int tds_b200_constrained_dynamics_vjp_host(tds_b200_sim* sim, const double* q, c
                                            const double* local, int dims, double damping, const double* G_qdd, const double* G_f,
                                            double* g_q, double* g_qd, double* g_tau, double* g_par);
 
+/* ---- Coriolis matrix C(q, qd) (DESIGN.md section 7.22) ---------------------------------------------------------------------------------
+ * At the fp32-rounded q and qd (qd may be NULL, meaning zero: C = 0), C [n_qd * n_qd] fp64 in the coordinates and layout of
+ * tds_b200_mass_matrix (entry (r, c) at r * n_qd + c; a floating base's qd[0:6] is the base-frame twist [w; v]):
+ *     C = sum over the bodies i of J_i^T (I_i J_i' + B(I_i, v_i) J_i),  B(I, v) = 1/2 ((v x*) I + bar(I v) - I (v x)),
+ *   I_i the spatial inertia of body i (a floating base counts) in world axes about the world origin, J_i its spatial Jacobian in the
+ *   coordinates of M (v_i = J_i qd), J_i' its time derivative along qd, bar(f) u = u x* f (Echeandia & Wensing 2021; Pinocchio's
+ *   computeCoriolisMatrix).  So C qd = h(q, qd) - h(q, 0) with h the bias forces of tds_b200_inverse_dynamics without joint damping,
+ *   C + C^T = M' (the time derivative of M along the motion with velocity qd; M' - 2 C is skew-symmetric), and on coordinates whose rates
+ *   are the velocities C is the Christoffel matrix C_ij = sum_k 1/2 (dM_ij/dq_k + dM_ik/dq_j - dM_jk/dq_i) qd_k.  Every entry is written;
+ *   a world of several multibodies gives exact zeros between multibodies.
+ * While a parameter set is installed, each environment's masses, centres of mass and inertias (links and floating base) are used;
+ * stiffness, damping, friction and restitution do not enter.
+ * Argument checks: NULL q, no output (C, or t_C for _jvp), no cotangent G, m < 1, every tangent NULL, or no gradient output -> -1; t_par /
+ * g_par without an installed set -> -4.
+ *   device: q [n_q][n_stride], qd [n_qd][n_stride] fp32; C [n_qd * n_qd][n_stride] fp64.  Asynchronous.
+ *   host:   q [n][n_q], qd [n][n_qd] fp64 (rounded to fp32); C [n][n_qd * n_qd].  Synchronous.
+ * _jvp: dC along m tangents of q, qd and the installed parameters (each may be NULL: zero, not all); C (may be NULL) receives the value.
+ *   Device t_q [n_q * m][n_stride], t_qd [n_qd * m][n_stride], t_par [k * m][n_stride], t_C [n_qd * n_qd * m][n_stride] (entry (r, j) at
+ *   (r * m + j) * n_stride + e); host t_q [n][n_q][m], t_qd [n][n_qd][m], t_par [n][k][m], t_C [n][n_qd * n_qd][m].
+ * _vjp: g_x[c] = <G, dC/dx_c> for x = q, qd and, while a set is installed, the parameters, for the cotangent G in C's layout: the JVP along
+ *   the n_q + n_qd (+ k) identity tangents contracted with G on the device.  Any of g_q, g_qd, g_par may be NULL, not all.  Device g_q
+ *   [n_q][n_stride], g_qd [n_qd][n_stride], g_par [k][n_stride] fp64 (asynchronous); host g_q [n][n_q], g_qd [n][n_qd], g_par [n][k]
+ *   (synchronous). */
+int tds_b200_coriolis_device(tds_b200_sim* sim, const float* q, const float* qd, double* C, void* stream);
+int tds_b200_coriolis_host(tds_b200_sim* sim, const double* q, const double* qd, double* C);
+int tds_b200_coriolis_jvp_device(tds_b200_sim* sim, const float* q, const float* qd, int m, const double* t_q, const double* t_qd,
+                                 const double* t_par, double* C, double* t_C, void* stream);
+int tds_b200_coriolis_jvp_host(tds_b200_sim* sim, const double* q, const double* qd, int m, const double* t_q, const double* t_qd,
+                               const double* t_par, double* C, double* t_C);
+int tds_b200_coriolis_vjp_device(tds_b200_sim* sim, const float* q, const float* qd, const double* G, double* g_q, double* g_qd, double* g_par,
+                                 void* stream);
+int tds_b200_coriolis_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* G, double* g_q, double* g_qd, double* g_par);
+
 /* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
  * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
  * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,

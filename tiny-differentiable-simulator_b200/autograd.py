@@ -62,6 +62,10 @@ constrained_dynamics(sim, q, qd=None, tau=None, links=None, local=None, dims=3, 
 the points of a table held in place and the constraint forces f (float64, DESIGN.md section 7.21), with a backward rule
 (BatchSim.constrained_dynamics_vjp_device: float32 q.grad, qd.grad, tau.grad, float64 params.grad) and a forward-mode rule
 (BatchSim.constrained_dynamics_jvp_device).
+
+coriolis(sim, q, qd=None, params=None) is the Coriolis matrix C(q, qd) [n_envs, n_qd, n_qd] (float64, DESIGN.md section 7.22) with a
+backward rule (BatchSim.coriolis_vjp_device: float32 q.grad, qd.grad, float64 params.grad) and a forward-mode rule
+(BatchSim.coriolis_jvp_device).
 """
 from collections import namedtuple
 
@@ -340,7 +344,7 @@ def _state_soa(sim, q, qd, qdd):
 
 class _Query(torch.autograd.Function):
     """The dynamics queries (mass_matrix, inverse_dynamics, centroidal, forward_kinematics, point_motion, regressor, mass_inverse,
-    constrained_dynamics) as one Function over a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
+    constrained_dynamics, coriolis) as one Function over a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
     float64 output buffers, every C-ABI call ordered on a side stream, and the gradients as float32 (q, qd, qdd) and float64 (params).
     An input the query does not take, or the call leaves out, is None and gets no gradient; a tangent on it is ignored.  With params
     the forward installs their values, and the backward and forward-mode rule reinstall the values of this call (a later call of the
@@ -815,3 +819,24 @@ def constrained_dynamics(sim, q, qd=None, tau=None, links=None, local=None, dims
     p = _CdPoints(*sim._points([] if links is None else links, np.zeros((0, 3)) if local is None else local), int(dims), float(damping))
     qdd, f = _Query.apply(_CONSTRAINED_DYNAMICS, sim, p, q, qd, tau, params)
     return qdd, (f if p.K else None)
+
+
+_CORIOLIS = _QuerySpec(
+    rows=lambda sim, p: [sim.n_qd * sim.n_qd],
+    unpack=lambda sim, p, C: C.reshape(sim.n_envs, sim.n_qd, sim.n_qd).contiguous(),
+    pack=lambda sim, p, gC: [_cot(gC, sim)],
+    value=lambda sim, p, x, out, st: sim.coriolis_device(x.q, x.qd, *out, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.coriolis_jvp_device(x.q, x.qd, 1, t.q, t.qd, t.params, *out, stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.coriolis_vjp_device(x.q, x.qd, *G, g.q, g.qd, g.params, stream=st))
+
+
+def coriolis(sim, q, qd=None, params=None):
+    """The Coriolis matrix C(q, qd) of every environment of `sim` (a BatchSim), DESIGN.md section 7.22: [n_envs, n_qd, n_qd] float64 in
+    the coordinates of mass_matrix, in fp64 at the fp32-rounded q [n_envs, n_q] and qd [n_envs, n_qd] float32 CUDA tensors (qd None:
+    zero, C = 0).  C is Echeandia & Wensing's factorisation, so C qd is the velocity part of the bias forces (inverse_dynamics(sim, q, qd)
+    - inverse_dynamics(sim, q) without joint damping) and C + C^T is the time derivative of M along qd (M' - 2 C is skew-symmetric).
+    params: None, or a float64 CUDA tensor [n_envs, k] of values for the parameters installed by sim.set_physical_params (then also
+    differentiated).  Differentiable in reverse mode (float32 q.grad, qd.grad, float64 params.grad) and forward mode."""
+    _check_state(sim, q, qd)
+    _check_params(sim, params)
+    return _Query.apply(_CORIOLIS, sim, None, q, qd, None, params)

@@ -99,6 +99,10 @@ extern "C" int tds_launch_mass_inverse_jvp(const DevModel* M, const StepIO* io, 
                                            int m, int n_dirs, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_osim(const double* J, const double* dJ, const double* Mi, const double* dMi, double* L, int K, int n_qd, int m,
                                int n, int ns, cudaStream_t stream);
+// Coriolis matrix C(q, qd) and its Jacobian-vector products (tds_coriolis.cu)
+extern "C" int tds_launch_coriolis(const DevModel* M, const StepIO* io, const ParMap* pm, char* gscratch, cudaStream_t stream);
+extern "C" int tds_launch_coriolis_jvp(const DevModel* M, const StepIO* io, const ParMap* pm, const double* t_in, const double* t_par, int m,
+                                       int n_dirs, char* gscratch, cudaStream_t stream);
 // the rows and the solve of the point-constrained forward dynamics (tds_constrained.cu)
 extern "C" int tds_launch_cdyn(const TdsCdynCall* c, int dual, int n, int ns, cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
@@ -925,7 +929,7 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
 
 // what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14, 7.16 and 7.17,
 // or the step with its contact records (section 7.15)
-enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, regressor, minv };
+enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, regressor, minv, cor };
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
 // inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
@@ -933,7 +937,7 @@ enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, r
 // contacts: as step, with the rows q' | qd' | records; centroidal: t_in = the q | qd tangents (qd in the step's qd), outputs `cen`;
 // motion: t_in = the q | qd | qdd tangents (qd and qdd as for inv), the point table and outputs `mot`; wrench: as step, with the point
 // table, wrenches and wrench tangents `ext`; regressor: t_in = the q | qd | qdd tangents (as for inv), Y in jac and the
-// energy outputs `reg`; minv: as mass, M^-1 in jac
+// energy outputs `reg`; minv: as mass, M^-1 in jac; cor: t_in = the q | qd tangents (qd in the step's qd), C in jac
 struct JvpTangents {
   const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr;
   const TdsCenCall* cen = nullptr; const TdsMotCall* mot = nullptr; const TdsExtCall* ext = nullptr;
@@ -1020,6 +1024,7 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
           break;
         case Query::regressor: rc = tds_launch_regressor_jvp(&s->dm_ad, &s->P, &io, jv->reg, jv->t_in, jv->m, nd, s->jac_scratch, sm); break;
         case Query::minv: rc = tds_launch_mass_inverse_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
+        case Query::cor: rc = tds_launch_coriolis_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
       }
     }
     if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
@@ -1681,6 +1686,122 @@ int tds_b200_centroidal_vjp_host(tds_b200_sim* s, const double* q, const double*
   double* g_d = s->vjp_g + R.all() * ns;
   CUDA_TRY(put_parts<double>(s->vjp_g, {{G_com, R.com}, {G_A, R.A}, {G_bias, R.bias}}, n, ns, s->stream));
   if (int rc = cen_vjp_run(s, s->q, qd_d, s->vjp_g, g_d, g_par ? g_d + (size_t)n_in * ns : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_par, k}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- Coriolis matrix C(q, qd) (DESIGN.md section 7.22): the COR instances of the world-frame kernel (tds_coriolis.cu).  The inputs
+// q | qd are those of the centroidal quantities (cen_n_in, put_cen_inputs). ------------------------------------------------------------
+// C [n_qd * n_qd][ns] from q [n_q][ns] and qd [n_qd][ns] fp32 (NULL: zero)
+static int cor_run(tds_b200_sim* s, const float* q, const float* qd, double* C, cudaStream_t sm) {
+  return value_run(s, "coriolis", q, qd, nullptr, C, [&](const StepIO* io, const ParMap* pm) {
+    return tds_launch_coriolis(&s->dm_m, io, pm, s->jac_scratch, sm);
+  });
+}
+
+// t_C [n_qd * n_qd * m][ns] along t_in [(n_q + n_qd) * m][ns] (q | qd tangents, contiguous) and t_par (either may be NULL); C, if not
+// NULL, receives the value
+static int cor_jvp_run(tds_b200_sim* s, const float* q, const float* qd, int m, const double* t_in, const double* t_par, double* C, double* t_C,
+                       cudaStream_t sm) {
+  if (C) { if (int rc = cor_run(s, q, qd, C, sm)) return rc; }
+  const JvpTangents jv{t_in, t_par, m, Query::cor};
+  return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, nullptr, t_C, sm, false, &jv);
+}
+
+// g_in [n_q + n_qd][ns] (q | qd, contiguous) and g_par [k][ns] (NULL: not wanted) = <G, dC>
+static int cor_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const double* G, double* g_in, double* g_par, cudaStream_t sm) {
+  const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
+  return vjp_by_eye(s, "coriolis", cen_n_in(s), nn, G, g_in, g_par, sm, [&](int nd, const double* t_in, const double* t_par, double* dC) {
+    return cor_jvp_run(s, q, qd, nd, t_in, t_par, nullptr, dC, sm);
+  });
+}
+
+int tds_b200_coriolis_device(tds_b200_sim* s, const float* q, const float* qd, double* C, void* stream) {
+  if (!s || !q || !C) return -1;
+  return cor_run(s, q, qd, C, (cudaStream_t)stream);
+}
+
+int tds_b200_coriolis_host(tds_b200_sim* s, const double* q, const double* qd, double* C) {
+  if (!s || !q || !C) return -1;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
+  const float* qd_d;
+  if (int rc = put_cen_inputs(s, q, qd, &qd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * nn * s->ns));
+  if (int rc = cor_run(s, s->q, qd_d, s->jac_dev, s->stream)) return rc;
+  CUDA_TRY(get_rows(C, s->jac_dev, nn, s->n, s->ns, s->stream));
+  return 0;
+}
+
+static int cor_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_qd, const void* t_par, const void* t_C) {
+  if (!s || !q || !t_C || m < 1 || (!t_q && !t_qd && !t_par)) return -1;
+  return par_without_installed(s, t_par, "coriolis jvp: parameter tangents");
+}
+
+int tds_b200_coriolis_jvp_device(tds_b200_sim* s, const float* q, const float* qd, int m, const double* t_q, const double* t_qd,
+                                 const double* t_par, double* C, double* t_C, void* stream) {
+  if (int rc = cor_jvp_check(s, q, m, t_q, t_qd, t_par, t_C)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  cudaStream_t sm = (cudaStream_t)stream;
+  double* tin = nullptr;
+  if (t_q || t_qd) {   // the kernel reads the q | qd tangents as one array
+    CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (size_t)cen_n_in(s) * m * s->ns));
+    tin = s->jac_dev;
+    CUDA_TRY(put_parts_d2d<double>(tin, {{t_q, n_q * m}, {t_qd, nd * m}}, s->ns, sm));
+  }
+  return cor_jvp_run(s, q, qd, m, tin, t_par, C, t_C, sm);
+}
+
+int tds_b200_coriolis_jvp_host(tds_b200_sim* s, const double* q, const double* qd, int m, const double* t_q, const double* t_qd,
+                               const double* t_par, double* C, double* t_C) {
+  if (int rc = cor_jvp_check(s, q, m, t_q, t_qd, t_par, t_C)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; q | qd (contiguous, zero where NULL, none if both are), t_par, t_C, C
+  const size_t ti = (t_q || t_qd) ? (size_t)cen_n_in(s) * m : 0, tp = (size_t)(t_par ? s->par.n : 0) * m, to = nn * m;
+  const float* qd_d;
+  if (int rc = put_cen_inputs(s, q, qd, &qd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + tp + to + nn) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + (ti + tp) * ns;
+  if (ti) CUDA_TRY(put_parts<double>(d, {{t_q, n_q * m}, {t_qd, nd * m}}, n, ns, s->stream));
+  if (t_par) CUDA_TRY(put_rows(d + ti * ns, t_par, tp, n, ns, s->stream));
+  if (int rc = cor_jvp_run(s, s->q, qd_d, m, ti ? d : nullptr, t_par ? d + ti * ns : nullptr, C ? to_d + to * ns : nullptr, to_d, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{t_C, to}, {C, nn}}, to_d, n, ns, s->stream));
+  return 0;
+}
+
+static int cor_vjp_check(tds_b200_sim* s, const void* q, const void* G, const void* g_q, const void* g_qd, const void* g_par) {
+  if (!s || !q || !G || (!g_q && !g_qd && !g_par)) return -1;
+  return par_without_installed(s, g_par, "coriolis vjp: parameter cotangents");
+}
+
+int tds_b200_coriolis_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const double* G, double* g_q, double* g_qd, double* g_par,
+                                 void* stream) {
+  if (int rc = cor_vjp_check(s, q, G, g_q, g_qd, g_par)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  cudaStream_t sm = (cudaStream_t)stream;
+  // g_q | g_qd are one array for the contraction: computed in s->vjp_g, then copied out
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (size_t)cen_n_in(s) * s->ns));
+  if (int rc = cor_vjp_run(s, q, qd, G, s->vjp_g, g_par, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, n_q}, {g_qd, nd}}, s->vjp_g, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_coriolis_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* G, double* g_q, double* g_qd, double* g_par) {
+  if (int rc = cor_vjp_check(s, q, G, g_q, g_qd, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, n_in = cen_n_in(s);
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd, k = s->par.n;
+  const float* qd_d;
+  if (int rc = put_cen_inputs(s, q, qd, &qd_d)) return rc;
+  // G | g_q | g_qd | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (nn + n_in + k + 1) * ns));
+  double* g_d = s->vjp_g + nn * ns;
+  CUDA_TRY(put_rows(s->vjp_g, G, nn, n, ns, s->stream));
+  if (int rc = cor_vjp_run(s, s->q, qd_d, s->vjp_g, g_d, g_par ? g_d + (size_t)n_in * ns : nullptr, s->stream)) return rc;
   CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_par, k}}, g_d, n, ns, s->stream));
   return 0;
 }

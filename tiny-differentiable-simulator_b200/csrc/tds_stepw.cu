@@ -176,9 +176,17 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // dinv), overwrites L's off-diagonal blocks with those of W = L^-1 column by column, and writes M^-1 = W^T W in place of the dense M: one
 // sum per pair (r >= c) written to (r, c) and (c, r).  The padding dofs hold an identity, so the first n_qd rows and columns of the
 // padded inverse are M^-1; they are not written.
+// COR: the Coriolis matrix C(q, qd) of Echeandia & Wensing (DESIGN.md section 7.22), launched in MODE_NOCONTACT with qd in io.qd_in (null:
+// zero).  Pass 1 as CEN's (v_i and the rigid inertias r_i about O in the link records).  Pass 2 carries, next to the composite Ic_i, the
+// composite rate Ic_i' = sum r_k' (r' = v x* r - r v x, a rigid-inertia record with m' = 0) and momentum h_i = sum r_k v_k of the subtree
+// in the accumulators' ABA words, so that the composite B_i u = 1/2 (Ic_i' u + u x* h_i).  With S' = v_i x S for the columns of link i and
+// v_j x S for those of an ancestor j (the base twist's: v_b x S), C(a, a') = S_a . F_a' within link i and C(b, a) = S_b . F_a, C(a, b) =
+// (B_i^T S_a - v_j x* (Ic_i S_a)) . S_b against its ancestors' columns b, F_a = Ic_i S_a' + B_i S_a (B_i^T = 1/2 (Ic_i' - h_i x*) is
+// B_i with the skew part negated).  A floating base's own block after the sweep from the whole tree's composites.  Every entry is
+// written: zeros first, C [n_qd * n_qd] at io.jac as MASS writes M (padding dofs not written).  ABA and integration are not compiled in.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
           bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false, bool REG = false,
-          bool MINV = false>
+          bool MINV = false, bool COR = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
@@ -301,7 +309,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // input directions of the differentiable instance: q | qd | tau or action | kp, kd, max_force (with PD)
   const int in0 = M.n_q + n;
   for (int k = 0; k < M.n_q; ++k) qv[k * ST] = seed(RQ(io.q_in[(size_t)k * ns + e]), k);
-  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(((INV || CEN || MOT) && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
+  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(((INV || CEN || MOT || COR) && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
   for (int k = 0; k < n; ++k) tauv[k * ST] = RQ(0.f);
   if (!MASS && use_pd) {
     const RQ kp = seed(RQ(E.kp), in0 + E.n_act), kd = seed(RQ(E.kd), in0 + E.n_act + 1), fmax_ = seed(RQ(E.max_force), in0 + E.n_act + 2);
@@ -1017,6 +1025,43 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     Ia.M.xx -= a.bot.x * b.bot.x; Ia.M.xy -= a.bot.x * b.bot.y; Ia.M.xz -= a.bot.x * b.bot.z;
     Ia.M.yy -= a.bot.y * b.bot.y; Ia.M.yz -= a.bot.y * b.bot.z; Ia.M.zz -= a.bot.z * b.bot.z;
   };
+  // COR: entry k of C; the rate r' of a rigid inertia r about O moving with v = [w; u]: h' = m u + w x h, I' = [w]x I - I [w]x +
+  // 2 (h . u) 1 - u h^T - h u^T; B u and B^T u of the composites (D = Ic', h); the composites handed from an adjacent child
+  auto cor_put = [&](int k, const RC& x) {
+    if constexpr (COR) {
+      if (!live || !io.jac) return;
+      if constexpr (AD) io.jac[((size_t)k * io.jac_n_in + jcol) * ns + e] = x.d;
+      else io.jac[(size_t)k * ns + e] = x;
+    }
+  };
+  auto cor_rate = [&](const Rbi<RC>& r, const Sv<RC>& v) -> Rbi<RC> {
+    Rbi<RC> o;
+    const V3<RC> w = v.top, u = v.bot;
+    o.m = RC(0);
+    o.h = u * r.m + cross(w, r.h);
+    const V3<RC> a0 = cross(w, v3<RC>(r.I.xx, r.I.xy, r.I.xz)), a1 = cross(w, v3<RC>(r.I.xy, r.I.yy, r.I.yz)),
+                 a2 = cross(w, v3<RC>(r.I.xz, r.I.yz, r.I.zz));   // the columns of [w]x I
+    const RC hu = dot(r.h, u);
+    o.I.xx = RC(2) * (a0.x + hu - u.x * r.h.x); o.I.yy = RC(2) * (a1.y + hu - u.y * r.h.y); o.I.zz = RC(2) * (a2.z + hu - u.z * r.h.z);
+    o.I.xy = a1.x + a0.y - u.x * r.h.y - r.h.x * u.y;
+    o.I.xz = a2.x + a0.z - u.x * r.h.z - r.h.x * u.z;
+    o.I.yz = a2.y + a1.z - u.y * r.h.z - r.h.y * u.z;
+    return o;
+  };
+  auto cor_B = [&](const Rbi<RC>& D, const Sv<RC>& h, const Sv<RC>& u, bool transposed) -> Sv<RC> {
+    const Sv<RC> a = rbi_mul(D, u), b = cross_mf(u, h);
+    const RC s = transposed ? RC(-0.5) : RC(0.5);
+    Sv<RC> o;
+    o.top = a.top * RC(0.5) + b.top * s;
+    o.bot = a.bot * RC(0.5) + b.bot * s;
+    return o;
+  };
+  typename std::conditional<COR, Rbi<RC>, NoPar>::type cor_cD{};
+  typename std::conditional<COR, Sv<RC>, NoPar>::type cor_cH{};
+  if constexpr (COR) {
+    static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the COR instances run in one scalar type");
+    for (int k = 0; k < n * n; ++k) cor_put(k, RC(0));
+  }
   for (int i = n_links - 1; i >= 0; --i) {
     const int p = M.parent[i];
     const int fl = M.flags[i];
@@ -1033,14 +1078,27 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
         pA.top = pA.top - w.top; pA.bot = pA.bot - w.bot;
       }
     }
-    if (fl & TDS_LF_CHILD_ADJ) { if constexpr (!MASS && !CEN) { abi_add(Ia, cA); pA = pA + cP; } rbi_add(Ic, cC); }
+    // COR: the link's own rate and momentum, then its children's composites (in the accumulators' ABA words: rate 10, momentum 6)
+    typename std::conditional<COR, Rbi<RC>, NoPar>::type cor_D{};
+    typename std::conditional<COR, Sv<RC>, NoPar>::type cor_h{};
+    if constexpr (COR) { cor_D = cor_rate(Ic, v); cor_h = rbi_mul(Ic, v); }
+    if (fl & TDS_LF_CHILD_ADJ) {
+      if constexpr (!MASS && !CEN && !COR) { abi_add(Ia, cA); pA = pA + cP; }
+      rbi_add(Ic, cC);
+      if constexpr (COR) { rbi_add(cor_D, cor_cD); cor_h = cor_h + cor_cH; }
+    }
     if (M.acc_slot[i] >= 0) {
-      if constexpr (!MASS && !CEN) {
+      if constexpr (!MASS && !CEN && !COR) {
         Abi<RA> sa; Sv<RA> sp;
         acc_ld27<RA>(A.ptr<RA>(M.x_acc + M.acc_slot[i] * M.x_acc_words), ST, sa, sp);
         abi_add(Ia, sa); pA = pA + sp;
       }
       rbi_add(Ic, ld_rbi<RC>(A.ptr<RC>(M.x_acc + M.acc_slot[i] * M.x_acc_words + M.x_acc_ic_word), ST));
+      if constexpr (COR) {
+        const RC* pc = A.ptr<RC>(M.x_acc + M.acc_slot[i] * M.x_acc_words);
+        rbi_add(cor_D, ld_rbi<RC>(pc, ST));
+        cor_h = cor_h + ld6<RC>(pc + 10 * ST, ST);
+      }
     }
     Sv<RA> pa = pA;
     // U (6), invD, u overwrite the rigid-inertia record.  The RA and RC views interleave lanes differently, so
@@ -1062,6 +1120,34 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
         const Sv<RC> F = rbi_mul(Ic, S_col(i, a));
         for (int b = 0; b <= a; ++b) Mset(d0 + a, d0 + b, RS(dot(S_col(i, b), F)));
         crba_ancestors(i, d0 + a, F);
+      }
+    } else if constexpr (COR) {   // C's entries between link i's dofs and those of i and its ancestors, column a of i at a time
+      const int d0 = M.qd_idx[i], nc = n_cols(i);
+      for (int a = 0; a < nc; ++a) {
+        const Sv<RC> S = S_col(i, a);
+        const Sv<RC> G = rbi_mul(Ic, S), Hs = cor_B(cor_D, cor_h, S, true);   // Ic S_a, B^T S_a
+        const Sv<RC> F = rbi_mul(Ic, cross_mm(v, S)) + cor_B(cor_D, cor_h, S, false);
+        for (int b = 0; b < nc; ++b) cor_put((d0 + b) * n + d0 + a, dot(S_col(i, b), F));
+        for (int j = M.parent[i]; j >= 0; j = M.parent[j]) {
+          const int ncj = n_cols(j);
+          if (ncj == 0) continue;
+          const Sv<RC> Y = cross_mf(ld6<RC>(A.ptr<RC>(M.x_link + j * LWD + VOFF), ST), G);
+          Sv<RC> X; X.top = Hs.top - Y.top; X.bot = Hs.bot - Y.bot;   // G_a . (v_j x S_b) = -(v_j x* G_a) . S_b
+          for (int b = 0; b < ncj; ++b) {
+            const Sv<RC> Sb = S_col(j, b);
+            cor_put((d0 + a) * n + M.qd_idx[j] + b, dot(X, Sb));
+            cor_put((M.qd_idx[j] + b) * n + d0 + a, dot(Sb, F));
+          }
+        }
+        if (M.floating) {   // the base twist's columns [R_b e_k; 0], [0; R_b e_k]: a dot product with one is a base-frame component
+          const Sv<RC> Y = cross_mf(v_base, G);
+          const V3<RC> xt = mulT(Rb, Hs.top - Y.top), xb = mulT(Rb, Hs.bot - Y.bot);
+          const V3<RC> ft = mulT(Rb, F.top), fb = mulT(Rb, F.bot);
+          const int r = (d0 + a) * n;
+          cor_put(r, xt.x); cor_put(r + 1, xt.y); cor_put(r + 2, xt.z); cor_put(r + 3, xb.x); cor_put(r + 4, xb.y); cor_put(r + 5, xb.z);
+          cor_put(d0 + a, ft.x); cor_put(n + d0 + a, ft.y); cor_put(2 * n + d0 + a, ft.z);
+          cor_put(3 * n + d0 + a, fb.x); cor_put(4 * n + d0 + a, fb.y); cor_put(5 * n + d0 + a, fb.z);
+        }
       }
     } else if (fl & TDS_LF_FIXED) {
       Sv<RA> z; z.top = v3<RA>(RA(0), RA(0), RA(0)); z.bot = z.top;
@@ -1171,14 +1257,48 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       }
     }
     // hand (Ia, pa, Ic) to the parent: plain sums in the common frame
-    if (fl & TDS_LF_PARENT_ADJ) { cA = Ia; cP = pa; cC = Ic; }
-    else {
+    if (fl & TDS_LF_PARENT_ADJ) {
+      cA = Ia; cP = pa; cC = Ic;
+      if constexpr (COR) { cor_cD = cor_D; cor_cH = cor_h; }
+    } else {
       const int slot = (p >= 0) ? M.acc_slot[p] : M.base_acc;
       if (slot >= 0) {
-        if constexpr (!MASS && !CEN) acc_add27<RA>(A.ptr<RA>(M.x_acc + slot * M.x_acc_words), ST, Ia, pa);
+        if constexpr (!MASS && !CEN && !COR) acc_add27<RA>(A.ptr<RA>(M.x_acc + slot * M.x_acc_words), ST, Ia, pa);
         rbi_acc<RC>(A.ptr<RC>(M.x_acc + slot * M.x_acc_words + M.x_acc_ic_word), ST, Ic);
+        if constexpr (COR) {
+          RC* pc = A.ptr<RC>(M.x_acc + slot * M.x_acc_words);
+          rbi_acc<RC>(pc, ST, cor_D);
+          st6<RC>(pc + 10 * ST, ST, ld6<RC>(pc + 10 * ST, ST) + cor_h);
+        }
       }
     }
+  }
+  if constexpr (COR) {
+    if (M.floating) {   // the base's own block from the whole tree's composites, the base body's included (in world axes about O)
+      Rbi<RC> Ib = model_rbi_of<RC>(M.base_rbi);
+      if constexpr (PAR) { if (pm.any_base) installed_base(Ib); }
+      Rbi<RC> Ic; Ic.m = Ib.m; Ic.h = mul(Rb, Ib.h); Ic.I = rot_sym(Rb, Ib.I);
+      Rbi<RC> D = cor_rate(Ic, v_base);
+      Sv<RC> h = rbi_mul(Ic, v_base);
+      if (n_links > 0 && M.parent[0] < 0) { rbi_add(Ic, cC); rbi_add(D, cor_cD); h = h + cor_cH; }
+      if (M.base_acc >= 0) {
+        const RC* pc = A.ptr<RC>(M.x_acc + M.base_acc * M.x_acc_words);
+        rbi_add(Ic, ld_rbi<RC>(A.ptr<RC>(M.x_acc + M.base_acc * M.x_acc_words + M.x_acc_ic_word), ST));
+        rbi_add(D, ld_rbi<RC>(pc, ST));
+        h = h + ld6<RC>(pc + 10 * ST, ST);
+      }
+      const Sv<RC> z = Sv<RC>{v3<RC>(RC(0), RC(0), RC(0)), v3<RC>(RC(0), RC(0), RC(0))};
+      for (int k = 0; k < 6; ++k) {
+        const V3<RC> u = k % 3 == 0 ? col_x(Rb) : (k % 3 == 1 ? col_y(Rb) : col_z(Rb));
+        Sv<RC> S = z;
+        if (k < 3) S.top = u; else S.bot = u;
+        const Sv<RC> F = rbi_mul(Ic, cross_mm(v_base, S)) + cor_B(D, h, S, false);
+        const V3<RC> ft = mulT(Rb, F.top), fb = mulT(Rb, F.bot);
+        cor_put(k, ft.x); cor_put(n + k, ft.y); cor_put(2 * n + k, ft.z);
+        cor_put(3 * n + k, fb.x); cor_put(4 * n + k, fb.y); cor_put(5 * n + k, fb.z);
+      }
+    }
+    return;
   }
   if constexpr (CEN) {
     if (M.floating) {   // the base twist's unit columns [R_b e_k; 0], [0; R_b e_k] move every body: the momentum is the total inertia's

@@ -966,6 +966,66 @@ class BatchSim:
         self._check(self._L.tds_b200_mass_inverse_vjp_device(self._h, _ptr(q), K, lp, cp, _ptr(G_Minv), _ptr(G_Linv), _ptr(g_q), _ptr(g_par),
                                                              st), "mass_inverse_vjp_device")
 
+    # ---- Coriolis matrix C(q, qd) (DESIGN.md section 7.22) ----
+    def coriolis_host(self, q, qd=None):
+        """C [n, n_qd, n_qd] float64 at the fp32-rounded q [n, n_q] and qd [n, n_qd] (None: zero, C = 0), in the coordinates of
+        mass_matrix_host: Echeandia & Wensing's factorisation, so that C qd is the velocity part of the bias forces (inverse_dynamics_host(q,
+        qd) - inverse_dynamics_host(q) without joint damping) and C + C^T is the time derivative of M along qd.  Installed masses, centres
+        of mass and inertias apply per environment; stiffness, damping, friction and restitution do not enter (include/tds_b200.h)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd = self._inv_in(qd, self.n_qd, "qd")
+        C = np.zeros((self.n_envs, self.n_qd, self.n_qd))
+        self._check(self._L.tds_b200_coriolis_host(self._h, _dp(q), _dp(qd), _dp(C)), "coriolis_host")
+        return C
+
+    def coriolis_device(self, q, qd, C, stream=None):
+        """Device version of coriolis_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd [n_qd, n_stride] (or None), C
+        float64 [n_qd * n_qd, n_stride], entry (r, c) at row r * n_qd + c.  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_coriolis_device(self._h, _ptr(q), _ptr(qd), _ptr(C), st), "coriolis_device")
+
+    def coriolis_jvp_host(self, q, qd=None, t_q=None, t_qd=None, t_par=None):
+        """Directional derivatives of C along m tangents t_q [n, n_q, m], t_qd [n, n_qd, m] and t_par [n, k, m] of the installed
+        parameters (each may be None, not all): (C, dC [n, n_qd, n_qd, m]); tangents given as [n, dim] are m = 1 and drop the last axis."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd = self._inv_in(qd, self.n_qd, "qd")
+        if all(t is None for t in (t_q, t_qd, t_par)):
+            raise ValueError("at least one tangent is expected")
+        (tq, tqd, tp), m, single = self._tangents([(t_q, self.n_q), (t_qd, self.n_qd), (t_par, len(self.param_ids))])
+        n, nd = self.n_envs, self.n_qd
+        C, dC = np.zeros((n, nd, nd)), np.zeros((n, nd, nd, m))
+        self._check(self._L.tds_b200_coriolis_jvp_host(self._h, _dp(q), _dp(qd), m, _dp(tq), _dp(tqd), _dp(tp), _dp(C), _dp(dC)),
+                    "coriolis_jvp_host")
+        return C, (dC[..., 0] if single else dC)
+
+    def coriolis_jvp_device(self, q, qd, m, t_q, t_qd, t_par, t_C, C=None, stream=None):
+        """Device version of coriolis_jvp_host: q float32 [n_q, n_stride], qd [n_qd, n_stride] (or None); t_q [n_q * m, n_stride], t_qd
+        [n_qd * m, n_stride], t_par [k * m, n_stride] (each may be None, not all), t_C [n_qd^2 * m, n_stride] and C [n_qd^2, n_stride] (or
+        None) float64 CUDA tensors, entry (r, j) at row r * m + j.  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_coriolis_jvp_device(self._h, _ptr(q), _ptr(qd), int(m), _ptr(t_q), _ptr(t_qd), _ptr(t_par), _ptr(C),
+                                                         _ptr(t_C), st), "coriolis_jvp_device")
+
+    def coriolis_vjp_host(self, q, qd, G):
+        """Cotangent G [n, n_qd, n_qd] of C -> (g_q [n, n_q], g_qd [n, n_qd], g_par [n, k] or None without installed parameters)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd = self._inv_in(qd, self.n_qd, "qd")
+        n = self.n_envs
+        G = self._inv_in(np.reshape(G, (n, -1)), self.n_qd * self.n_qd, "G")
+        k = len(self.param_ids)
+        g_q, g_qd = np.zeros((n, self.n_q)), np.zeros((n, self.n_qd))
+        g_par = np.zeros((n, k)) if k else None
+        self._check(self._L.tds_b200_coriolis_vjp_host(self._h, _dp(q), _dp(qd), _dp(G), _dp(g_q), _dp(g_qd), _dp(g_par)), "coriolis_vjp_host")
+        return g_q, g_qd, g_par
+
+    def coriolis_vjp_device(self, q, qd, G, g_q, g_qd=None, g_par=None, stream=None):
+        """Device version of coriolis_vjp_host: q float32 [n_q, n_stride], qd [n_qd, n_stride] (or None), G float64 [n_qd * n_qd, n_stride]
+        in C's layout, g_q [n_q, n_stride], g_qd [n_qd, n_stride], g_par [k, n_stride] float64 CUDA tensors (each may be None, not all).
+        Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_coriolis_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(G), _ptr(g_q), _ptr(g_qd), _ptr(g_par), st),
+                    "coriolis_vjp_device")
+
     # ---- point-constrained forward dynamics (DESIGN.md section 7.21) ----
     def _cd_points(self, links, local, dims, damping):
         """The point table (None: no points, K = 0), dims and damping of the constrained_dynamics methods."""
