@@ -531,6 +531,43 @@ int tds_b200_coriolis_vjp_device(tds_b200_sim* sim, const float* q, const float*
                                  void* stream);
 int tds_b200_coriolis_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* G, double* g_q, double* g_qd, double* g_par);
 
+/* ---- derivatives of the inverse dynamics d tau / dq and d tau / dqd (DESIGN.md section 7.23) ----------------------------------------
+ * The linearisation of tds_b200_inverse_dynamics at (q, qd, qdd), each [n_qd * n_qd] fp64 per environment, row-major as
+ * tds_b200_mass_matrix: row r is tau_r, column c a tangent direction.  d tau / dqdd is M (tds_b200_mass_matrix).  tau is exactly that
+ * query's tau: stiffness and damping terms (the spherical joints' axis-angle stiffness included), a floating base's wrench rows in the
+ * base frame with gravity rotated into it, and the installed parameter set.  Inputs are rounded to fp32; qd or qdd may be NULL (zero).
+ * The columns are in M's coordinates, not q's: column k of d tau / dq is d/de tau(q (+) e e_k) at e = 0, where q (+) e d is the
+ * motion with velocity d, whose coordinate rate is dq_dt(q, d) (a floating base: 1/2 q_b (x) (w, 0) and R_b v; a spherical joint: 1/2 q
+ * (x) (w, 0); a REVOLUTE_AXIS joint: |axis| d; other joints: d).  So d tau / dq . d equals tds_b200_inverse_dynamics_jvp along
+ * t_q = dq_dt(q, d), and the matrices compose with M, C and the point Jacobians.  Every entry is written; a world of several
+ * multibodies gives exact zeros between multibodies.
+ * Argument checks: NULL q, no output (neither matrix, or neither tangent for _jvp), no cotangent, m < 1, every tangent NULL, or no
+ * gradient output -> -1; t_par / g_par without an installed set -> -4.
+ *   device: q [n_q][n_stride], qd, qdd [n_qd][n_stride] fp32; dtau_dq, dtau_dqd [n_qd * n_qd][n_stride] fp64 (either may be NULL).
+ *           Asynchronous.
+ *   host:   q [n][n_q], qd, qdd [n][n_qd] fp64 (rounded to fp32); dtau_dq, dtau_dqd [n][n_qd * n_qd].  Synchronous.
+ * _jvp: the tangents of both matrices along m tangents of q (n_q coordinates), qd, qdd and the installed parameters (each may be NULL:
+ *   zero, not all), the layout of tds_b200_inverse_dynamics_jvp; dtau_dq, dtau_dqd (may be NULL) receive the values.  Device t_dtau_dq,
+ *   t_dtau_dqd [n_qd * n_qd * m][n_stride] (either may be NULL, not both); host [n][n_qd * n_qd][m].
+ * _vjp: g_x[c] = <G_dq, d(dtau_dq)/dx_c> + <G_dqd, d(dtau_dqd)/dx_c> for x = q, qd, qdd and, while a set is installed, the parameters
+ *   (the JVP along identity tangents contracted on the device).  G_dq or G_dqd may be NULL (zero), not both; any of g_q, g_qd, g_qdd,
+ *   g_par may be NULL, not all.  Layouts as tds_b200_inverse_dynamics_vjp. */
+int tds_b200_inverse_dynamics_derivatives_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, double* dtau_dq,
+                                                 double* dtau_dqd, void* stream);
+int tds_b200_inverse_dynamics_derivatives_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, double* dtau_dq,
+                                               double* dtau_dqd);
+int tds_b200_inverse_dynamics_derivatives_jvp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, int m,
+                                                     const double* t_q, const double* t_qd, const double* t_qdd, const double* t_par,
+                                                     double* dtau_dq, double* dtau_dqd, double* t_dtau_dq, double* t_dtau_dqd, void* stream);
+int tds_b200_inverse_dynamics_derivatives_jvp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, int m,
+                                                   const double* t_q, const double* t_qd, const double* t_qdd, const double* t_par,
+                                                   double* dtau_dq, double* dtau_dqd, double* t_dtau_dq, double* t_dtau_dqd);
+int tds_b200_inverse_dynamics_derivatives_vjp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* qdd, const double* G_dq,
+                                                     const double* G_dqd, double* g_q, double* g_qd, double* g_qdd, double* g_par,
+                                                     void* stream);
+int tds_b200_inverse_dynamics_derivatives_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, const double* G_dq,
+                                                   const double* G_dqd, double* g_q, double* g_qd, double* g_qdd, double* g_par);
+
 /* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
  * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
  * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,

@@ -194,6 +194,18 @@ def lib():
     L.tds_b200_mass_inverse_vjp_device.argtypes = [vp, fp, ci, vp, dp, vp, vp, vp, vp, vp]
     L.tds_b200_mass_inverse_vjp_host.restype = ci
     L.tds_b200_mass_inverse_vjp_host.argtypes = [vp, dp, ci, vp, dp, dp, dp, dp, dp]
+    L.tds_b200_inverse_dynamics_derivatives_device.restype = ci
+    L.tds_b200_inverse_dynamics_derivatives_device.argtypes = [vp, fp, fp, fp, vp, vp, vp]
+    L.tds_b200_inverse_dynamics_derivatives_host.restype = ci
+    L.tds_b200_inverse_dynamics_derivatives_host.argtypes = [vp, dp, dp, dp, dp, dp]
+    L.tds_b200_inverse_dynamics_derivatives_jvp_device.restype = ci
+    L.tds_b200_inverse_dynamics_derivatives_jvp_device.argtypes = [vp, fp, fp, fp, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.tds_b200_inverse_dynamics_derivatives_jvp_host.restype = ci
+    L.tds_b200_inverse_dynamics_derivatives_jvp_host.argtypes = [vp, dp, dp, dp, ci, dp, dp, dp, dp, dp, dp, dp, dp]
+    L.tds_b200_inverse_dynamics_derivatives_vjp_device.restype = ci
+    L.tds_b200_inverse_dynamics_derivatives_vjp_device.argtypes = [vp, fp, fp, fp, vp, vp, vp, vp, vp, vp, vp]
+    L.tds_b200_inverse_dynamics_derivatives_vjp_host.restype = ci
+    L.tds_b200_inverse_dynamics_derivatives_vjp_host.argtypes = [vp, dp, dp, dp, dp, dp, dp, dp, dp, dp]
     L.tds_b200_coriolis_device.restype = ci
     L.tds_b200_coriolis_device.argtypes = [vp, fp, fp, vp, vp]
     L.tds_b200_coriolis_host.restype = ci
@@ -354,6 +366,9 @@ DECLARED_SYMBOLS = [
     "tds_b200_mass_inverse_vjp_device", "tds_b200_mass_inverse_vjp_host",
     "tds_b200_coriolis_device", "tds_b200_coriolis_host", "tds_b200_coriolis_jvp_device", "tds_b200_coriolis_jvp_host",
     "tds_b200_coriolis_vjp_device", "tds_b200_coriolis_vjp_host",
+    "tds_b200_inverse_dynamics_derivatives_device", "tds_b200_inverse_dynamics_derivatives_host",
+    "tds_b200_inverse_dynamics_derivatives_jvp_device", "tds_b200_inverse_dynamics_derivatives_jvp_host",
+    "tds_b200_inverse_dynamics_derivatives_vjp_device", "tds_b200_inverse_dynamics_derivatives_vjp_host",
     "tds_b200_constrained_dynamics_device", "tds_b200_constrained_dynamics_host", "tds_b200_constrained_dynamics_jvp_device",
     "tds_b200_constrained_dynamics_jvp_host", "tds_b200_constrained_dynamics_vjp_device", "tds_b200_constrained_dynamics_vjp_host",
     "tds_b200_step_contacts_device", "tds_b200_step_contacts_host", "tds_b200_step_contacts_jvp_device", "tds_b200_step_contacts_jvp_host",

@@ -66,6 +66,10 @@ the points of a table held in place and the constraint forces f (float64, DESIGN
 coriolis(sim, q, qd=None, params=None) is the Coriolis matrix C(q, qd) [n_envs, n_qd, n_qd] (float64, DESIGN.md section 7.22) with a
 backward rule (BatchSim.coriolis_vjp_device: float32 q.grad, qd.grad, float64 params.grad) and a forward-mode rule
 (BatchSim.coriolis_jvp_device).
+
+inverse_dynamics_derivatives(sim, q, qd=None, qdd=None, params=None) is (d tau / dq, d tau / dqd) [n_envs, n_qd, n_qd] of the inverse
+dynamics (float64, DESIGN.md section 7.23) with a backward rule (BatchSim.inverse_dynamics_derivatives_vjp_device: float32 q.grad, qd.grad,
+qdd.grad, float64 params.grad) and a forward-mode rule (BatchSim.inverse_dynamics_derivatives_jvp_device).
 """
 from collections import namedtuple
 
@@ -344,7 +348,7 @@ def _state_soa(sim, q, qd, qdd):
 
 class _Query(torch.autograd.Function):
     """The dynamics queries (mass_matrix, inverse_dynamics, centroidal, forward_kinematics, point_motion, regressor, mass_inverse,
-    constrained_dynamics, coriolis) as one Function over a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
+    constrained_dynamics, coriolis, inverse_dynamics_derivatives) as one Function over a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
     float64 output buffers, every C-ABI call ordered on a side stream, and the gradients as float32 (q, qd, qdd) and float64 (params).
     An input the query does not take, or the call leaves out, is None and gets no gradient; a tangent on it is ignored.  With params
     the forward installs their values, and the backward and forward-mode rule reinstall the values of this call (a later call of the
@@ -840,3 +844,25 @@ def coriolis(sim, q, qd=None, params=None):
     _check_state(sim, q, qd)
     _check_params(sim, params)
     return _Query.apply(_CORIOLIS, sim, None, q, qd, None, params)
+
+
+_INVERSE_DYNAMICS_DERIVATIVES = _QuerySpec(
+    rows=lambda sim, p: [sim.n_qd * sim.n_qd, sim.n_qd * sim.n_qd],
+    unpack=lambda sim, p, a, b: (a.reshape(sim.n_envs, sim.n_qd, sim.n_qd).contiguous(), b.reshape(sim.n_envs, sim.n_qd, sim.n_qd).contiguous()),
+    pack=lambda sim, p, ga, gb: [_cot(ga, sim), _cot(gb, sim)],
+    value=lambda sim, p, x, out, st: sim.inverse_dynamics_derivatives_device(x.q, x.qd, x.qdd, *out, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.inverse_dynamics_derivatives_jvp_device(x.q, x.qd, x.qdd, 1, *t, *out, stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.inverse_dynamics_derivatives_vjp_device(x.q, x.qd, x.qdd, *G, *g, stream=st))
+
+
+def inverse_dynamics_derivatives(sim, q, qd=None, qdd=None, params=None):
+    """The derivatives (d tau / dq, d tau / dqd) of inverse_dynamics(sim, q, qd, qdd, params) for every environment of `sim` (a
+    BatchSim), DESIGN.md section 7.23: two [n_envs, n_qd, n_qd] float64 tensors, row r = tau_r, in fp64 at the fp32-rounded q [n_envs,
+    n_q], qd and qdd [n_envs, n_qd] float32 CUDA tensors (qd or qdd None: zero).  The columns are in the coordinates of mass_matrix: column
+    k of d tau / dq is the derivative along the motion with velocity e_k (include/tds_b200.h), so the matrices compose with M, C and the
+    point Jacobians; d tau / dqdd is mass_matrix(sim, q).  params: None, or a float64 CUDA tensor [n_envs, k] of values for the parameters
+    installed by sim.set_physical_params (then also differentiated).  Differentiable in reverse mode (float32 q.grad, qd.grad, qdd.grad,
+    float64 params.grad: second-order terms) and forward mode."""
+    _check_state(sim, q, qd, qdd)
+    _check_params(sim, params)
+    return _Query.apply(_INVERSE_DYNAMICS_DERIVATIVES, sim, None, q, qd, qdd, params)

@@ -101,6 +101,11 @@ extern "C" int tds_launch_osim(const double* J, const double* dJ, const double* 
                                int n, int ns, cudaStream_t stream);
 // Coriolis matrix C(q, qd) and its Jacobian-vector products (tds_coriolis.cu)
 extern "C" int tds_launch_coriolis(const DevModel* M, const StepIO* io, const ParMap* pm, char* gscratch, cudaStream_t stream);
+// Derivatives d tau / dq, d tau / dqd of the inverse dynamics and their Jacobian-vector products (tds_dynamics_derivatives.cu)
+extern "C" int tds_launch_dynamics_derivatives(const DevModel* M, const SimParams* P, const StepIO* io, const ParMap* pm, char* gscratch,
+                                               cudaStream_t stream);
+extern "C" int tds_launch_dynamics_derivatives_jvp(const DevModel* M, const SimParams* P, const StepIO* io, const ParMap* pm, const double* t_in,
+                                                   const double* t_par, int m, int n_dirs, char* gscratch, cudaStream_t stream);
 extern "C" int tds_launch_coriolis_jvp(const DevModel* M, const StepIO* io, const ParMap* pm, const double* t_in, const double* t_par, int m,
                                        int n_dirs, char* gscratch, cudaStream_t stream);
 // the rows and the solve of the point-constrained forward dynamics (tds_constrained.cu)
@@ -929,7 +934,7 @@ int tds_b200_jacobian_dims(const tds_b200_sim* s, int mode, int use_pd, int dims
 
 // what a Jacobian-vector product differentiates: the step, one of the dynamics queries of DESIGN.md sections 7.12-7.14, 7.16 and 7.17,
 // or the step with its contact records (section 7.15)
-enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, regressor, minv, cor };
+enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, regressor, minv, cor, der };
 
 // tangents of a Jacobian-vector product: t_in [cols * m][ns], t_par [k * m][ns] (either may be null).  step: t_in = the step's
 // inputs; mass: t_in = the q tangents (the step's arguments are not read); kin: the kinematics of the point table and outputs `kin`
@@ -937,11 +942,12 @@ enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, r
 // contacts: as step, with the rows q' | qd' | records; centroidal: t_in = the q | qd tangents (qd in the step's qd), outputs `cen`;
 // motion: t_in = the q | qd | qdd tangents (qd and qdd as for inv), the point table and outputs `mot`; wrench: as step, with the point
 // table, wrenches and wrench tangents `ext`; regressor: t_in = the q | qd | qdd tangents (as for inv), Y in jac and the
-// energy outputs `reg`; minv: as mass, M^-1 in jac; cor: t_in = the q | qd tangents (qd in the step's qd), C in jac
+// energy outputs `reg`; minv: as mass, M^-1 in jac; cor: t_in = the q | qd tangents (qd in the step's qd), C in jac; der: t_in as for
+// inv, d tau / dq in jac and d tau / dqd in der_dqd (either may be NULL)
 struct JvpTangents {
   const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr;
   const TdsCenCall* cen = nullptr; const TdsMotCall* mot = nullptr; const TdsExtCall* ext = nullptr;
-  const TdsRegCall* reg = nullptr;
+  const TdsRegCall* reg = nullptr; double* der_dqd = nullptr;
 };
 
 // the installed physical parameters as a launch argument in *pmv, or NULL without any
@@ -970,6 +976,11 @@ static size_t wrench_arena_bytes(const tds_b200_sim* s, const DevModel& M, int s
   return (size_t)(s->n + 31) / 32 * (size_t)words * 32 * 4;
 }
 
+// scratch of one launch of the dynamics-derivative instances (tds_dynamics_derivatives.cu) on layout M with RC of size_rc bytes
+static size_t der_arena_bytes(const tds_b200_sim* s, const DevModel& M, int size_rc) {
+  return (size_t)(s->n + 31) / 32 * (size_t)tds_der_layout_w(&M, size_rc) * 32 * 4;
+}
+
 // directions (Jacobian columns or tangents) one launch of the dual instance takes: the scratch (arena bytes per direction) stays within
 // 2 GB
 static int dir_chunk_of(const tds_b200_sim* s, size_t arena) {
@@ -992,7 +1003,10 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   io.n = s->n; io.n_stride = s->ns;
   ParMap pmv;
   const ParMap* pm = installed_par(s, &pmv);
-  const size_t arena = (jv && jv->query == Query::wrench) ? wrench_arena_bytes(s, s->dm_ad, 16) : lane_arena_bytes(s, s->dm_ad);
+  const size_t arena = (jv && jv->query == Query::wrench) ? wrench_arena_bytes(s, s->dm_ad, 16)
+                       : (jv && jv->query == Query::der)  ? der_arena_bytes(s, s->dm_ad, 16)
+                                                          : lane_arena_bytes(s, s->dm_ad);
+  if (jv && jv->query == Query::der) io.g_in = jv->der_dqd;
   const int chunk = std::min(dir_chunk_of(s, arena), n_dirs);
   CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, arena * chunk));
   const cudaStream_t sm = (cudaStream_t)stream;
@@ -1025,6 +1039,9 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
         case Query::regressor: rc = tds_launch_regressor_jvp(&s->dm_ad, &s->P, &io, jv->reg, jv->t_in, jv->m, nd, s->jac_scratch, sm); break;
         case Query::minv: rc = tds_launch_mass_inverse_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
         case Query::cor: rc = tds_launch_coriolis_jvp(&s->dm_ad, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm); break;
+        case Query::der:
+          rc = tds_launch_dynamics_derivatives_jvp(&s->dm_ad, &s->P, &io, pm, jv->t_in, jv->t_par, jv->m, nd, s->jac_scratch, sm);
+          break;
       }
     }
     if (rc) { set_err(std::string(jv ? "jvp launch: " : "jacobian launch: ") + cudaGetErrorString((cudaError_t)rc)); return rc; }
@@ -1687,6 +1704,143 @@ int tds_b200_centroidal_vjp_host(tds_b200_sim* s, const double* q, const double*
   CUDA_TRY(put_parts<double>(s->vjp_g, {{G_com, R.com}, {G_A, R.A}, {G_bias, R.bias}}, n, ns, s->stream));
   if (int rc = cen_vjp_run(s, s->q, qd_d, s->vjp_g, g_d, g_par ? g_d + (size_t)n_in * ns : nullptr, s->stream)) return rc;
   CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_par, k}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- derivatives of the inverse dynamics d tau / dq, d tau / dqd (DESIGN.md section 7.23): the DER instances of the world-frame kernel
+// (tds_dynamics_derivatives.cu).  The inputs q | qd | qdd are those of the inverse dynamics (inv_n_in, put_inv_inputs). ----------------
+// d tau / dq and d tau / dqd [n_qd * n_qd][ns] (either may be NULL) from q [n_q][ns], qd and qdd [n_qd][ns] fp32 (either NULL: zero)
+static int der_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* dq, double* dqd, cudaStream_t sm) {
+  CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, der_arena_bytes(s, s->dm_m, 8)));
+  return value_run(s, "inverse dynamics derivatives", q, qd, qdd, dq, [&](const StepIO* io, const ParMap* pm) {
+    StepIO d = *io;
+    d.g_in = dqd;
+    return tds_launch_dynamics_derivatives(&s->dm_m, &s->P, &d, pm, s->jac_scratch, sm);
+  });
+}
+
+// t_dq, t_dqd [n_qd * n_qd * m][ns] (either may be NULL) along t_in [(n_q + 2 n_qd) * m][ns] (q | qd | qdd tangents, contiguous) and
+// t_par (either may be NULL); dq, dqd, if not NULL, receive the values
+static int der_jvp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int m, const double* t_in, const double* t_par,
+                       double* dq, double* dqd, double* t_dq, double* t_dqd, cudaStream_t sm) {
+  if (dq || dqd) { if (int rc = der_run(s, q, qd, qdd, dq, dqd, sm)) return rc; }
+  JvpTangents jv{t_in, t_par, m, Query::der};
+  jv.der_dqd = t_dqd;
+  return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, qdd, t_dq, sm, false, &jv);
+}
+
+// g_in [(n_q + 2 n_qd)][ns] (q | qd | qdd, contiguous) and g_par [k][ns] (NULL: not wanted) = <G, d(d tau / dq | d tau / dqd)> for the
+// cotangent G [2 n_qd^2][ns] of both matrices
+static int der_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const double* G, double* g_in, double* g_par,
+                       cudaStream_t sm) {
+  const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
+  return vjp_by_eye(s, "inverse dynamics derivatives", inv_n_in(s), 2 * nn, G, g_in, g_par, sm,
+                    [&](int nd, const double* t_in, const double* t_par, double* dO) {
+                      return der_jvp_run(s, q, qd, qdd, nd, t_in, t_par, nullptr, nullptr, dO, dO + nn * nd * s->ns, sm);
+                    });
+}
+
+int tds_b200_inverse_dynamics_derivatives_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* dtau_dq,
+                                                 double* dtau_dqd, void* stream) {
+  if (!s || !q || (!dtau_dq && !dtau_dqd)) return -1;
+  return der_run(s, q, qd, qdd, dtau_dq, dtau_dqd, (cudaStream_t)stream);
+}
+
+int tds_b200_inverse_dynamics_derivatives_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, double* dtau_dq,
+                                               double* dtau_dqd) {
+  if (!s || !q || (!dtau_dq && !dtau_dqd)) return -1;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const size_t nn = (size_t)s->dm[0].n_qd * s->dm[0].n_qd;
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (2 * nn + 1) * s->ns));
+  double* d = s->jac_dev;
+  if (int rc = der_run(s, s->q, qd_d, qdd_d, dtau_dq ? d : nullptr, dtau_dqd ? d + nn * s->ns : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{dtau_dq, nn}, {dtau_dqd, nn}}, d, s->n, s->ns, s->stream));
+  return 0;
+}
+
+static int der_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_qd, const void* t_qdd, const void* t_par,
+                         const void* t_dq, const void* t_dqd) {
+  if (!s || !q || (!t_dq && !t_dqd) || m < 1 || (!t_q && !t_qd && !t_qdd && !t_par)) return -1;
+  return par_without_installed(s, t_par, "inverse dynamics derivatives jvp: parameter tangents");
+}
+
+int tds_b200_inverse_dynamics_derivatives_jvp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int m,
+                                                     const double* t_q, const double* t_qd, const double* t_qdd, const double* t_par,
+                                                     double* dtau_dq, double* dtau_dqd, double* t_dtau_dq, double* t_dtau_dqd, void* stream) {
+  if (int rc = der_jvp_check(s, q, m, t_q, t_qd, t_qdd, t_par, t_dtau_dq, t_dtau_dqd)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd;
+  cudaStream_t sm = (cudaStream_t)stream;
+  double* tin = nullptr;
+  if (t_q || t_qd || t_qdd) {   // the kernel reads the q | qd | qdd tangents as one array
+    CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (size_t)inv_n_in(s) * m * s->ns));
+    tin = s->jac_dev;
+    CUDA_TRY(put_parts_d2d<double>(tin, {{t_q, n_q * m}, {t_qd, nd * m}, {t_qdd, nd * m}}, s->ns, sm));
+  }
+  return der_jvp_run(s, q, qd, qdd, m, tin, t_par, dtau_dq, dtau_dqd, t_dtau_dq, t_dtau_dqd, sm);
+}
+
+int tds_b200_inverse_dynamics_derivatives_jvp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, int m,
+                                                   const double* t_q, const double* t_qd, const double* t_qdd, const double* t_par,
+                                                   double* dtau_dq, double* dtau_dqd, double* t_dtau_dq, double* t_dtau_dqd) {
+  if (int rc = der_jvp_check(s, q, m, t_q, t_qd, t_qdd, t_par, t_dtau_dq, t_dtau_dqd)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; q | qd | qdd (contiguous, zero where NULL, none if all are), t_par, the
+  // tangents of d tau / dq and d tau / dqd, their values
+  const size_t ti = (t_q || t_qd || t_qdd) ? (size_t)inv_n_in(s) * m : 0, tp = (size_t)(t_par ? s->par.n : 0) * m, to = nn * m;
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + tp + 2 * to + 2 * nn + 1) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + (ti + tp) * ns;
+  double* v_d = to_d + 2 * to * ns;
+  if (ti) CUDA_TRY(put_parts<double>(d, {{t_q, n_q * m}, {t_qd, nd * m}, {t_qdd, nd * m}}, n, ns, s->stream));
+  if (t_par) CUDA_TRY(put_rows(d + ti * ns, t_par, tp, n, ns, s->stream));
+  if (int rc = der_jvp_run(s, s->q, qd_d, qdd_d, m, ti ? d : nullptr, t_par ? d + ti * ns : nullptr, dtau_dq ? v_d : nullptr,
+                           dtau_dqd ? v_d + nn * ns : nullptr, t_dtau_dq ? to_d : nullptr, t_dtau_dqd ? to_d + to * ns : nullptr, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{t_dtau_dq, to}, {t_dtau_dqd, to}, {dtau_dq, nn}, {dtau_dqd, nn}}, to_d, n, ns, s->stream));
+  return 0;
+}
+
+static int der_vjp_check(tds_b200_sim* s, const void* q, const void* G_dq, const void* G_dqd, const void* g_q, const void* g_qd,
+                         const void* g_qdd, const void* g_par) {
+  if (!s || !q || (!G_dq && !G_dqd) || (!g_q && !g_qd && !g_qdd && !g_par)) return -1;
+  return par_without_installed(s, g_par, "inverse dynamics derivatives vjp: parameter cotangents");
+}
+
+int tds_b200_inverse_dynamics_derivatives_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, const double* G_dq,
+                                                     const double* G_dqd, double* g_q, double* g_qd, double* g_qdd, double* g_par,
+                                                     void* stream) {
+  if (int rc = der_vjp_check(s, q, G_dq, G_dqd, g_q, g_qd, g_qdd, g_par)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd;
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the cotangent G_dq | G_dqd (zero where NULL) and g_q | g_qd | g_qdd are one array each: in s->vjp_g, then copied out
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (2 * nn + (size_t)inv_n_in(s)) * s->ns));
+  double* g_d = s->vjp_g + 2 * nn * s->ns;
+  CUDA_TRY(put_parts_d2d<double>(s->vjp_g, {{G_dq, nn}, {G_dqd, nn}}, s->ns, sm));
+  if (int rc = der_vjp_run(s, q, qd, qdd, s->vjp_g, g_d, g_par, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}}, g_d, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_inverse_dynamics_derivatives_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* qdd, const double* G_dq,
+                                                   const double* G_dqd, double* g_q, double* g_qd, double* g_qdd, double* g_par) {
+  if (int rc = der_vjp_check(s, q, G_dq, G_dqd, g_q, g_qd, g_qdd, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns, n_in = inv_n_in(s);
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd, k = s->par.n;
+  const float *qd_d, *qdd_d;
+  if (int rc = put_inv_inputs(s, q, qd, qdd, &qd_d, &qdd_d)) return rc;
+  // G_dq | G_dqd | g_q | g_qd | g_qdd | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (2 * nn + n_in + k + 1) * ns));
+  double* g_d = s->vjp_g + 2 * nn * ns;
+  CUDA_TRY(put_parts<double>(s->vjp_g, {{G_dq, nn}, {G_dqd, nn}}, n, ns, s->stream));
+  if (int rc = der_vjp_run(s, s->q, qd_d, qdd_d, s->vjp_g, g_d, g_par ? g_d + (size_t)n_in * ns : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_qdd, nd}, {g_par, k}}, g_d, n, ns, s->stream));
   return 0;
 }
 

@@ -343,6 +343,13 @@ TDS_HOST_INLINE int tds_ext_layout_w(const DevModel* D, int size_ra, int* x_tota
   return x_ext;
 }
 
+// Layout of the world-frame kernel's dynamics-derivative instances (tds_stepw.cu, template flag DER; DESIGN.md section 7.23): the layout D
+// followed by a_i and f_i of every link, 12 RC words per link, 16-byte aligned.  Returns the words per lane of the grown layout, whose last
+// 12 RC n_links words the kernel addresses; D itself is unchanged.
+TDS_HOST_INLINE int tds_der_layout_w(const DevModel* D, int size_rc) {
+  return ((D->x_total + 3) & ~3) + D->n_links * 12 * (size_rc / 4);
+}
+
 // ---- physical parameter ids (include/tds_b200.h, tds_b200_set_physical_params_*) ----------------------------------------------------
 // 0 friction, 1 restitution, 2 + 10 b + c body b (0 = base, i + 1 = link i; c: mass, com x y z, I_com xx xy xz yy yz zz),
 // 2 + 10 (n_links + 1) + 2 i + c link i (c: joint stiffness, joint damping)

@@ -184,9 +184,22 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // (B_i^T S_a - v_j x* (Ic_i S_a)) . S_b against its ancestors' columns b, F_a = Ic_i S_a' + B_i S_a (B_i^T = 1/2 (Ic_i' - h_i x*) is
 // B_i with the skew part negated).  A floating base's own block after the sweep from the whole tree's composites.  Every entry is
 // written: zeros first, C [n_qd * n_qd] at io.jac as MASS writes M (padding dofs not written).  ABA and integration are not compiled in.
+// DER: the derivatives d tau / dq and d tau / dqd of INV's tau (DESIGN.md section 7.23), launched as INV, in the tangent coordinates of
+// the velocities: the tangent of q along the motion with velocity e_k.  Pass 1 carries v_i and a_i as INV does and keeps a_i and f_i =
+// r_i a_i + v_i x* (r_i v_i) per link in a region of 12 RC words per link at the end of the arena (x_total - 12 RCW n_links: the launch
+// grows the layout, tds_der_layout_w).  Pass 2 carries COR's composites Ic_i, Ic_i' and h_i and the subtree force F_i = sum f_k.  A column
+// S (link j's, or the base twist's) with the parent's velocity v_l and acceleration a_l (the base's: 0 and -g) moves the subtree of j
+// rigidly (q) or adds S to its velocities (qd); what does not move with it is alpha = v_l x S, gamma = a_l x S + v_l x alpha (q) or S,
+// psi = (v_l + v_j) x S (qd), and each body k of the subtree adds F(gamma, alpha) = r_k gamma + r_k' alpha + alpha x* (r_k v_k) to its
+// force, the covariant S x* f_k besides (q).  So row b of link i against column S of an ancestor-or-self j is S_b . F_i(gamma, alpha)
+// (qd: F_i(psi, S)), = (Ic_i S_b) . gamma + (Ic_i' S_b - S_b x* h_i) . alpha, and row b of a strict ancestor against S of link i is
+// S_b . (F_i(gamma, alpha) + S x* F_i) (qd: S_b . F_i(psi, S)).  The stiffness and damping terms go into link i's own block, a spherical
+// joint's axis-angle stiffness along its three tangents by a local dual number; a floating base's own block after the sweep from the
+// whole tree's composites.  Every entry is written: zeros first, d tau / dq [n_qd * n_qd] at io.jac and d tau / dqd at io.g_in (either
+// may be null), row-major as MASS writes M.  ABA and integration are not compiled in.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
           bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false, bool REG = false,
-          bool MINV = false, bool COR = false>
+          bool MINV = false, bool COR = false, bool DER = false>
 __global__ void __launch_bounds__(128, 1)
 tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ SimParams P,
                  const __grid_constant__ EnvParams E, const StepIO io, const int mode, const int use_pd,
@@ -277,18 +290,27 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   auto n_cols = [&](int j) -> int { return (M.flags[j] & TDS_LF_FIXED) ? 0 : ((M.flags[j] & TDS_LF_SPHERICAL) ? 3 : 1); };
   const int LWD = M.x_link_words;
   const int VOFF = LWD - 6 * RAW;                  // word offset of v/c/a inside a link record
+  // DER: a_i at derw + 12 i ST and f_i behind it (the region the DER launches add at the end of the layout)
+  RC* const derw = [&]() -> RC* {
+    if constexpr (DER) return A.ptr<RC>(M.x_total - 12 * RCW * n_links);
+    else return nullptr;
+  }();
   RS* const Mb = A.ptr<RS>(M.x_M);
   RS* const dinv = A.ptr<RS>(M.x_dinv);
   RS* const wv = A.ptr<RS>(M.x_w);
   // INV only (the step's own statements of these two stay inline: its code must not change).  quaternion_axis_angle(q) of spherical
   // joint i, the vector its stiffness multiplies (forward_dynamics.hpp:69-74, tiny_algebra.hpp:509-527)
+  // (of the quaternion's components in any scalar type: DER evaluates it on a local dual number for its q-derivative)
+  auto axis_angle_of = [&](auto qx, auto qy, auto qz, auto qw) {
+    typedef decltype(qx) T;
+    const T nrm = sqrt_t(qx * qx + qy * qy + qz * qz);
+    const T theta = T(2) * atan2_t(nrm, qw);
+    const T scaling = nrm < T(1.220703125e-4) ? T(1) / (T(0.5) + theta * theta * T(1.0 / 48.0)) : theta / nrm;   // eps^(1/4)
+    return v3<T>(scaling * qx, scaling * qy, scaling * qz);
+  };
   auto axis_angle = [&](int i) -> V3<RC> {
     const int q0 = M.q_idx[i];
-    const RC qx = RC(qv[q0 * ST]), qy = RC(qv[(q0 + 1) * ST]), qz = RC(qv[(q0 + 2) * ST]), qw = RC(qv[(q0 + 3) * ST]);
-    const RC nrm = sqrt_t(qx * qx + qy * qy + qz * qz);
-    const RC theta = RC(2) * atan2_t(nrm, qw);
-    const RC scaling = nrm < RC(1.220703125e-4) ? RC(1) / (RC(0.5) + theta * theta * RC(1.0 / 48.0)) : theta / nrm;   // eps^(1/4)
-    return v3<RC>(scaling * qx, scaling * qy, scaling * qz);
+    return axis_angle_of(RC(qv[q0 * ST]), RC(qv[(q0 + 1) * ST]), RC(qv[(q0 + 2) * ST]), RC(qv[(q0 + 3) * ST]));
   };
   // installed base quantities: (m, h, I about the origin) packed per lane as tds_rbi_pack does on the host (the block after pass 2)
   auto installed_base = [&](Rbi<RP>& bp) {
@@ -309,7 +331,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // input directions of the differentiable instance: q | qd | tau or action | kp, kd, max_force (with PD)
   const int in0 = M.n_q + n;
   for (int k = 0; k < M.n_q; ++k) qv[k * ST] = seed(RQ(io.q_in[(size_t)k * ns + e]), k);
-  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(((INV || CEN || MOT || COR) && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
+  for (int k = 0; k < n; ++k) qdv[k * ST] = (MASS || KIN) ? RQ(0.f) : seed(RQ(((INV || CEN || MOT || COR || DER) && !io.qd_in) ? 0.f : io.qd_in[(size_t)k * ns + e]), M.n_q + k);
   for (int k = 0; k < n; ++k) tauv[k * ST] = RQ(0.f);
   if (!MASS && use_pd) {
     const RQ kp = seed(RQ(E.kp), in0 + E.n_act), kd = seed(RQ(E.kd), in0 + E.n_act + 1), fmax_ = seed(RQ(E.max_force), in0 + E.n_act + 2);
@@ -322,7 +344,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       f = min_t(max_t(f, -fmax_), fmax_);
       tauv[M.qd_idx[li] * ST] = f;
     }
-  } else if (!MASS && !INV && !MOT && io.tau_in) {
+  } else if (!MASS && !INV && !MOT && !DER && io.tau_in) {
     const int off = M.floating ? 6 : 0;
     for (int k = off; k < n; ++k) tauv[k * ST] = seed(RQ(io.tau_in[(size_t)(k - off) * ns + e]), in0 + k - off);
   }
@@ -623,7 +645,7 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   // INV: qdd of dof k (seeded at input n_q + n_qd + k); the acceleration of the previous link, of the base; the sum of the link forces
   auto qdd_in = [&](int k) -> RQ { return seed(RQ(io.tau_in ? io.tau_in[(size_t)k * ns + e] : 0.f), M.n_q + n + k); };
   // (empty placeholders in the other instances, whose code must not change)
-  typedef typename std::conditional<INV || MOT, Sv<RC>, NoPar>::type SvInv;
+  typedef typename std::conditional<INV || MOT || DER, Sv<RC>, NoPar>::type SvInv;
   const SvInv a_base_inv = [&]() -> SvInv {
     if constexpr (MOT) {   // the base's acceleration without gravity: zero, or the base-frame qdd[0:6] in the common frame
       static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the MOT instances run in one scalar type");
@@ -635,8 +657,8 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
         a.bot = mul(Rb, v3<RC>(qdd_in(3), qdd_in(4), qdd_in(5)));
       }
       return a;
-    } else if constexpr (INV) {
-      static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the INV instances run in one scalar type");
+    } else if constexpr (INV || DER) {
+      static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the INV and DER instances run in one scalar type");
       const V3<RC> g = v3<RC>(RC(P.gravity[0]), RC(P.gravity[1]), RC(P.gravity[2]));
       Sv<RC> a;
       a.top = v3<RC>(RC(0), RC(0), RC(0));
@@ -816,6 +838,24 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       st6<RC>(A.ptr<RC>(M.x_link + i * LWD), ST, a);
       a_prev_inv = a;
       mot_link(i, Ri, pi, v, a);
+    }
+    if constexpr (DER) {   // a_i as INV carries it and f_i, kept in the derivative region
+      Sv<RC> a;
+      if (fl & TDS_LF_PARENT_ADJ) a = a_prev_inv;
+      else if (p >= 0) a = ld6<RC>(derw + 12 * p * ST, ST);
+      else a = a_base_inv;
+      Sv<RC> vJ; vJ.top = v3<RC>(RC(0), RC(0), RC(0)); vJ.bot = vJ.top;
+      for (int c = 0; c < n_cols(i); ++c) {
+        const Sv<RC> Sc = S_col(i, c);
+        const RC qdc = qdv[(M.qd_idx[i] + c) * ST], qddc = qdd_in(M.qd_idx[i] + c);
+        vJ.top = axpy(Sc.top, qdc, vJ.top); vJ.bot = axpy(Sc.bot, qdc, vJ.bot);
+        a.top = axpy(Sc.top, qddc, a.top); a.bot = axpy(Sc.bot, qddc, a.bot);
+      }
+      a = a + cross_mm(v, vJ);
+      const Rbi<RC> r = ld_rbi<RC>(A.ptr<RC>(M.x_link + i * LWD), ST);
+      st6<RC>(derw + 12 * i * ST, ST, a);
+      st6<RC>(derw + (12 * i + 6) * ST, ST, rbi_mul(r, a) + cross_mf(v, rbi_mul(r, v)));
+      a_prev_inv = a;
     }
     R_prev = Ri; p_prev = pi; v_prev = v;
   }
@@ -1056,11 +1096,46 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     o.bot = a.bot * RC(0.5) + b.bot * s;
     return o;
   };
-  typename std::conditional<COR, Rbi<RC>, NoPar>::type cor_cD{};
-  typename std::conditional<COR, Sv<RC>, NoPar>::type cor_cH{};
+  typename std::conditional<COR || DER, Rbi<RC>, NoPar>::type cor_cD{};
+  typename std::conditional<COR || DER, Sv<RC>, NoPar>::type cor_cH{};
   if constexpr (COR) {
     static_assert(std::is_same<RA, RC>::value && std::is_same<RC, RQ>::value, "the COR instances run in one scalar type");
     for (int k = 0; k < n * n; ++k) cor_put(k, RC(0));
+  }
+  // DER: entry k of d tau / dq (o = 0) or d tau / dqd (o = 1); the subtree force handed from an adjacent child; column c of link j (-1:
+  // the floating base's twist column c) with the quantities that do not move with the subtree (see the comment on the kernel)
+  auto der_put = [&](int o, int k, const RC& x) {
+    if constexpr (DER) {
+      double* out = o ? io.g_in : io.jac;
+      if (!live || !out) return;
+      if constexpr (AD) out[((size_t)k * io.jac_n_in + jcol) * ns + e] = x.d;
+      else out[(size_t)k * ns + e] = x;
+    }
+  };
+  typename std::conditional<DER, Sv<RC>, NoPar>::type der_cF{};
+  auto der_col = [&](int j, int c, Sv<RC>& S, Sv<RC>& al, Sv<RC>& ga, Sv<RC>& ps) {
+    if constexpr (DER) {
+      const Sv<RC> z = Sv<RC>{v3<RC>(RC(0), RC(0), RC(0)), v3<RC>(RC(0), RC(0), RC(0))};
+      Sv<RC> vl = z, al_ = z, vj = v_base;   // the base's: the world's velocity and acceleration (-g)
+      al_.bot = v3<RC>(RC(-P.gravity[0]), RC(-P.gravity[1]), RC(-P.gravity[2]));
+      if (j >= 0) {
+        const int pj = M.parent[j];
+        if (pj >= 0) { vl = ld6<RC>(A.ptr<RC>(M.x_link + pj * LWD + VOFF), ST); al_ = ld6<RC>(derw + 12 * pj * ST, ST); }
+        else { vl = v_base; al_ = a_base_inv; }
+        vj = ld6<RC>(A.ptr<RC>(M.x_link + j * LWD + VOFF), ST);
+        S = S_col(j, c);
+      } else {
+        const V3<RC> u = c % 3 == 0 ? col_x(Rb) : (c % 3 == 1 ? col_y(Rb) : col_z(Rb));
+        S = z;
+        if (c < 3) S.top = u; else S.bot = u;
+      }
+      al = cross_mm(vl, S);
+      ga = cross_mm(al_, S) + cross_mm(vl, al);
+      ps = cross_mm(vl + vj, S);
+    }
+  };
+  if constexpr (DER) {
+    for (int k = 0; k < n * n; ++k) { der_put(0, k, RC(0)); der_put(1, k, RC(0)); }
   }
   for (int i = n_links - 1; i >= 0; --i) {
     const int p = M.parent[i];
@@ -1079,25 +1154,30 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
       }
     }
     // COR: the link's own rate and momentum, then its children's composites (in the accumulators' ABA words: rate 10, momentum 6)
-    typename std::conditional<COR, Rbi<RC>, NoPar>::type cor_D{};
-    typename std::conditional<COR, Sv<RC>, NoPar>::type cor_h{};
-    if constexpr (COR) { cor_D = cor_rate(Ic, v); cor_h = rbi_mul(Ic, v); }
+    // DER: these and the subtree force (rate 10, momentum 6, force 6)
+    typename std::conditional<COR || DER, Rbi<RC>, NoPar>::type cor_D{};
+    typename std::conditional<COR || DER, Sv<RC>, NoPar>::type cor_h{};
+    typename std::conditional<DER, Sv<RC>, NoPar>::type der_F{};
+    if constexpr (COR || DER) { cor_D = cor_rate(Ic, v); cor_h = rbi_mul(Ic, v); }
+    if constexpr (DER) der_F = ld6<RC>(derw + (12 * i + 6) * ST, ST);
     if (fl & TDS_LF_CHILD_ADJ) {
-      if constexpr (!MASS && !CEN && !COR) { abi_add(Ia, cA); pA = pA + cP; }
+      if constexpr (!MASS && !CEN && !COR && !DER) { abi_add(Ia, cA); pA = pA + cP; }
       rbi_add(Ic, cC);
-      if constexpr (COR) { rbi_add(cor_D, cor_cD); cor_h = cor_h + cor_cH; }
+      if constexpr (COR || DER) { rbi_add(cor_D, cor_cD); cor_h = cor_h + cor_cH; }
+      if constexpr (DER) der_F = der_F + der_cF;
     }
     if (M.acc_slot[i] >= 0) {
-      if constexpr (!MASS && !CEN && !COR) {
+      if constexpr (!MASS && !CEN && !COR && !DER) {
         Abi<RA> sa; Sv<RA> sp;
         acc_ld27<RA>(A.ptr<RA>(M.x_acc + M.acc_slot[i] * M.x_acc_words), ST, sa, sp);
         abi_add(Ia, sa); pA = pA + sp;
       }
       rbi_add(Ic, ld_rbi<RC>(A.ptr<RC>(M.x_acc + M.acc_slot[i] * M.x_acc_words + M.x_acc_ic_word), ST));
-      if constexpr (COR) {
+      if constexpr (COR || DER) {
         const RC* pc = A.ptr<RC>(M.x_acc + M.acc_slot[i] * M.x_acc_words);
         rbi_add(cor_D, ld_rbi<RC>(pc, ST));
         cor_h = cor_h + ld6<RC>(pc + 10 * ST, ST);
+        if constexpr (DER) der_F = der_F + ld6<RC>(pc + 16 * ST, ST);
       }
     }
     Sv<RA> pa = pA;
@@ -1147,6 +1227,66 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
           cor_put(r, xt.x); cor_put(r + 1, xt.y); cor_put(r + 2, xt.z); cor_put(r + 3, xb.x); cor_put(r + 4, xb.y); cor_put(r + 5, xb.z);
           cor_put(d0 + a, ft.x); cor_put(n + d0 + a, ft.y); cor_put(2 * n + d0 + a, ft.z);
           cor_put(3 * n + d0 + a, fb.x); cor_put(4 * n + d0 + a, fb.y); cor_put(5 * n + d0 + a, fb.z);
+        }
+      }
+    } else if constexpr (DER) {   // link i's rows and columns against those of i and its ancestors, column a of i at a time
+      const int d0 = M.qd_idx[i], nc = n_cols(i);
+      for (int a = 0; a < nc; ++a) {
+        Sv<RC> S, al, ga, ps;
+        der_col(i, a, S, al, ga, ps);
+        const Sv<RC> G = rbi_mul(Ic, S), Sh = cross_mf(S, cor_h);
+        Sv<RC> H = rbi_mul(cor_D, S);   // row a against a column: (Ic S_a) . gamma + H . alpha
+        H.top = H.top - Sh.top; H.bot = H.bot - Sh.bot;
+        const Sv<RC> Fn = rbi_mul(Ic, ga) + rbi_mul(cor_D, al) + cross_mf(al, cor_h);
+        const Sv<RC> Fd = rbi_mul(Ic, ps) + rbi_mul(cor_D, S) + cross_mf(S, cor_h);
+        const Sv<RC> Fq = Fn + cross_mf(S, der_F);
+        for (int b = 0; b < nc; ++b) {
+          const Sv<RC> Sb = S_col(i, b);
+          RC kq = RC(0), kd = RC(0);   // the stiffness and damping terms
+          if (fl & TDS_LF_SPHERICAL) {
+            if (a == b) kd = joint_par(i, 1, M.damping[i]);
+            if (M.stiffness[i] != 0.f || joint_slot(i, 0) >= 0) {   // d/de axis_angle(q (+) e e_a), q' = 1/2 q (x) (e_a, 0)
+              typedef tds::Dual<RC> T;
+              const int q0 = M.q_idx[i];
+              const RC x = qv[q0 * ST], y = qv[(q0 + 1) * ST], z = qv[(q0 + 2) * ST], w = qv[(q0 + 3) * ST];
+              const V3<RC> ea = v3<RC>(RC(a == 0), RC(a == 1), RC(a == 2));
+              const V3<RC> dv = (ea * w + cross(v3<RC>(x, y, z), ea)) * RC(0.5);
+              const V3<T> aa = axis_angle_of(T(x, dv.x), T(y, dv.y), T(z, dv.z), T(w, RC(-0.5) * dot(v3<RC>(x, y, z), ea)));
+              kq = joint_par(i, 0, M.stiffness[i]) * (b == 0 ? aa.x : (b == 1 ? aa.y : aa.z)).d;
+            }
+          } else {
+            kd = joint_par(i, 1, M.damping[i]);
+            kq = joint_par(i, 0, M.stiffness[i]);
+            if (M.jtype[i] == TDSJ_REVOLUTE_AXIS && !(fl & TDS_LF_PRISMATIC)) {   // q' = |axis| along the unit tangent
+              const V3<RC> ax = v3<RC>(RC(M.axis[i][0]), RC(M.axis[i][1]), RC(M.axis[i][2]));
+              kq = kq * sqrt_t(dot(ax, ax));
+            }
+          }
+          der_put(0, (d0 + b) * n + d0 + a, dot(Sb, Fn) + kq);
+          der_put(1, (d0 + b) * n + d0 + a, dot(Sb, Fd) + kd);
+        }
+        for (int j = M.parent[i]; j >= 0; j = M.parent[j]) {
+          for (int b = 0; b < n_cols(j); ++b) {
+            Sv<RC> Sb, alb, gab, psb;
+            der_col(j, b, Sb, alb, gab, psb);
+            const int rj = M.qd_idx[j] + b;
+            der_put(0, rj * n + d0 + a, dot(Sb, Fq));
+            der_put(1, rj * n + d0 + a, dot(Sb, Fd));
+            der_put(0, (d0 + a) * n + rj, dot(G, gab) + dot(H, alb));
+            der_put(1, (d0 + a) * n + rj, dot(G, psb) + dot(H, Sb));
+          }
+        }
+        if (M.floating) {   // the base twist's columns: a dot product with one is a base-frame component
+          const V3<RC> qt = mulT(Rb, Fq.top), qb = mulT(Rb, Fq.bot), dt = mulT(Rb, Fd.top), db = mulT(Rb, Fd.bot);
+          const RC fq[6] = {qt.x, qt.y, qt.z, qb.x, qb.y, qb.z}, fd[6] = {dt.x, dt.y, dt.z, db.x, db.y, db.z};
+          for (int k = 0; k < 6; ++k) {
+            Sv<RC> Sb, alb, gab, psb;
+            der_col(-1, k, Sb, alb, gab, psb);
+            der_put(0, k * n + d0 + a, fq[k]);
+            der_put(1, k * n + d0 + a, fd[k]);
+            der_put(0, (d0 + a) * n + k, dot(G, gab));
+            der_put(1, (d0 + a) * n + k, dot(G, psb) + dot(H, Sb));
+          }
         }
       }
     } else if (fl & TDS_LF_FIXED) {
@@ -1259,19 +1399,48 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
     // hand (Ia, pa, Ic) to the parent: plain sums in the common frame
     if (fl & TDS_LF_PARENT_ADJ) {
       cA = Ia; cP = pa; cC = Ic;
-      if constexpr (COR) { cor_cD = cor_D; cor_cH = cor_h; }
+      if constexpr (COR || DER) { cor_cD = cor_D; cor_cH = cor_h; }
+      if constexpr (DER) der_cF = der_F;
     } else {
       const int slot = (p >= 0) ? M.acc_slot[p] : M.base_acc;
       if (slot >= 0) {
-        if constexpr (!MASS && !CEN && !COR) acc_add27<RA>(A.ptr<RA>(M.x_acc + slot * M.x_acc_words), ST, Ia, pa);
+        if constexpr (!MASS && !CEN && !COR && !DER) acc_add27<RA>(A.ptr<RA>(M.x_acc + slot * M.x_acc_words), ST, Ia, pa);
         rbi_acc<RC>(A.ptr<RC>(M.x_acc + slot * M.x_acc_words + M.x_acc_ic_word), ST, Ic);
-        if constexpr (COR) {
+        if constexpr (COR || DER) {
           RC* pc = A.ptr<RC>(M.x_acc + slot * M.x_acc_words);
           rbi_acc<RC>(pc, ST, cor_D);
           st6<RC>(pc + 10 * ST, ST, ld6<RC>(pc + 10 * ST, ST) + cor_h);
+          if constexpr (DER) st6<RC>(pc + 16 * ST, ST, ld6<RC>(pc + 16 * ST, ST) + der_F);
         }
       }
     }
+  }
+  if constexpr (DER) {
+    if (M.floating) {   // the base's own block from the whole tree's composites, the base body's included (in world axes about O)
+      Rbi<RC> Ib = model_rbi_of<RC>(M.base_rbi);
+      if constexpr (PAR) { if (pm.any_base) installed_base(Ib); }
+      Rbi<RC> Ic; Ic.m = Ib.m; Ic.h = mul(Rb, Ib.h); Ic.I = rot_sym(Rb, Ib.I);
+      Rbi<RC> D = cor_rate(Ic, v_base);
+      Sv<RC> h = rbi_mul(Ic, v_base);
+      if (n_links > 0 && M.parent[0] < 0) { rbi_add(Ic, cC); rbi_add(D, cor_cD); h = h + cor_cH; }
+      if (M.base_acc >= 0) {
+        const RC* pc = A.ptr<RC>(M.x_acc + M.base_acc * M.x_acc_words);
+        rbi_add(Ic, ld_rbi<RC>(A.ptr<RC>(M.x_acc + M.base_acc * M.x_acc_words + M.x_acc_ic_word), ST));
+        rbi_add(D, ld_rbi<RC>(pc, ST));
+        h = h + ld6<RC>(pc + 10 * ST, ST);
+      }
+      for (int k = 0; k < 6; ++k) {   // alpha = 0: the twist columns do not move the world
+        Sv<RC> S, al, ga, ps;
+        der_col(-1, k, S, al, ga, ps);
+        const Sv<RC> Fn = rbi_mul(Ic, ga), Fd = rbi_mul(Ic, ps) + rbi_mul(D, S) + cross_mf(S, h);
+        const V3<RC> nt = mulT(Rb, Fn.top), nb_ = mulT(Rb, Fn.bot), dt = mulT(Rb, Fd.top), db = mulT(Rb, Fd.bot);
+        der_put(0, k, nt.x); der_put(0, n + k, nt.y); der_put(0, 2 * n + k, nt.z);
+        der_put(0, 3 * n + k, nb_.x); der_put(0, 4 * n + k, nb_.y); der_put(0, 5 * n + k, nb_.z);
+        der_put(1, k, dt.x); der_put(1, n + k, dt.y); der_put(1, 2 * n + k, dt.z);
+        der_put(1, 3 * n + k, db.x); der_put(1, 4 * n + k, db.y); der_put(1, 5 * n + k, db.z);
+      }
+    }
+    return;
   }
   if constexpr (COR) {
     if (M.floating) {   // the base's own block from the whole tree's composites, the base body's included (in world axes about O)

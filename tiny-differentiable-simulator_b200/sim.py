@@ -435,6 +435,80 @@ class BatchSim:
         self._check(self._L.tds_b200_inverse_dynamics_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(G), _ptr(g_q), _ptr(g_qd),
                                                                  _ptr(g_qdd), _ptr(g_par), st), "inverse_dynamics_vjp_device")
 
+    # ---- derivatives of the inverse dynamics (DESIGN.md section 7.23) ----
+    def inverse_dynamics_derivatives_host(self, q, qd=None, qdd=None):
+        """(dtau_dq, dtau_dqd) [n, n_qd, n_qd] float64: the derivatives of inverse_dynamics_host's tau at the fp32-rounded q [n, n_q], qd,
+        qdd [n, n_qd] (None: zero), row r = tau_r, column c = a tangent direction in M's coordinates: column k of dtau_dq is the
+        derivative along the motion with velocity e_k, i.e. inverse_dynamics_jvp_host along t_q = dq_dt(q, e_k) (include/tds_b200.h).
+        dtau / dqdd is mass_matrix_host(q)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        a, b = np.zeros((self.n_envs, self.n_qd, self.n_qd)), np.zeros((self.n_envs, self.n_qd, self.n_qd))
+        self._check(self._L.tds_b200_inverse_dynamics_derivatives_host(self._h, _dp(q), _dp(qd), _dp(qdd), _dp(a), _dp(b)),
+                    "inverse_dynamics_derivatives_host")
+        return a, b
+
+    def inverse_dynamics_derivatives_device(self, q, qd, qdd, dtau_dq, dtau_dqd, stream=None):
+        """Device version of inverse_dynamics_derivatives_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd and qdd
+        [n_qd, n_stride] (either may be None), dtau_dq and dtau_dqd float64 [n_qd * n_qd, n_stride] (either may be None, not both).
+        Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_inverse_dynamics_derivatives_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(dtau_dq), _ptr(dtau_dqd),
+                                                                         st), "inverse_dynamics_derivatives_device")
+
+    def inverse_dynamics_derivatives_jvp_host(self, q, qd, qdd, t_q=None, t_qd=None, t_qdd=None, t_par=None):
+        """Directional derivatives of (dtau_dq, dtau_dqd): each [n, n_qd, n_qd, m] along the m tangents t_q [n, n_q, m], t_qd and t_qdd
+        [n, n_qd, m] and t_par [n, k, m] (each may be None, not all; [n, dim] is m = 1 and gives [n, n_qd, n_qd]).  Returns (dtau_dq,
+        dtau_dqd, t_dtau_dq, t_dtau_dqd)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        if all(t is None for t in (t_q, t_qd, t_qdd, t_par)):
+            raise ValueError("at least one tangent is expected")
+        ts, m, single = self._tangents([(t_q, self.n_q), (t_qd, self.n_qd), (t_qdd, self.n_qd), (t_par, len(self.param_ids))])
+        nd = self.n_qd
+        a, b = np.zeros((self.n_envs, nd, nd)), np.zeros((self.n_envs, nd, nd))
+        ta, tb = np.zeros((self.n_envs, nd, nd, m)), np.zeros((self.n_envs, nd, nd, m))
+        self._check(self._L.tds_b200_inverse_dynamics_derivatives_jvp_host(self._h, _dp(q), _dp(qd), _dp(qdd), m, *(_dp(t) for t in ts),
+                                                                           _dp(a), _dp(b), _dp(ta), _dp(tb)),
+                    "inverse_dynamics_derivatives_jvp_host")
+        return (a, b, ta[..., 0], tb[..., 0]) if single else (a, b, ta, tb)
+
+    def inverse_dynamics_derivatives_jvp_device(self, q, qd, qdd, m, t_q, t_qd, t_qdd, t_par, t_dtau_dq, t_dtau_dqd, dtau_dq=None,
+                                                dtau_dqd=None, stream=None):
+        """Device version of inverse_dynamics_derivatives_jvp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None);
+        t_q [n_q * m, n_stride], t_qd and t_qdd [n_qd * m, n_stride], t_par [k * m, n_stride] (each may be None, not all), t_dtau_dq and
+        t_dtau_dqd [n_qd * n_qd * m, n_stride] (either may be None, not both) and the values [n_qd * n_qd, n_stride] (or None) float64
+        CUDA tensors, entry (c, j) at row c * m + j.  Asynchronous."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_inverse_dynamics_derivatives_jvp_device(
+            self._h, _ptr(q), _ptr(qd), _ptr(qdd), int(m), _ptr(t_q), _ptr(t_qd), _ptr(t_qdd), _ptr(t_par), _ptr(dtau_dq), _ptr(dtau_dqd),
+            _ptr(t_dtau_dq), _ptr(t_dtau_dqd), st), "inverse_dynamics_derivatives_jvp_device")
+
+    def inverse_dynamics_derivatives_vjp_host(self, q, qd, qdd, G_dq=None, G_dqd=None):
+        """Cotangents G_dq, G_dqd [n, n_qd, n_qd] of (dtau_dq, dtau_dqd) (either may be None, not both) -> (g_q [n, n_q], g_qd [n, n_qd],
+        g_qdd [n, n_qd], g_par [n, k] or None without installed parameters)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, qdd = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(qdd, self.n_qd, "qdd")
+        nn = self.n_qd * self.n_qd
+        G_dq = None if G_dq is None else self._inv_in(np.reshape(G_dq, (self.n_envs, nn)), nn, "G_dq")
+        G_dqd = None if G_dqd is None else self._inv_in(np.reshape(G_dqd, (self.n_envs, nn)), nn, "G_dqd")
+        k = len(self.param_ids)
+        g_q, g_qd, g_qdd = np.zeros((self.n_envs, self.n_q)), np.zeros((self.n_envs, self.n_qd)), np.zeros((self.n_envs, self.n_qd))
+        g_par = np.zeros((self.n_envs, k)) if k else None
+        self._check(self._L.tds_b200_inverse_dynamics_derivatives_vjp_host(self._h, _dp(q), _dp(qd), _dp(qdd), _dp(G_dq), _dp(G_dqd), _dp(g_q),
+                                                                           _dp(g_qd), _dp(g_qdd), _dp(g_par)),
+                    "inverse_dynamics_derivatives_vjp_host")
+        return g_q, g_qd, g_qdd, g_par
+
+    def inverse_dynamics_derivatives_vjp_device(self, q, qd, qdd, G_dq, G_dqd, g_q, g_qd, g_qdd, g_par=None, stream=None):
+        """Device version of inverse_dynamics_derivatives_vjp_host: q float32 [n_q, n_stride], qd and qdd [n_qd, n_stride] (or None),
+        G_dq and G_dqd float64 [n_qd * n_qd, n_stride] (either may be None, not both), g_q [n_q, n_stride], g_qd and g_qdd [n_qd,
+        n_stride], g_par [k, n_stride] float64 CUDA tensors (each may be None, not all).  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_inverse_dynamics_derivatives_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(qdd), _ptr(G_dq), _ptr(G_dqd),
+                                                                             _ptr(g_q), _ptr(g_qd), _ptr(g_qdd), _ptr(g_par), st),
+                    "inverse_dynamics_derivatives_vjp_device")
+
     # ---- centre of mass, centroidal momentum matrix and its bias (DESIGN.md section 7.16) ----
     def centroidal_host(self, q, qd=None):
         """(m [n], c [n, 3], I_G [n, 3, 3], A [n, 6, n_qd], bias [n, 6]) float64 at the fp32-rounded q [n, n_q] and qd [n, n_qd] (None:
