@@ -568,6 +568,52 @@ int tds_b200_inverse_dynamics_derivatives_vjp_device(tds_b200_sim* sim, const fl
 int tds_b200_inverse_dynamics_derivatives_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* qdd, const double* G_dq,
                                                    const double* G_dqd, double* g_q, double* g_qd, double* g_qdd, double* g_par);
 
+/* ---- derivatives of the forward dynamics d qdd / dq, d qdd / dqd, d qdd / dtau (DESIGN.md section 7.24) ---------------------------
+ * The linearisation of the unconstrained forward dynamics qdd = M^-1 (tau - h) at the fp32-rounded q, qd and tau (qd or tau may be NULL:
+ * zero) and the installed parameters, in fp64 per environment:
+ *   qdd [n_qd]: tds_b200_constrained_dynamics_* with K = 0, bit for bit;
+ *   d qdd / dq [n_qd * n_qd]: -M^-1 d tau / dq, with d tau / dq of tds_b200_inverse_dynamics_derivatives_* taken at (q, qd, qdd) and qdd
+ *     read in fp64 (that entry point reads it in fp32);
+ *   d qdd / dqd [n_qd * n_qd]: -M^-1 d tau / dqd at the same point;
+ *   d qdd / dtau [n_qd * n_qd]: M^-1, tds_b200_mass_inverse_* bit for bit.
+ * Row-major as tds_b200_mass_matrix: row r is qdd_r, column c a tangent direction.  The columns are in M's coordinates: column k of
+ * d qdd / dq is the derivative along the motion with velocity e_k (see tds_b200_inverse_dynamics_derivatives_*), so d qdd / dq . d equals
+ * tds_b200_constrained_dynamics_jvp (K = 0) along t_q = dq_dt(q, d).  The stiffness and damping terms (the spherical joints' axis-angle
+ * stiffness included) enter as they enter tds_b200_inverse_dynamics_*.  A floating base's tau rows 0..5 are the applied wrench on the base
+ * in the base frame; as for K = 0 of tds_b200_constrained_dynamics_*, qdd is then not the MODE_FD step's qdd (the reference's
+ * floating-base forward dynamics does not invert its own M), and these are not that step's derivatives.  A world of several multibodies
+ * gives exact zeros between multibodies in all three matrices.  Each output may be NULL, not all four.
+ * Argument checks -> -1: NULL q; no output (no tangent output for _jvp, no cotangent for _vjp); m < 1 or every tangent NULL; no gradient
+ * output.  -> -4: t_par / g_par without an installed set.
+ *   device: q [n_q][n_stride], qd and tau [n_qd][n_stride] fp32; qdd [n_qd][n_stride], the matrices [n_qd * n_qd][n_stride] fp64.
+ *           Asynchronous on `stream`.
+ *   host:   q [n][n_q], qd and tau [n][n_qd] fp64 (rounded to fp32); qdd [n][n_qd], the matrices [n][n_qd * n_qd].  Synchronous.
+ * _jvp: the tangents of the four outputs along m tangents of q (n_q coordinates), qd, tau and the installed parameters (each may be NULL:
+ *   zero, not all), second-order terms included, in chunks of tangents; the values (each may be NULL) are written too.  Layouts as
+ *   tds_b200_constrained_dynamics_jvp: device t_q [n_q * m][n_stride], t_qd and t_tau [n_qd * m][n_stride], t_par [k * m][n_stride],
+ *   t_qdd [n_qd * m][n_stride], t_dqdd_* [n_qd * n_qd * m][n_stride] (entry (r, j) at (r * m + j) * n_stride + e); host [n][dim][m].
+ * _vjp: g_x[c] = <G_qdd, dqdd/dx_c> + <G_dq, d(dqdd_dq)/dx_c> + <G_dqd, d(dqdd_dqd)/dx_c> + <G_dtau, d(dqdd_dtau)/dx_c> for x = q, qd, tau
+ *   and, while a set is installed, the parameters: the JVP along the n_q + 2 n_qd (+ k) identity tangents contracted on the device.  Each
+ *   G may be NULL (zero), not all; any of g_q, g_qd, g_tau, g_par may be NULL, not all.  Layouts as tds_b200_constrained_dynamics_vjp. */
+int tds_b200_forward_dynamics_derivatives_device(tds_b200_sim* sim, const float* q, const float* qd, const float* tau, double* qdd,
+                                                 double* dqdd_dq, double* dqdd_dqd, double* dqdd_dtau, void* stream);
+int tds_b200_forward_dynamics_derivatives_host(tds_b200_sim* sim, const double* q, const double* qd, const double* tau, double* qdd,
+                                               double* dqdd_dq, double* dqdd_dqd, double* dqdd_dtau);
+int tds_b200_forward_dynamics_derivatives_jvp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* tau, int m,
+                                                     const double* t_q, const double* t_qd, const double* t_tau, const double* t_par,
+                                                     double* qdd, double* dqdd_dq, double* dqdd_dqd, double* dqdd_dtau, double* t_qdd,
+                                                     double* t_dqdd_dq, double* t_dqdd_dqd, double* t_dqdd_dtau, void* stream);
+int tds_b200_forward_dynamics_derivatives_jvp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* tau, int m,
+                                                   const double* t_q, const double* t_qd, const double* t_tau, const double* t_par,
+                                                   double* qdd, double* dqdd_dq, double* dqdd_dqd, double* dqdd_dtau, double* t_qdd,
+                                                   double* t_dqdd_dq, double* t_dqdd_dqd, double* t_dqdd_dtau);
+int tds_b200_forward_dynamics_derivatives_vjp_device(tds_b200_sim* sim, const float* q, const float* qd, const float* tau, const double* G_qdd,
+                                                     const double* G_dq, const double* G_dqd, const double* G_dtau, double* g_q, double* g_qd,
+                                                     double* g_tau, double* g_par, void* stream);
+int tds_b200_forward_dynamics_derivatives_vjp_host(tds_b200_sim* sim, const double* q, const double* qd, const double* tau, const double* G_qdd,
+                                                   const double* G_dq, const double* G_dqd, const double* G_dtau, double* g_q, double* g_qd,
+                                                   double* g_tau, double* g_par);
+
 /* ---- the step with its contacts (DESIGN.md section 7.15) -----------------------------------------------------------------
  * One step (MODE_FULL or MODE_WORLD) that also reports what the contact solve did: one record of 10 rows per contact candidate of the
  * model (n_points of tds_b200_get_dims, in the order of tds_b200_contact_pairs and contact_dist), row r of candidate k at row 10 k + r,

@@ -206,6 +206,18 @@ def lib():
     L.tds_b200_inverse_dynamics_derivatives_vjp_device.argtypes = [vp, fp, fp, fp, vp, vp, vp, vp, vp, vp, vp]
     L.tds_b200_inverse_dynamics_derivatives_vjp_host.restype = ci
     L.tds_b200_inverse_dynamics_derivatives_vjp_host.argtypes = [vp, dp, dp, dp, dp, dp, dp, dp, dp, dp]
+    L.tds_b200_forward_dynamics_derivatives_device.restype = ci
+    L.tds_b200_forward_dynamics_derivatives_device.argtypes = [vp, fp, fp, fp, vp, vp, vp, vp, vp]
+    L.tds_b200_forward_dynamics_derivatives_host.restype = ci
+    L.tds_b200_forward_dynamics_derivatives_host.argtypes = [vp, dp, dp, dp, dp, dp, dp, dp]
+    L.tds_b200_forward_dynamics_derivatives_jvp_device.restype = ci
+    L.tds_b200_forward_dynamics_derivatives_jvp_device.argtypes = [vp, fp, fp, fp, ci] + [vp] * 13
+    L.tds_b200_forward_dynamics_derivatives_jvp_host.restype = ci
+    L.tds_b200_forward_dynamics_derivatives_jvp_host.argtypes = [vp, dp, dp, dp, ci] + [dp] * 12
+    L.tds_b200_forward_dynamics_derivatives_vjp_device.restype = ci
+    L.tds_b200_forward_dynamics_derivatives_vjp_device.argtypes = [vp, fp, fp, fp] + [vp] * 9
+    L.tds_b200_forward_dynamics_derivatives_vjp_host.restype = ci
+    L.tds_b200_forward_dynamics_derivatives_vjp_host.argtypes = [vp, dp, dp, dp] + [dp] * 8
     L.tds_b200_coriolis_device.restype = ci
     L.tds_b200_coriolis_device.argtypes = [vp, fp, fp, vp, vp]
     L.tds_b200_coriolis_host.restype = ci
@@ -369,6 +381,9 @@ DECLARED_SYMBOLS = [
     "tds_b200_inverse_dynamics_derivatives_device", "tds_b200_inverse_dynamics_derivatives_host",
     "tds_b200_inverse_dynamics_derivatives_jvp_device", "tds_b200_inverse_dynamics_derivatives_jvp_host",
     "tds_b200_inverse_dynamics_derivatives_vjp_device", "tds_b200_inverse_dynamics_derivatives_vjp_host",
+    "tds_b200_forward_dynamics_derivatives_device", "tds_b200_forward_dynamics_derivatives_host",
+    "tds_b200_forward_dynamics_derivatives_jvp_device", "tds_b200_forward_dynamics_derivatives_jvp_host",
+    "tds_b200_forward_dynamics_derivatives_vjp_device", "tds_b200_forward_dynamics_derivatives_vjp_host",
     "tds_b200_constrained_dynamics_device", "tds_b200_constrained_dynamics_host", "tds_b200_constrained_dynamics_jvp_device",
     "tds_b200_constrained_dynamics_jvp_host", "tds_b200_constrained_dynamics_vjp_device", "tds_b200_constrained_dynamics_vjp_host",
     "tds_b200_step_contacts_device", "tds_b200_step_contacts_host", "tds_b200_step_contacts_jvp_device", "tds_b200_step_contacts_jvp_host",

@@ -70,6 +70,11 @@ backward rule (BatchSim.coriolis_vjp_device: float32 q.grad, qd.grad, float64 pa
 inverse_dynamics_derivatives(sim, q, qd=None, qdd=None, params=None) is (d tau / dq, d tau / dqd) [n_envs, n_qd, n_qd] of the inverse
 dynamics (float64, DESIGN.md section 7.23) with a backward rule (BatchSim.inverse_dynamics_derivatives_vjp_device: float32 q.grad, qd.grad,
 qdd.grad, float64 params.grad) and a forward-mode rule (BatchSim.inverse_dynamics_derivatives_jvp_device).
+
+forward_dynamics_derivatives(sim, q, qd=None, tau=None, params=None) is (qdd [n_envs, n_qd], d qdd / dq, d qdd / dqd, d qdd / dtau
+[n_envs, n_qd, n_qd]) of the forward dynamics (float64, DESIGN.md section 7.24) with a backward rule
+(BatchSim.forward_dynamics_derivatives_vjp_device: float32 q.grad, qd.grad, tau.grad, float64 params.grad) and a forward-mode rule
+(BatchSim.forward_dynamics_derivatives_jvp_device).
 """
 from collections import namedtuple
 
@@ -348,7 +353,7 @@ def _state_soa(sim, q, qd, qdd):
 
 class _Query(torch.autograd.Function):
     """The dynamics queries (mass_matrix, inverse_dynamics, centroidal, forward_kinematics, point_motion, regressor, mass_inverse,
-    constrained_dynamics, coriolis, inverse_dynamics_derivatives) as one Function over a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
+    constrained_dynamics, coriolis, inverse_dynamics_derivatives, forward_dynamics_derivatives) as one Function over a _QuerySpec: the inputs in the SoA layout (float32 state, float64 tangents, environments padded with zeros to n_stride), zeroed
     float64 output buffers, every C-ABI call ordered on a side stream, and the gradients as float32 (q, qd, qdd) and float64 (params).
     An input the query does not take, or the call leaves out, is None and gets no gradient; a tangent on it is ignored.  With params
     the forward installs their values, and the backward and forward-mode rule reinstall the values of this call (a later call of the
@@ -866,3 +871,33 @@ def inverse_dynamics_derivatives(sim, q, qd=None, qdd=None, params=None):
     _check_state(sim, q, qd, qdd)
     _check_params(sim, params)
     return _Query.apply(_INVERSE_DYNAMICS_DERIVATIVES, sim, None, q, qd, qdd, params)
+
+
+def _square(sim, x):
+    return x.reshape(sim.n_envs, sim.n_qd, sim.n_qd).contiguous()
+
+
+_FORWARD_DYNAMICS_DERIVATIVES = _QuerySpec(
+    rows=lambda sim, p: [sim.n_qd] + [sim.n_qd * sim.n_qd] * 3,
+    unpack=lambda sim, p, qdd, a, b, c: (qdd.contiguous(), _square(sim, a), _square(sim, b), _square(sim, c)),
+    pack=lambda sim, p, *G: [_cot(g, sim) for g in G],
+    value=lambda sim, p, x, out, st: sim.forward_dynamics_derivatives_device(x.q, x.qd, x.qdd, *out, stream=st),
+    jvp=lambda sim, p, x, t, out, st: sim.forward_dynamics_derivatives_jvp_device(x.q, x.qd, x.qdd, 1, *t, *out, stream=st),
+    vjp=lambda sim, p, x, G, g, st: sim.forward_dynamics_derivatives_vjp_device(x.q, x.qd, x.qdd, *G, *g, stream=st))
+
+
+def forward_dynamics_derivatives(sim, q, qd=None, tau=None, params=None):
+    """The forward dynamics qdd = M^-1 (tau - h) and its derivatives (d qdd / dq, d qdd / dqd, d qdd / dtau) for every environment of
+    `sim` (a BatchSim), DESIGN.md section 7.24: qdd [n_envs, n_qd] and three [n_envs, n_qd, n_qd] float64 tensors, row r = qdd_r, in fp64
+    at the fp32-rounded q [n_envs, n_q], qd and tau [n_envs, n_qd] float32 CUDA tensors (qd or tau None: zero).  qdd is
+    constrained_dynamics(sim, q, qd, tau)'s, d qdd / dtau is mass_inverse(sim, q)'s M^-1, and d qdd / dq = -M^-1 d tau / dq, d qdd / dqd =
+    -M^-1 d tau / dqd with the inverse dynamics' derivatives at that qdd in fp64.  The columns are in the coordinates of mass_matrix: column
+    k of d qdd / dq is the derivative along the motion with velocity e_k (include/tds_b200.h).  A floating base's tau rows 0..5 are the
+    base wrench in the base frame (this qdd is not the MODE_FD step's there).  params: None, or a float64 CUDA tensor [n_envs, k] of values
+    for the parameters installed by sim.set_physical_params (then also differentiated).  Differentiable in reverse mode (float32 q.grad,
+    qd.grad, tau.grad, float64 params.grad: second-order terms) and forward mode."""
+    _check_state(sim, q, qd)
+    if tau is not None and (tau.dtype != torch.float32 or not tau.is_cuda or tuple(tau.shape) != (sim.n_envs, sim.n_qd)):
+        raise ValueError("tau: a float32 CUDA tensor [n_envs, n_qd] is expected")
+    _check_params(sim, params)
+    return _Query.apply(_FORWARD_DYNAMICS_DERIVATIVES, sim, None, q, qd, tau, params)

@@ -110,6 +110,8 @@ extern "C" int tds_launch_coriolis_jvp(const DevModel* M, const StepIO* io, cons
                                        int n_dirs, char* gscratch, cudaStream_t stream);
 // the rows and the solve of the point-constrained forward dynamics (tds_constrained.cu)
 extern "C" int tds_launch_cdyn(const TdsCdynCall* c, int dual, int n, int ns, cudaStream_t stream);
+// the product -M^-1 [d tau / dq | d tau / dqd] of the forward dynamics' derivatives (tds_fd_derivatives.cu)
+extern "C" int tds_launch_fdd(const TdsFddCall* c, int dual, int n, int ns, cudaStream_t stream);
 static_assert(TDS_B200_MAX_KIN_POINTS == TDS_MAX_KIN_POINTS, "the point table of the kernel argument holds the C-ABI's maximum");
 
 // candidate contact points of a model, reference enumeration order: (link_a, link_b) per point
@@ -463,6 +465,7 @@ struct tds_b200_sim {
   double* mass_dev = nullptr; size_t mass_dev_bytes = 0; // dynamics queries' VJPs: identity tangents | output columns of a chunk
   double* minv_dev = nullptr; size_t minv_dev_bytes = 0; // the inverse mass matrix's intermediates: M^-1, J and their tangents
   double* cdyn_dev = nullptr; size_t cdyn_dev_bytes = 0; // the constrained dynamics' intermediates: h, M^-1, J, drift, solve, tangents
+                                                         // (and those of the forward dynamics' derivatives)
   // installed physical parameters (tds_b200_set_physical_params_*): slot map (par.n == 0: none) and values [k][ns] fp64
   ParMap par;
   double* par_dev = nullptr; size_t par_dev_bytes = 0;
@@ -943,11 +946,11 @@ enum class Query { step, mass, kin, inv, contacts, centroidal, motion, wrench, r
 // motion: t_in = the q | qd | qdd tangents (qd and qdd as for inv), the point table and outputs `mot`; wrench: as step, with the point
 // table, wrenches and wrench tangents `ext`; regressor: t_in = the q | qd | qdd tangents (as for inv), Y in jac and the
 // energy outputs `reg`; minv: as mass, M^-1 in jac; cor: t_in = the q | qd tangents (qd in the step's qd), C in jac; der: t_in as for
-// inv, d tau / dq in jac and d tau / dqd in der_dqd (either may be NULL)
+// inv, d tau / dq in jac and d tau / dqd in der_dqd (either may be NULL), qdd from the fp64 der_qdd [n_qd][ns] when not NULL
 struct JvpTangents {
   const double* t_in; const double* t_par; int m; Query query = Query::step; const TdsKinCall* kin = nullptr;
   const TdsCenCall* cen = nullptr; const TdsMotCall* mot = nullptr; const TdsExtCall* ext = nullptr;
-  const TdsRegCall* reg = nullptr; double* der_dqd = nullptr;
+  const TdsRegCall* reg = nullptr; double* der_dqd = nullptr; const double* der_qdd = nullptr;
 };
 
 // the installed physical parameters as a launch argument in *pmv, or NULL without any
@@ -1006,7 +1009,7 @@ static int jacobian_run(tds_b200_sim* s, int mode, int use_pd, const float* q, c
   const size_t arena = (jv && jv->query == Query::wrench) ? wrench_arena_bytes(s, s->dm_ad, 16)
                        : (jv && jv->query == Query::der)  ? der_arena_bytes(s, s->dm_ad, 16)
                                                           : lane_arena_bytes(s, s->dm_ad);
-  if (jv && jv->query == Query::der) io.g_in = jv->der_dqd;
+  if (jv && jv->query == Query::der) { io.g_in = jv->der_dqd; io.g_out = jv->der_qdd; }
   const int chunk = std::min(dir_chunk_of(s, arena), n_dirs);
   CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, arena * chunk));
   const cudaStream_t sm = (cudaStream_t)stream;
@@ -1709,23 +1712,27 @@ int tds_b200_centroidal_vjp_host(tds_b200_sim* s, const double* q, const double*
 
 // ---- derivatives of the inverse dynamics d tau / dq, d tau / dqd (DESIGN.md section 7.23): the DER instances of the world-frame kernel
 // (tds_dynamics_derivatives.cu).  The inputs q | qd | qdd are those of the inverse dynamics (inv_n_in, put_inv_inputs). ----------------
-// d tau / dq and d tau / dqd [n_qd * n_qd][ns] (either may be NULL) from q [n_q][ns], qd and qdd [n_qd][ns] fp32 (either NULL: zero)
-static int der_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* dq, double* dqd, cudaStream_t sm) {
+// d tau / dq and d tau / dqd [n_qd * n_qd][ns] (either may be NULL) from q [n_q][ns], qd and qdd [n_qd][ns] fp32 (either NULL: zero), or
+// at the fp64 qdd64 [n_qd][ns] in place of qdd when that is not NULL (the forward dynamics' derivatives)
+static int der_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, double* dq, double* dqd, cudaStream_t sm,
+                   const double* qdd64 = nullptr) {
   CUDA_TRY(grow_dev(&s->jac_scratch, &s->jac_scratch_bytes, der_arena_bytes(s, s->dm_m, 8)));
   return value_run(s, "inverse dynamics derivatives", q, qd, qdd, dq, [&](const StepIO* io, const ParMap* pm) {
     StepIO d = *io;
     d.g_in = dqd;
+    d.g_out = qdd64;
     return tds_launch_dynamics_derivatives(&s->dm_m, &s->P, &d, pm, s->jac_scratch, sm);
   });
 }
 
 // t_dq, t_dqd [n_qd * n_qd * m][ns] (either may be NULL) along t_in [(n_q + 2 n_qd) * m][ns] (q | qd | qdd tangents, contiguous) and
-// t_par (either may be NULL); dq, dqd, if not NULL, receive the values
+// t_par (either may be NULL); dq, dqd, if not NULL, receive the values.  qdd64: as for der_run.
 static int der_jvp_run(tds_b200_sim* s, const float* q, const float* qd, const float* qdd, int m, const double* t_in, const double* t_par,
-                       double* dq, double* dqd, double* t_dq, double* t_dqd, cudaStream_t sm) {
-  if (dq || dqd) { if (int rc = der_run(s, q, qd, qdd, dq, dqd, sm)) return rc; }
+                       double* dq, double* dqd, double* t_dq, double* t_dqd, cudaStream_t sm, const double* qdd64 = nullptr) {
+  if (dq || dqd) { if (int rc = der_run(s, q, qd, qdd, dq, dqd, sm, qdd64)) return rc; }
   JvpTangents jv{t_in, t_par, m, Query::der};
   jv.der_dqd = t_dqd;
+  jv.der_qdd = qdd64;
   return jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, qdd, t_dq, sm, false, &jv);
 }
 
@@ -2443,6 +2450,52 @@ static int cdyn_launch(tds_b200_sim* s, const TdsCdynCall& c, bool dual, cudaStr
   return rc;
 }
 
+// h = ID(q, qd, 0) [n_qd][ns] and M^-1 [n_qd^2][ns] from q [n_q][ns] and qd [n_qd][ns] fp32 (NULL: zero) by the INV and MINV value
+// launches: what the constrained dynamics and the forward dynamics' derivatives start from (`what` names the call in errors)
+static int h_minv_run(tds_b200_sim* s, const char* what, const float* q, const float* qd, double* h, double* Mi, cudaStream_t sm) {
+  if (int rc = inv_run(s, q, qd, nullptr, h, sm)) return rc;
+  return value_run(s, what, q, nullptr, nullptr, Mi, [&](const StepIO* io, const ParMap* pm) {
+    return tds_launch_mass_inverse(&s->dm_m, io, pm, s->jac_scratch, sm);
+  });
+}
+
+// The tangents of directions [j0, j0 + mc) of m that the constrained dynamics and the forward dynamics' derivatives share, laid out from
+// w: T = the q | qd | 0 tangents [(n_q + 2 n_qd) * mc][ns] of the INV (and MOT) JVPs, Tp = t_par [k * mc], Tt = t_tau [n_qd * mc], and
+// dh [n_qd * mc] and dM^-1 [n_qd^2 * mc] by the INV and MINV JVPs where the tangents given reach them (d_h, d_Mi).  `end` is where the
+// caller's own tangents of the chunk begin; chunk_tangent_words(s) words per direction come before it.
+struct ChunkTangents { double *T, *Tp, *Tt, *dh, *dMi, *end; bool d_h, d_Mi; };
+static size_t chunk_tangent_words(const tds_b200_sim* s) {
+  const size_t nd = s->dm[0].n_qd;
+  return (size_t)inv_n_in(s) + s->par.n + 2 * nd + nd * nd;
+}
+static int chunk_tangents(tds_b200_sim* s, const float* q, const float* qd, int m, int j0, int mc, const double* t_q, const double* t_qd,
+                          const double* t_tau, const double* t_par, double* w, ChunkTangents* c, cudaStream_t sm) {
+  const int nd = s->dm[0].n_qd, n_q = s->dm[0].n_q, k = s->par.n;
+  const size_t ns = s->ns, nn = (size_t)nd * nd, n_in = (size_t)inv_n_in(s);
+  c->T = w;
+  c->Tp = c->T + n_in * mc * ns;
+  c->Tt = c->Tp + (size_t)k * mc * ns;
+  c->dh = c->Tt + (size_t)nd * mc * ns;
+  c->dMi = c->dh + (size_t)nd * mc * ns;
+  c->end = c->dMi + nn * mc * ns;
+  c->d_h = t_q || t_qd || t_par;
+  c->d_Mi = t_q || t_par;
+  CUDA_TRY(tangent_slice(c->T, t_q, n_q, m, j0, mc, ns, sm));
+  CUDA_TRY(tangent_slice(c->T + (size_t)n_q * mc * ns, t_qd, nd, m, j0, mc, ns, sm));
+  CUDA_TRY(tangent_slice(c->T + (size_t)(n_q + nd) * mc * ns, nullptr, nd, m, j0, mc, ns, sm));
+  if (t_par) CUDA_TRY(tangent_slice(c->Tp, t_par, k, m, j0, mc, ns, sm));
+  if (t_tau) CUDA_TRY(tangent_slice(c->Tt, t_tau, nd, m, j0, mc, ns, sm));
+  if (c->d_h) {
+    const JvpTangents jv{c->T, t_par ? c->Tp : nullptr, mc, Query::inv};
+    if (int rc = jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, nullptr, c->dh, sm, false, &jv)) return rc;
+  }
+  if (c->d_Mi) {   // (the qd tangents do not enter M^-1)
+    const JvpTangents jv{t_q ? c->T : nullptr, t_par ? c->Tp : nullptr, mc, Query::minv};
+    if (int rc = jacobian_run(s, TDS_B200_MODE_FULL, 0, q, nullptr, nullptr, c->dMi, sm, false, &jv)) return rc;
+  }
+  return 0;
+}
+
 // qdd [n_qd][ns] and f [R][ns] (R = dims K; either may be NULL) from q [n_q][ns], qd and tau [n_qd][ns] fp32 (either NULL: zero) and,
 // with m >= 1 tangents t_q [n_q * m][ns], t_qd and t_tau [n_qd * m][ns], t_par [k * m][ns] (each may be NULL: zero), their tangents
 // t_qdd [n_qd * m][ns] and t_f [R * m][ns] (either may be NULL).  Everything else goes to s->cdyn_dev: the values of h, M^-1, J, the
@@ -2451,12 +2504,12 @@ static int cdyn_run(tds_b200_sim* s, const float* q, const float* qd, const floa
                     const double* t_q, const double* t_qd, const double* t_tau, const double* t_par, double* t_qdd, double* t_f,
                     cudaStream_t sm) {
   const DevModel& D = s->dm[0];
-  const int K = cc.K, nd = D.n_qd, n_q = D.n_q, k = s->par.n;
+  const int K = cc.K, nd = D.n_qd;
   const size_t ns = s->ns, nn = (size_t)nd * nd, nJ = (size_t)6 * K * nd, nA = (size_t)6 * K, R = (size_t)cc.dims * K;
-  const size_t n_in = (size_t)inv_n_in(s), scr = R * nd + R * R + R;
+  const size_t scr = R * nd + R * R + R;
   const bool tan = m > 0 && (t_qdd || t_f);
-  // per tangent of a chunk: q | qd | 0 tangents, t_par, t_tau, dh, dM^-1, dJ, d drift, and the (value, tangent) pairs of the scratch
-  const size_t per = n_in + k + 2 * (size_t)nd + nn + nJ + nA + 2 * scr;
+  // per tangent of a chunk: the shared tangents (chunk_tangents), dJ, d drift, and the (value, tangent) pairs of the scratch
+  const size_t per = chunk_tangent_words(s) + nJ + nA + 2 * scr;
   const size_t fit = std::max<size_t>(1, ((size_t)1 << 30) / (sizeof(double) * per * ns));
   const int chunk = tan ? (int)std::min<size_t>(std::min<size_t>((size_t)m, 65535), fit) : 0;   // (gridDim.y, gridDim.z)
   CUDA_TRY(grow_dev(&s->cdyn_dev, &s->cdyn_dev_bytes, sizeof(double) * (nd + nn + nJ + nA + scr + per * chunk + 1) * ns));
@@ -2466,11 +2519,7 @@ static int cdyn_run(tds_b200_sim* s, const float* q, const float* qd, const floa
   double* const acc = J + nJ * ns;
   double* const Y = acc + nA * ns;
   double* const w = Y + scr * ns;
-  if (int rc = inv_run(s, q, qd, nullptr, h, sm)) return rc;
-  int rc = value_run(s, "constrained dynamics", q, nullptr, nullptr, Mi, [&](const StepIO* io, const ParMap* pm) {
-    return tds_launch_mass_inverse(&s->dm_m, io, pm, s->jac_scratch, sm);
-  });
-  if (rc) return rc;
+  if (int rc = h_minv_run(s, "constrained dynamics", q, qd, h, Mi, sm)) return rc;
   if (K > 0) {
     const TdsMotCall mc{K, cc.links, cc.local, J, nullptr, acc};
     if (int rc = mot_run(s, q, qd, nullptr, &mc, sm)) return rc;
@@ -2485,37 +2534,21 @@ static int cdyn_run(tds_b200_sim* s, const float* q, const float* qd, const floa
     if (int rc = cdyn_launch(s, c, false, sm)) return rc;
   }
   if (!tan) return 0;
-  const bool d_h = t_q || t_qd || t_par, d_Mi = t_q || t_par, d_J = K > 0 && (t_q || t_qd);
+  const bool d_J = K > 0 && (t_q || t_qd);
   for (int j0 = 0; j0 < m; j0 += chunk) {
     const int mc = std::min(chunk, m - j0);
-    double* const T = w;   // q | qd | qdd tangents of the INV and MOT JVPs, the qdd ones zero
-    double* const Tp = T + n_in * mc * ns;
-    double* const Tt = Tp + (size_t)k * mc * ns;
-    double* const dh = Tt + (size_t)nd * mc * ns;
-    double* const dMi = dh + (size_t)nd * mc * ns;
-    double* const dJ = dMi + nn * mc * ns;
+    ChunkTangents ct;
+    if (int rc = chunk_tangents(s, q, qd, m, j0, mc, t_q, t_qd, t_tau, t_par, w, &ct, sm)) return rc;
+    double* const dJ = ct.end;
     double* const dacc = dJ + nJ * mc * ns;
     double* const P = dacc + nA * mc * ns;   // Y | dY | A | dA | b | db
-    CUDA_TRY(tangent_slice(T, t_q, n_q, m, j0, mc, ns, sm));
-    CUDA_TRY(tangent_slice(T + (size_t)n_q * mc * ns, t_qd, nd, m, j0, mc, ns, sm));
-    CUDA_TRY(tangent_slice(T + (size_t)(n_q + nd) * mc * ns, nullptr, nd, m, j0, mc, ns, sm));
-    if (t_par) CUDA_TRY(tangent_slice(Tp, t_par, k, m, j0, mc, ns, sm));
-    if (t_tau) CUDA_TRY(tangent_slice(Tt, t_tau, nd, m, j0, mc, ns, sm));
-    if (d_h) {
-      const JvpTangents jv{T, t_par ? Tp : nullptr, mc, Query::inv};
-      if (int rc = jacobian_run(s, TDS_B200_MODE_FULL, 0, q, qd, nullptr, dh, sm, false, &jv)) return rc;
-    }
-    if (d_Mi) {   // (the qd tangents do not enter M^-1)
-      const JvpTangents jv{t_q ? T : nullptr, t_par ? Tp : nullptr, mc, Query::minv};
-      if (int rc = jacobian_run(s, TDS_B200_MODE_FULL, 0, q, nullptr, nullptr, dMi, sm, false, &jv)) return rc;
-    }
     if (d_J) {
       const TdsMotCall dmc{K, cc.links, cc.local, dJ, nullptr, dacc};
-      if (int rc = mot_jvp_run(s, q, qd, nullptr, &dmc, mc, T, sm)) return rc;
+      if (int rc = mot_jvp_run(s, q, qd, nullptr, &dmc, mc, ct.T, sm)) return rc;
     }
     TdsCdynCall dc = c;
     dc.m = mc; dc.j0 = j0; dc.m_out = m;
-    dc.dtau = t_tau ? Tt : nullptr; dc.dh = d_h ? dh : nullptr; dc.dMi = d_Mi ? dMi : nullptr;
+    dc.dtau = t_tau ? ct.Tt : nullptr; dc.dh = ct.d_h ? ct.dh : nullptr; dc.dMi = ct.d_Mi ? ct.dMi : nullptr;
     dc.dJ = d_J ? dJ : nullptr; dc.dacc = d_J ? dacc : nullptr;
     dc.Y = P; dc.dY = dc.Y + R * nd * mc * ns; dc.A = dc.dY + R * nd * mc * ns; dc.dA = dc.A + R * R * mc * ns;
     dc.b = dc.dA + R * R * mc * ns; dc.db = dc.b + R * mc * ns;
@@ -2653,6 +2686,212 @@ int tds_b200_constrained_dynamics_vjp_host(tds_b200_sim* s, const double* q, con
   double* g_d = s->vjp_g + (nd + R) * ns;
   CUDA_TRY(put_parts<double>(s->vjp_g, {{G_qdd, nd}, {G_f, R}}, n, ns, s->stream));
   if (int rc = cdyn_vjp_run(s, s->q, qd_d, tau_d, cc, s->vjp_g, g_d, g_par ? g_d + n_in * ns : nullptr, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_tau, nd}, {g_par, g_par ? k : 0}}, g_d, n, ns, s->stream));
+  return 0;
+}
+
+// ---- derivatives of the forward dynamics d qdd / dq, d qdd / dqd, d qdd / dtau (DESIGN.md section 7.24): h and M^-1 from the INV and
+// MINV instances and qdd from the constrained dynamics' solve at K = 0 (the launches of cdyn_run), d tau / dq and d tau / dqd from the DER
+// instances at that fp64 qdd (der_run, der_jvp_run), then the product kernel of tds_fd_derivatives.cu.  The inputs q | qd | tau are those
+// of the constrained dynamics (inv_n_in, put_inv_inputs).
+// The four outputs qdd [n_qd][ns], d qdd / dq, d qdd / dqd and d qdd / dtau [n_qd * n_qd][ns] (each may be NULL), or their tangents
+// [rows * m][ns]
+struct FddOut { double* qdd; double* dq; double* dqd; double* dtau; };
+
+static int fdd_launch(tds_b200_sim* s, const TdsFddCall& c, bool dual, cudaStream_t sm) {
+  const int rc = tds_launch_fdd(&c, dual ? 1 : 0, s->n, s->ns, sm);
+  if (rc) set_err(std::string("forward dynamics derivatives launch: ") + cudaGetErrorString((cudaError_t)rc));
+  return rc;
+}
+
+// The outputs o from q [n_q][ns], qd and tau [n_qd][ns] fp32 (either NULL: zero) and, with m >= 1 tangents t_q [n_q * m][ns], t_qd and
+// t_tau [n_qd * m][ns], t_par [k * m][ns] (each may be NULL: zero), their tangents t.  Everything else goes to s->cdyn_dev: the values of
+// h, M^-1 (unless o.dtau takes it), qdd (unless o.qdd takes it), d tau / dq and d tau / dqd, then the tangents of one chunk of directions
+// (within 1 GB) after another.  dM^-1 of a chunk serves both the solve and the product.
+static int fdd_run(tds_b200_sim* s, const float* q, const float* qd, const float* tau, const FddOut& o, int m, const double* t_q,
+                   const double* t_qd, const double* t_tau, const double* t_par, const FddOut& t, cudaStream_t sm) {
+  const DevModel& D = s->dm[0];
+  const int nd = D.n_qd, n_q = D.n_q;
+  const size_t ns = s->ns, nn = (size_t)nd * nd;
+  const bool tan = m > 0 && (t.qdd || t.dq || t.dqd || t.dtau), tan_A = tan && (t.dq || t.dqd);
+  const bool want_A = o.dq || o.dqd || tan_A;
+  // per tangent of a chunk: the shared tangents (chunk_tangents), d(d tau / dq), d(d tau / dqd)
+  const size_t per = chunk_tangent_words(s) + 2 * nn;
+  const size_t fit = std::max<size_t>(1, ((size_t)1 << 30) / (sizeof(double) * per * ns));
+  const int chunk = tan ? (int)std::min<size_t>(std::min<size_t>((size_t)m, 65535), fit) : 0;   // (gridDim.z)
+  CUDA_TRY(grow_dev(&s->cdyn_dev, &s->cdyn_dev_bytes, sizeof(double) * (3 * (size_t)nd + 3 * nn + per * chunk + 1) * ns));
+  double* const h = s->cdyn_dev;
+  double* const Mi = o.dtau ? o.dtau : h + nd * ns;
+  double* const qdd = o.qdd ? o.qdd : h + (nd + nn) * ns;
+  double* const Aq = h + (2 * nd + nn) * ns;
+  double* const Aqd = Aq + nn * ns;
+  double* const w = Aqd + nn * ns;
+  if (int rc = h_minv_run(s, "forward dynamics derivatives", q, qd, h, Mi, sm)) return rc;
+  TdsCdynCall c;   // the constrained dynamics' solve without points: qdd = M^-1 (tau - h)
+  memset(&c, 0, sizeof(c));
+  c.dims = 3; c.n_qd = nd; c.m = 1; c.m_out = 1;
+  c.tau = tau; c.h = h; c.Mi = Mi; c.qdd = qdd;
+  if (int rc = cdyn_launch(s, c, false, sm)) return rc;
+  if (want_A) { if (int rc = der_run(s, q, qd, nullptr, Aq, Aqd, sm, qdd)) return rc; }
+  TdsFddCall pc;
+  memset(&pc, 0, sizeof(pc));
+  pc.n_qd = nd; pc.m = 1; pc.m_out = 1; pc.Mi = Mi; pc.Aq = Aq; pc.Aqd = Aqd;
+  if (o.dq || o.dqd) {
+    pc.dq = o.dq; pc.dqd = o.dqd;
+    if (int rc = fdd_launch(s, pc, false, sm)) return rc;
+  }
+  if (!tan) return 0;
+  for (int j0 = 0; j0 < m; j0 += chunk) {
+    const int mc = std::min(chunk, m - j0);
+    ChunkTangents ct;
+    if (int rc = chunk_tangents(s, q, qd, m, j0, mc, t_q, t_qd, t_tau, t_par, w, &ct, sm)) return rc;
+    double* const Tqdd = ct.T + (size_t)(n_q + nd) * mc * ns;   // the qdd tangents: zero for the INV JVP, then the solve's dqdd
+    double* const dAq = ct.end;
+    double* const dAqd = dAq + nn * mc * ns;
+    TdsCdynCall dc = c;   // dqdd into the qdd tangents of the DER JVP
+    dc.m = mc; dc.j0 = 0; dc.m_out = mc;
+    dc.dtau = t_tau ? ct.Tt : nullptr; dc.dh = ct.d_h ? ct.dh : nullptr; dc.dMi = ct.d_Mi ? ct.dMi : nullptr;
+    dc.qdd = Tqdd;
+    if (int rc = cdyn_launch(s, dc, true, sm)) return rc;
+    if (t.qdd)
+      CUDA_TRY(cudaMemcpy2DAsync(t.qdd + (size_t)j0 * ns, sizeof(double) * m * ns, Tqdd, sizeof(double) * mc * ns, sizeof(double) * mc * ns,
+                                 nd, cudaMemcpyDeviceToDevice, sm));
+    if (tan_A) {
+      if (int rc = der_jvp_run(s, q, qd, nullptr, mc, ct.T, t_par ? ct.Tp : nullptr, nullptr, nullptr, t.dq ? dAq : nullptr,
+                               t.dqd ? dAqd : nullptr, sm, qdd))
+        return rc;
+    }
+    if (!tan_A && !t.dtau) continue;
+    TdsFddCall dp = pc;
+    dp.m = mc; dp.j0 = j0; dp.m_out = m;
+    dp.dMi = ct.d_Mi ? ct.dMi : nullptr; dp.dAq = dAq; dp.dAqd = dAqd;
+    dp.dq = t.dq; dp.dqd = t.dqd; dp.dtau = t.dtau;
+    if (int rc = fdd_launch(s, dp, true, sm)) return rc;
+  }
+  return 0;
+}
+
+// g_in [n_q + 2 n_qd][ns] (q | qd | tau, contiguous) and g_par [k][ns] (NULL: not wanted) = <G, d(qdd | d qdd / dq | d qdd / dqd |
+// d qdd / dtau)>, G [n_qd + 3 n_qd^2][ns]
+static int fdd_vjp_run(tds_b200_sim* s, const float* q, const float* qd, const float* tau, const double* G, double* g_in, double* g_par,
+                       cudaStream_t sm) {
+  const size_t ns = s->ns, n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd;
+  return vjp_by_eye(s, "forward dynamics derivatives", inv_n_in(s), nd + 3 * nn, G, g_in, g_par, sm,
+                    [&](int m, const double* t_in, const double* t_par, double* dO) {
+                      const size_t r = (size_t)m * ns;
+                      const FddOut t{dO, dO + nd * r, dO + (nd + nn) * r, dO + (nd + 2 * nn) * r};
+                      return fdd_run(s, q, qd, tau, FddOut{}, m, t_in, t_in + n_q * r, t_in + (n_q + nd) * r, t_par, t, sm);
+                    });
+}
+
+static bool fdd_any(const void* a, const void* b, const void* c, const void* d) { return a || b || c || d; }
+
+int tds_b200_forward_dynamics_derivatives_device(tds_b200_sim* s, const float* q, const float* qd, const float* tau, double* qdd,
+                                                 double* dqdd_dq, double* dqdd_dqd, double* dqdd_dtau, void* stream) {
+  if (!s || !q || !fdd_any(qdd, dqdd_dq, dqdd_dqd, dqdd_dtau)) return -1;
+  return fdd_run(s, q, qd, tau, FddOut{qdd, dqdd_dq, dqdd_dqd, dqdd_dtau}, 0, nullptr, nullptr, nullptr, nullptr, FddOut{},
+                 (cudaStream_t)stream);
+}
+
+int tds_b200_forward_dynamics_derivatives_host(tds_b200_sim* s, const double* q, const double* qd, const double* tau, double* qdd,
+                                               double* dqdd_dq, double* dqdd_dqd, double* dqdd_dtau) {
+  if (!s || !q || !fdd_any(qdd, dqdd_dq, dqdd_dqd, dqdd_dtau)) return -1;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t nd = s->dm[0].n_qd, nn = nd * nd;
+  const float *qd_d, *tau_d;
+  if (int rc = put_inv_inputs(s, q, qd, tau, &qd_d, &tau_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (nd + 3 * nn + 1) * ns));
+  double* d = s->jac_dev;
+  const FddOut o{qdd ? d : nullptr, dqdd_dq ? d + nd * ns : nullptr, dqdd_dqd ? d + (nd + nn) * ns : nullptr,
+                 dqdd_dtau ? d + (nd + 2 * nn) * ns : nullptr};
+  if (int rc = fdd_run(s, s->q, qd_d, tau_d, o, 0, nullptr, nullptr, nullptr, nullptr, FddOut{}, s->stream)) return rc;
+  CUDA_TRY(get_parts<double>({{qdd, nd}, {dqdd_dq, nn}, {dqdd_dqd, nn}, {dqdd_dtau, nn}}, d, n, ns, s->stream));
+  return 0;
+}
+
+static int fdd_jvp_check(tds_b200_sim* s, const void* q, int m, const void* t_q, const void* t_qd, const void* t_tau, const void* t_par,
+                         const FddOut& t) {
+  if (!s || !q || !fdd_any(t.qdd, t.dq, t.dqd, t.dtau) || m < 1 || !fdd_any(t_q, t_qd, t_tau, t_par)) return -1;
+  return par_without_installed(s, t_par, "forward dynamics derivatives jvp: parameter tangents");
+}
+
+int tds_b200_forward_dynamics_derivatives_jvp_device(tds_b200_sim* s, const float* q, const float* qd, const float* tau, int m,
+                                                     const double* t_q, const double* t_qd, const double* t_tau, const double* t_par,
+                                                     double* qdd, double* dqdd_dq, double* dqdd_dqd, double* dqdd_dtau, double* t_qdd,
+                                                     double* t_dqdd_dq, double* t_dqdd_dqd, double* t_dqdd_dtau, void* stream) {
+  const FddOut t{t_qdd, t_dqdd_dq, t_dqdd_dqd, t_dqdd_dtau};
+  if (int rc = fdd_jvp_check(s, q, m, t_q, t_qd, t_tau, t_par, t)) return rc;
+  return fdd_run(s, q, qd, tau, FddOut{qdd, dqdd_dq, dqdd_dqd, dqdd_dtau}, m, t_q, t_qd, t_tau, t_par, t, (cudaStream_t)stream);
+}
+
+int tds_b200_forward_dynamics_derivatives_jvp_host(tds_b200_sim* s, const double* q, const double* qd, const double* tau, int m,
+                                                   const double* t_q, const double* t_qd, const double* t_tau, const double* t_par,
+                                                   double* qdd, double* dqdd_dq, double* dqdd_dqd, double* dqdd_dtau, double* t_qdd,
+                                                   double* t_dqdd_dq, double* t_dqdd_dqd, double* t_dqdd_dtau) {
+  if (int rc = fdd_jvp_check(s, q, m, t_q, t_qd, t_tau, t_par, FddOut{t_qdd, t_dqdd_dq, t_dqdd_dqd, t_dqdd_dtau})) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd;
+  // tangents: host [n][dim][m] <-> device [dim * m][ns]; t_q | t_qd | t_tau | t_par | the four output tangents | the four values
+  const size_t tq = (t_q ? n_q : 0) * m, tqd = (t_qd ? nd : 0) * m, tt = (t_tau ? nd : 0) * m, tp = (size_t)(t_par ? s->par.n : 0) * m;
+  const size_t ti = tq + tqd + tt + tp, to = (nd + 3 * nn) * m;
+  const float *qd_d, *tau_d;
+  if (int rc = put_inv_inputs(s, q, qd, tau, &qd_d, &tau_d)) return rc;
+  CUDA_TRY(grow_dev(&s->jac_dev, &s->jac_dev_bytes, sizeof(double) * (ti + to + nd + 3 * nn + 1) * ns));
+  double* d = s->jac_dev;
+  double* to_d = d + ti * ns;
+  double* v_d = to_d + to * ns;
+  CUDA_TRY(put_parts<double>(d, {{t_q, tq}, {t_qd, tqd}, {t_tau, tt}, {t_par, tp}}, n, ns, s->stream));
+  const size_t r = (size_t)m * ns;
+  const FddOut o{qdd ? v_d : nullptr, dqdd_dq ? v_d + nd * ns : nullptr, dqdd_dqd ? v_d + (nd + nn) * ns : nullptr,
+                 dqdd_dtau ? v_d + (nd + 2 * nn) * ns : nullptr};
+  const FddOut t{t_qdd ? to_d : nullptr, t_dqdd_dq ? to_d + nd * r : nullptr, t_dqdd_dqd ? to_d + (nd + nn) * r : nullptr,
+                 t_dqdd_dtau ? to_d + (nd + 2 * nn) * r : nullptr};
+  if (int rc = fdd_run(s, s->q, qd_d, tau_d, o, m, t_q ? d : nullptr, t_qd ? d + tq * ns : nullptr, t_tau ? d + (tq + tqd) * ns : nullptr,
+                       t_par ? d + (tq + tqd + tt) * ns : nullptr, t, s->stream))
+    return rc;
+  CUDA_TRY(get_parts<double>({{t_qdd, nd * m}, {t_dqdd_dq, nn * m}, {t_dqdd_dqd, nn * m}, {t_dqdd_dtau, nn * m}, {qdd, nd}, {dqdd_dq, nn},
+                              {dqdd_dqd, nn}, {dqdd_dtau, nn}},
+                             to_d, n, ns, s->stream));
+  return 0;
+}
+
+static int fdd_vjp_check(tds_b200_sim* s, const void* q, const void* G_qdd, const void* G_dq, const void* G_dqd, const void* G_dtau,
+                         const void* g_q, const void* g_qd, const void* g_tau, const void* g_par) {
+  if (!s || !q || !fdd_any(G_qdd, G_dq, G_dqd, G_dtau) || !fdd_any(g_q, g_qd, g_tau, g_par)) return -1;
+  return par_without_installed(s, g_par, "forward dynamics derivatives vjp: parameter cotangents");
+}
+
+int tds_b200_forward_dynamics_derivatives_vjp_device(tds_b200_sim* s, const float* q, const float* qd, const float* tau, const double* G_qdd,
+                                                     const double* G_dq, const double* G_dqd, const double* G_dtau, double* g_q, double* g_qd,
+                                                     double* g_tau, double* g_par, void* stream) {
+  if (int rc = fdd_vjp_check(s, q, G_qdd, G_dq, G_dqd, G_dtau, g_q, g_qd, g_tau, g_par)) return rc;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd, k = s->par.n, n_in = inv_n_in(s), rows = nd + 3 * nn;
+  cudaStream_t sm = (cudaStream_t)stream;
+  // the concatenated cotangent (zero where a part is NULL), then g_q | g_qd | g_tau | g_par as one array for the contraction
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (rows + n_in + k) * s->ns));
+  double* g_d = s->vjp_g + rows * s->ns;
+  CUDA_TRY(put_parts_d2d<double>(s->vjp_g, {{G_qdd, nd}, {G_dq, nn}, {G_dqd, nn}, {G_dtau, nn}}, s->ns, sm));
+  if (int rc = fdd_vjp_run(s, q, qd, tau, s->vjp_g, g_d, g_par ? g_d + n_in * s->ns : nullptr, sm)) return rc;
+  CUDA_TRY(get_parts_d2d<double>({{g_q, n_q}, {g_qd, nd}, {g_tau, nd}, {g_par, g_par ? k : 0}}, g_d, s->ns, sm));
+  return 0;
+}
+
+int tds_b200_forward_dynamics_derivatives_vjp_host(tds_b200_sim* s, const double* q, const double* qd, const double* tau, const double* G_qdd,
+                                                   const double* G_dq, const double* G_dqd, const double* G_dtau, double* g_q, double* g_qd,
+                                                   double* g_tau, double* g_par) {
+  if (int rc = fdd_vjp_check(s, q, G_qdd, G_dq, G_dqd, G_dtau, g_q, g_qd, g_tau, g_par)) return rc;
+  if (int rc = enter_derivative_host(s)) return rc;
+  const int n = s->n, ns = s->ns;
+  const size_t n_q = s->dm[0].n_q, nd = s->dm[0].n_qd, nn = nd * nd, k = s->par.n, n_in = inv_n_in(s), rows = nd + 3 * nn;
+  const float *qd_d, *tau_d;
+  if (int rc = put_inv_inputs(s, q, qd, tau, &qd_d, &tau_d)) return rc;
+  // G (qdd | d qdd / dq | d qdd / dqd | d qdd / dtau, zero where a part is NULL) | g_q | g_qd | g_tau | g_par
+  CUDA_TRY(grow_dev(&s->vjp_g, &s->vjp_g_bytes, sizeof(double) * (rows + n_in + k + 1) * ns));
+  double* g_d = s->vjp_g + rows * ns;
+  CUDA_TRY(put_parts<double>(s->vjp_g, {{G_qdd, nd}, {G_dq, nn}, {G_dqd, nn}, {G_dtau, nn}}, n, ns, s->stream));
+  if (int rc = fdd_vjp_run(s, s->q, qd_d, tau_d, s->vjp_g, g_d, g_par ? g_d + n_in * ns : nullptr, s->stream)) return rc;
   CUDA_TRY(get_parts<double>({{g_q, n_q}, {g_qd, nd}, {g_tau, nd}, {g_par, g_par ? k : 0}}, g_d, n, ns, s->stream));
   return 0;
 }

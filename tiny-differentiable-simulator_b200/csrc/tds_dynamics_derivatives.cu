@@ -12,7 +12,7 @@
 // (the DER lanes run in MODE_NOCONTACT without PD, as INV's: no contact detection; P supplies the gravity)
 
 // d tau / dq (io->jac) and d tau / dqd (io->g_in) [n_qd * n_qd][ns] (either may be null) from io->q_in, io->qd_in and io->tau_in = qdd (either
-// of the last two may be null: zero).  M: the 8-byte layout (tds_build_layout_w(..., 8, 8, 8, -1, 8)); gscratch: ceil(n / 32) blocks of
+// of the last two may be null: zero), or qdd in fp64 from io->g_out [n_qd][ns] when that is not null (DESIGN.md section 7.24).  M: the 8-byte layout (tds_build_layout_w(..., 8, 8, 8, -1, 8)); gscratch: ceil(n / 32) blocks of
 // tds_der_layout_w(M, 8) * 128 bytes.  pm: the installed parameters, or null.
 extern "C" int tds_launch_dynamics_derivatives(const DevModel* M, const SimParams* P, const StepIO* io, const ParMap* pm, char* gscratch,
                                                cudaStream_t stream) {

@@ -196,7 +196,8 @@ template <typename T> TDS_D Tape<T> f32_round(Tape<T> x) { x.v = (T)(float)x.v; 
 // S_b . (F_i(gamma, alpha) + S x* F_i) (qd: S_b . F_i(psi, S)).  The stiffness and damping terms go into link i's own block, a spherical
 // joint's axis-angle stiffness along its three tangents by a local dual number; a floating base's own block after the sweep from the
 // whole tree's composites.  Every entry is written: zeros first, d tau / dq [n_qd * n_qd] at io.jac and d tau / dqd at io.g_in (either
-// may be null), row-major as MASS writes M.  ABA and integration are not compiled in.
+// may be null), row-major as MASS writes M.  qdd is INV's fp32 tau_in, or the fp64 io.g_out [n_qd][ns] when that is not null (the
+// forward dynamics' derivatives, section 7.24).  ABA and integration are not compiled in.
 template <typename RA, typename RC, typename RS, typename RQ, bool SMEM, bool PAR = false, bool JV = false, bool MASS = false,
           bool KIN = false, bool INV = false, bool CF = false, bool CEN = false, bool MOT = false, bool EXT = false, bool REG = false,
           bool MINV = false, bool COR = false, bool DER = false>
@@ -642,8 +643,13 @@ tds_stepw_kernel(const __grid_constant__ DevModel M, const __grid_constant__ Sim
   { RC* px = A.ptr<RC>(M.x_xw); st9<RC>(px, ST, R_base); st3<RC>(px + 9 * ST, ST, p_base); }
   if (want_contacts) emit_geoms(-1, R_base, p_base);
   if constexpr (KIN) kin_link(-1, R_base, p_base);
-  // INV: qdd of dof k (seeded at input n_q + n_qd + k); the acceleration of the previous link, of the base; the sum of the link forces
-  auto qdd_in = [&](int k) -> RQ { return seed(RQ(io.tau_in ? io.tau_in[(size_t)k * ns + e] : 0.f), M.n_q + n + k); };
+  // INV: qdd of dof k (seeded at input n_q + n_qd + k); the acceleration of the previous link, of the base; the sum of the link forces.
+  // DER reads qdd in fp64 from io.g_out [n_qd][ns] when the launch gives it (the forward dynamics' derivatives, DESIGN.md section 7.24;
+  // no DER lane reads g_out otherwise), else from tau_in as INV does.
+  auto qdd_in = [&](int k) -> RQ {
+    if constexpr (DER) { if (io.g_out) return seed(RQ(io.g_out[(size_t)k * ns + e]), M.n_q + n + k); }
+    return seed(RQ(io.tau_in ? io.tau_in[(size_t)k * ns + e] : 0.f), M.n_q + n + k);
+  };
   // (empty placeholders in the other instances, whose code must not change)
   typedef typename std::conditional<INV || MOT || DER, Sv<RC>, NoPar>::type SvInv;
   const SvInv a_base_inv = [&]() -> SvInv {

@@ -184,6 +184,16 @@ struct TdsCdynCall {
   double *qdd, *f;
 };
 
+// One call of the product kernel of the forward dynamics' derivatives (tds_fd_derivatives.cu, DESIGN.md section 7.24): from M^-1 and
+// the inverse dynamics' derivatives A_q = d tau / dq, A_qd = d tau / dqd (each [n_qd * n_qd][ns]; the dual instance also reads their
+// tangents dMi, dAq, dAqd [n_qd^2 * m][ns], each may be null: zero), the outputs dq = -M^-1 A_q, dqd = -M^-1 A_qd and dtau = M^-1
+// [n_qd * n_qd] (each may be null): values, or tangent j at row r * m_out + j0 + j.
+struct TdsFddCall {
+  int n_qd, m, j0, m_out;
+  const double *Mi, *dMi, *Aq, *dAq, *Aqd, *dAqd;
+  double *dq, *dqd, *dtau;
+};
+
 // The energy outputs of one call of the regressor instances (tds_regressor.cu, DESIGN.md section 7.19): yT [n_pi][ns] and yV [n_pi][ns]
 // (each may be null; columns of an m-column block in the JVP).  Y itself goes to StepIO::jac.
 struct TdsRegCall { double* yT; double* yV; };

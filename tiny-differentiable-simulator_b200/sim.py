@@ -1191,6 +1191,88 @@ class BatchSim:
                                                                      _ptr(G_f), _ptr(g_q), _ptr(g_qd), _ptr(g_tau), _ptr(g_par), st),
                     "constrained_dynamics_vjp_device")
 
+    # ---- derivatives of the forward dynamics (DESIGN.md section 7.24) ----
+    def forward_dynamics_derivatives_host(self, q, qd=None, tau=None):
+        """(qdd [n, n_qd], dqdd_dq, dqdd_dqd, dqdd_dtau [n, n_qd, n_qd]) float64 at the fp32-rounded q [n, n_q], qd and tau [n, n_qd] (None:
+        zero): qdd = M^-1 (tau - h) is constrained_dynamics_host's qdd without points, dqdd_dq = -M^-1 dtau_dq and dqdd_dqd = -M^-1
+        dtau_dqd with the inverse dynamics' derivatives taken at that qdd in fp64, dqdd_dtau = M^-1 (mass_inverse_host's).  Row r = qdd_r,
+        columns in M's coordinates: column k of dqdd_dq is constrained_dynamics_jvp_host along t_q = dq_dt(q, e_k) (include/tds_b200.h)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, tau = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(tau, self.n_qd, "tau")
+        n, nd = self.n_envs, self.n_qd
+        qdd, a, b, c = np.zeros((n, nd)), np.zeros((n, nd, nd)), np.zeros((n, nd, nd)), np.zeros((n, nd, nd))
+        self._check(self._L.tds_b200_forward_dynamics_derivatives_host(self._h, _dp(q), _dp(qd), _dp(tau), _dp(qdd), _dp(a), _dp(b), _dp(c)),
+                    "forward_dynamics_derivatives_host")
+        return qdd, a, b, c
+
+    def forward_dynamics_derivatives_device(self, q, qd, tau, qdd, dqdd_dq, dqdd_dqd, dqdd_dtau, stream=None):
+        """Device version of forward_dynamics_derivatives_host on the SoA layout: q float32 CUDA tensor [n_q, n_stride], qd and tau [n_qd,
+        n_stride] (either may be None); qdd [n_qd, n_stride] and the matrices [n_qd * n_qd, n_stride] float64 CUDA tensors (each may be
+        None, not all).  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_forward_dynamics_derivatives_device(self._h, _ptr(q), _ptr(qd), _ptr(tau), _ptr(qdd), _ptr(dqdd_dq),
+                                                                         _ptr(dqdd_dqd), _ptr(dqdd_dtau), st),
+                    "forward_dynamics_derivatives_device")
+
+    def forward_dynamics_derivatives_jvp_host(self, q, qd=None, tau=None, t_q=None, t_qd=None, t_tau=None, t_par=None):
+        """Directional derivatives of the four outputs of forward_dynamics_derivatives_host along m tangents t_q [n, n_q, m], t_qd and t_tau
+        [n, n_qd, m] and t_par [n, k, m] (each may be None, not all): (qdd, dqdd_dq, dqdd_dqd, dqdd_dtau, t_qdd [n, n_qd, m], t_dqdd_dq,
+        t_dqdd_dqd, t_dqdd_dtau [n, n_qd, n_qd, m]); tangents given as [n, dim] are m = 1 and drop the last axis."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, tau = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(tau, self.n_qd, "tau")
+        if all(t is None for t in (t_q, t_qd, t_tau, t_par)):
+            raise ValueError("at least one tangent is expected")
+        ts, m, single = self._tangents([(t_q, self.n_q), (t_qd, self.n_qd), (t_tau, self.n_qd), (t_par, len(self.param_ids))])
+        n, nd = self.n_envs, self.n_qd
+        vals = [np.zeros((n, nd))] + [np.zeros((n, nd, nd)) for _ in range(3)]
+        tans = [np.zeros((n, nd, m))] + [np.zeros((n, nd, nd, m)) for _ in range(3)]
+        self._check(self._L.tds_b200_forward_dynamics_derivatives_jvp_host(self._h, _dp(q), _dp(qd), _dp(tau), m, *(_dp(t) for t in ts),
+                                                                           *(_dp(x) for x in vals + tans)),
+                    "forward_dynamics_derivatives_jvp_host")
+        if single:
+            tans = [t[..., 0] for t in tans]
+        return tuple(vals + tans)
+
+    def forward_dynamics_derivatives_jvp_device(self, q, qd, tau, m, t_q, t_qd, t_tau, t_par, t_qdd, t_dqdd_dq, t_dqdd_dqd, t_dqdd_dtau,
+                                                qdd=None, dqdd_dq=None, dqdd_dqd=None, dqdd_dtau=None, stream=None):
+        """Device version of forward_dynamics_derivatives_jvp_host: q float32 [n_q, n_stride], qd and tau [n_qd, n_stride] (or None); t_q
+        [n_q * m, n_stride], t_qd and t_tau [n_qd * m, n_stride], t_par [k * m, n_stride] (each may be None, not all); t_qdd [n_qd * m,
+        n_stride] and the matrices' tangents [n_qd * n_qd * m, n_stride] (each may be None, not all), and the values (or None) float64
+        CUDA tensors, entry (r, j) at row r * m + j.  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_forward_dynamics_derivatives_jvp_device(
+            self._h, _ptr(q), _ptr(qd), _ptr(tau), int(m), _ptr(t_q), _ptr(t_qd), _ptr(t_tau), _ptr(t_par), _ptr(qdd), _ptr(dqdd_dq),
+            _ptr(dqdd_dqd), _ptr(dqdd_dtau), _ptr(t_qdd), _ptr(t_dqdd_dq), _ptr(t_dqdd_dqd), _ptr(t_dqdd_dtau), st),
+            "forward_dynamics_derivatives_jvp_device")
+
+    def forward_dynamics_derivatives_vjp_host(self, q, qd=None, tau=None, G_qdd=None, G_dq=None, G_dqd=None, G_dtau=None):
+        """Cotangents G_qdd [n, n_qd], G_dq, G_dqd, G_dtau [n, n_qd, n_qd] of the four outputs (each may be None: zero, not all) -> (g_q [n,
+        n_q], g_qd [n, n_qd], g_tau [n, n_qd], g_par [n, k] or None without installed parameters)."""
+        q = self._inv_in(q, self.n_q, "q")
+        qd, tau = self._inv_in(qd, self.n_qd, "qd"), self._inv_in(tau, self.n_qd, "tau")
+        if all(G is None for G in (G_qdd, G_dq, G_dqd, G_dtau)):
+            raise ValueError("at least one cotangent is expected")
+        n, nd, nn, k = self.n_envs, self.n_qd, self.n_qd * self.n_qd, len(self.param_ids)
+        G_qdd = None if G_qdd is None else self._inv_in(G_qdd, nd, "G_qdd")
+        G_dq, G_dqd, G_dtau = (None if G is None else self._inv_in(np.reshape(G, (n, nn)), nn, w)
+                               for G, w in ((G_dq, "G_dq"), (G_dqd, "G_dqd"), (G_dtau, "G_dtau")))
+        g_q, g_qd, g_tau = np.zeros((n, self.n_q)), np.zeros((n, nd)), np.zeros((n, nd))
+        g_par = np.zeros((n, k)) if k else None
+        self._check(self._L.tds_b200_forward_dynamics_derivatives_vjp_host(self._h, _dp(q), _dp(qd), _dp(tau), _dp(G_qdd), _dp(G_dq), _dp(G_dqd),
+                                                                           _dp(G_dtau), _dp(g_q), _dp(g_qd), _dp(g_tau), _dp(g_par)),
+                    "forward_dynamics_derivatives_vjp_host")
+        return g_q, g_qd, g_tau, g_par
+
+    def forward_dynamics_derivatives_vjp_device(self, q, qd, tau, G_qdd, G_dq, G_dqd, G_dtau, g_q, g_qd, g_tau, g_par=None, stream=None):
+        """Device version of forward_dynamics_derivatives_vjp_host: q float32 [n_q, n_stride], qd and tau [n_qd, n_stride] (or None),
+        cotangents float64 in the layouts of forward_dynamics_derivatives_device (each may be None, not all), g_q [n_q, n_stride], g_qd and
+        g_tau [n_qd, n_stride], g_par [k, n_stride] float64 CUDA tensors (each may be None, not all).  Asynchronous on the stream."""
+        st = _stream(stream)
+        self._check(self._L.tds_b200_forward_dynamics_derivatives_vjp_device(self._h, _ptr(q), _ptr(qd), _ptr(tau), _ptr(G_qdd), _ptr(G_dq),
+                                                                             _ptr(G_dqd), _ptr(G_dtau), _ptr(g_q), _ptr(g_qd), _ptr(g_tau),
+                                                                             _ptr(g_par), st),
+                    "forward_dynamics_derivatives_vjp_device")
+
     def jacobian_chunk(self):
         """Directions (Jacobian columns or JVP tangents) one launch of the dual-number step takes; more run in several launches."""
         return self._L.tds_b200_jacobian_chunk(self._h)
